@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py -- stream-updates/s of the Precise streaming-inference hot path on B200.
+"""bench.py -- stream-updates/s of the Precise streaming-inference hot path on H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams-per-gpu S] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--streams-per-gpu S] [--impl b200|reference] [--dump-outputs DIR]
 
 One "step" = one tick: every stream on the GPU receives one 1024-sample (2048-byte) chunk and is
 fully classified: PCM -> MFCC frames -> 29-step GRU scan -> sigmoid -> threshold decode -> trigger
@@ -10,7 +10,7 @@ stream-update; ``value`` = stream-updates/s over all GPUs, weak scaling (S strea
 
 Workload (``config.workload``): the per-GPU shard of BASELINE.json configs[3] (1M default-parameter
 streams over 8 GPUs; 131072 = 2^17 streams per GPU so that one tick's PCM, 268 MB, exceeds the
-126 MB L2), default 'hey-mycroft' parameters (n_fft 512, 20 filters, 13 MFCCs, GRU 20).  configs[1]
+50 MB L2 of an H100 several times over), default 'hey-mycroft' parameters (n_fft 512, 20 filters, 13 MFCCs, GRU 20).  configs[1]
 (1k streams) is reported beside it under ``small_batch`` with an explicit L2 flush between steps.
 Synthetic data: Gaussian sigma=3000 LSB int16 PCM, 1 % silent and 1 % full-scale-DC streams, seeded
 random weights (no trained model ships with the reference).
@@ -19,6 +19,8 @@ The JSON line carries ``roofline`` (MFCC kernel vs measured HBM bandwidth; per-l
 events inside the timed region), ``roofline_gru`` (fp32-FMA bound scan kernel), ``e2e`` (same metric
 through the host-buffer C-ABI call, pinned host PCM in / confidences out inside the timed region),
 ``cpu_baseline`` (the numpy oracle port on the host cores) and ``clocks``.
+
+--dump-outputs DIR: the last timed tick's outputs on rank 0 as DIR/<name>.npy (seeded inputs: builds compare output for output).
 """
 import argparse
 import json
@@ -41,12 +43,14 @@ CHUNK = 1024
 PRIME = 24                # ticks that fill a 29-frame window: (24 * 1024 - 1600) // 800 + 1 = 29 frames
 ALG_BYTES_PER_UPDATE = 2048 + 1.28 * 13 * 4           # SURVEY 8d: 2114.56 B (F=13)
 ALG_FLOP_PER_UPDATE_GRU = 2 * (29 * (13 + 20) * 60 + 20)   # 114 880
-FP32_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12     # 74.4 (148 SMs x 128 lanes x 2 x max clock)
+FP32_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12      # 66.9 (H100 SXM: 132 SMs x 128 lanes x 2 x max boost clock)
 K2_BYTES_PER_UPDATE = 29 * 240 + 4 + 8 + 1 + 8 + 1.28 * (52 + 240)   # 29 cached projection rows + raw, conf, fired, trigger state + the tick's new frames (MFCC row in, projection out)
 K2_MMA_FLOP_PER_UPDATE = 29 * 27 * (4096 + 2048) // 16   # per 16-stream tile and step 27 m16n8k16 + 27 m16n8k8 fp16 MMAs (fp16x3 split included)
-K1_NAMES = {0: 'mfcc_tc3_plan_kernel + mfcc_tc3_kernel (K1: int16 split exactly into fp16 pieces, both DFT stages on tcgen05 / TMEM) -- default from 49152 streams per tick',
-            2: 'mfcc_fast_stream_kernel<LEAN> (K1, FFT on the CUDA cores)', 3: 'mfcc_fast_stream_kernel (K1, FFT, 64-bit set-up)',
-            4: 'mfcc_tc2_stream_kernel (K1, DFT stage 2 on tcgen05)', 5: 'mfcc_tc3_plan_kernel + mfcc_tc3_kernel (K1, both DFT stages on tcgen05)'}
+K1_NAMES = {0: 'mfcc_fast_stream_kernel<LEAN> (K1, FFT on the CUDA cores)', 2: 'mfcc_fast_stream_kernel<LEAN> (K1, FFT on the CUDA cores)',
+            3: 'mfcc_fast_stream_kernel (K1, FFT, 64-bit set-up)',
+            4: 'mfcc_mma_plan_kernel + mfcc_mma_kernel<false> (K1, DFT stage 2 on mma.sync)',
+            5: 'mfcc_mma_plan_kernel + mfcc_mma_kernel<true> (K1, both DFT stages on mma.sync)',
+            6: 'mfcc_mma_plan_kernel + mfcc_mma_kernel<true, true> (K1, both DFT stages on mma.sync, shuffle epilogue)'}
 
 
 def peaks():
@@ -56,7 +60,7 @@ def peaks():
             return float(json.load(open(p))['hbm_gbs']), 'measured'
         except Exception:
             pass
-    return 6650.0, 'fallback'
+    return 3350.0, 'fallback: H100 SXM data sheet'
 
 
 def synth_pcm(n_streams, n_samples, seed, stream_offset=0):
@@ -368,6 +372,15 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------ GPU arm
+def dump_outputs(d, out, count):
+    """What StreamBatch.update returned for the last timed tick and the running detection count, as float32 / float64 .npy
+    files (S = 131072: 2.6 MB)."""
+    os.makedirs(d, exist_ok=True)
+    arrays = {'raw': out['raw'].float(), 'conf': out['conf'].double(), 'fired': out['fired'].float(), 'count': count.double().reshape(1)}
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + '.npy'), a.cpu().numpy())
+
+
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -425,9 +438,10 @@ def run_b200(args):
     def step(t):
         if flush is not None:
             flush.add_(1)                      # rewrite 256 MB: evicts L2 between iterations
-        sb.update(dev_ticks[t % NT])
+        out = sb.update(dev_ticks[t % NT])
         if world > 1:
             counter.all_reduce_overlapped()    # snapshot on this stream, NCCL on a side stream under the next tick's K1
+        return out
 
     # ---- value: inputs resident in HBM
     # Priming (untimed, before the warm-up): PRIME ticks fill every stream's 29-frame window, so that each timed update
@@ -452,7 +466,7 @@ def run_b200(args):
         barrier()
     e0.record()
     for t in range(K):
-        step(W + t)
+        last = step(W + t)
     counter.wait()                              # the last tick's all-reduce is inside the timed region
     e1.record()
     barrier()
@@ -466,6 +480,8 @@ def run_b200(args):
     value = S * world * K / (ms_all * 1e-3)
     torch.cuda.synchronize()
     total_fired = int(counter.total.item()) if world > 1 else int(sb.count.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, sb.count)
 
     # ---- e2e: host buffers through pb_update_host (H2D of the PCM and D2H of the results inside)
     pins = []
@@ -595,7 +611,7 @@ def run_b200(args):
         return
 
     hbm_peak, which = peaks()
-    k1_name = K1_NAMES.get(args.k1_mode, 'k1 mode %d' % args.k1_mode) if (args.k1_mode or S >= 49152) else K1_NAMES[2]
+    k1_name = K1_NAMES.get(args.k1_mode, 'k1 mode %d' % args.k1_mode)
     k1_ms = kms[0] / max(1, klaunch[0])
     k2_ms = kms[1] / max(1, klaunch[1])
     k1_gbs = S * ALG_BYTES_PER_UPDATE / (k1_ms * 1e-3) / 1e9 if k1_ms > 0 else None
@@ -605,13 +621,6 @@ def run_b200(args):
         bf16_peak = float(json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['bf16_tflops_sustained'])
     except Exception:
         pass
-    traffic = None
-    tp = os.path.join(ROOT, 'profiles', 'k1_traffic.json')
-    if os.path.isfile(tp):
-        try:
-            traffic = json.load(open(tp)).get('bytes_per_launch')
-        except Exception:
-            traffic = None
     line = {
         'metric': 'stream-updates/s (16 kHz int16 PCM, 1024-sample chunk -> decoded confidence + trigger)',
         'value': value, 'unit': 'stream-updates/s', 'n_gpus': world, 'steps': K, 'warmup': W,
@@ -622,10 +631,9 @@ def run_b200(args):
         'realtime_streams': value / 15.625,
         'detections': total_fired,
         'roofline': {'kernel': k1_name, 'bound': 'hbm', 'achieved': k1_gbs, 'peak': hbm_peak, 'unit': 'GB/s',
-                     'frac': (k1_gbs / hbm_peak) if k1_gbs else None, 'of': which, 'traffic': traffic,
-                     'traffic_source': 'profiles/k1_traffic.json (one ncu --set full capture of this kernel, not a live counter)' if traffic else None,
+                     'frac': (k1_gbs / hbm_peak) if k1_gbs else None, 'of': which,
                      'algorithmic_bytes_per_launch': S * ALG_BYTES_PER_UPDATE, 'ms_per_launch': k1_ms, 'launches': klaunch[0],
-                     'note': 'ms_per_launch = one tick of K1 (for the tcgen05 path: plan kernel + main kernel, both inside the CUDA-event bracket)'},
+                     'note': 'ms_per_launch = one tick of K1 (CUDA events around the launch)'},
         # K2 (scan over cached projections) against both of its ceilings: HBM for the bytes it must move (29 cached projection rows of
         # 240 B per update, the results, and the new frames' MFCC rows in / projections out) and the tensor pipe for the MMA FLOPs it
         # executes (fp16 x 3 split: 27 m16n8k16 + 27 m16n8k8 per 16 streams and step = 300 672 FLOP per update) against the measured
@@ -639,7 +647,7 @@ def run_b200(args):
                                    'frac': (S * K2_MMA_FLOP_PER_UPDATE / (k2_ms * 1e-3) / 1e12 / bf16_peak) if (bf16_peak and k2_ms > 0) else None},
                         'algorithmic_flop_per_update': ALG_FLOP_PER_UPDATE_GRU},
         'e2e': e2e,
-        'gpu_launches': int(sum(klaunch)) + (int(klaunch[0]) if (args.k1_mode in (0, 5) and S >= 49152) else 0),     # K1 on the tcgen05 path = plan kernel + main kernel
+        'gpu_launches': int(sum(klaunch)) + (int(klaunch[0]) if args.k1_mode >= 4 else 0),     # K1 on mma.sync = plan kernel + main kernel
         'cpu_baseline': ({'value': cpu[0], 'unit': 'stream-updates/s', 'cores': cpu[1], 'kind': 'port', 'sample': cpu[2]} if cpu else None),
         'cpu_baseline_c': ({'value': cpu_c[0], 'unit': 'stream-updates/s', 'cores': cpu_c[1], 'kind': 'port', 'sample': cpu_c[2]} if cpu_c else None),
         'cpu_baseline_batched': cpu_batched,
@@ -669,9 +677,13 @@ def main():
     ap.add_argument('--no-latency', dest='latency', action='store_false')
     ap.add_argument('--no-config3', dest='config3', action='store_false')
     ap.add_argument('--no-numa-bind', action='store_true', help='do not pin the process to the CPUs of its GPU\'s NUMA node')
-    ap.add_argument('--gru-mode', type=int, default=0, help='debug: 0 auto, 1 CUDA-core, 2 mma.sync, 3 tcgen05, 7 mma.sync with 32-stream tiles')
-    ap.add_argument('--k1-mode', type=int, default=0, help='debug (A/B runs only): 0 default MFCC kernel choice, 2 FFT kernel, 3 FFT kernel with 64-bit set-up, 4 tcgen05 stage 2 only, 5 both DFT stages on tcgen05')
+    ap.add_argument('--gru-mode', type=int, default=0, help='debug: 0 auto, 1 CUDA-core, 2 mma.sync, 7 mma.sync with 32-stream tiles')
+    ap.add_argument('--k1-mode', type=int, default=0, help='debug (A/B runs only): 0 default MFCC kernel choice, 2 FFT kernel, 3 FFT kernel with 64-bit set-up, 4 / 5 / 6 DFT on mma.sync (stage 2 / both stages / both with shuffle epilogue)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed tick (rank 0) as DIR/<name>.npy')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == 'reference':

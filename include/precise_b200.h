@@ -1,5 +1,5 @@
 /*
- * precise_b200.h -- C ABI of libprecise_b200.so: the B200 (sm_100a) implementation of the
+ * precise_b200.h -- C ABI of libprecise_b200.so: the H100 (sm_90a) implementation of the
  * Mycroft Precise streaming-inference hot path
  *
  *      int16 PCM -> MFCC -> GRU window scan + Dense + sigmoid -> threshold decode -> trigger
@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define PB_ABI_VERSION 1
+#define PB_ABI_VERSION 2
 #define PB_MAX_THRESHOLDS 8
 
 typedef enum pb_status {
@@ -197,29 +197,25 @@ int pb_set_cdf(pb_handle* h, const double* h_cd, int64_t len);
 int pb_debug_force_generic(pb_handle* h, int on);
 /* Test / A-B hook for the default network (H=20, F=13): 0 = automatic choice (warp-per-stream kernel up to 8192 streams per tick; above,
  * the fp16x3 mma.sync scan over bulk-copy-staged cached projections, which also projects the tick's new frames), 1 = CUDA-core
- * thread-per-stream kernel, 2 = tensor-core kernel also for small batches, 3 = tcgen05 scan, 7 = 3xTF32 scan with 32-stream warp
- * tiles, 8 = tcgen05 scan over cached projections, 9 = 3xTF32 scan over cached projections without staging, 10 = with staging,
- * 11 = the default scan at 5 CTAs per SM.  All variants are parity-tested on B200 (tests/test_gpu_parity.py). */
+ * thread-per-stream kernel, 2 = tensor-core kernel also for small batches, 7 = 3xTF32 scan with 32-stream warp tiles,
+ * 9 = 3xTF32 scan over cached projections without staging, 10 = with staging, 11 = the default scan at 5 CTAs per SM.
+ * All variants are parity-tested (tests/test_gpu_parity.py). */
 int pb_debug_gru_mode(pb_handle* h, int mode);
-/* Test / A-B hook for the stateful tick's MFCC kernel (aligned default geometry).  0 = automatic: from 49 152 streams per tick on the
- * kernel with both DFT stages on the tensor cores (csrc/mfcc_tc3.cuh: int16 samples split exactly into two fp16 pieces, tcgen05
- * MMAs with TMEM accumulators), below that the FFT kernel on the CUDA cores (csrc/mfcc_fast.cuh); 2 = always the FFT kernel;
- * 3 = the FFT kernel with its original 64-bit set-up; 4 = csrc/mfcc_tc2.cuh (radix-16 butterflies on the CUDA cores, second DFT
- * stage on tcgen05); 5 = always mfcc_tc3; 100 + w = mfcc_tc3 with the phase timeline of warp w in pb_debug_counters.  All variants
- * are parity-tested on B200 (tests/test_gpu_parity.py). */
+/* Test / A-B hook for the stateful tick's MFCC kernel (aligned default geometry).  0 = automatic: the FFT kernel on the CUDA
+ * cores (csrc/mfcc_fast.cuh) where the geometry allows it, else the generic kernel; 2 = always the FFT kernel; 3 = the FFT kernel
+ * with its original 64-bit set-up; 4 / 5 / 6 = csrc/mfcc_mma.cuh, the DFT on mma.sync (stage 2 / both stages / both with a
+ * shuffle epilogue; hop >= 512, chunk >= hop).  All variants are parity-tested (tests/test_gpu_parity.py). */
 int pb_debug_k1_mode(pb_handle* h, int mode);
-/* CPU model of that kernel's DFT for one frame of 512 int16 samples -> |X[k]|^2, k = 0..256 (same butterfly, operand tables
- * and layout arithmetic; no device needed).  Test hook. */
+/* CPU model of a tensor-core formulation of the DFT (csrc/mfcc_tc.cuh: radix-16 butterflies, second stage as an fp16 hi / lo
+ * matrix product) for one frame of 512 int16 samples -> |X[k]|^2, k = 0..256.  No device needed.  Test hook. */
 int pb_debug_tc_dft_power(const int16_t* x512, double* power257);
-/* ... and of the whole kernel for one frame (accumulators + mel / log / DCT epilogue with the tables this configuration
- * would upload) -> out[min(n_filt, n_mfcc)].  No device needed.  Test hook. */
+/* CPU model of the k1 mode 4-6 kernel's DFT (csrc/mfcc_mma.cuh, its own tables) -> |X[k]|^2, k = 0..256.  Test hook. */
+int pb_debug_mma_dft_power(const int16_t* x512, double* power257);
+/* ... and of the whole MFCC for one frame (accumulators + mel / log / DCT epilogue with the tables of this configuration) -> out[min(n_filt, n_mfcc)].  No device needed.  Test hook. */
 int pb_debug_tc_mfcc_frame(const pb_config* cfg, const int16_t* x512, float* out);
-/* The same for k1 mode 5 (csrc/mfcc_tc3.cuh: both DFT stages on the tensor cores, int16 split exactly into two fp16 pieces);
- * power257 (optional) receives |X[k]|^2 of the raw samples as that kernel's accumulators hold it.  No device needed.  Test hook. */
+/* The same with both DFT stages as matrix products (csrc/mfcc_tc3.cuh: int16 split exactly into two fp16 pieces);
+ * power257 (optional) receives |X[k]|^2 of the raw samples as the model's accumulators hold it.  No device needed.  Test hook. */
 int pb_debug_tc3_mfcc_frame(const pb_config* cfg, const int16_t* x512, float* out, double* power257);
-/* Test/profiling hook: the first call arms, later calls read four device-side cycle counters of the wide-network
- * tensor-core kernel's MMA-issuer thread (operand wait, weight-tile wait, issue, total) for CTA 0. */
-int pb_debug_counters(pb_handle* h, long long out[4]);
 
 const char* pb_last_error(void);
 int pb_abi_version(void);

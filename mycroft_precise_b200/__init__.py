@@ -1,4 +1,4 @@
-"""mycroft_precise_b200 -- B200 (sm_100a) implementation of Mycroft Precise's streaming-inference
+"""mycroft_precise_b200 -- H100 (sm_90a) implementation of Mycroft Precise's streaming-inference
 hot path (MFCC -> GRU window scan -> threshold decode -> trigger) behind the reference's own
 interfaces.  The compute lives in csrc/libprecise_b200.so (hand-written CUDA, C ABI declared in
 include/precise_b200.h); this package is the thin Python host that mirrors

@@ -12,7 +12,7 @@ from .params import ListenerParams
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 PB_MAX_THRESHOLDS = 8
-PB_ABI_VERSION = 1
+PB_ABI_VERSION = 2
 
 
 class PBError(RuntimeError):
@@ -65,9 +65,9 @@ SYMBOLS = {
     'pb_debug_gru_mode': (C.c_int, [_VP, C.c_int]),
     'pb_debug_k1_mode': (C.c_int, [_VP, C.c_int]),
     'pb_debug_tc_dft_power': (C.c_int, [_VP, _VP]),
+    'pb_debug_mma_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_tc_mfcc_frame': (C.c_int, [_VP, _VP, _VP]),
     'pb_debug_tc3_mfcc_frame': (C.c_int, [_VP, _VP, _VP, _VP]),
-    'pb_debug_counters': (C.c_int, [_VP, C.POINTER(C.c_longlong)]),
     'pb_last_error': (C.c_char_p, []),
     'pb_abi_version': (C.c_int, []),
     'pb_build_info': (C.c_char_p, []),
@@ -369,11 +369,6 @@ class PreciseB200:
                                       C.cast(C.byref(cnt), C.c_void_p)))
         return int(cnt.value)
 
-    def debug_counters(self):
-        out = (C.c_longlong * 4)()
-        check(self.lib.pb_debug_counters(self._h, out))
-        return list(out)
-
     def gru_mode(self, mode):
         check(self.lib.pb_debug_gru_mode(self._h, int(mode)))
 
@@ -381,7 +376,8 @@ class PreciseB200:
         check(self.lib.pb_debug_force_generic(self._h, int(on)))
 
     def k1_mode(self, mode):
-        """1 = experimental tensor-core DFT tick (csrc/mfcc_tc.cuh, not yet validated on hardware), 0 = default kernels."""
+        """0 = default MFCC kernel choice, 2 = the FFT kernel, 3 = the FFT kernel with its 64-bit set-up, 4 / 5 / 6 = the DFT on
+        mma.sync (stage 2 only / both stages / both stages with a shuffle epilogue)."""
         check(self.lib.pb_debug_k1_mode(self._h, int(mode)))
 
     # ---- profiling / introspection

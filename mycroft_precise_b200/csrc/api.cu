@@ -19,13 +19,12 @@
 
 #include "../../include/precise_b200.h"
 #include "gru_kernels.cuh"
+#include "gru_wide.cuh"
 #include "mfcc_kernels.cuh"
 #include "mfcc_fast.cuh"
-#include "gru_tc5.cuh"
-#include "gru_tc5_big.cuh"
 #include "mfcc_tc.cuh"
-#include "mfcc_tc2.cuh"
 #include "mfcc_tc3.cuh"
+#include "mfcc_mma.cuh"
 
 using namespace pb;
 
@@ -63,7 +62,7 @@ struct ProfSlot {
 
 struct pb_handle {
     pb_config cfg;
-    int sm_count = 148;
+    int sm_count = 132;
     // derived
     int used = 0, n_bins = 0, n_out = 0, feat = 0, ring_rows = 0, row_stride = 0, tail_cap = 0, max_new = 0;
     int rel_window = 0;              // samples before frame 0 is released: window_samples (sonopy), window_samples + hop_samples (speechpy drops the last complete frame)
@@ -74,16 +73,12 @@ struct pb_handle {
     float *d_proj_w = nullptr, *d_proj_b = nullptr;
     size_t k1_batch_smem = 0, k1_stream_smem = 0, k1_fast_smem = 0;
     bool force_generic = false;      // tests: exercise the generic kernels on the aligned geometry
-    int k1_mode = 0;                 // 0 = default (mfcc_tc3 from TC3_MIN_STREAMS streams per tick on, else the FFT kernel with 32-bit set-up), 2 = always the FFT kernel, 3 = FFT kernel with the original 64-bit set-up, 4 = tcgen05 stage-2 kernel (mfcc_tc2), 5 = both DFT stages on tcgen05 (mfcc_tc3), 100 + w = 5 with warp w's timeline
-    bool tcd_ok = false;             // geometry the tensor-core DFT tables cover (CPU model + kernel)
-    bool tc2_ok = false;             // ... and by mfcc_tc2_stream_kernel<Tc2Geo20> (run-time mel tables equal its compile-time ones)
-    std::vector<float> h_wrise, h_wfall; std::vector<int> h_grid;      // host copies for the lazily built tcd tables
-    uint4* d_tcd_b = nullptr; float* d_tcd_tw = nullptr; float* d_tcd_dct = nullptr;
-    bool tc3_ok = false;             // ... and by mfcc_tc3_kernel<Tc2Geo20> (both DFT stages on the tensor cores; needs chunk >= hop)
-    uint4 *d_tc3_b1 = nullptr, *d_tc3_b2 = nullptr; float* d_tc3_tw = nullptr;
-    Tc3Rec* d_tc3_recs = nullptr; unsigned int* d_tc3_counters = nullptr;
-    int tc3_parity = 0;              // which of the two frame counters the next tick's plan kernel fills
-    float tcd_tot_scale = 0.f;
+    int k1_mode = 0;                 // 0 = default (the FFT kernel with 32-bit set-up where the geometry allows it), 2 = always the FFT kernel, 3 = FFT kernel with the original 64-bit set-up, 4 / 5 / 6 = the mma.sync DFT tick (mfcc_mma.cuh): stage 1 on the CUDA cores / on the tensor cores / the latter with a shuffle epilogue
+    bool mma_ok = false;             // geometry mfcc_mma_kernel covers (n_fft = frame = 512, hop >= 512, chunk >= hop, MFCC vectorizer)
+    uint2 *d_mm_b1 = nullptr, *d_mm_b2 = nullptr; float2* d_mm_tw = nullptr;
+    MmRec* d_mm_recs = nullptr; unsigned int* d_mm_counters = nullptr;
+    int mm_parity = 0;               // which of the two frame counters the next tick's plan kernel fills
+    std::vector<float> h_wrise, h_wfall; std::vector<int> h_grid;      // mel tables of the CPU model of the matrix-product DFT (pb_debug_tc*_mfcc_frame)
     bool fast_ok = false;            // aligned geometry: warp-autonomous kernels (mfcc_fast.cuh)
     int npl = 0, maxc = 0, nol = 0;
     float4* d_ptab = nullptr;
@@ -109,12 +104,10 @@ struct pb_handle {
     uint4* d_bfrag16 = nullptr;      // ... recurrent part as fp16 hi / lo fragments (gru_mma16_kernel)
     uint4* d_xfrag16 = nullptr;      // ... and the input part (the scan projects a tick's new frames itself)
     float *d_mma_bias = nullptr, *d_mma_wd = nullptr;
-    long long* d_dbg = nullptr;       // optional debug counters (pb_debug_counters)
-    float *d_tcb = nullptr;           // tcgen05 wide-network GRU: [b1 tiles | b2 tiles | bias(384) | wd(128)]
-    bool tcb_ok = false;
-    int tcb_kx = 0;
-    float *d_tc5 = nullptr;           // tcgen05 GRU: [b1_hi | b1_lo | b2_hi | b2_lo | bias(80) | wd(24)]
-    int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core small kernel, 2 = force tensor-core kernel, 3 = tcgen05 scan, 7 = tensor-core kernel with 32-stream warp tiles, 8 = tcgen05 scan over cached projections (opt-in, unvalidated)
+    bool wide_ok = false;            // gru_wide_kernel covers the network (H <= 128, F <= 40)
+    int wg_fp = 0, wg_hp = 0;
+    uint4 *d_wg_b1 = nullptr, *d_wg_b2 = nullptr; float* d_wg_bias = nullptr;
+    int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core kernel, 2 = force tensor-core kernel, 7 = tensor-core kernel with 32-stream warp tiles, 9 / 10 / 11 = A/B variants of the cached-projection scan
     float bd = 0.f;
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -240,7 +233,7 @@ static cudaError_t ensure_dyn_smem(K kernel, size_t bytes) {
 
 PB_API int pb_abi_version(void) { return PB_ABI_VERSION; }
 PB_API const char* pb_last_error(void) { return g_err; }
-PB_API const char* pb_build_info(void) { return "precise_b200 sm_100a " __DATE__ " " __TIME__; }
+PB_API const char* pb_build_info(void) { return "precise_b200 sm_90a " __DATE__ " " __TIME__; }
 
 PB_API int pb_config_default(pb_config* cfg) {
     if (!cfg) return fail(PB_ERR_INVALID, "cfg is null");
@@ -274,12 +267,12 @@ PB_API void pb_destroy(pb_handle* h) {
     if (!h) return;
     cudaSetDevice(h->cfg.device);
     cudaFree(h->d_wrise); cudaFree(h->d_wfall); cudaFree(h->d_dct); cudaFree(h->d_grid);
-    cudaFree(h->d_tcd_b); cudaFree(h->d_tcd_tw); cudaFree(h->d_tcd_dct);
-    cudaFree(h->d_tc3_b1); cudaFree(h->d_tc3_b2); cudaFree(h->d_tc3_tw); cudaFree(h->d_tc3_recs); cudaFree(h->d_tc3_counters);
+    cudaFree(h->d_mm_b1); cudaFree(h->d_mm_b2); cudaFree(h->d_mm_tw); cudaFree(h->d_mm_recs); cudaFree(h->d_mm_counters);
+    cudaFree(h->d_wg_b1); cudaFree(h->d_wg_b2); cudaFree(h->d_wg_bias);
     cudaFree(h->d_tw_stage); cudaFree(h->d_tw_post); cudaFree(h->d_tw_any); cudaFree(h->d_cd); cudaFree(h->d_ptab); cudaFree(h->d_ctab); cudaFree(h->d_dct_t);
     cudaFree(h->st.n_samples); cudaFree(h->st.tail); cudaFree(h->st.ring); cudaFree(h->st.trig);
     cudaFree(h->d_wcat); cudaFree(h->d_bias); cudaFree(h->d_wd); cudaFree(h->d_count);
-    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_bfrag); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd); cudaFree(h->d_proj_w); cudaFree(h->d_proj_b); cudaFree(h->d_proj_ring); cudaFree(h->d_tc5); cudaFree(h->d_tcb); cudaFree(h->d_dbg);
+    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_bfrag); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd); cudaFree(h->d_proj_w); cudaFree(h->d_proj_b); cudaFree(h->d_proj_ring);
     if (h->h_count_pinned) cudaFreeHost(h->h_count_pinned);
     for (int i = 0; i < HOST_PIPE; ++i) {
         cudaFree(h->d_stage_pcm[i]); cudaFree(h->d_stage_ids[i]); cudaFree(h->d_stage_raw[i]);
@@ -382,13 +375,8 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
         for (int pp = seg_first[j + 1]; pp < seg_first[j + 2]; ++pp) ctab[(size_t)j * h->maxc + w++] = (unsigned char)(64 + pp);
     }
     h->fast_ok = c.n_fft == 512 && h->used == 512 && c.hop_samples % 8 == 0 && n_pieces <= 64 && h->npl <= 4;
-    h->h_wrise = wrise; h->h_wfall = wfall; h->h_grid = grid;
-    h->tcd_ok = h->fast_ok && c.vectorizer == PB_VEC_MFCCS && c.n_filt <= TCD_MAX_FILT && h->n_out <= TCD_MAX_OUT &&
-                c.chunk_samples % 8 == 0 && c.chunk_samples >= 512 && (c.chunk_samples + c.hop_samples - 1) / c.hop_samples <= TC2_MAX_NEW;
-    h->tc2_ok = h->tcd_ok && c.hop_samples >= 512 && c.hop_samples <= 16384 && h->ring_rows <= 255 && h->n_out >= 1 &&
-                (c.chunk_samples + c.hop_samples - 1) / c.hop_samples <= TC2_MAX_NEW &&
-                tc2_geo_matches<Tc2Geo20>(c.n_filt, h->n_bins, grid, wrise, wfall);
-    h->tc3_ok = h->tc2_ok && c.chunk_samples >= c.hop_samples && c.chunk_samples <= 32760;
+    h->mma_ok = h->fast_ok && c.vectorizer == PB_VEC_MFCCS && c.n_filt <= MM_MAX_FILT && h->n_out <= MM_MAX_FILT && !c.use_delta &&
+                c.chunk_samples % 8 == 0 && c.hop_samples >= 512 && c.chunk_samples >= c.hop_samples && c.chunk_samples <= 32760;
     h->k1_fast_smem = K1F_WARPS * sizeof(K1FWarp) + (size_t)h->npl * 128 * sizeof(float4) +
                       (size_t)c.n_filt * 16 * h->nol * sizeof(float) + (((size_t)c.n_filt * h->maxc + 15) & ~(size_t)15);
     // DCT-II, norm='ortho' (scipy.fftpack.dct as sonopy.mfcc_spec calls it), first n_out rows
@@ -578,6 +566,7 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
             CK(upload(&h->d_xfrag16, xf16));
             CK(ensure_dyn_smem(gru_mma16_kernel<20, 13, 4>, (size_t)K2_STAGED_SMEM));
             CK(ensure_dyn_smem(gru_mma16_kernel<20, 13, 5>, (size_t)K2_STAGED_SMEM));
+            CK(ensure_dyn_smem(gru_mma_kernel<20, 13, true, true, 1, true>, (size_t)K2_STAGED_SMEM));
         }
         {   // input projection table: wx[f][col], col = gate * 24 + unit (same column order as the accumulator tiles)
             std::vector<float> pw((size_t)F * PROJ_COLS, 0.f), pbias(PROJ_COLS, 0.f);
@@ -599,77 +588,51 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
         CK(upload(&h->d_bfrag, bf));
         CK(upload(&h->d_mma_bias, mb));
         CK(upload(&h->d_mma_wd, mw));
-        {   // tcgen05 operand tiles (gru_tc5.cuh): B[k/4][n][k%4], k = x feature (0..15) then hidden unit (16..39)
-            const int n1 = TC5_N1, n2 = TC5_N2, sz1 = 10 * n1 * 4, sz2 = 10 * n2 * 4;
-            std::vector<float> t((size_t)2 * sz1 + 2 * sz2 + 80 + 24, 0.f);
-            float *b1h = t.data(), *b1l = b1h + sz1, *b2h = b1l + sz1, *b2l = b2h + sz2, *tb = b2l + sz2, *tw = tb + 80;
-            auto wv = [&](int k, int gate, int unit) -> float {
-                if (unit >= H) return 0.f;
-                if (k < 16) return k < F ? kernel[(size_t)k * H3 + gate * H + unit] : 0.f;
-                const int hu = k - 16;
-                return hu < H ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
-            };
-            for (int k = 0; k < 40; ++k) {
-                for (int c = 0; c < n1; ++c) {
-                    const float v = wv(k, c / 24, c % 24), vh = tf32(v);
-                    b1h[((size_t)(k / 4) * n1 + c) * 4 + k % 4] = vh;
-                    b1l[((size_t)(k / 4) * n1 + c) * 4 + k % 4] = tf32(v - vh);
-                }
-                for (int c = 0; c < n2; ++c) {
-                    const float v = wv(k, 2, c), vh = tf32(v);
-                    b2h[((size_t)(k / 4) * n2 + c) * 4 + k % 4] = vh;
-                    b2l[((size_t)(k / 4) * n2 + c) * 4 + k % 4] = tf32(v - vh);
-                }
-            }
-            for (int u = 0; u < H; ++u) { tb[u] = bias[u]; tb[24 + u] = bias[H + u]; tb[48 + u] = bias[2 * H + u]; tw[u] = dense_w[u]; }
-            cudaFree(h->d_tc5); h->d_tc5 = nullptr;
-            CK(upload(&h->d_tc5, t));
-            CK(ensure_dyn_smem(gru_mma_kernel<20, 13, true, true, 1, true>, (size_t)K2_STAGED_SMEM));
-            CK(ensure_dyn_smem(gru_tc5_kernel<20, 13, true>, (size_t)(sizeof(Tc5Smem) + 128)));
-            CK(ensure_dyn_smem(gru_tc5_kernel<20, 13, false>, (size_t)(sizeof(Tc5Smem) + 128)));
-            CK(ensure_dyn_smem(gru_tc5_kernel<20, 13, true, true>, (size_t)(sizeof(Tc5Smem) + 128)));
-        }
         memcpy(h->w_small.W, kernel, sizeof(h->w_small.W));
         memcpy(h->w_small.U, recurrent, sizeof(h->w_small.U));
         memcpy(h->w_small.b, bias, sizeof(h->w_small.b));
         memcpy(h->w_small.wd, dense_w, sizeof(h->w_small.wd));
         h->w_small.bd = dense_b;
     } else {
-        h->tcb_ok = H <= TCB_HP && F <= 8 * TCB_MAX_KX && !h->cfg.use_delta;
-        if (h->tcb_ok) {
-            // weight tiles of gru_tcb_kernel: per k-step s one contiguous tile [hi: chunk0[N][4], chunk1[N][4] | lo: same];
-            // k-step s < kx covers x features 8s..8s+7, s >= kx hidden units 8(s-kx)..; phase 1: N = 256 (z | r), phase 2: N = 128
+        h->wide_ok = H <= WG_MAX_H && F <= WG_MAX_F;
+        if (h->wide_ok) {
+            // fragment-ordered, TF32-split weights of gru_wide_kernel: k = 8 s + t (+ 4) is x feature k (k < FP) or hidden unit k - FP;
+            // phase-1 column n = 8 nt + g is z unit n (n < HP) or r unit n - HP, phase-2 column n is candidate unit n
             auto tf32 = [](float x) { uint32_t u; memcpy(&u, &x, 4); u = (u + 0x1000u) & 0xffffe000u; float r; memcpy(&r, &u, 4); return r; };
-            const int kx = (F + 7) / 8, ks = kx + TCB_KH;
-            h->tcb_kx = kx;
-            std::vector<float> t((size_t)ks * 4096 + (size_t)ks * 2048 + 3 * TCB_HP + TCB_HP, 0.f);
-            float* b1 = t.data(); float* b2 = b1 + (size_t)ks * 4096; float* tb = b2 + (size_t)ks * 2048; float* tw = tb + 3 * TCB_HP;
-            auto wv = [&](int s, int j, int gate, int unit) -> float {
+            const int FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
+            h->wg_fp = FP; h->wg_hp = HP;
+            auto wv = [&](int k, int gate, int unit) -> float {
                 if (unit >= H) return 0.f;
-                if (s < kx) { const int f = 8 * s + j; return f < F ? kernel[(size_t)f * H3 + gate * H + unit] : 0.f; }
-                const int hu = 8 * (s - kx) + j;
+                if (k < FP) return k < F ? kernel[(size_t)k * H3 + gate * H + unit] : 0.f;
+                const int hu = k - FP;
                 return hu < H ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
             };
-            for (int s = 0; s < ks; ++s)
-                for (int j = 0; j < 8; ++j) {
-                    for (int c = 0; c < 256; ++c) {
-                        const float v = wv(s, j, c / TCB_HP, c % TCB_HP), vh = tf32(v);
-                        const size_t o = (size_t)s * 4096 + ((size_t)(j / 4) * 256 + c) * 4 + j % 4;
-                        b1[o] = vh; b1[o + 2048] = tf32(v - vh);
+            auto frag = [&](int s, int lane, int gate, int unit) {
+                const int t = lane & 3;
+                const float v0 = wv(8 * s + t, gate, unit), v1 = wv(8 * s + t + 4, gate, unit);
+                const float h0 = tf32(v0), h1 = tf32(v1), l0 = tf32(v0 - h0), l1 = tf32(v1 - h1);
+                uint4 r; memcpy(&r.x, &h0, 4); memcpy(&r.y, &h1, 4); memcpy(&r.z, &l0, 4); memcpy(&r.w, &l1, 4);
+                return r;
+            };
+            std::vector<uint4> b1((size_t)KS * (HP / 4) * 32), b2((size_t)KS * (HP / 8) * 32);
+            for (int s = 0; s < KS; ++s)
+                for (int lane = 0; lane < 32; ++lane) {
+                    for (int nt = 0; nt < HP / 4; ++nt) {
+                        const int c = 8 * nt + (lane >> 2);
+                        b1[((size_t)s * (HP / 4) + nt) * 32 + lane] = frag(s, lane, c < HP ? 0 : 1, c % HP);
                     }
-                    for (int c = 0; c < 128; ++c) {
-                        const float v = wv(s, j, 2, c), vh = tf32(v);
-                        const size_t o = (size_t)s * 2048 + ((size_t)(j / 4) * 128 + c) * 4 + j % 4;
-                        b2[o] = vh; b2[o + 1024] = tf32(v - vh);
-                    }
+                    for (int nt = 0; nt < HP / 8; ++nt) b2[((size_t)s * (HP / 8) + nt) * 32 + lane] = frag(s, lane, 2, 8 * nt + (lane >> 2));
                 }
-            for (int g = 0; g < 3; ++g)
-                for (int u = 0; u < H; ++u) tb[g * TCB_HP + u] = bias[g * H + u];
-            for (int u = 0; u < H; ++u) tw[u] = dense_w[u];
-            cudaFree(h->d_tcb); h->d_tcb = nullptr;
-            CK(upload(&h->d_tcb, t));
-            CK(ensure_dyn_smem(gru_tcb_kernel<true>, (size_t)(sizeof(TcbSmem) + 128)));
-            CK(ensure_dyn_smem(gru_tcb_kernel<false>, (size_t)(sizeof(TcbSmem) + 128)));
+            std::vector<float> wb((size_t)3 * HP, 0.f);
+            for (int g3 = 0; g3 < 3; ++g3)
+                for (int u = 0; u < H; ++u) wb[(size_t)g3 * HP + u] = bias[g3 * H + u];
+            cudaFree(h->d_wg_b1); cudaFree(h->d_wg_b2); cudaFree(h->d_wg_bias);
+            h->d_wg_b1 = h->d_wg_b2 = nullptr; h->d_wg_bias = nullptr;
+            CK(upload(&h->d_wg_b1, b1));
+            CK(upload(&h->d_wg_b2, b2));
+            CK(upload(&h->d_wg_bias, wb));
+            CK(ensure_dyn_smem(gru_wide_kernel<true>, wg_smem(FP, HP)));
+            CK(ensure_dyn_smem(gru_wide_kernel<false>, wg_smem(FP, HP)));
         }
         size_t smem = (size_t)(F + 3 * H) * K2_TILE_STREAMS * sizeof(float);
         if (smem > 200 * 1024) return fail(PB_ERR_UNSUPPORTED, "feature_size + 3*hidden = %d is too large for the tiled GRU kernel", F + 3 * H);
@@ -705,30 +668,19 @@ struct ProfScope {
     ~ProfScope() { if (idx >= 0) cudaEventRecord(h->prof[slot].ev[idx + 1], s); }
 };
 
-PB_API int pb_debug_counters(pb_handle* h, long long out[4]) {
-    if (!h || !out) return fail(PB_ERR_INVALID, "null argument");
-    CK(cudaSetDevice(h->cfg.device));
-    if (!h->d_dbg) { CK(cudaMalloc((void**)&h->d_dbg, 4 * sizeof(long long))); CK(cudaMemset(h->d_dbg, 0, 4 * sizeof(long long))); }
-    CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(out, h->d_dbg, 4 * sizeof(long long), cudaMemcpyDeviceToHost));
-    return PB_OK;
-}
-
 PB_API int pb_debug_gru_mode(pb_handle* h, int mode) { if (!h) return fail(PB_ERR_INVALID, "null handle"); h->gru_mode = mode; return PB_OK; }
 
 PB_API int pb_debug_k1_mode(pb_handle* h, int mode) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
-    if (mode >= 100 && mode <= 116 && h->tc3_ok) { h->k1_mode = mode; return PB_OK; }      // mode 5 with the phase timeline of warp (mode - 100) in pb_debug_counters
-    if (mode < 0 || mode > 6 || mode == 1) return fail(PB_ERR_INVALID, "k1 mode must be 0 (automatic), 2 (FFT kernel, lean set-up), 3 (FFT kernel), 4 (tensor-core DFT kernel, stage 2 only) or 5 (both DFT stages on the tensor cores)");
-    if (mode >= 5 && mode <= 6 && !h->tc3_ok) return fail(PB_ERR_UNSUPPORTED, "the two-stage tensor-core MFCC tick needs the default mel geometry, hop >= 512 and chunk >= hop, a multiple of 8");
-    if (mode == 4 && !h->tc2_ok) return fail(PB_ERR_UNSUPPORTED, "the tensor-core MFCC tick needs the default mel geometry (20 filters, 16 kHz, n_fft 512), chunk >= 512 and a multiple of 8");
-    if (mode == 2 && !h->fast_ok) return fail(PB_ERR_UNSUPPORTED, "k1 mode 2 needs the aligned geometry of the fast MFCC kernels");
+    if (mode < 0 || mode > 6 || mode == 1) return fail(PB_ERR_INVALID, "k1 mode must be 0 (automatic), 2 (FFT kernel, lean set-up), 3 (FFT kernel), 4 (tensor-core DFT stage 2), 5 (both DFT stages on the tensor cores) or 6 (5 with a shuffle epilogue)");
+    if (mode >= 4 && !h->mma_ok) return fail(PB_ERR_UNSUPPORTED, "the tensor-core MFCC tick needs n_fft = 512 = frame length, hop >= 512 (a multiple of 8), chunk >= hop (a multiple of 8), n_filt <= 32, MFCC vectorizer");
+    if ((mode == 2 || mode == 3) && !h->fast_ok) return fail(PB_ERR_UNSUPPORTED, "k1 mode 2 needs the aligned geometry of the fast MFCC kernels");
     h->k1_mode = mode;
     return PB_OK;
 }
 
-// CPU model of the tensor-core DFT for one 512-sample frame (mfcc_tc.cuh: same butterfly, same operand tables and layout
-// arithmetic as the kernel).  No device needed; used by the CPU tests to pin the host-side half of that design.
+// CPU model of the matrix-product DFT for one 512-sample frame (mfcc_tc.cuh: butterfly, operand tables and layout arithmetic
+// of a tensor-core formulation).  No device needed; used by the CPU tests to pin that design.
 PB_API int pb_debug_tc_dft_power(const int16_t* x512, double* power257) {
     if (!x512 || !power257) return fail(PB_ERR_INVALID, "null argument");
     tcd_host_power(x512, power257);
@@ -737,8 +689,8 @@ PB_API int pb_debug_tc_dft_power(const int16_t* x512, double* power257) {
 
 static void tcd_host_tables(const pb_handle* h, std::vector<float4>& etab, std::vector<float>& dct, float* tot_scale);
 
-// CPU model of the whole experimental kernel for one frame: accumulator row (as above) + the epilogue (mel, log, DCT, c0) with
-// the tables a handle of this configuration would upload.  Needs no device: only the mel-table part of pb_create runs.
+// CPU model of the whole matrix-product MFCC for one frame: accumulator row (as above) + the epilogue (mel, log, DCT, c0) with
+// the tables of a handle of this configuration.  Needs no device: only the mel-table part of pb_create runs.
 PB_API int pb_debug_tc_mfcc_frame(const pb_config* cfg, const int16_t* x512, float* out) {
     if (!cfg || !x512 || !out) return fail(PB_ERR_INVALID, "null argument");
     if (cfg->n_fft != 512 || cfg->n_filt < 1 || cfg->n_filt > TCD_MAX_FILT || cfg->vectorizer != PB_VEC_MFCCS)
@@ -762,7 +714,7 @@ PB_API int pb_debug_tc_mfcc_frame(const pb_config* cfg, const int16_t* x512, flo
     return rc;
 }
 
-// ... and of the kernel with both DFT stages on the tensor cores (mfcc_tc3.cuh): exact int16 split, stage-1 matrix passes, twiddle,
+// ... and of the formulation with both DFT stages as matrix products (mfcc_tc3.cuh): exact int16 split, stage-1 matrix passes, twiddle,
 // fp16 split, stage-2 passes, its own epilogue order.  No device needed.  Test hook.
 PB_API int pb_debug_tc3_mfcc_frame(const pb_config* cfg, const int16_t* x512, float* out, double* power257) {
     if (!cfg || !x512 || !out) return fail(PB_ERR_INVALID, "null argument");
@@ -796,6 +748,13 @@ PB_API int pb_debug_tc3_mfcc_frame(const pb_config* cfg, const int16_t* x512, fl
     }
     delete h;
     return rc;
+}
+
+// CPU model of the mma.sync MFCC tick's DFT (mfcc_mma.cuh: its fragment tables, splits and bin assembly) for one frame.  Test hook.
+PB_API int pb_debug_mma_dft_power(const int16_t* x512, double* power257) {
+    if (!x512 || !power257) return fail(PB_ERR_INVALID, "null argument");
+    mm_host_power(x512, power257);
+    return PB_OK;
 }
 
 PB_API int pb_debug_force_generic(pb_handle* h, int on) { if (!h) return fail(PB_ERR_INVALID, "null handle"); h->force_generic = on != 0; return PB_OK; }
@@ -901,16 +860,6 @@ static int launch_gru(pb_handle* h, const K2In& in, bool ring, int64_t n, const 
         const int grid = (int)((n + 3) / 4);
         if (ring) gru_warp_kernel<20, 13, true><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
         else gru_warp_kernel<20, 13, false><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
-    } else if (h->small_path && (h->gru_mode == 3 || h->gru_mode == 8)) {   // tcgen05 + TMEM scan (8: over cached projections, opt-in)
-        GruTc5W w;
-        const int sz1 = 10 * TC5_N1 * 4, sz2 = 10 * TC5_N2 * 4;
-        w.b1_hi = h->d_tc5; w.b1_lo = w.b1_hi + sz1; w.b2_hi = w.b1_lo + sz1; w.b2_lo = w.b2_hi + sz2;
-        w.bias = w.b2_lo + sz2; w.wd = w.bias + 80; w.bd = h->bd;
-        const int grid = (int)((n + TC5_THREADS - 1) / TC5_THREADS);
-        const size_t smem = sizeof(Tc5Smem) + 128;
-        if (ring && in.proj != nullptr && h->gru_mode == 8) gru_tc5_kernel<20, 13, true, true><<<grid, TC5_BLOCK, smem, s>>>(w, in, n, dp, o);
-        else if (ring) gru_tc5_kernel<20, 13, true><<<grid, TC5_BLOCK, smem, s>>>(w, in, n, dp, o);
-        else gru_tc5_kernel<20, 13, false><<<grid, TC5_BLOCK, smem, s>>>(w, in, n, dp, o);
     } else if (h->small_path && h->gru_mode != 1) {               // tensor-core scan (mma.sync TF32 x3)
         GruMmaW w;
         w.bfrag = h->d_bfrag; w.bias = h->d_mma_bias; w.wd = h->d_mma_wd; w.bd = h->bd;
@@ -941,16 +890,14 @@ static int launch_gru(pb_handle* h, const K2In& in, bool ring, int64_t n, const 
         const int grid = (int)((n + per_cta - 1) / per_cta);
         if (ring) gru_small_kernel<20, 13, true><<<grid, K2_SMALL_THREADS, 0, s>>>(h->w_small, in, n, dp, o);
         else gru_small_kernel<20, 13, false><<<grid, K2_SMALL_THREADS, 0, s>>>(h->w_small, in, n, dp, o);
-    } else if (h->tcb_ok && h->gru_mode != 1) {                    // wide network on tcgen05 + TMEM, weights via TMA pipeline
-        GruTcbW w;
-        const int ks = h->tcb_kx + TCB_KH;
-        w.b1 = h->d_tcb; w.b2 = w.b1 + (size_t)ks * 4096; w.bias = w.b2 + (size_t)ks * 2048; w.wd = w.bias + 3 * TCB_HP;
-        w.bd = h->bd; w.kx = h->tcb_kx; w.F = h->feat; w.H = h->cfg.hidden; w.act = h->cfg.activation; w.ract = h->cfg.recurrent_activation;
-        w.dbg = h->d_dbg;
-        const int grid = (int)((n + 127) / 128);
-        const size_t smem = sizeof(TcbSmem) + 128;
-        if (ring) gru_tcb_kernel<true><<<grid, TCB_BLOCK, smem, s>>>(w, in, n, dp, o);
-        else gru_tcb_kernel<false><<<grid, TCB_BLOCK, smem, s>>>(w, in, n, dp, o);
+    } else if (h->wide_ok && h->gru_mode != 1) {                  // tensor-core scan (mma.sync 3xTF32) for other networks
+        GruWideW w;
+        w.b1 = h->d_wg_b1; w.b2 = h->d_wg_b2; w.bias = h->d_wg_bias; w.wd = h->d_wd; w.bd = h->bd;
+        w.H = h->cfg.hidden; w.F = h->feat; w.FP = h->wg_fp; w.HP = h->wg_hp; w.act = h->cfg.activation; w.ract = h->cfg.recurrent_activation;
+        const int grid = (int)((n + WG_STREAMS - 1) / WG_STREAMS);
+        const size_t smem = wg_smem(w.FP, w.HP);
+        if (ring) gru_wide_kernel<true><<<grid, WG_THREADS, smem, s>>>(w, in, n, dp, o);
+        else gru_wide_kernel<false><<<grid, WG_THREADS, smem, s>>>(w, in, n, dp, o);
     } else {
         GruTiledW w;
         w.wcat = h->d_wcat; w.bias = h->d_bias; w.wd = h->d_wd; w.bd = h->bd;
@@ -998,7 +945,7 @@ static int check_tick(pb_handle* h, const void* pcm, int64_t n) {
     return PB_OK;
 }
 
-// tables of the experimental tensor-core MFCC tick (host part: shared by the device upload and the CPU model)
+// tables of the CPU model of the matrix-product MFCC
 static void tcd_host_tables(const pb_handle* h, std::vector<float4>& etab, std::vector<float>& dct, float* tot_scale) {
     const float inv = 1.0f / 32768.0f, scale = inv * inv / (float)h->cfg.n_fft, pscale = scale / (TCD_A_SCALE * TCD_A_SCALE);
     tcd_build_etab(etab, h->h_wrise, h->h_wfall, h->h_grid, h->cfg.n_filt, pscale);
@@ -1012,42 +959,20 @@ static void tcd_host_tables(const pb_handle* h, std::vector<float4>& etab, std::
     *tot_scale = pscale;
 }
 
-// ... built on first use (never on the default path)
-static int ensure_tcd_tables(pb_handle* h) {
-    if (h->d_tcd_b) return PB_OK;
-    std::vector<__half> bh, bl;
-    tcd_build_b(bh, bl);
-    std::vector<__half> both(bh);
-    both.insert(both.end(), bl.begin(), bl.end());
-    std::vector<float4> etab;
-    std::vector<float> dct, tw;
-    tcd_host_tables(h, etab, dct, &h->tcd_tot_scale);
-    tcd_build_tw(tw);
-    CK(cudaMalloc((void**)&h->d_tcd_b, both.size() * sizeof(__half)));
-    CK(cudaMemcpy(h->d_tcd_b, both.data(), both.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    CK(upload(&h->d_tcd_tw, tw));
-    CK(upload(&h->d_tcd_dct, dct));
-    CK(ensure_dyn_smem(mfcc_tc2_stream_kernel<Tc2Geo20>, sizeof(Tc2Smem) + 128));
-    return PB_OK;
-}
-
-static int ensure_tc3_tables(pb_handle* h) {
-    if (h->d_tc3_b1) return PB_OK;
-    int rc = ensure_tcd_tables(h);                       // DCT table and the power scale are shared with mfcc_tc2
-    if (rc != PB_OK) return rc;
-    std::vector<__half> b1, b2;
-    std::vector<float> tw;
-    tc3_build_b1(b1); tc3_build_b2(b2); tc3_build_tw(tw);
-    CK(cudaMalloc((void**)&h->d_tc3_b2, b2.size() * sizeof(__half)));
-    CK(cudaMemcpy(h->d_tc3_b2, b2.data(), b2.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    CK(upload(&h->d_tc3_tw, tw));
-    CK(cudaMalloc((void**)&h->d_tc3_recs, (size_t)h->cfg.max_streams * (size_t)std::max(1, h->max_new) * sizeof(Tc3Rec)));
-    CK(cudaMalloc((void**)&h->d_tc3_counters, 2 * sizeof(unsigned int)));
-    CK(cudaMemset(h->d_tc3_counters, 0, 2 * sizeof(unsigned int)));
-    CK(ensure_dyn_smem(mfcc_tc3_kernel<Tc2Geo20, false>, sizeof(Tc3Smem) + 128));
-    CK(ensure_dyn_smem(mfcc_tc3_kernel<Tc2Geo20, true>, sizeof(Tc3Smem) + 128));
-    CK(cudaMalloc((void**)&h->d_tc3_b1, b1.size() * sizeof(__half)));      // last: its presence marks the set as complete
-    CK(cudaMemcpy(h->d_tc3_b1, b1.data(), b1.size() * sizeof(__half), cudaMemcpyHostToDevice));
+static int ensure_mma_tables(pb_handle* h) {
+    if (h->d_mm_b1) return PB_OK;
+    std::vector<uint2> b1, b2;
+    std::vector<float2> tw;
+    mm_build_tables(b1, b2, tw);
+    CK(upload(&h->d_mm_b2, b2));
+    CK(upload(&h->d_mm_tw, tw));
+    CK(cudaMalloc((void**)&h->d_mm_recs, (size_t)h->cfg.max_streams * (size_t)std::max(1, h->max_new) * sizeof(MmRec)));
+    CK(cudaMalloc((void**)&h->d_mm_counters, 2 * sizeof(unsigned int)));
+    CK(cudaMemset(h->d_mm_counters, 0, 2 * sizeof(unsigned int)));
+    CK(ensure_dyn_smem(mfcc_mma_kernel<false, false>, sizeof(MmSmem)));
+    CK(ensure_dyn_smem(mfcc_mma_kernel<true, false>, sizeof(MmSmem)));
+    CK(ensure_dyn_smem(mfcc_mma_kernel<true, true>, sizeof(MmSmem)));
+    CK(upload(&h->d_mm_b1, b1));                         // last: its presence marks the set as complete
     return PB_OK;
 }
 
@@ -1058,43 +983,31 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
     const int grid = (int)std::min<int64_t>(tiles, (int64_t)h->sm_count * 4);
     const float inv = 1.0f / 32768.0f, scale = inv * inv / (float)h->cfg.n_fft;
     ProfScope ps(h, 0, s);
-    // Default choice (k1_mode 0): from TC3_MIN_STREAMS streams on, the tick's MFCCs come from the kernel with both DFT stages on the
-    // tensor cores (measured on B200: 116 vs 128 us at 65 536 streams, 208 vs 228 us at 131 072, 392 vs 414 us at 262 144; below
-    // that its persistent pipeline does not fill and the FFT kernel wins: 71 vs 64 us at 32 768).
-    const bool tc3_auto = h->k1_mode == 0 && n >= TC3_MIN_STREAMS;
-    if ((h->k1_mode == 5 || h->k1_mode == 6 || h->k1_mode >= 100 || tc3_auto) && h->tc3_ok && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
-        int rc = ensure_tc3_tables(h);
+    if (h->k1_mode >= 4 && h->mma_ok && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
+        int rc = ensure_mma_tables(h);
         if (rc != PB_OK) return rc;
-        Tc3Tables t;
-        t.b1 = h->d_tc3_b1; t.b2 = h->d_tc3_b2; t.tw = h->d_tc3_tw; t.dct = h->d_tcd_dct; t.n_out = h->n_out; t.pscale = h->tcd_tot_scale;
-        const int par = h->tc3_parity;
-        h->tc3_parity ^= 1;
-        mfcc_tc3_plan_kernel<<<(int)((n + TC3_PLAN_THREADS - 1) / TC3_PLAN_THREADS), TC3_PLAN_THREADS, 0, s>>>(
-            d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, h->st, h->d_tc3_recs, h->d_tc3_counters, par);
-        const int64_t max_tiles = (n * std::max(1, h->max_new) + TC3_TILE - 1) / TC3_TILE;
-        const int g3 = (int)std::min<int64_t>(max_tiles, h->sm_count);
-        if (h->k1_mode >= 100)          // phase timeline of one warp (pb_debug_counters): separate instantiation, the counters cost registers
-            mfcc_tc3_kernel<Tc2Geo20, true><<<g3, TC3_THREADS, sizeof(Tc3Smem) + 128, s>>>(t, h->d_tc3_recs, h->d_tc3_counters, par, h->k1_mode, h->d_dbg);
+        MmTables t;
+        t.b1 = h->d_mm_b1; t.b2 = h->d_mm_b2; t.tw = h->d_mm_tw;
+        t.pscale = inv * inv / (float)h->cfg.n_fft * 1024.f;             // the accumulators hold 2^-5 X
+        const int par = h->mm_parity;
+        h->mm_parity ^= 1;
+        mfcc_mma_plan_kernel<<<(int)((n + MM_PLAN_THREADS - 1) / MM_PLAN_THREADS), MM_PLAN_THREADS, 0, s>>>(
+            d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, h->st, h->d_mm_recs, h->d_mm_counters, par);
+        const int64_t max_tiles = (n * std::max(1, h->max_new) + MM_FRAMES - 1) / MM_FRAMES;
+        const int gm = (int)std::min<int64_t>((max_tiles + MM_WARPS - 1) / MM_WARPS, h->sm_count);
+        if (h->k1_mode == 4)
+            mfcc_mma_kernel<false, false><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), h->d_mm_recs, h->d_mm_counters, par);
+        else if (h->k1_mode == 5)
+            mfcc_mma_kernel<true, false><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), h->d_mm_recs, h->d_mm_counters, par);
         else
-            mfcc_tc3_kernel<Tc2Geo20, false><<<g3, TC3_THREADS, sizeof(Tc3Smem) + 128, s>>>(t, h->d_tc3_recs, h->d_tc3_counters, par, h->k1_mode == 6 ? 8 : 0, nullptr);   // 6: A/B of the epilogue's shuffle-gather tail
-    } else if (h->k1_mode == 4 && h->tc2_ok && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
-        int rc = ensure_tcd_tables(h);
-        if (rc != PB_OK) return rc;
-        Tc2Tables t;
-        t.b = h->d_tcd_b; t.tw = h->d_tcd_tw; t.dct = h->d_tcd_dct; t.n_out = h->n_out; t.pscale = h->tcd_tot_scale;
-        // super-groups: one per SM where the batch allows it, a multiple of 32 streams, at most TC2_SG_MAX
-        int sg = (int)((n + h->sm_count - 1) / h->sm_count);
-        sg = std::min(TC2_SG_MAX, std::max(128, (sg + 31) & ~31));
-        const int groups = (int)((n + sg - 1) / sg);
-        mfcc_tc2_stream_kernel<Tc2Geo20><<<std::min(groups, h->sm_count), TC2_THREADS, sizeof(Tc2Smem) + 128, s>>>(
-            d_pcm, d_ids, (int)n, sg, h->cfg.chunk_samples, h->cfg.hop_samples, t, h->st);
+            mfcc_mma_kernel<true, true><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), h->d_mm_recs, h->d_mm_counters, par);
     } else if (h->fast_ok && h->max_new <= 8 && h->cfg.chunk_samples % 8 == 0 && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
         // streams per warp tile: 16 at scale; fewer when the batch cannot fill the machine's warps
         const int64_t warps_total = (int64_t)h->sm_count * 4 * K1F_WARPS;
         const int spw = (int)std::max<int64_t>(1, std::min<int64_t>(K1F_STREAMS_PER_WARP, (n + warps_total - 1) / warps_total));
         const int64_t tilesf = (n + spw - 1) / spw;
         const int gridf = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
-        if (h->k1_mode != 3)                     // default: the 32-bit per-pass set-up (bit-identical rows, 3 % faster on B200); 3 = the 64-bit original
+        if (h->k1_mode != 3)                     // default: the 32-bit per-pass set-up (bit-identical rows); 3 = the 64-bit original
             mfcc_fast_stream_kernel<true><<<gridf, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
                                                                                       mel_tables(h), fast_tables(h), h->st);
         else
@@ -1126,7 +1039,7 @@ PB_API int pb_update_vectors(pb_handle* h, const int16_t* d_pcm, const int32_t* 
 
 // Does a tick of n streams run the scan that reads cached input projections (gru_mma_kernel<.., PROJ>)?
 static bool wants_projection(const pb_handle* h, int64_t n) {
-    return h->has_proj && h->small_path && n > K2_WARP_PATH_MAX && (h->gru_mode == 0 || h->gru_mode == 2 || h->gru_mode == 7 || h->gru_mode == 8 || h->gru_mode == 9 || h->gru_mode == 10 || h->gru_mode == 11);
+    return h->has_proj && h->small_path && n > K2_WARP_PATH_MAX && (h->gru_mode == 0 || h->gru_mode == 2 || h->gru_mode == 7 || h->gru_mode == 9 || h->gru_mode == 10 || h->gru_mode == 11);
 }
 
 // Recompute the projection of every ring row once (all streams), then the cache is maintained incrementally.

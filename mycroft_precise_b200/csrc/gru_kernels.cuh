@@ -202,10 +202,8 @@ __device__ __forceinline__ void gate_dot(const float (*Wt)[KP], int j, float bia
 
 // One thread owns K2_NS adjacent streams; h, z, r*h live in registers.  The weights sit in shared
 // memory transposed -- column j of [W;U] is one contiguous row of KP = roundup4(F + H) floats -- and are
-// fetched with warp-uniform (broadcast) 16-byte loads.  sm_100a has no constant-operand FFMA (ptxas
-// turns __grid_constant__/__constant__ weights into one LDCU per FFMA: measured 2008 LDCU for 2073
-// FFMA per step), so shared-memory broadcast with 2-way register blocking is the cheapest weight path:
-// 9 LDS.128 per 66 FFMA.
+// fetched with warp-uniform (broadcast) 16-byte loads: with 2-way register blocking that is 9 LDS.128
+// per 66 FFMA.
 template <int H, int F, bool RING>
 __global__ void __launch_bounds__(K2_SMALL_THREADS, 3)
 gru_small_kernel(const __grid_constant__ GruSmallW<H, F> P, K2In in, long long n, DecodeParams dp, K2Out out) {

@@ -1,4 +1,5 @@
-// mfcc_tc.cuh -- host tables, CPU model and device helpers of the tensor-core MFCC tick (the kernel itself: mfcc_tc2.cuh).
+// mfcc_tc.cuh -- host tables and CPU model of an MFCC frame whose second DFT stage is an fp16 matrix product (the shape a
+// tensor-core MFCC tick computes: mfcc_mma.cuh, k1 mode 4).
 //
 // Replaces, per frame, np.fft.rfft(frame, n=512), the power spectrum, the mel filterbank, log, DCT and c0 of
 // sonopy.mfcc_spec as the reference calls it (precise/vectorization.py:36-39), for the stateful tick
@@ -26,9 +27,6 @@
 
 #include <vector>
 
-#include "gru_tc5.cuh"        // tc5_desc, tc5_commit, tcgen05 fences
-#include "mfcc_fast.cuh"      // mbarrier helpers
-#include "mfcc_kernels.cuh"   // StreamState, frames_ready, K1_EPS
 
 namespace pb {
 
@@ -39,7 +37,7 @@ constexpr int TCD_MAX_OUT = 16;
 constexpr int TCD_TW_STRIDE = 18;             // floats per input n2 in the twiddle table: (cos, -sin) of r = 1..8, + 2 of padding
 constexpr float TCD_IN_SCALE = 0.015625f;     // 2^-6 folded into the int16 -> float conversion; the butterfly returns 2 Y
 constexpr float TCD_A_SCALE = 0.03125f;       // => A operands hold Z * 2^-5: |A| <= 16384, and <= 32768 < fp16 max after the shift below
-// The kernel transforms x - x[0] (a constant only moves X[0]; constant input then gives exact zeros everywhere else, like the
+// The model transforms x - x[0] (a constant only moves X[0]; constant input then gives exact zeros everywhere else, like the
 // float64 reference and the FFT kernels): Y_0 loses 16 x[0], i.e. the butterfly output 2 * 16 * IN_SCALE * x[0], and the
 // X[0] accumulator gets 32 times that back.
 constexpr float TCD_X0_Y = 32.f * TCD_IN_SCALE;          // 0.5
@@ -153,7 +151,7 @@ static inline void tcd_build_tw(std::vector<float>& tw) {
 }
 
 // One input's nine block operands from its 16-point DFT (yr, yi scaled as rdft16_x2 returns them): Z_0 = Y_0 - shift (real),
-// Z_r = Y_r w512^(n2 r).  Host + device: the kernel and the CPU model share this arithmetic.
+// Z_r = Y_r w512^(n2 r).  Host + device.
 __host__ __device__ __forceinline__ void tcd_twiddle(const float (&yr)[9], const float (&yi)[9], const float* tw, float x0_shift,
                                                      float (&zr)[9], float (&zi)[9]) {
     zr[0] = yr[0] - x0_shift; zi[0] = 0.f;
@@ -169,8 +167,7 @@ __host__ __device__ __forceinline__ void tcd_twiddle(const float (&yr)[9], const
 }
 
 // wrise / wfall / grid as built by api.cu (build_mel); pscale turns (re^2 + im^2) of the scaled accumulators into power / n_fft.
-// etab[k] = (rising-edge weight, falling-edge weight, segment) of bin k  (CPU model of the epilogue only; the kernel has the same
-// numbers at compile time, mfcc_tc2.cuh)
+// etab[k] = (rising-edge weight, falling-edge weight, segment) of bin k  (CPU model of the epilogue)
 static inline void tcd_build_etab(std::vector<float4>& etab, const std::vector<float>& wrise, const std::vector<float>& wfall,
                                   const std::vector<int>& grid, int n_filt, float pscale) {
     etab.assign(257, make_float4(0.f, 0.f, 0.f, 0.f));
@@ -219,7 +216,7 @@ static inline void tcd_host_accumulators(const int16_t* x, float (*d)[64]) {
                 }
             d[b][n] = acc;
         }
-    d[0][0] += TCD_X0_D * (float)x[0];     // the kernel transforms x - x[0] (exact zeros for constant input) and restores X[0] here
+    d[0][0] += TCD_X0_D * (float)x[0];     // the model transforms x - x[0] (exact zeros for constant input) and restores X[0] here
 }
 
 // |X[k]|^2 of the raw samples, k = 0..256
@@ -262,33 +259,6 @@ static inline void tcd_host_epilogue(const float (*d)[64], const float4* etab, c
         for (int j = 0; j < n_filt; ++j) v = fmaf(dct[(size_t)o * 24 + j], lg[j], v);
         out[o] = o == 0 ? logf(fmaxf(tot * pscale, eps)) : v;
     }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// instruction descriptor: kind::f16, A and B fp16 K-major, fp32 accumulate, M = 128
-__device__ __forceinline__ uint32_t tcd_idesc(int n) {
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-__device__ __forceinline__ void tcd_mma(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-                 ::"r"(d_tmem), "l"(a), "l"(b), "r"(idesc), "r"(accumulate), "r"(0), "r"(0), "r"(0), "r"(0) : "memory");
-}
-
-// int16 pair (already XORed with 0x80008000) -> two floats scaled by 2^-6 (TCD_IN_SCALE), exact: drop the biased 16-bit value
-// into the mantissa of 2^17 (ulp 2^-6) and subtract 2^17 + 32768 * 2^-6.
-__device__ __forceinline__ void tcd_cvt2(uint32_t v, float& lo, float& hi) {
-    lo = __uint_as_float(__byte_perm(v, 0x48000000u, 0x7610)) - 131584.f;
-    hi = __uint_as_float(__byte_perm(v, 0x48000000u, 0x7632)) - 131584.f;
-}
-
-// four floats -> fp16 hi and lo pieces, one 8-byte store each
-__device__ __forceinline__ void tcd_put4(__half* hi_dst, __half* lo_dst, float v0, float v1, float v2, float v3) {
-    const __half2 h0 = __floats2half2_rn(v0, v1), h1 = __floats2half2_rn(v2, v3);
-    const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-    const __half2 l0 = __floats2half2_rn(v0 - f0.x, v1 - f0.y), l1 = __floats2half2_rn(v2 - f1.x, v3 - f1.y);
-    *reinterpret_cast<uint2*>(hi_dst) = make_uint2(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1));
-    *reinterpret_cast<uint2*>(lo_dst) = make_uint2(*reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
 }
 
 }  // namespace pb

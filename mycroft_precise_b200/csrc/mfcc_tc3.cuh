@@ -1,55 +1,27 @@
-// mfcc_tc3.cuh -- K1 with BOTH DFT stages on the 5th-generation tensor cores (tcgen05 + TMEM): the stateful MFCC tick for the
-// reference's default geometry (n_fft 512, 20 mel filters at 16 kHz; precise/params.py:140-144).
+// mfcc_tc3.cuh -- CPU model of an MFCC frame with BOTH DFT stages as fp16 matrix products (the reference's default geometry:
+// n_fft 512, 20 mel filters at 16 kHz; precise/params.py:140-144).  It specifies the decomposition and splits that the tensor-core
+// MFCC tick (mfcc_mma.cuh) computes; that kernel's own fragment tables and bin assembly are checked by mm_host_power.
 //
 // Replaces, per frame, np.fft.rfft(frame, n=512) -> power -> mel filterbank -> log -> DCT -> c0 of sonopy.mfcc_spec as the
-// reference calls it (precise/vectorization.py:36-39) and the carry-buffer bookkeeping of Listener.update_vectors
-// (precise/network_runner.py:125-146).
+// reference calls it (precise/vectorization.py:36-39).
 //
 // n = n2 + 32 q (n2 < 32, q < 16), k = 16 m + r:
-//   stage 1 (tensor cores):  Y_r[n2] = sum_q x[n2 + 32 q] w16^(q r), r = 0..8.  The int16 samples are split EXACTLY into two fp16
-//            pieces (x - x0 = 256 hi + lo, |lo| <= 128, balanced so that a quiet signal has hi = 0), which needs no floating-point
-//            work: bytes are dropped into the mantissa of 1024.0h and the bias removed by one half2 add.  The operand is the PCM
-//            in its natural order (MN-major A: 8 consecutive samples = 8 rows of one K index); rows of an MMA = (frame, n2).
-//   between (CUDA cores):    Z_r[n2] = Y_r[n2] w512^(n2 r) (the lane owns n2: its eight twiddles come from a 2 KB table), fp16 hi / lo
-//            split, one 4-byte store per block and piece into the stage-2 operand.
-//   stage 2 (tensor cores):  X[16 m + r] = sum_n2 Z_r[n2] w32^(n2 m), X[16 m + 16 - r] from conj(Z_r): nine 64-column blocks
-//            sharing one 64 x 64 matrix (mfcc_tc.cuh); rows of an MMA = (frame, h), four rows per frame.
-//   epilogue (CUDA cores):   power, mel edge sums with compile-time bins and weights, log, DCT, ring row.
-//
-// Organisation: a persistent CTA per SM, 16 worker warps that all walk the same phases (no warp specialisation of the heavy
-// loops: the instruction cache sees one small loop at a time -- the warp-specialised predecessor, mfcc_tc2.cuh, spent 40 % of
-// its issue slots waiting for instructions) plus one warp that only issues the MMAs.  Per tile of 32 frames:
-//     INT(k)   workers     tcgen05.ld of stage 1's result, twiddle, split, stores into the stage-2 operand
-//     P(k)     warps 0-7   EPI(k-1), then a quarter of CONV(k+2)
-//              warps 8-15  new tails of tile k+1, frame records of tile k+4 (+ L2 prefetch), three quarters of CONV(k+2)
-//              CONV = raw PCM copied by cp.async into the stage-1 operand buffer (L2-prefetched four tiles earlier), split in place
-//     warp 16  follows mbarriers only: MMA1(k+1) once CONV(k+1) is complete and every worker has read tile k's stage-1 result,
-//              MMA2(k) once INT(k)'s operand is complete and the epilogue has drained the accumulator buffer
-// with one barrier of the worker warps per tile; the MMAs of a tile run under the CUDA-core phases of its neighbours.  The
-// frame list (which frames complete this tick, where their samples are, the split of the first sample, new tail) is built
-// by mfcc_tc3_plan_kernel with every pointer ready to use.  Measurements and the history of this organisation: DESIGN.md.
+//   stage 1 (matrix product): Y_r[n2] = sum_q x[n2 + 32 q] w16^(q r), r = 0..8.  The int16 samples are split EXACTLY into two fp16
+//            pieces (x - x0 = 256 hi + lo, |lo| <= 128, balanced so that a quiet signal has hi = 0).
+//   between:                  Z_r[n2] = Y_r[n2] w512^(n2 r), fp16 hi / lo split.
+//   stage 2 (matrix product): X[16 m + r] = sum_n2 Z_r[n2] w32^(n2 m), X[16 m + 16 - r] from conj(Z_r): nine 64-column blocks
+//            sharing one 64 x 64 matrix (mfcc_tc.cuh).
+//   epilogue:                 power, mel edge sums, log, DCT.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "mfcc_tc2.cuh"
+#include "mfcc_tc.cuh"
 
 namespace pb {
 
-constexpr int TC3_WORKERS = 512;                // 16 worker warps
-constexpr int TC3_THREADS = TC3_WORKERS + 32;   // + the MMA-issuing warp
-constexpr int TC3_TILE = 32;                    // frames per tile
-constexpr int TC3_SLOTS = 3;                    // 64-column stage-2 MMA slots per tile row
-constexpr int TC3_D1_COLS = 128;                // stage-1 accumulators: 8 groups of 4 frames x 16 columns
-constexpr int TC3_D2_COLS = 64 * TC3_SLOTS;     // stage-2 accumulators of a tile (two tiles resident)
-constexpr int TC3_A1_TILE = 4096;               // stage-1 operand of one group and piece: 128 rows x 16 K (MN-major: SBO 128, LBO 2048)
-constexpr int TC3_A2_LBO = 2048 + 16;           // bytes between K-groups of a stage-2 operand tile (16 B of padding: conflict-free 4-byte stores)
-constexpr int TC3_A2_TILE = 4 * TC3_A2_LBO;     // one (piece, stage, slot) tile: 4 K-groups x 128 rows x 16 bytes
-constexpr int TC3_REC_RING = 8;                 // tiles of frame records resident in shared memory
 constexpr float TC3_Z_SCALE = 0.03125f;         // stage-2 operands hold Z * 2^-5 (= TCD_A_SCALE): |.| <= 32768 < fp16 max
-constexpr int TC3_PLAN_THREADS = 256;
-constexpr int TC3_MIN_STREAMS = 49152;          // streams per tick from which this kernel is the default (api.cu: launch_stream_mfcc)
 
 // block r -> tile row h (of the frame's four) and MMA slot: rows hold 64, 64, 64 and 65 bins
 __host__ __device__ constexpr int tc3_blk_h(int b) { constexpr int t[9] = {3, 0, 0, 1, 1, 2, 2, 3, 3}; return t[b]; }
@@ -59,17 +31,6 @@ __host__ __device__ constexpr int tc3_hs_blk(int h, int s) { constexpr int t[12]
 __host__ __device__ constexpr int tc3_kslot(int j, int im) { return 2 * j + im; }
 // stage-1 output column: 0 = Y_0, 1 = Y_8, 2 r / 2 r + 1 = Re / Im Y_r (r = 1..7)
 __host__ __device__ constexpr int tc3_y_col(int r, int im) { return r == 0 ? 0 : r == 8 ? 1 : 2 * r + im; }
-
-struct __align__(16) Tc3Rec {          // one frame completed by this tick, everything the main kernel needs in ready-to-use form
-    const int16_t* frame;              // sample 0 of the frame in chunk coordinates (pcm row + dj; only samples >= 8 len0c are read); nullptr: padding
-    int16_t* tail;                     // the stream's tail buffer (holds the frame's first 8 len0c samples; receives the new tail)
-    float* row;                        // the frame's MFCC ring row
-    unsigned short c_lo, c_hi;         // fp16 constants of the exact split: -(1152 + lo0), -(9 + hi0 / 128) with x0 = 256 hi0 + lo0 the frame's first sample
-    unsigned char len0c;               // 16-byte chunks of the frame that come from the tail
-    unsigned char tail_nv;             // first frame of a stream only: 16-byte chunks of the new tail (0: nothing to copy)
-    unsigned short tail_delta;         // ... which starts 8 tail_delta samples after `frame`
-};
-static_assert(sizeof(Tc3Rec) == 32, "frame records are loaded as two 16-byte vectors");
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Host tables.
@@ -99,7 +60,7 @@ static inline void tc3_build_b1(std::vector<__half>& b1) {
             }
         }
 }
-//   B2 (stage 2): the 64 x 64 matrix of mfcc_tc.cuh with the K order of this kernel (tc3_kslot), pieces hi then lo.
+//   B2 (stage 2): the 64 x 64 matrix of mfcc_tc.cuh with the K order of this model (tc3_kslot), pieces hi then lo.
 static inline void tc3_build_b2(std::vector<__half>& b2) {
     b2.assign((size_t)2 * 8 * 64 * 8, __float2half_rn(0.f));
     const double PI2 = 6.283185307179586476925286766559;
@@ -153,7 +114,7 @@ __host__ __device__ __forceinline__ void tc3_twiddle(const float (&y)[16], const
     zr[8] = y[1] * tw[14]; zi[8] = y[1] * tw[15];
 }
 
-// CPU model of the kernel's arithmetic for ONE frame of 512 int16 samples (same splits, tables, pass order and layout
+// CPU model of the arithmetic for ONE frame of 512 int16 samples (same splits, tables, pass order and layout
 // arithmetic; fp16 products accumulated in fp32): d[9][64] = the frame's stage-2 accumulator columns block by block, X[0]
 // restored.  What tests/test_tc_dft_host_model.py checks without a device.
 static inline void tc3_host_accumulators(const int16_t* x, float (*d)[64]) {
@@ -205,7 +166,7 @@ static inline void tc3_host_accumulators(const int16_t* x, float (*d)[64]) {
     d[0][0] += TCD_X0_D * (float)x[0];
 }
 
-// The epilogue's arithmetic for one frame (fp32), as the kernel orders it: per segment s = 1..19 the power sum and the
+// The epilogue's arithmetic for one frame (fp32), in this order: per segment s = 1..19 the power sum and the
 // rising-edge sum (falling edge = sum - rising), segment 20 with its falling weights, log, DCT, c0.
 static inline void tc3_host_epilogue(const float (*d)[64], const std::vector<float>& wrise, const std::vector<float>& wfall,
                                      const std::vector<int>& grid, const float* dct, int n_filt, int n_out, float pscale, float* out) {
@@ -235,575 +196,6 @@ static inline void tc3_host_epilogue(const float (*d)[64], const std::vector<flo
         for (int j = 0; j < n_filt; ++j) v = fmaf(dct[(size_t)o * 24 + j], lg[j], v);
         out[o] = o == 0 ? logf(fmaxf(tot * pscale, eps)) : v;
     }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// The frame list of a tick (cf. Listener.update_vectors, network_runner.py:137-144): per stream the frames the new chunk
-// completes.  counters[parity] receives the number of frames (zeroed by the main kernel of the previous tick).
-__global__ void __launch_bounds__(TC3_PLAN_THREADS)
-mfcc_tc3_plan_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids, int n, int chunk, int hop, StreamState st,
-                     Tc3Rec* __restrict__ recs, unsigned int* __restrict__ counters, int parity) {
-    __shared__ int warp_tot[TC3_PLAN_THREADS / 32];
-    __shared__ unsigned int base_sh;
-    constexpr int used = 512;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int i = blockIdx.x * TC3_PLAN_THREADS + tid;
-    int cnt = 0, d = 0, slot0 = 0, sid = 0;
-    if (i < n) {
-        sid = ids ? ids[i] : i;
-        const long long n0 = st.n_samples[sid];
-        const long long c0 = frames_ready(n0, used, hop);
-        cnt = (int)(frames_ready(n0 + chunk, used, hop) - c0);
-        d = (int)(c0 * hop - n0);
-        slot0 = (int)(c0 % st.ring_rows);
-        st.n_samples[sid] = n0 + chunk;
-    }
-    int incl = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-    if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();
-    if (tid == 0) {
-        int t = 0;
-        for (int w = 0; w < TC3_PLAN_THREADS / 32; ++w) { const int v = warp_tot[w]; warp_tot[w] = t; t += v; }
-        base_sh = t ? atomicAdd(&counters[parity], (unsigned int)t) : 0u;
-    }
-    __syncthreads();
-    if (i >= n) return;
-    const unsigned int off0 = base_sh + warp_tot[warp] + (incl - cnt);
-    const int16_t* chunk_p = pcm + (long long)i * chunk;
-    const int tail_off = min(d + cnt * hop, chunk);
-    for (int j = 0; j < cnt; ++j) {
-        Tc3Rec r;
-        const int dj = d + j * hop;
-        const int x0 = dj >= 0 ? chunk_p[dj] : st.tail[(long long)sid * st.tail_cap + j * hop];
-        int hi0, lo0;
-        tc3_split16(x0, hi0, lo0);
-        int sl = slot0 + j;
-        if (sl >= st.ring_rows) sl -= st.ring_rows;
-        r.frame = chunk_p + dj;
-        r.tail = st.tail + (long long)sid * st.tail_cap;
-        r.row = st.ring + ((long long)sid * st.ring_rows + sl) * st.row_stride;
-        r.c_lo = __half_as_ushort(__float2half_rn(-(float)(1152 + lo0)));
-        r.c_hi = __half_as_ushort(__float2half_rn(-(9.f + (float)hi0 * 0.0078125f)));
-        r.len0c = (unsigned char)(dj < 0 ? min(used, -dj) >> 3 : 0);
-        r.tail_nv = (unsigned char)(j == 0 ? (chunk - tail_off) >> 3 : 0);
-        r.tail_delta = (unsigned short)(j == 0 ? (tail_off - dj) >> 3 : 0);
-        int4* dst = reinterpret_cast<int4*>(recs + off0 + j);
-        dst[0] = reinterpret_cast<const int4*>(&r)[0];
-        dst[1] = reinterpret_cast<const int4*>(&r)[1];
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int TC3_PART_STRIDE = 28;     // floats per epilogue thread in the partial-sum exchange (24 used; 112-byte rows: conflict-free 16-byte accesses)
-constexpr int TC3_LGM_STRIDE = 20;      // floats per frame in the log-mel exchange (80-byte rows: conflict-free 16-byte accesses)
-
-struct Tc3Smem {
-    __half b2[2][8][64][8];                              // stage-2 matrix, pieces hi / lo
-    __half b1[4][2][16][8];                              // stage-1 matrices (tc3_build_b1)
-    unsigned char a1[8][2][TC3_A1_TILE];                 // stage-1 operands [group of 4 frames][piece hi / lo]
-    unsigned char a2[2][2][TC3_SLOTS][TC3_A2_TILE];      // stage-2 operands [piece][K half][slot]
-    float part[256][TC3_PART_STRIDE];                    // mel sums (20) + total power of the 8 epilogue threads of every frame
-    float lgm[TC3_TILE][TC3_LGM_STRIDE];                 // log-mel values of the tile's frames
-    float c0v[TC3_TILE];
-    float dct[TCD_MAX_OUT][24];
-    float tw[32][16];                                    // twiddles of input n2 = lane (tc3_build_tw)
-    Tc3Rec rec[TC3_REC_RING][TC3_TILE];
-    unsigned long long m1_done, m2_done, d1_free, a1_ready, a2_ready, d2_free[2];
-    uint32_t tmem_base;
-    unsigned int n_frames;
-};
-
-struct Tc3Tables {               // device pointers
-    const uint4* b1;             // 4 x 512 bytes
-    const uint4* b2;             // 2 x 8192 bytes
-    const float* tw;             // [32][16]
-    const float* dct;            // [TCD_MAX_OUT][24]
-    int n_out;
-    float pscale;
-};
-
-__device__ __forceinline__ void tc3_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tc3_wait_ld16(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :: "memory");
-}
-__device__ __forceinline__ uint32_t tc3_hadd2(uint32_t a, uint32_t b) {
-    uint32_t d;
-    asm("add.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-    return d;
-}
-__device__ __forceinline__ uint32_t tc3_hfma2(uint32_t a, uint32_t b, uint32_t c) {       // no .ftz: a may be subnormal
-    uint32_t d;
-    asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-__device__ __forceinline__ void tc3_l2_prefetch(const void* p, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
-// instruction descriptors: kind::f16, fp32 accumulate, M = 128; stage 1 reads A MN-major
-__device__ __forceinline__ uint32_t tc3_idesc(int n, bool a_mn) {
-    return (1u << 4) | (a_mn ? (1u << 15) : 0u) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-
-// The mel sums of one 64-column block B of a tile row (cf. tc2_block_bins): per segment the power sum and the rising-edge sum;
-// the last segment (no rising edge) keeps its falling-edge sum.
-template <class G, int B>
-__device__ __forceinline__ void tc3_block_bins(uint32_t taddr, float x0f, float (&rise)[G::n_filt + 1], float (&seg)[G::n_filt + 1]) {
-    tc2_static_for<2>([&](auto hh) {
-        constexpr int half = decltype(hh)::value;
-        constexpr bool any = tcd_col_bin(B, 32 * half) >= 0 || tcd_col_bin(B, 32 * half + 15) >= 0;
-        if constexpr (any) {
-            uint32_t v[32];
-            tc2_ld32(taddr + 32 * half, v);
-            tc2_wait_ld(v);
-            tc2_static_for<16>([&](auto mm) {
-                constexpr int m = decltype(mm)::value;
-                constexpr int bin = tcd_col_bin(B, 32 * half + m);
-                if constexpr (bin >= 0) {
-                    float re = __uint_as_float(v[m]);
-                    const float im = __uint_as_float(v[16 + m]);
-                    float p;
-                    if constexpr (bin == 0) { re = fmaf(TCD_X0_D, x0f, re); p = re * re; }          // undo the constant subtracted from the frame
-                    else if constexpr (bin == 256) p = re * re;
-                    else p = fmaf(im, im, re * re);
-                    constexpr int s = tc2_seg<G>(bin);
-                    seg[s] += p;
-                    if constexpr (s < G::n_filt) {
-                        constexpr float wr = tc2_wrise<G>(bin);
-                        if constexpr (wr != 0.f) rise[s] = fmaf(wr, p, rise[s]);
-                    } else {
-                        constexpr float wf = tc2_wfall<G>(bin);
-                        rise[s] = fmaf(wf, p, rise[s]);              // rise[n_filt] holds the last segment's falling-edge sum
-                    }
-                }
-            });
-        }
-    });
-}
-
-template <class G, bool TIMED = false>
-__global__ void __launch_bounds__(TC3_THREADS, 1)
-mfcc_tc3_kernel(Tc3Tables tab, const Tc3Rec* __restrict__ recs, unsigned int* __restrict__ counters, int parity, int dbg, long long* __restrict__ dbg_clk) {
-    extern __shared__ __align__(128) unsigned char tc3_raw[];
-    Tc3Smem& sm = *reinterpret_cast<Tc3Smem*>(tc3_raw);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q4 = warp & 3, wg = warp >> 2;               // TMEM lane quadrant of this warp; warp group 0..3 (workers)
-    static_assert(G::n_filt == 20, "the epilogue distributes 20 filters over the eight threads of a frame");
-
-    // ---- one-time set-up
-    if (tid == 0) {
-        mbar_init(&sm.m1_done, 1); mbar_init(&sm.m2_done, 1); mbar_init(&sm.d1_free, TC3_WORKERS);
-        mbar_init(&sm.a1_ready, TC3_WORKERS); mbar_init(&sm.a2_ready, TC3_WORKERS);
-        mbar_init(&sm.d2_free[0], TC3_WORKERS / 2); mbar_init(&sm.d2_free[1], TC3_WORKERS / 2);
-        fence_mbar_init();
-        sm.n_frames = counters[parity];
-        if (blockIdx.x == 0) counters[parity ^ 1] = 0;        // the next tick's plan kernel counts from zero
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    for (int e = tid; e < 1024; e += TC3_THREADS) reinterpret_cast<uint4*>(&sm.b2[0][0][0][0])[e] = __ldg(tab.b2 + e);
-    if (tid < 128) reinterpret_cast<uint4*>(&sm.b1[0][0][0][0])[tid] = __ldg(tab.b1 + tid);
-    for (int e = tid; e < TCD_MAX_OUT * 24; e += TC3_THREADS) (&sm.dct[0][0])[e] = __ldg(tab.dct + e);
-    for (int e = tid; e < 32 * 16; e += TC3_THREADS) (&sm.tw[0][0])[e] = __ldg(tab.tw + e);
-    fence_proxy_async();
-    tc5_fence_before();
-    __syncthreads();
-    tc5_fence_after();
-    const uint32_t tmem = sm.tmem_base;
-    const int n_frames = (int)sm.n_frames;
-    const int n_tiles = (n_frames + TC3_TILE - 1) / TC3_TILE;
-    const int K = (int)blockIdx.x < n_tiles ? (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    auto tile_of = [&](int k) { return (int)blockIdx.x + k * (int)gridDim.x; };
-
-    // ---- helpers
-    // the two halves of the record of (tile k, frame f); frame == nullptr and the split constants of x0 = 0 pad the last tile
-    auto fetch_rec = [&](int k, int f, int4& a, int4& b) {
-        a = make_int4(0, 0, 0, 0); b = make_int4(0, 0, (int)0xC880E480u, 0);
-        if (k < K) {
-            const int idx = tile_of(k) * TC3_TILE + f;
-            if (idx < n_frames) {
-                const int4* p = reinterpret_cast<const int4*>(recs + idx);
-                a = __ldg(p); b = __ldg(p + 1);
-            }
-        }
-    };
-    auto store_rec = [&](int k, int f, const int4& a, const int4& b) {
-        int4* p = reinterpret_cast<int4*>(&sm.rec[k & (TC3_REC_RING - 1)][f]);
-        p[0] = a; p[1] = b;
-    };
-    // CONV: warp 8 + w8 converts frames 3 w8 .. 3 w8 + 2 of a tile, warp w < 8 frame 24 + w; lane (c4, l8) owns chunks 4 l8 + c4 and
-    // 32 + 4 l8 + c4 (8 samples each).  The raw PCM is first copied asynchronously (cp.async: no registers, no waiting) into the
-    // lo-piece position of the stage-1 operand it will become; conv_tile later splits it in place.
-    const int c4 = lane >> 3, l8 = lane & 7, cch = 4 * l8 + c4;
-    const int cv_n = warp < 8 ? 1 : 3, cv_f0 = warp < 8 ? 24 + warp : 3 * (warp - 8);
-    auto a1_lo = [&](int fi) { return &sm.a1[fi >> 2][1][0] + (4 * (fi & 3) + c4) * 128 + l8 * 16; };
-    auto stage_tile = [&](int k) {
-#pragma unroll
-        for (int m = 0; m < 3; ++m) {
-            if (m < cv_n) {
-                const int fi = cv_f0 + m;
-                const Tc3Rec& r = sm.rec[k & (TC3_REC_RING - 1)][fi];
-                const int16_t* fp = r.frame;
-                unsigned char* dst = a1_lo(fi);
-                if (fp != nullptr) {
-                    const int l0 = r.len0c;
-                    const int16_t* tp = r.tail;
-                    const int16_t* s0 = (cch < l0 ? tp : fp) + 8 * cch;
-                    const int16_t* s1 = (cch + 32 < l0 ? tp : fp) + 8 * (cch + 32);
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(s0) : "memory");
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst + 2048)), "l"(s1) : "memory");
-                } else {                                         // padding of the last tile: zero samples (split constants of x0 = 0)
-                    *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
-                    *reinterpret_cast<uint4*>(dst + 2048) = make_uint4(0u, 0u, 0u, 0u);
-                }
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    // staged PCM -> the two fp16 pieces of x - x0 (exact), in place
-    auto conv_tile = [&](int k) {
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-#pragma unroll
-        for (int m = 0; m < 3; ++m) {
-            if (m < cv_n) {
-                const int fi = cv_f0 + m;
-                const uint32_t cc = *reinterpret_cast<const uint32_t*>(&sm.rec[k & (TC3_REC_RING - 1)][fi].c_lo);     // c_lo | c_hi << 16
-                const uint32_t c_lo = __byte_perm(cc, 0, 0x1010), c_hi = __byte_perm(cc, 0, 0x3232);
-                unsigned char* dst = a1_lo(fi);
-#pragma unroll
-                for (int hf = 0; hf < 2; ++hf) {
-                    const uint4 raw = *reinterpret_cast<const uint4*>(dst + hf * 2048);
-                    const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
-                    uint32_t ah[4], al[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const uint32_t vx = w[e] ^ 0x80008000u;
-                        const uint32_t lo_magic = (vx & 0x00FF00FFu) ^ 0x64806480u;         // 1024 + (lo ^ 0x80)
-                        al[e] = tc3_hadd2(lo_magic, c_lo);                                    // lo_b - lo0
-                        const uint32_t hi_magic = __byte_perm(vx, 0x64646464u, 0x4341);       // 1024 + hi + 128
-                        const uint32_t mb = w[e] & 0x00800080u;                               // bit 7 of the low byte as fp16 subnormal 2^-17
-                        const uint32_t t = tc3_hfma2(hi_magic, 0x20002000u, c_hi);            // (hi_floor - hi0) / 128   (0x2000 = 2^-7)
-                        ah[e] = tc3_hfma2(mb, 0x64006400u, t);                                // + carry / 128            (0x6400 = 1024)
-                    }
-                    *reinterpret_cast<uint4*>(dst + hf * 2048 - TC3_A1_TILE) = make_uint4(ah[0], ah[1], ah[2], ah[3]);
-                    *reinterpret_cast<uint4*>(dst + hf * 2048) = make_uint4(al[0], al[1], al[2], al[3]);
-                }
-            }
-        }
-    };
-
-    // ---- prologue: records of tiles 0, 1; PCM of tile 0
-    if (tid < 2 * TC3_TILE) {
-        int4 a, b;
-        fetch_rec(tid >> 5, lane, a, b);
-        store_rec(tid >> 5, lane, a, b);
-    }
-    __syncthreads();
-
-    // Per-lane stage-2 store offset (INT): input n2 = lane -> K half (lane >> 4), K-group ((lane >> 2) & 3), 4-byte word (lane & 3)
-    const uint32_t int_lane_off = (uint32_t)((lane >> 4) * (TC3_SLOTS * TC3_A2_TILE) + ((lane >> 2) & 3) * TC3_A2_LBO + (lane & 3) * 4);
-    constexpr uint32_t A2_PIECE = 2 * TC3_SLOTS * TC3_A2_TILE;
-
-    if (warp == 16) {
-        // ================= the MMA-issuing warp: after INT(k), stage 1 of tile k + 1 and stage 2 of tile k
-        const uint32_t idesc1 = tc3_idesc(16, true), idesc2 = tc3_idesc(64, false);
-        const uint32_t a_lbo = 2048u, a_sbo = 128u;             // MN-major operand: K-group stride, 8-row-group stride
-        const bool itimed = TIMED && dbg_clk != nullptr && blockIdx.x == 0 && lane == 0 && dbg == 116;
-        long long ti1 = 0, ti2 = 0, tq = 0;
-        // Decoupled from the workers' barrier: it waits only for the data of the MMAs it is about to issue.
-        //   MMA1(t): operand written (a1_ready: CONV(t)) and tile t - 1's stage-1 result read (d1_free: INT(t - 1))
-        //   MMA2(t): operand written (a2_ready: INT(t)) and the accumulator buffer drained (d2_free[t & 1]: EPI(t - 2))
-        if (lane == 0) {
-#pragma unroll 1
-            for (int t = 0; t <= K; ++t) {
-                if (t < K) {
-                    mbar_wait(&sm.a1_ready, t & 1);
-                    if (t >= 1) mbar_wait(&sm.d1_free, (t - 1) & 1);
-                    if (itimed) tq = clock64();
-                    tc5_fence_after();
-                    uint64_t db[4];
-#pragma unroll
-                    for (int v = 0; v < 4; ++v) db[v] = tc5_desc(&sm.b1[v][0][0][0], 256, 128);
-#pragma unroll 1
-                    for (int i = 0; i < 8; ++i) {
-                        const uint64_t dah = tc5_desc(&sm.a1[i][0][0], a_lbo, a_sbo), dal = tc5_desc(&sm.a1[i][1][0], a_lbo, a_sbo);
-                        const uint32_t d = tmem + 16 * i;
-                        tcd_mma(d, dal, db[3], idesc1, 0);
-                        tcd_mma(d, dal, db[2], idesc1, 1);
-                        tcd_mma(d, dah, db[1], idesc1, 1);
-                        tcd_mma(d, dah, db[0], idesc1, 1);
-                    }
-                    tc5_commit(&sm.m1_done);
-                    if (itimed) ti1 += clock64() - tq;
-                }
-                if (t >= 1) {
-                    const int k = t - 1;
-                    mbar_wait(&sm.a2_ready, k & 1);
-                    if (k >= 2) mbar_wait(&sm.d2_free[k & 1], ((k - 2) >> 1) & 1);
-                    if (itimed) tq = clock64();
-                    tc5_fence_after();
-                    const uint32_t dcol = tmem + TC3_D1_COLS + (k & 1) * TC3_D2_COLS;
-#pragma unroll 1
-                    for (int stage = 0; stage < 2; ++stage) {
-                        const uint64_t da_hi = tc5_desc(&sm.a2[0][stage][0][0], TC3_A2_LBO, 128), da_lo = tc5_desc(&sm.a2[1][stage][0][0], TC3_A2_LBO, 128);
-                        const uint64_t db_hi = tc5_desc(&sm.b2[0][4 * stage][0][0], 1024, 128), db_lo = tc5_desc(&sm.b2[1][4 * stage][0][0], 1024, 128);
-#pragma unroll
-                        for (int kk = 0; kk < 2; ++kk)
-#pragma unroll
-                            for (int sl = 0; sl < TC3_SLOTS; ++sl) {
-                                const uint64_t off = (uint64_t)((sl * TC3_A2_TILE + 2 * kk * TC3_A2_LBO) >> 4);
-                                const uint64_t dbh = db_hi + (uint64_t)(2 * kk * 64), dbl = db_lo + (uint64_t)(2 * kk * 64);
-                                const uint32_t d = dcol + 64 * sl;
-                                tcd_mma(d, da_lo + off, dbh, idesc2, (stage | kk) != 0);
-                                tcd_mma(d, da_hi + off, dbl, idesc2, 1);
-                                tcd_mma(d, da_hi + off, dbh, idesc2, 1);
-                            }
-                    }
-                    tc5_commit(&sm.m2_done);
-                    if (itimed) ti2 += clock64() - tq;
-                }
-            }
-        }
-        __syncwarp();
-        if (itimed) { dbg_clk[0] = ti1; dbg_clk[1] = ti2; dbg_clk[2] = 0; dbg_clk[3] = K; }
-    } else {
-        // optional timeline of one warp of CTA 0 (pb_debug_counters): cycles in INT, waiting at (A), in P, waiting at (B)
-        const bool timed = TIMED && dbg_clk != nullptr && dbg >= 100 && blockIdx.x == 0 && lane == 0 && warp == dbg - 100;
-        long long t_int = 0, t_wa = 0, t_p = 0, t_wb = 0, t0 = 0, t1 = 0;
-#pragma unroll 1
-        for (int k = -2; k <= K; ++k) {
-            if (timed) t0 = clock64();
-            // ================= INT(k): stage-1 result -> twiddle -> split -> stage-2 operand
-            if (k >= 0 && k < K) {
-                mbar_wait(&sm.m1_done, k & 1);
-                tc5_fence_after();
-                uint32_t yv[2][16];
-                tc3_ld16(tmem + ((uint32_t)(q4 * 32) << 16) + 32 * wg, yv[0]);
-                tc3_ld16(tmem + ((uint32_t)(q4 * 32) << 16) + 32 * wg + 16, yv[1]);
-                tc3_wait_ld16(yv[0]);
-                tc3_wait_ld16(yv[1]);
-                tc5_fence_before();
-                mbar_arrive(&sm.d1_free);                        // the stage-1 accumulators may be overwritten
-                if (k >= 1) mbar_wait(&sm.m2_done, (k - 1) & 1); // the tensor core has read the previous tile's operands (long ago)
-                float tw[16];
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float4 t4 = *reinterpret_cast<const float4*>(&sm.tw[lane][4 * q]);
-                    tw[4 * q] = t4.x; tw[4 * q + 1] = t4.y; tw[4 * q + 2] = t4.z; tw[4 * q + 3] = t4.w;
-                }
-#pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                    float y[16], zr[9], zi[9];
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) y[e] = __uint_as_float(yv[u][e]);
-                    tc3_twiddle(y, tw, zr, zi);
-                    const int fr = 4 * (2 * wg + u) + q4;
-                    unsigned char* base = &sm.a2[0][0][0][0] + int_lane_off + fr * 16;
-#pragma unroll
-                    for (int b = 0; b < TCD_BLOCKS; ++b) {
-                        const __half2 hh = __floats2half2_rn(zr[b], zi[b]);
-                        const float2 hf = __half22float2(hh);
-                        const __half2 ll = __floats2half2_rn(zr[b] - hf.x, zi[b] - hf.y);
-                        const int o = tc3_blk_s(b) * TC3_A2_TILE + 32 * tc3_blk_h(b) * 16;
-                        *reinterpret_cast<uint32_t*>(base + o) = *reinterpret_cast<const uint32_t*>(&hh);
-                        *reinterpret_cast<uint32_t*>(base + A2_PIECE + o) = *reinterpret_cast<const uint32_t*>(&ll);
-                    }
-                }
-                fence_proxy_async();
-                mbar_arrive(&sm.a2_ready);                       // the stage-2 operand of tile k is complete once all workers are here
-            }
-            if (timed) { t1 = clock64(); t_int += t1 - t0; t0 = t1; }
-
-            // ================= P(k)
-            if (warp < 8) {
-                // ---- EPI(k - 1): row (frame = lane, h = q4), part wg: one 64-column block (row 3, part 1: blocks 0 and 8)
-                if (k >= 1) {
-                    const int ke = k - 1;
-                    if (k == K) mbar_wait(&sm.m2_done, ke & 1);
-                    tc5_fence_after();
-                    const Tc3Rec& r = sm.rec[ke & (TC3_REC_RING - 1)][lane];
-                    // x0 = 256 hi0 + lo0 from the split constants: lo0 = -c_lo - 1152, hi0 / 128 = -c_hi - 9
-                    const float x0f = fmaf(-32768.f, __half2float(__ushort_as_half(r.c_hi)) + 9.f, -__half2float(__ushort_as_half(r.c_lo)) - 1152.f);
-                    const uint32_t t_row = tmem + ((uint32_t)(q4 * 32) << 16) + TC3_D1_COLS + (ke & 1) * TC3_D2_COLS;
-                    float rise[G::n_filt + 1], seg[G::n_filt + 1];
-#pragma unroll
-                    for (int j = 0; j <= G::n_filt; ++j) { rise[j] = 0.f; seg[j] = 0.f; }
-                    if (wg == 0) {
-                        if (q4 == 0) tc3_block_bins<G, 1>(t_row, x0f, rise, seg);
-                        else if (q4 == 1) tc3_block_bins<G, 3>(t_row, x0f, rise, seg);
-                        else if (q4 == 2) tc3_block_bins<G, 5>(t_row, x0f, rise, seg);
-                        else tc3_block_bins<G, 7>(t_row, x0f, rise, seg);
-                    } else {
-                        if (q4 == 0) tc3_block_bins<G, 2>(t_row + 64, x0f, rise, seg);
-                        else if (q4 == 1) tc3_block_bins<G, 4>(t_row + 64, x0f, rise, seg);
-                        else if (q4 == 2) tc3_block_bins<G, 6>(t_row + 64, x0f, rise, seg);
-                        else { tc3_block_bins<G, 0>(t_row + 64, x0f, rise, seg); tc3_block_bins<G, 8>(t_row + 128, x0f, rise, seg); }
-                    }
-                    tc5_fence_before();
-                    mbar_arrive(&sm.d2_free[ke & 1]);            // this accumulator buffer may be overwritten (by tile ke + 2)
-                    // PCM of tile k + 2 on its way (the copies land under the rest of the epilogue)
-                    if (k + 2 < K) { mbar_wait(&sm.m1_done, (k + 1) & 1); stage_tile(k + 2); }
-                    // this thread's share of the 20 mel sums and of the total power: one row of the exchange buffer, six 16-byte stores
-                    {
-                        float pv[24];
-                        float tot = seg[0];
-#pragma unroll
-                        for (int j = 0; j < G::n_filt; ++j) {
-                            const float fall = j + 1 < G::n_filt ? seg[j + 1] - rise[j + 1] : rise[G::n_filt];
-                            pv[j] = rise[j] + fall;
-                            tot += seg[j + 1];
-                        }
-                        pv[20] = tot; pv[21] = 0.f; pv[22] = 0.f; pv[23] = 0.f;
-                        float4* pr = reinterpret_cast<float4*>(sm.part[tid]);
-#pragma unroll
-                        for (int q = 0; q < 6; ++q) pr[q] = make_float4(pv[4 * q], pv[4 * q + 1], pv[4 * q + 2], pv[4 * q + 3]);
-                    }
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
-                    if ((dbg & 8) && dbg < 100) {
-                        // Variant (A/B): after the exchange, warp w takes frames 4 w .. 4 w + 3 of the tile, eight lanes per frame: lane j8 < 5 sums the
-                        // eight partial sums of filters 4 j8 .. 4 j8 + 3 and takes their logs, lane 5 the total power; the 20 log-mels are gathered
-                        // inside the 8-lane group by shuffles, and lane j8 forms DCT rows j8 and j8 + 8.  No second barrier.
-                        const int fr = 4 * warp + (lane >> 3), j8 = lane & 7;
-                        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (j8 < 6) {
-#pragma unroll
-                            for (int v = 0; v < 8; ++v) {
-                                const float4 a = *reinterpret_cast<const float4*>(&sm.part[32 * v + fr][4 * j8]);
-                                acc.x += a.x; acc.y += a.y; acc.z += a.z; acc.w += a.w;
-                            }
-                        }
-                        float lg4[4];
-                        lg4[0] = __logf(fmaxf(acc.x * tab.pscale, K1_EPS)); lg4[1] = __logf(fmaxf(acc.y * tab.pscale, K1_EPS));
-                        lg4[2] = __logf(fmaxf(acc.z * tab.pscale, K1_EPS)); lg4[3] = __logf(fmaxf(acc.w * tab.pscale, K1_EPS));
-                        float lg[G::n_filt];
-                        const int grp = lane & ~7;
-#pragma unroll
-                        for (int q = 0; q < G::n_filt; ++q) lg[q] = __shfl_sync(0xffffffffu, lg4[q & 3], grp | (q >> 2));
-                        const float c0 = __shfl_sync(0xffffffffu, lg4[0], grp | 5);
-                        const Tc3Rec& rr = sm.rec[ke & (TC3_REC_RING - 1)][fr];
-                        if (rr.frame != nullptr) {
-                            float* rowp = rr.row;
-                            for (int o = j8; o < tab.n_out; o += 8) {
-                                const float4* d4 = reinterpret_cast<const float4*>(sm.dct[o]);
-                                float v0 = 0.f, v1 = 0.f;
-#pragma unroll
-                                for (int q = 0; q < G::n_filt / 4; ++q) {
-                                    const float4 dd = d4[q];
-                                    v0 = fmaf(dd.x, lg[4 * q], v0); v1 = fmaf(dd.y, lg[4 * q + 1], v1);
-                                    v0 = fmaf(dd.z, lg[4 * q + 2], v0); v1 = fmaf(dd.w, lg[4 * q + 3], v1);
-                                }
-                                rowp[o] = o == 0 ? c0 : v0 + v1;
-                            }
-                        }
-                    } else {
-                        const int t8 = q4 + 4 * wg;                  // 0..7: thread t8 < 5 sums and logs filters 4 t8 .. 4 t8 + 3, thread 5 the total power
-                        if (t8 < 6) {
-                            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    #pragma unroll
-                            for (int v = 0; v < 8; ++v) {
-                                const float4 a = *reinterpret_cast<const float4*>(&sm.part[32 * v + lane][4 * t8]);
-                                acc.x += a.x; acc.y += a.y; acc.z += a.z; acc.w += a.w;
-                            }
-                            if (t8 < 5) {
-                                float4 lg;
-                                lg.x = __logf(fmaxf(acc.x * tab.pscale, K1_EPS)); lg.y = __logf(fmaxf(acc.y * tab.pscale, K1_EPS));
-                                lg.z = __logf(fmaxf(acc.z * tab.pscale, K1_EPS)); lg.w = __logf(fmaxf(acc.w * tab.pscale, K1_EPS));
-                                *reinterpret_cast<float4*>(&sm.lgm[lane][4 * t8]) = lg;
-                            } else {
-                                sm.c0v[lane] = __logf(fmaxf(acc.x * tab.pscale, K1_EPS));
-                            }
-                        }
-                        asm volatile("bar.sync 1, 256;" ::: "memory");
-                        if (r.frame != nullptr) {
-                            float* rowp = r.row;
-                            float lg[G::n_filt];
-    #pragma unroll
-                            for (int q = 0; q < G::n_filt / 4; ++q) {
-                                const float4 a = *reinterpret_cast<const float4*>(&sm.lgm[lane][4 * q]);
-                                lg[4 * q] = a.x; lg[4 * q + 1] = a.y; lg[4 * q + 2] = a.z; lg[4 * q + 3] = a.w;
-                            }
-                            for (int o = t8; o < tab.n_out; o += 8) {
-                                const float4* d4 = reinterpret_cast<const float4*>(sm.dct[o]);
-                                float v0 = 0.f, v1 = 0.f;
-    #pragma unroll
-                                for (int q = 0; q < G::n_filt / 4; ++q) {
-                                    const float4 dd = d4[q];
-                                    v0 = fmaf(dd.x, lg[4 * q], v0); v1 = fmaf(dd.y, lg[4 * q + 1], v1);
-                                    v0 = fmaf(dd.z, lg[4 * q + 2], v0); v1 = fmaf(dd.w, lg[4 * q + 3], v1);
-                                }
-                                rowp[o] = o == 0 ? sm.c0v[lane] : v0 + v1;
-                            }
-                        }
-                    }
-                }
-            } else {
-                // ---- new tails of tile k + 1 (converted one phase ago: the old tails are no longer needed): warp w8 takes frames 4 w8 .. 4 w8 + 3
-                if (k + 1 >= 0 && k + 1 < K) {
-                    const int w8 = warp - 8;
-                    uint4 tv[4][2];
-                    uint4* tdst[4];
-                    int tnv[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {                // all loads first: one memory latency, not four
-                        const Tc3Rec& r = sm.rec[(k + 1) & (TC3_REC_RING - 1)][4 * w8 + u];
-                        tnv[u] = r.frame != nullptr ? (int)r.tail_nv : 0;
-                        tdst[u] = reinterpret_cast<uint4*>(r.tail);
-                        const uint4* src = reinterpret_cast<const uint4*>(r.frame + 8 * (int)r.tail_delta);
-                        if (lane < tnv[u]) tv[u][0] = __ldg(src + lane);
-                        if (lane + 32 < tnv[u]) tv[u][1] = __ldg(src + lane + 32);
-                    }
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        if (lane < tnv[u]) tdst[u][lane] = tv[u][0];
-                        if (lane + 32 < tnv[u]) tdst[u][lane + 32] = tv[u][1];
-                    }
-                }
-                // ---- frame records of tile k + 4 (warp 15), with an L2 prefetch of everything that tile will read
-                if (warp == 15) {
-                    int4 a, b;
-                    fetch_rec(k + 4, lane, a, b);
-                    Tc3Rec r;
-                    reinterpret_cast<int4*>(&r)[0] = a; reinterpret_cast<int4*>(&r)[1] = b;
-                    if (r.frame != nullptr) {                    // everything tile k + 4 will read: into L2 now, line by line
-                        const char* fp = reinterpret_cast<const char*>(r.frame) + 16 * (int)r.len0c;
-                        for (int o = 0; o < 16 * (64 - (int)r.len0c); o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(fp + o));
-                        const char* tp = reinterpret_cast<const char*>(r.frame) + 16 * (int)r.tail_delta;
-                        for (int o = 0; o < 16 * (int)r.tail_nv; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(tp + o));
-                    }
-                    store_rec(k + 4, lane, a, b);
-                }
-            }
-            // ---- CONV(k + 2), every worker its share.  Stage 1 of tile k + 1 must have read the operand buffer before the raw PCM
-            // of tile k + 2 is copied into it (epilogue warps with an epilogue to run have staged already, see above).
-            if (k + 2 < K) {
-                if (!(warp < 8 && k >= 1)) {
-                    if (k + 2 >= 1) mbar_wait(&sm.m1_done, (k + 1) & 1);
-                    stage_tile(k + 2);
-                }
-                conv_tile(k + 2);
-                fence_proxy_async();
-                mbar_arrive(&sm.a1_ready);                       // the stage-1 operand of tile k + 2 is complete once all workers are here
-            }
-            if (timed) { t1 = clock64(); t_p += t1 - t0; }
-            asm volatile("bar.sync 2, 512;" ::: "memory");       // workers only: frame records and exchange buffers change hands
-            if (timed) t_wb += clock64() - t1;
-        }
-        if (timed) { dbg_clk[0] = t_int; dbg_clk[1] = t_wa; dbg_clk[2] = t_p; dbg_clk[3] = t_wb; }
-    }
-    tc5_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(512) : "memory");
 }
 
 }  // namespace pb

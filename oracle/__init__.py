@@ -18,13 +18,11 @@ Parity pinning status
 * ``decoder.py``, ``trigger.py``, ``params.py``, ``listener.py`` (state machine): PINNED.  The
   reference's own ``precise/threshold_decoder.py``, ``precise/functions.py``,
   ``precise/params.py``, ``runner/precise_runner/runner.py`` and the real
-  ``precise.network_runner.Listener`` class were imported unmodified from ``/root/reference``
-  in the build container and their outputs committed as ``tests/golden/*.npz`` by
+  ``precise.network_runner.Listener`` class were imported unmodified from a reference checkout and their outputs committed as ``tests/golden/*.npz`` by
   ``tests/golden/make_golden.py``; ``tests/test_oracle_golden.py`` replays them.
 * ``mfcc.py`` (sonopy 0.1.2, pinned in reference ``requirements.txt:35``) and ``gru.py``
   (Keras<=2.1.5 / TF 1.13 GRU+Dense, reference ``setup.py:75-78``): **PARITY UNPINNED**.
-  Neither sonopy nor Keras/TF source is under ``/root/reference``, in the image, or in the
-  offline wheelhouse, and the reference's tests hold no golden vectors for this path
+  Neither sonopy nor Keras/TF source is in the reference tree or installable for Python 3.12, and the reference's tests hold no golden vectors for this path
   (``test/scripts/test_engine.py:50`` asserts only an output regex).  These two files restate
   the published algorithms of those libraries; they are anchored on the reference's call
   sites (``precise/vectorization.py:36-39``, ``precise/model.py:77-82``), on analytic

@@ -1,6 +1,6 @@
 """Oracle restatement of the MFCC featuriser.  TEST INFRASTRUCTURE ONLY.  ** PARITY UNPINNED **
 
-The arithmetic lives in a third-party dependency that is absent from ``/root/reference``:
+The arithmetic lives in a third-party dependency that is absent from the reference tree:
 ``sonopy==0.1.2`` (reference ``requirements.txt:35``; call sites
 ``precise/vectorization.py:24`` and ``:32-39``).  This file restates sonopy's published
 ``mfcc_spec`` / ``mel_spec`` / ``power_spec`` / ``filterbanks`` algorithm as the reference

@@ -1,5 +1,5 @@
 """K2 A/B at the bench size (pb_debug_gru_mode): 0 = default (fp16x3 scan, staged projection blocks, projects its own new frames, 4 CTAs/SM),
-11 = the same at 5 CTAs/SM, 10 = 3xTF32 staged, 9 = 3xTF32 with LDG loads, 7 = 3xTF32 32-stream tiles, 8 = tcgen05 scan over the cache."""
+11 = the same at 5 CTAs/SM, 10 = 3xTF32 staged, 9 = 3xTF32 with LDG loads, 7 = 3xTF32 32-stream tiles."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch, mycroft_precise_b200 as m

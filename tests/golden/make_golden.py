@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """Generate the committed golden fixtures from the REAL reference code.
 
-Run in the build container only (needs /root/reference, which the GPU box does not have):
+Needs a checkout of the reference (mycroft-precise, commit e1a635e); the tests only read the committed outputs:
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py /path/to/mycroft-precise
 
 What is taken from the reference, unmodified, by import:
   * precise.params.ListenerParams            -> params_golden.json
@@ -29,8 +29,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.dont_write_bytecode = True
 sys.path.insert(0, ROOT)
-sys.path.insert(0, '/root/reference')
-sys.path.insert(0, '/root/reference/runner')
+REF = os.path.abspath(sys.argv[1])
+sys.path.insert(0, REF)
+sys.path.insert(0, os.path.join(REF, 'runner'))
 
 sys.path.insert(0, HERE)
 from cases import DECODER_CASES, TRIGGER_CASES, LISTENER_CASES, make_pcm   # noqa: E402

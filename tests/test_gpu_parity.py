@@ -194,9 +194,9 @@ def test_predict_small_path(core, scale):
         assert np.median(np.abs(p - p64)) < 1e-5
 
 
-@pytest.mark.parametrize('mode', [0, 1, 2, 3])
+@pytest.mark.parametrize('mode', [0, 1, 2])
 def test_default_network_kernel_variants(core, mode):
-    """warp-per-stream (auto, small n), thread-per-stream CUDA-core (1) and tensor-core mma.sync 3xTF32 (2) and tcgen05/TMEM (3) kernels."""
+    """warp-per-stream (auto, small n), thread-per-stream CUDA-core (1) and tensor-core mma.sync 3xTF32 (2) kernels."""
     w = og.GruWeights.random(13, 20, seed=11, scale=0.1)
     core.load_weights(w.kernel, w.recurrent, w.bias, w.dense_w, w.dense_b)
     core.gru_mode(mode)
@@ -221,7 +221,7 @@ def test_stream_tick_kernel_variants_agree():
     model = m.GruModel.random(13, 20, seed=6, scale=0.1)
     model.dense_b = 3.0                                   # pushes the confidence over the trigger threshold
     outs = []
-    for mode in (0, 1, 2, 3):
+    for mode in (0, 1, 2):
         sb = m.StreamBatch(model, S, chunk_samples=chunk)
         sb.core.gru_mode(mode)
         raws, fired = [], []
@@ -303,7 +303,7 @@ def _generic_case(pr_kw, H, act='linear', ract='hard_sigmoid', N=200, seed=5, mo
 ])
 @pytest.mark.parametrize('mode', [0, 1])
 def test_predict_tiled_path(H, kw, act, ract, mode):
-    """mode 0: automatic choice (tcgen05 wide-network kernel where it applies), mode 1: CUDA-core tiled kernel."""
+    """mode 0: automatic choice, mode 1: CUDA-core tiled kernel."""
     err = _generic_case(kw, H, act, ract, mode=mode, N=333)
     print('generic GRU err', err)
     assert err < 1e-5
@@ -727,8 +727,9 @@ def test_runner_plugin_predict_shape():
 @pytest.mark.parametrize('k1_mode', [3, 4, 5, 6], ids=['fft_64bit_setup', 'tensor_core', 'tensor_core_two_stage', 'two_stage_shuffle_epilogue'])
 def test_alternative_mfcc_tick_kernels(k1_mode):
     """pb_debug_k1_mode against the default kernel (FFT on the CUDA cores, 32-bit per-pass set-up): 3 = the same kernel with its
-    original 64-bit set-up (must be bit-identical: same arithmetic, different address computation), 4 = stage 2 of the DFT on
-    tcgen05 (mfcc_tc2), 5 = both stages on tcgen05 from exactly split int16 samples (mfcc_tc3).  All validated on B200."""
+    original 64-bit set-up (must be bit-identical: same arithmetic, different address computation), 4 = the mma.sync DFT tick
+    (mfcc_mma.cuh) with stage 1 on the CUDA cores, 5 = both stages on the tensor cores from exactly split int16 samples,
+    6 = 5 with the shuffle epilogue."""
     m = _mod()
     chunk, S, K = 1024, 300, 40
     pcm = noise(S, K * chunk, seed=51)
@@ -752,7 +753,7 @@ def test_alternative_mfcc_tick_kernels(k1_mode):
 
 @pytest.mark.parametrize('chunk', [1024, 800, 2000, 1600])
 def test_two_stage_tensor_core_mfcc_vs_oracle_ragged(chunk):
-    """k1 mode 5 (mfcc_tc3: plan kernel + both DFT stages on tcgen05) against independent oracle Listeners: windows after every
+    """k1 mode 5 (mfcc_mma.cuh: plan kernel + both DFT stages on mma.sync) against independent oracle Listeners: windows after every
     tick, with streams of different ages in one batch (id subsets skip ticks), several frames per tick (chunk 1600 / 2000), silent,
     full-scale DC, near-silent and boundary-hovering streams, and a partial last tile (frames not a multiple of 32)."""
     import torch
@@ -790,8 +791,9 @@ def test_two_stage_tensor_core_mfcc_vs_oracle_ragged(chunk):
 
 
 def test_default_kernel_choice_large_tick_matches_fft_kernel():
-    """From 49 152 streams per tick on, the default MFCC kernel is mfcc_tc3 (tcgen05); its windows, network outputs and detections
-    must agree with the FFT kernel's on the same audio (many tiles per CTA, several CTAs per SM count, partial last tile)."""
+    """A large tick (49 189 streams: 16 streams per warp tile, several tiles per warp, partial last tile) through the default
+    MFCC kernel (FFT, 32-bit per-pass set-up) must give the same windows, network outputs and detections as the FFT kernel
+    with its original 64-bit set-up on the same audio: the two differ only in address arithmetic."""
     m = _mod()
     chunk, S, K = 1024, 49152 + 37, 30
     base = noise(256, K * chunk, seed=77)
@@ -801,6 +803,34 @@ def test_default_kernel_choice_large_tick_matches_fft_kernel():
     model.dense_b = 3.0
     a = m.StreamBatch(model, S, chunk_samples=chunk, sensitivity=0.9, trigger_level=0)
     b = m.StreamBatch(model, S, chunk_samples=chunk, sensitivity=0.9, trigger_level=0)
+    b.core.k1_mode(3)
+    worst = 0.0
+    for k in range(K):
+        c = cuda(np.ascontiguousarray(pcm[:, k * chunk:(k + 1) * chunk]))
+        ra, rb = a.update(c), b.update(c)
+        worst = max(worst, float((ra['raw'] - rb['raw']).abs().max().item()))
+        if k % 7 == 6 or k == K - 1:
+            wa, wb = a.core.read_window(S), b.core.read_window(S)
+            assert torch.equal(wa, wb), k
+    assert worst == 0.0
+    ca, cb = int(a.count.item()), int(b.count.item())
+    assert ca > 0 and ca == cb, (ca, cb)
+    a.core.close(); b.core.close()
+
+
+def test_two_stage_tensor_core_mfcc_large_tick_matches_fft_kernel():
+    """k1 mode 5 (mfcc_mma.cuh) at 20 011 streams per tick (2 500 to 3 200 tiles of 8 frames: several tiles per warp, partial last tile)
+    against the FFT kernel on the same audio: windows, network outputs and detections."""
+    m = _mod()
+    chunk, S, K = 1024, 20011, 30
+    base = noise(256, K * chunk, seed=78)
+    base[3] = 0; base[4] = 32767; base[5] = np.round(np.random.RandomState(2).randn(K * chunk) * 2)
+    pcm = np.tile(base, (S // 256 + 1, 1))[:S]
+    model = m.GruModel.random(13, 20, seed=9, scale=0.1)
+    model.dense_b = 3.0
+    a = m.StreamBatch(model, S, chunk_samples=chunk, sensitivity=0.9, trigger_level=0)
+    b = m.StreamBatch(model, S, chunk_samples=chunk, sensitivity=0.9, trigger_level=0)
+    a.core.k1_mode(5)
     b.core.k1_mode(2)
     worst = 0.0
     for k in range(K):
@@ -829,20 +859,3 @@ def test_detection_counter_overlapped_allreduce_single_rank():
     torch.cuda.synchronize()
     assert int(c.total.item()) == int(local.item()) == 28
 
-
-def test_tcgen05_scan_over_cached_projections():
-    m = _mod()
-    S, K, chunk = 9000, 36, 1024
-    pcm = noise(64, K * chunk, seed=61)
-    pcm = np.tile(pcm, (S // 64 + 1, 1))[:S].copy()
-    model = m.GruModel.random(13, 20, seed=8, scale=0.1)
-    model.dense_b = 3.0
-    res = []
-    for mode in (8, 1):
-        sb = m.StreamBatch(model, S, chunk_samples=chunk)
-        sb.core.gru_mode(mode)
-        raws = [sb.update(cuda(pcm[:, k * chunk:(k + 1) * chunk]))['raw'].cpu().numpy().copy() for k in range(K)]
-        res.append((np.array(raws), int(sb.count.item())))
-        sb.core.close()
-    assert np.max(np.abs(res[0][0] - res[1][0])) < 1e-5
-    assert res[0][1] > 0 and abs(res[0][1] - res[1][1]) <= 3

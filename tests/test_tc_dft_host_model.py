@@ -1,7 +1,7 @@
-"""CPU: the host-side half of the experimental tensor-core MFCC kernel (csrc/mfcc_tc.cuh) -- the 16-point real-DFT butterfly,
-the fp16 hi/lo twiddle operands in the UMMA K-major layout (with the K permutation the producer threads write) and the
-accumulator-column -> bin map -- reproduces a float64 power spectrum.  The library exports a CPU model built from exactly
-those pieces (pb_debug_tc_dft_power); no device is needed."""
+"""CPU: the tensor-core formulation of the MFCC DFT -- the 16-point real-DFT butterfly, the fp16 hi/lo operands of the 64 x 64
+stage-2 matrix and the accumulator-column -> bin map (csrc/mfcc_tc.cuh, csrc/mfcc_tc3.cuh) -- reproduces a float64 power
+spectrum, and so does the DFT of the mma.sync MFCC tick read through that kernel's own fragment tables (csrc/mfcc_mma.cuh).
+The library exports these CPU models (pb_debug_tc_dft_power, pb_debug_mma_dft_power, ...); no device is needed."""
 import ctypes as C
 
 import numpy as np
@@ -43,6 +43,26 @@ def test_host_model_matches_float64_fft(name, x):
 
 def test_silence_is_exactly_zero():
     assert np.all(_power(np.zeros(512, np.int16)) == 0.0)
+
+
+def _mma_power(x):
+    lib = get_lib()
+    x = np.ascontiguousarray(x, dtype=np.int16)
+    out = np.zeros(257, np.float64)
+    assert lib.pb_debug_mma_dft_power(x.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)) == 0
+    return out
+
+
+@pytest.mark.parametrize('name,x', list(_cases()), ids=[n for n, _ in _cases()])
+def test_mma_kernel_tables_match_float64_fft(name, x):
+    """mfcc_mma.cuh's fragment tables (mm_build_tables), exact sample split, twiddles and bin assembly."""
+    x = np.asarray(x).astype(np.int16)
+    ref = np.abs(np.fft.rfft(x.astype(np.float64))) ** 2
+    got = _mma_power(x)
+    peak = max(ref.max(), 1.0)
+    assert np.max(np.abs(got - ref)) / peak < 3e-6, name
+    if np.all(x == x[0]):                                              # constant frame: exact zeros outside bin 0
+        assert np.all(got[1:] == 0.0)
 
 
 def _mfcc_frame(pr, x512):
