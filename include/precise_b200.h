@@ -33,6 +33,7 @@ extern "C" {
 
 #define PB_ABI_VERSION 2
 #define PB_MAX_THRESHOLDS 8
+#define PB_MAX_MODELS 8           /* networks a handle's model bank holds (pb_add_model), slot 0 included */
 
 typedef enum pb_status {
     PB_OK = 0,
@@ -151,6 +152,31 @@ int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, i
               float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_count,
               void* stream);
 
+/* Model bank: several networks scored per tick over the handle's one MFCC front end (e.g. a wake word and a wake-up word,
+ * each a Listener + TriggerDetector of its own fed the same chunk).  Slot 0 is the handle's own network (pb_create /
+ * pb_load_weights); pb_add_model appends slot 1, 2, ... up to PB_MAX_MODELS models in all.  Models cannot be removed.
+ *
+ * pb_add_model: cfg supplies the model's network (hidden, activation, recurrent_activation), ThresholdDecoder
+ * (n_thresholds, threshold_mu / _std, threshold_center, decode_legacy_f64) and TriggerDetector (sensitivity, trigger_level)
+ * fields.  Its front-end fields (sample_rate, window_samples, hop_samples, n_fft, n_filt, n_mfcc, n_features, use_delta,
+ * vectorizer, chunk_samples, device) must equal the handle's, else PB_ERR_INVALID naming the field; max_streams is taken
+ * from the handle.  Weights as pb_load_weights (HOST pointers, Keras layout).  h_cd (optional, may be NULL = the built-in
+ * table) is the model's CDF table of cd_len entries, as pb_set_cdf takes it.  *slot (optional) receives the model's slot.
+ * Allocates the weights, tables and a [max_streams] int32 trigger state; no second ring, tail or projection cache.
+ * Synchronous. */
+int pb_add_model(pb_handle* h, const pb_config* cfg, const float* h_kernel, const float* h_recurrent,
+                 const float* h_bias, const float* h_dense_w, float dense_b, const double* h_cd, int64_t cd_len,
+                 int32_t* slot);
+/* Number of models in the bank (>= 1), or a negative pb_status. */
+int pb_num_models(const pb_handle* h);
+/* Bank tick: the pb_update tick for every model of the bank, MFCC computed once.  Outputs are model-major, M = pb_num_models:
+ *   d_raw [M][n] float32 (optional), d_conf [M][n] float64, d_fired [M][n] uint8 (optional),
+ *   d_count [M] uint64 (optional; d_count[m] += streams model m fired for this tick).
+ * d_pcm / d_stream_ids as pb_update.  PB_ERR_STATE if slot 0 has no weights.  Slot 0's cached input projections are not
+ * maintained by this tick; a later pb_update rebuilds them. */
+int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, int64_t n,
+                     float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_count, void* stream);
+
 /* Listener.update_vectors only (network_runner.py:125-146): advance stream state, no network. */
 int pb_update_vectors(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, int64_t n,
                       void* stream);
@@ -166,7 +192,7 @@ int pb_update_host(pb_handle* h, const int16_t* h_pcm, const int32_t* h_stream_i
  * given streams: d_out [n][n_features][pb_mfcc_width()] float32, oldest row first. */
 int pb_read_window(pb_handle* h, const int32_t* d_stream_ids, int64_t n, float* d_out, void* stream);
 
-/* Replaces Listener.clear (network_runner.py:121-123) and re-arms the stream's trigger counter.
+/* Replaces Listener.clear (network_runner.py:121-123) and re-arms the stream's trigger counter (of every bank model).
  * d_stream_ids NULL => streams 0..n-1. */
 int pb_clear(pb_handle* h, const int32_t* d_stream_ids, int64_t n, void* stream);
 
@@ -175,7 +201,7 @@ int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);
 
 /* Per-kernel device timing (CUDA events on the launching stream), for bench.py's roofline.
- * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel, 2 = decode-only kernel.
+ * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel (a bank tick: all its network kernels), 2 = decode-only kernel.
  * pb_profile_read synchronises the recorded events, returns accumulated ms and launch counts
  * since the last pb_profile_reset. */
 int pb_profile_enable(pb_handle* h, int on);

@@ -20,7 +20,30 @@ class StreamBatch:
         self.core.load_weights(model.kernel, model.recurrent, model.bias, model.dense_w, model.dense_b)
         torch = self.core.torch
         self.count = torch.zeros(1, dtype=torch.int64, device=self.core.device)
+        self.counts = torch.zeros(1, dtype=torch.int64, device=self.core.device)    # per bank model, update_models only
         self._out = None
+        self._bank_out = None
+
+    def add_model(self, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False) -> int:
+        """Score another network (GruModel or weights path) on the same streams' MFCC frames; returns its bank slot.
+        See PreciseB200.add_model."""
+        slot = self.core.add_model(model, params, sensitivity, trigger_level, decode_legacy_f64)
+        torch = self.core.torch
+        self.counts = torch.cat([self.counts, torch.zeros(1, dtype=torch.int64, device=self.core.device)])
+        self._bank_out = None
+        return slot
+
+    def update_models(self, pcm, ids=None):
+        """One tick for every bank model: pcm int16 CUDA [n, chunk_samples] -> dict(raw f32, conf f64, fired u8), each
+        [M, n].  ``self.counts`` (int64[M], device) accumulates each model's fired streams until reset_count()."""
+        n, M = pcm.shape[0], self.core.num_models
+        if self._bank_out is None or tuple(self._bank_out['conf'].shape) != (M, n):
+            torch = self.core.torch
+            dev = self.core.device
+            self._bank_out = dict(raw=torch.empty((M, n), dtype=torch.float32, device=dev),
+                                  conf=torch.empty((M, n), dtype=torch.float64, device=dev),
+                                  fired=torch.empty((M, n), dtype=torch.uint8, device=dev))
+        return self.core.update_models(pcm, ids, self._bank_out, self.counts)
 
     def update(self, pcm, ids=None):
         """pcm: int16 CUDA tensor [n, chunk_samples] -> dict(raw f32[n], conf f64[n], fired u8[n]).
@@ -39,6 +62,7 @@ class StreamBatch:
 
     def reset_count(self):
         self.count.zero_()
+        self.counts.zero_()
 
     def clear(self, ids=None):
         self.core.clear(ids=ids) if ids is not None else self.core.clear()

@@ -12,7 +12,11 @@ from .params import ListenerParams
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 PB_MAX_THRESHOLDS = 8
+PB_MAX_MODELS = 8
 PB_ABI_VERSION = 2
+# ListenerParams fields of the MFCC front end: the models of one handle's bank must agree on all of them
+FRONT_END_FIELDS = ('sample_rate', 'window_samples', 'hop_samples', 'n_fft', 'n_filt', 'n_mfcc', 'n_features',
+                    'use_delta', 'vectorizer')
 
 
 class PBError(RuntimeError):
@@ -49,6 +53,9 @@ SYMBOLS = {
     'pb_predict': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP]),
     'pb_decode': (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
     'pb_update': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
+    'pb_add_model': (C.c_int, [_VP, C.POINTER(pb_config), _VP, _VP, _VP, _VP, C.c_float, _VP, _I64, C.POINTER(_I32)]),
+    'pb_num_models': (C.c_int, [_VP]),
+    'pb_update_models': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
     'pb_update_vectors': (C.c_int, [_VP, _VP, _VP, _I64, _VP]),
     'pb_update_host': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP]),
     'pb_read_window': (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
@@ -230,16 +237,48 @@ class PreciseB200:
         return C.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)
 
     # ---- model
-    def load_weights(self, kernel, recurrent, bias, dense_w, dense_b):
-        F, H = self.feature_size, self.hidden
+    @staticmethod
+    def _weights(F, H, kernel, recurrent, bias, dense_w):
         k = np.ascontiguousarray(kernel, dtype=np.float32)
         u = np.ascontiguousarray(recurrent, dtype=np.float32)
         b = np.ascontiguousarray(bias, dtype=np.float32).reshape(-1)
         w = np.ascontiguousarray(dense_w, dtype=np.float32).reshape(-1)
         if k.shape != (F, 3 * H) or u.shape != (H, 3 * H) or b.shape != (3 * H,) or w.shape != (H,):
             raise ValueError('weight shapes %s %s %s %s do not match F=%d, H=%d' % (k.shape, u.shape, b.shape, w.shape, F, H))
+        return k, u, b, w
+
+    def load_weights(self, kernel, recurrent, bias, dense_w, dense_b):
+        k, u, b, w = self._weights(self.feature_size, self.hidden, kernel, recurrent, bias, dense_w)
         vp = lambda a: a.ctypes.data_as(C.c_void_p)
         check(self.lib.pb_load_weights(self._h, vp(k), vp(u), vp(b), vp(w), float(np.asarray(dense_b).reshape(-1)[0])))
+
+    # ---- model bank: more networks over the same MFCC front end (slot 0 is the network of load_weights)
+    def add_model(self, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False) -> int:
+        """Add a network to this handle's bank; returns its slot.  ``model`` is a GruModel or a .npz / .pb / .net path (its
+        .params file is read as the reference does).  ``params`` (else the model's .params, else this handle's params) gives
+        the model's decoder settings; its front end must equal this handle's."""
+        from .runner import _resolve_model
+        model, pr = _resolve_model(model)
+        pr = params or pr or self.params
+        diff = [f for f in FRONT_END_FIELDS if getattr(pr, f) != getattr(self.params, f)]
+        if diff:
+            raise ValueError('front end of the model differs from the handle in %s: the models of a bank share one MFCC front end'
+                             % ', '.join('%s (%r != %r)' % (f, getattr(pr, f), getattr(self.params, f)) for f in diff))
+        if model.feature_size != self.feature_size:
+            raise ValueError('model expects %d features, the handle computes %d' % (model.feature_size, self.feature_size))
+        cfg = make_config(pr, model.hidden, self.max_streams, self.chunk_samples, self.device.index, sensitivity,
+                          trigger_level, model.activation, model.recurrent_activation, decode_legacy_f64)
+        k, u, b, w = self._weights(self.feature_size, model.hidden, model.kernel, model.recurrent, model.bias, model.dense_w)
+        cd, lo, hi = numpy_cdf(pr.threshold_config)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        slot = C.c_int32(-1)
+        check(self.lib.pb_add_model(self._h, C.byref(cfg), vp(k), vp(u), vp(b), vp(w), float(model.dense_b),
+                                    vp(cd) if hi > lo else None, len(cd) if hi > lo else 0, C.byref(slot)))
+        return int(slot.value)
+
+    @property
+    def num_models(self) -> int:
+        return int(self.lib.pb_num_models(self._h))
 
     # ---- stateless pieces
     def mfcc_frames(self, n_samples: int) -> int:
@@ -330,6 +369,26 @@ class PreciseB200:
                        fired=torch.empty(n, dtype=torch.uint8, device=self.device))
         check(self.lib.pb_update(self._h, _ptr(pcm), _ptr(ids), n, _ptr(out.get('raw')), _ptr(out['conf']),
                                  _ptr(out.get('fired')), _ptr(count), self._stream()))
+        return out
+
+    def update_models(self, pcm, ids=None, out=None, counts=None):
+        """Bank tick: pcm [n, chunk_samples] int16 CUDA.  Returns dict(raw f32, conf f64, fired u8), each [M, n] for the M
+        models of the bank (slot order); ``counts`` (int64 [M]) accumulates each model's fired streams."""
+        torch = self.torch
+        n = self._check_pcm(pcm)
+        self._check_ids(ids, n)
+        M = self.num_models
+        if out is not None:
+            self._check_t("out['raw']", out.get('raw'), torch.float32, M * n)
+            self._check_t("out['conf']", out.get('conf'), torch.float64, M * n, optional=False)
+            self._check_t("out['fired']", out.get('fired'), torch.uint8, M * n)
+        self._check_t('counts', counts, torch.int64, M)
+        if out is None:
+            out = dict(raw=torch.empty((M, n), dtype=torch.float32, device=self.device),
+                       conf=torch.empty((M, n), dtype=torch.float64, device=self.device),
+                       fired=torch.empty((M, n), dtype=torch.uint8, device=self.device))
+        check(self.lib.pb_update_models(self._h, _ptr(pcm), _ptr(ids), n, _ptr(out.get('raw')), _ptr(out['conf']),
+                                        _ptr(out.get('fired')), _ptr(counts), self._stream()))
         return out
 
     def update_vectors(self, pcm, ids=None):

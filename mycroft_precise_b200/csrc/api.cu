@@ -19,6 +19,7 @@
 
 #include "../../include/precise_b200.h"
 #include "gru_kernels.cuh"
+#include "gru_bank.cuh"
 #include "gru_wide.cuh"
 #include "mfcc_kernels.cuh"
 #include "mfcc_fast.cuh"
@@ -119,6 +120,9 @@ struct pb_handle {
     uint8_t* d_stage_fired[HOST_PIPE] = {nullptr, nullptr, nullptr};
     unsigned long long* d_count = nullptr;
     unsigned long long* h_count_pinned = nullptr;
+    // model bank: slots 1..M-1 (pb_add_model).  Each is a handle without stream state of its own: network, decoder table and
+    // trigger settings, and a [max_streams] trigger array in st.trig; it reads this handle's ring.
+    std::vector<pb_handle*> bank;
     // profiling
     bool profiling = false;
     ProfSlot prof[N_PROFILE_SLOTS];
@@ -282,6 +286,7 @@ PB_API void pb_destroy(pb_handle* h) {
     }
     for (auto& p : h->prof)
         for (auto e : p.ev) cudaEventDestroy(e);
+    for (pb_handle* m : h->bank) pb_destroy(m);
     delete h;
 }
 
@@ -485,6 +490,63 @@ PB_API int pb_set_cdf(pb_handle* h, const double* cd, int64_t len) {
     return PB_OK;
 }
 
+// Networks gru_bank_kernel scores (and gru_mma16_kernel, for the default one): H <= 24, feature_size <= 16, no deltas.
+static bool bank_fused(const pb_handle* h) {
+    return h->cfg.hidden <= BANK_MAX_H && h->feat <= BANK_MAX_F && !h->cfg.use_delta;
+}
+
+// fp16 hi / lo weight fragments of the fused family (gru_mma16_kernel, gru_bank_kernel).  Column (nt, g) -> gate nt / 3,
+// unit 8 (nt % 3) + g.  Recurrent weights: k-tile 0 = hidden units 0..15 as an m16n8k16 B fragment (b0: k = 2t, 2t + 1;
+// b1: k = 2t + 8, 2t + 9), k-tile 1 = units 16..23 as an m16n8k8 one (b0 only).  Input weights: features 0..15 as one k16
+// fragment.  Bias and dense weights padded to 24 units per gate.
+static int upload_frag16(pb_handle* h, const float* kernel, const float* recurrent, const float* bias, const float* dense_w) {
+    const int H = h->cfg.hidden, F = h->feat, H3 = 3 * H;
+    auto h2 = [](float lo16, float hi16) {
+        const __half a = __float2half_rn(lo16), b = __float2half_rn(hi16);
+        uint16_t ua, ub; memcpy(&ua, &a, 2); memcpy(&ub, &b, 2);
+        return (uint32_t)ua | ((uint32_t)ub << 16);
+    };
+    auto res = [](float v) { return v - __half2float(__float2half_rn(v)); };
+    std::vector<uint4> bf16((size_t)2 * MMA_NT * 32);
+    for (int kt = 0; kt < 2; ++kt)
+        for (int nt = 0; nt < MMA_NT; ++nt)
+            for (int lane = 0; lane < 32; ++lane) {
+                const int g = lane >> 2, t = lane & 3, gate = nt / 3, unit = 8 * (nt % 3) + g;
+                float b[2][2];
+                for (int r = 0; r < 2; ++r)
+                    for (int j = 0; j < 2; ++j) {
+                        const int hu = 16 * kt + 8 * r + 2 * t + j;
+                        b[r][j] = (unit < H && hu < H && !(kt == 1 && r == 1)) ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
+                    }
+                bf16[((size_t)kt * MMA_NT + nt) * 32 + lane] = make_uint4(h2(b[0][0], b[0][1]), h2(b[1][0], b[1][1]),
+                                                                          h2(res(b[0][0]), res(b[0][1])), h2(res(b[1][0]), res(b[1][1])));
+            }
+    std::vector<uint4> xf16((size_t)MMA_NT * 32);
+    for (int nt = 0; nt < MMA_NT; ++nt)
+        for (int lane = 0; lane < 32; ++lane) {
+            const int g = lane >> 2, t = lane & 3, gate = nt / 3, unit = 8 * (nt % 3) + g;
+            float b[2][2];
+            for (int r = 0; r < 2; ++r)
+                for (int j = 0; j < 2; ++j) {
+                    const int f = 8 * r + 2 * t + j;
+                    b[r][j] = (unit < H && f < F) ? kernel[(size_t)f * H3 + gate * H + unit] : 0.f;
+                }
+            xf16[(size_t)nt * 32 + lane] = make_uint4(h2(b[0][0], b[0][1]), h2(b[1][0], b[1][1]),
+                                                      h2(res(b[0][0]), res(b[0][1])), h2(res(b[1][0]), res(b[1][1])));
+        }
+    std::vector<float> mb(72, 0.f), mw(24, 0.f);
+    for (int gate = 0; gate < 3; ++gate)
+        for (int u = 0; u < H; ++u) mb[gate * 24 + u] = bias[gate * H + u];
+    for (int u = 0; u < H; ++u) mw[u] = dense_w[u];
+    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd);
+    h->d_bfrag16 = nullptr; h->d_xfrag16 = nullptr; h->d_mma_bias = h->d_mma_wd = nullptr;
+    CK(upload(&h->d_bfrag16, bf16));
+    CK(upload(&h->d_xfrag16, xf16));
+    CK(upload(&h->d_mma_bias, mb));
+    CK(upload(&h->d_mma_wd, mw));
+    return PB_OK;
+}
+
 PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recurrent, const float* bias,
                     const float* dense_w, float dense_b) {
     if (!h || !kernel || !recurrent || !bias || !dense_w) return fail(PB_ERR_INVALID, "null argument");
@@ -524,46 +586,7 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
                     const float b0h = tf32(b[0]), b1h = tf32(b[1]);
                     bf[((size_t)kt * MMA_NT + nt) * 32 + lane] = make_float4(b0h, b1h, tf32(b[0] - b0h), tf32(b[1] - b1h));
                 }
-        {   // fp16 fragments of the recurrent weights (gru_mma16_kernel): k-tile 0 = hidden units 0..15 as an m16n8k16 B fragment
-            // (b0: k = 2t, 2t + 1; b1: k = 2t + 8, 2t + 9), k-tile 1 = units 16..23 as an m16n8k8 one (b0 only); column (nt, g) as above.
-            auto h2 = [](float lo16, float hi16) {
-                const __half a = __float2half_rn(lo16), b = __float2half_rn(hi16);
-                uint16_t ua, ub; memcpy(&ua, &a, 2); memcpy(&ub, &b, 2);
-                return (uint32_t)ua | ((uint32_t)ub << 16);
-            };
-            auto res = [](float v) { return v - __half2float(__float2half_rn(v)); };
-            std::vector<uint4> bf16((size_t)2 * MMA_NT * 32);
-            for (int kt = 0; kt < 2; ++kt)
-                for (int nt = 0; nt < MMA_NT; ++nt)
-                    for (int lane = 0; lane < 32; ++lane) {
-                        const int g = lane >> 2, t = lane & 3, gate = nt / 3, unit = 8 * (nt % 3) + g;
-                        float b[2][2];
-                        for (int r = 0; r < 2; ++r)
-                            for (int j = 0; j < 2; ++j) {
-                                const int hu = 16 * kt + 8 * r + 2 * t + j;
-                                b[r][j] = (unit < H && hu < H && !(kt == 1 && r == 1)) ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
-                            }
-                        bf16[((size_t)kt * MMA_NT + nt) * 32 + lane] = make_uint4(h2(b[0][0], b[0][1]), h2(b[1][0], b[1][1]),
-                                                                                  h2(res(b[0][0]), res(b[0][1])), h2(res(b[1][0]), res(b[1][1])));
-                    }
-            cudaFree(h->d_bfrag16); h->d_bfrag16 = nullptr;
-            CK(upload(&h->d_bfrag16, bf16));
-            // ... and of the input weights: features 0..15 as one k16 fragment (b0: k = 2t, 2t + 1; b1: k = 2t + 8, 2t + 9)
-            std::vector<uint4> xf16((size_t)MMA_NT * 32);
-            for (int nt = 0; nt < MMA_NT; ++nt)
-                for (int lane = 0; lane < 32; ++lane) {
-                    const int g = lane >> 2, t = lane & 3, gate = nt / 3, unit = 8 * (nt % 3) + g;
-                    float b[2][2];
-                    for (int r = 0; r < 2; ++r)
-                        for (int j = 0; j < 2; ++j) {
-                            const int f = 8 * r + 2 * t + j;
-                            b[r][j] = (unit < H && f < F) ? kernel[(size_t)f * H3 + gate * H + unit] : 0.f;
-                        }
-                    xf16[(size_t)nt * 32 + lane] = make_uint4(h2(b[0][0], b[0][1]), h2(b[1][0], b[1][1]),
-                                                              h2(res(b[0][0]), res(b[0][1])), h2(res(b[1][0]), res(b[1][1])));
-                }
-            cudaFree(h->d_xfrag16); h->d_xfrag16 = nullptr;
-            CK(upload(&h->d_xfrag16, xf16));
+        {   // fp16 fragments (gru_mma16_kernel): built below with the other networks of the fused family
             CK(ensure_dyn_smem(gru_mma16_kernel<20, 13, 4>, (size_t)K2_STAGED_SMEM));
             CK(ensure_dyn_smem(gru_mma16_kernel<20, 13, 5>, (size_t)K2_STAGED_SMEM));
             CK(ensure_dyn_smem(gru_mma_kernel<20, 13, true, true, 1, true>, (size_t)K2_STAGED_SMEM));
@@ -579,15 +602,8 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
             CK(upload(&h->d_proj_w, pw));
             CK(upload(&h->d_proj_b, pbias));
         }
-        std::vector<float> mb(72, 0.f), mw(24, 0.f);
-        for (int gate = 0; gate < 3; ++gate)
-            for (int u = 0; u < H; ++u) mb[gate * 24 + u] = bias[gate * H + u];
-        for (int u = 0; u < H; ++u) mw[u] = dense_w[u];
-        cudaFree(h->d_bfrag); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd);
-        h->d_bfrag = nullptr; h->d_mma_bias = h->d_mma_wd = nullptr;
+        cudaFree(h->d_bfrag); h->d_bfrag = nullptr;
         CK(upload(&h->d_bfrag, bf));
-        CK(upload(&h->d_mma_bias, mb));
-        CK(upload(&h->d_mma_wd, mw));
         memcpy(h->w_small.W, kernel, sizeof(h->w_small.W));
         memcpy(h->w_small.U, recurrent, sizeof(h->w_small.U));
         memcpy(h->w_small.b, bias, sizeof(h->w_small.b));
@@ -638,6 +654,10 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
         if (smem > 200 * 1024) return fail(PB_ERR_UNSUPPORTED, "feature_size + 3*hidden = %d is too large for the tiled GRU kernel", F + 3 * H);
         CK(ensure_dyn_smem(gru_tiled_kernel<true>, (size_t)(smem)));
         CK(ensure_dyn_smem(gru_tiled_kernel<false>, (size_t)(smem)));
+    }
+    if (bank_fused(h)) {
+        const int rc = upload_frag16(h, kernel, recurrent, bias, dense_w);
+        if (rc != PB_OK) return rc;
     }
     h->have_weights = true;
     h->proj_dirty = true;
@@ -854,8 +874,7 @@ PB_API int pb_mfcc_f32(pb_handle* h, const float* d_audio, int64_t n_streams, in
     return mfcc_impl<float>(h, d_audio, n_streams, L, d_out, (cudaStream_t)stream, 1.0f / (float)h->cfg.n_fft);
 }
 
-static int launch_gru(pb_handle* h, const K2In& in, bool ring, int64_t n, const DecodeParams& dp, const K2Out& o, cudaStream_t s) {
-    ProfScope ps(h, 1, s);
+static int launch_gru_kernels(pb_handle* h, const K2In& in, bool ring, int64_t n, const DecodeParams& dp, const K2Out& o, cudaStream_t s) {
     if (h->small_path && n <= K2_WARP_PATH_MAX && h->gru_mode == 0) {                 // latency path: a warp per stream
         const int grid = (int)((n + 3) / 4);
         if (ring) gru_warp_kernel<20, 13, true><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
@@ -909,6 +928,11 @@ static int launch_gru(pb_handle* h, const K2In& in, bool ring, int64_t n, const 
     }
     CK(cudaGetLastError());
     return PB_OK;
+}
+
+static int launch_gru(pb_handle* h, const K2In& in, bool ring, int64_t n, const DecodeParams& dp, const K2Out& o, cudaStream_t s) {
+    ProfScope ps(h, 1, s);
+    return launch_gru_kernels(h, in, ring, n, dp, o, s);
 }
 
 PB_API int pb_predict(pb_handle* h, const float* d_inputs, int64_t n, float* d_out, float* d_logit, void* stream) {
@@ -1100,6 +1124,126 @@ PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, i
     return launch_gru(h, in, true, n, decode_params(h), o, s);
 }
 
+// ------------------------------------------------------------------------------------------------
+// model bank
+PB_API int pb_add_model(pb_handle* h, const pb_config* cfg, const float* kernel, const float* recurrent, const float* bias,
+                        const float* dense_w, float dense_b, const double* cd, int64_t cd_len, int32_t* slot) {
+    if (!h || !cfg || !kernel || !recurrent || !bias || !dense_w) return fail(PB_ERR_INVALID, "null argument");
+    const pb_config& c = *cfg;
+    if (c.abi_version != PB_ABI_VERSION) return fail(PB_ERR_INVALID, "abi_version %d != %d", c.abi_version, PB_ABI_VERSION);
+#define PB_SAME_FRONT_END(f)                                                                                  \
+    if (c.f != h->cfg.f)                                                                                      \
+        return fail(PB_ERR_INVALID, "front-end field %s = %d differs from the handle's %d: the models of a bank share one MFCC front end", \
+                    #f, (int)c.f, (int)h->cfg.f)
+    PB_SAME_FRONT_END(sample_rate); PB_SAME_FRONT_END(window_samples); PB_SAME_FRONT_END(hop_samples); PB_SAME_FRONT_END(n_fft);
+    PB_SAME_FRONT_END(n_filt); PB_SAME_FRONT_END(n_mfcc); PB_SAME_FRONT_END(n_features); PB_SAME_FRONT_END(use_delta);
+    PB_SAME_FRONT_END(vectorizer); PB_SAME_FRONT_END(chunk_samples); PB_SAME_FRONT_END(device);
+#undef PB_SAME_FRONT_END
+    if ((int)h->bank.size() + 1 >= PB_MAX_MODELS) return fail(PB_ERR_INVALID, "a bank holds at most %d models", PB_MAX_MODELS);
+    if (c.hidden < 1) return fail(PB_ERR_INVALID, "hidden must be positive");
+    if (c.n_thresholds < 1 || c.n_thresholds > PB_MAX_THRESHOLDS) return fail(PB_ERR_INVALID, "n_thresholds must be in [1, %d]", PB_MAX_THRESHOLDS);
+    if (c.activation < 0 || c.activation > 1 || c.recurrent_activation < 0 || c.recurrent_activation > 1)
+        return fail(PB_ERR_UNSUPPORTED, "unsupported GRU activation");
+    CK(cudaSetDevice(c.device));
+    pb_handle* m = new (std::nothrow) pb_handle();
+    if (!m) return fail(PB_ERR_CUDA, "out of host memory");
+    m->cfg = c;
+    m->cfg.max_streams = h->cfg.max_streams;
+    m->sm_count = h->sm_count; m->used = h->used; m->n_bins = h->n_bins; m->n_out = h->n_out; m->feat = h->feat;
+    m->ring_rows = h->ring_rows; m->row_stride = h->row_stride; m->rel_window = h->rel_window; m->tail_cap = h->tail_cap; m->max_new = h->max_new;
+    build_cdf(m);
+    int rc = PB_OK;
+    if (cd && cd_len != (int64_t)m->cd.size()) rc = fail(PB_ERR_INVALID, "cdf length %lld != %zu", (long long)cd_len, m->cd.size());
+    else if (cd) memcpy(m->cd.data(), cd, cd_len * sizeof(double));
+    const size_t S = (size_t)h->cfg.max_streams;
+    cudaError_t e = cudaSuccess;
+    if (rc == PB_OK && (e = upload(&m->d_cd, m->cd)) == cudaSuccess && (e = cudaMalloc((void**)&m->st.trig, S * sizeof(int))) == cudaSuccess)
+        e = cudaMemset(m->st.trig, 0, S * sizeof(int));
+    if (rc == PB_OK && e != cudaSuccess) rc = fail(PB_ERR_CUDA, "model bank allocation failed: %s", cudaGetErrorString(e));
+    if (rc == PB_OK) rc = pb_load_weights(m, kernel, recurrent, bias, dense_w, dense_b);
+    if (rc != PB_OK) { pb_destroy(m); return rc; }
+    h->bank.push_back(m);
+    if (slot) *slot = (int32_t)h->bank.size();
+    return PB_OK;
+}
+
+PB_API int pb_num_models(const pb_handle* h) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    return 1 + (int)h->bank.size();
+}
+
+template <int NM>
+static int launch_bank_nm(pb_handle* h, const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
+    const size_t smem = (size_t)NM * BANK_MODEL_SMEM;
+    CK(ensure_dyn_smem(gru_bank_kernel<NM>, smem));
+    const int per_cta = (MMA_THREADS / 32) * 16;
+    gru_bank_kernel<NM><<<(int)((n + per_cta - 1) / per_cta), MMA_THREADS, smem, s>>>(P, in, n);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+static int launch_bank(pb_handle* h, const BankParams& P, int nm, const K2In& in, int64_t n, cudaStream_t s) {
+    switch (nm) {
+        case 1: return launch_bank_nm<1>(h, P, in, n, s);
+        case 2: return launch_bank_nm<2>(h, P, in, n, s);
+        case 3: return launch_bank_nm<3>(h, P, in, n, s);
+        case 4: return launch_bank_nm<4>(h, P, in, n, s);
+        case 5: return launch_bank_nm<5>(h, P, in, n, s);
+        case 6: return launch_bank_nm<6>(h, P, in, n, s);
+        case 7: return launch_bank_nm<7>(h, P, in, n, s);
+        case 8: return launch_bank_nm<8>(h, P, in, n, s);
+    }
+    return fail(PB_ERR_INVALID, "%d fused models", nm);
+}
+
+PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
+                            uint8_t* d_fired, unsigned long long* d_count, void* stream) {
+    int rc = check_tick(h, d_pcm, n);
+    if (rc != PB_OK) return rc;
+    if (!h->have_weights) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (n == 0) return PB_OK;
+    if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int M = 1 + (int)h->bank.size();
+    rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
+    if (rc != PB_OK) return rc;
+    h->proj_dirty = true;                                      // this tick's frames get no cached projection: pb_update rebuilds it
+    K2In in{};
+    in.ring = h->st.ring; in.n_samples = h->st.n_samples; in.ids = d_ids;
+    in.ring_rows = h->ring_rows; in.row_stride = h->row_stride; in.window = h->rel_window; in.hop = h->cfg.hop_samples;
+    in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
+    in.proj = nullptr;
+    in.proj_tiles = (h->cfg.max_streams + 15) / 16;
+    in.used = h->used;
+    in.chunk = h->cfg.chunk_samples;
+    ProfScope ps(h, 1, s);
+    // the fused family in one gru_bank_kernel launch; other networks one launch each of their own kernel, on the same ring
+    BankParams P{};
+    int nm = 0;
+    for (int m = 0; m < M; ++m) {
+        pb_handle* hm = m == 0 ? h : h->bank[m - 1];
+        K2Out o{};
+        o.raw = d_raw ? d_raw + (int64_t)m * n : nullptr;
+        o.conf = d_conf + (int64_t)m * n;
+        o.fired = d_fired ? d_fired + (int64_t)m * n : nullptr;
+        o.count = d_count ? d_count + m : nullptr;
+        o.trig = hm->st.trig;
+        if (bank_fused(hm)) {
+            BankModelW& w = P.w[nm];
+            w.bfrag = hm->d_bfrag16; w.xfrag = hm->d_xfrag16; w.bias = hm->d_mma_bias; w.wd = hm->d_mma_wd; w.bd = hm->bd;
+            w.act = hm->cfg.activation; w.ract = hm->cfg.recurrent_activation;
+            P.dp[nm] = decode_params(hm);
+            P.o[nm] = o;
+            ++nm;
+        } else {
+            rc = launch_gru_kernels(hm, in, true, n, decode_params(hm), o, s);
+            if (rc != PB_OK) return rc;
+        }
+    }
+    return nm ? launch_bank(h, P, nm, in, n, s) : PB_OK;
+}
+
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {
     // one thread per (item, row, column)
     const int Fb = in.F_base;
@@ -1141,6 +1285,11 @@ __global__ void clear_kernel(StreamState st, const int* ids, long long n) {
     st.trig[sid] = 0;
 }
 
+__global__ void clear_trig_kernel(int* trig, const int* ids, long long n) {
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) trig[ids ? ids[i] : (int)i] = 0;
+}
+
 PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (n < 0 || n > h->cfg.max_streams) return fail(PB_ERR_INVALID, "bad n");
@@ -1148,6 +1297,10 @@ PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream)
     CK(cudaSetDevice(h->cfg.device));
     clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->st, d_ids, n);
     CK(cudaGetLastError());
+    for (pb_handle* m : h->bank) {                             // the other models of the bank: their trigger counters
+        clear_trig_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(m->st.trig, d_ids, n);
+        CK(cudaGetLastError());
+    }
     return PB_OK;
 }
 
