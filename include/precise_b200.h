@@ -162,7 +162,7 @@ int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, i
  * vectorizer, chunk_samples, device) must equal the handle's, else PB_ERR_INVALID naming the field; max_streams is taken
  * from the handle.  Weights as pb_load_weights (HOST pointers, Keras layout).  h_cd (optional, may be NULL = the built-in
  * table) is the model's CDF table of cd_len entries, as pb_set_cdf takes it.  *slot (optional) receives the model's slot.
- * Allocates the weights, tables and a [max_streams] int32 trigger state; no second ring, tail or projection cache.
+ * Allocates the weights, tables and a [max_streams] int32 trigger state; no second ring or tail.
  * Synchronous. */
 int pb_add_model(pb_handle* h, const pb_config* cfg, const float* h_kernel, const float* h_recurrent,
                  const float* h_bias, const float* h_dense_w, float dense_b, const double* h_cd, int64_t cd_len,
@@ -172,8 +172,7 @@ int pb_num_models(const pb_handle* h);
 /* Bank tick: the pb_update tick for every model of the bank, MFCC computed once.  Outputs are model-major, M = pb_num_models:
  *   d_raw [M][n] float32 (optional), d_conf [M][n] float64, d_fired [M][n] uint8 (optional),
  *   d_count [M] uint64 (optional; d_count[m] += streams model m fired for this tick).
- * d_pcm / d_stream_ids as pb_update.  PB_ERR_STATE if slot 0 has no weights.  Slot 0's cached input projections are not
- * maintained by this tick; a later pb_update rebuilds them. */
+ * d_pcm / d_stream_ids as pb_update.  PB_ERR_STATE if slot 0 has no weights. */
 int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, int64_t n,
                      float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_count, void* stream);
 
@@ -201,7 +200,8 @@ int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);
 
 /* Per-kernel device timing (CUDA events on the launching stream), for bench.py's roofline.
- * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel (a bank tick: all its network kernels), 2 = decode-only kernel.
+ * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel (a bank tick: all its network kernels), 2 = decode-only kernel,
+ * 3 = unused (always 0).
  * pb_profile_read synchronises the recorded events, returns accumulated ms and launch counts
  * since the last pb_profile_reset. */
 int pb_profile_enable(pb_handle* h, int on);
@@ -222,10 +222,8 @@ int pb_set_cdf(pb_handle* h, const double* h_cd, int64_t len);
  * instead of the warp-autonomous fast kernels, so both implementations are covered by parity tests. */
 int pb_debug_force_generic(pb_handle* h, int on);
 /* Test / A-B hook for the default network (H=20, F=13): 0 = automatic choice (warp-per-stream kernel up to 8192 streams per tick; above,
- * the fp16x3 mma.sync scan over bulk-copy-staged cached projections, which also projects the tick's new frames), 1 = CUDA-core
- * thread-per-stream kernel, 2 = tensor-core kernel also for small batches, 7 = 3xTF32 scan with 32-stream warp tiles,
- * 9 = 3xTF32 scan over cached projections without staging, 10 = with staging, 11 = the default scan at 5 CTAs per SM.
- * All variants are parity-tested (tests/test_gpu_parity.py). */
+ * the fp16x3 mma.sync scan of csrc/gru_bank.cuh with one model), 1 = CUDA-core thread-per-stream kernel, 2 = the tensor-core scan
+ * also for small batches.  Any other mode: PB_ERR_INVALID.  All variants are parity-tested (tests/test_gpu_parity.py). */
 int pb_debug_gru_mode(pb_handle* h, int mode);
 /* Test / A-B hook for the stateful tick's MFCC kernel (aligned default geometry).  0 = automatic: the FFT kernel on the CUDA
  * cores (csrc/mfcc_fast.cuh) where the geometry allows it, else the generic kernel; 2 = always the FFT kernel; 3 = the FFT kernel

@@ -67,11 +67,6 @@ struct pb_handle {
     // derived
     int used = 0, n_bins = 0, n_out = 0, feat = 0, ring_rows = 0, row_stride = 0, tail_cap = 0, max_new = 0;
     int rel_window = 0;              // samples before frame 0 is released: window_samples (sonopy), window_samples + hop_samples (speechpy drops the last complete frame)
-    bool has_proj = false;           // default network: a second ring caches the input projections (gru_kernels.cuh)
-    float* d_proj_ring = nullptr;
-    bool proj_dirty = true;          // some ring rows lack a valid cached projection (weights changed / projection skipped)
-    bool host_tick_proj = false;     // inside a pb_update_host tick whose sub-batches use the cache: short sub-batches keep it valid too
-    float *d_proj_w = nullptr, *d_proj_b = nullptr;
     size_t k1_batch_smem = 0, k1_stream_smem = 0, k1_fast_smem = 0;
     bool force_generic = false;      // tests: exercise the generic kernels on the aligned geometry
     int k1_mode = 0;                 // 0 = default (the FFT kernel with 32-bit set-up where the geometry allows it), 2 = always the FFT kernel, 3 = FFT kernel with the original 64-bit set-up, 4 / 5 / 6 = the mma.sync DFT tick (mfcc_mma.cuh): stage 1 on the CUDA cores / on the tensor cores / the latter with a shuffle epilogue
@@ -101,14 +96,13 @@ struct pb_handle {
     bool small_path = false;
     GruSmallW<20, 13> w_small;
     float *d_wcat = nullptr, *d_bias = nullptr, *d_wd = nullptr;
-    float4* d_bfrag = nullptr;       // tensor-core GRU: pre-split, fragment-ordered weights
-    uint4* d_bfrag16 = nullptr;      // ... recurrent part as fp16 hi / lo fragments (gru_mma16_kernel)
-    uint4* d_xfrag16 = nullptr;      // ... and the input part (the scan projects a tick's new frames itself)
+    uint4* d_bfrag16 = nullptr;      // fused family (gru_bank_kernel): recurrent weights as fp16 hi / lo fragments
+    uint4* d_xfrag16 = nullptr;      // ... and the input weights
     float *d_mma_bias = nullptr, *d_mma_wd = nullptr;
     bool wide_ok = false;            // gru_wide_kernel covers the network (H <= 128, F <= 40)
     int wg_fp = 0, wg_hp = 0;
     uint4 *d_wg_b1 = nullptr, *d_wg_b2 = nullptr; float* d_wg_bias = nullptr;
-    int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core kernel, 2 = force tensor-core kernel, 7 = tensor-core kernel with 32-stream warp tiles, 9 / 10 / 11 = A/B variants of the cached-projection scan
+    int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core kernel, 2 = force tensor-core kernel
     float bd = 0.f;
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -276,7 +270,7 @@ PB_API void pb_destroy(pb_handle* h) {
     cudaFree(h->d_tw_stage); cudaFree(h->d_tw_post); cudaFree(h->d_tw_any); cudaFree(h->d_cd); cudaFree(h->d_ptab); cudaFree(h->d_ctab); cudaFree(h->d_dct_t);
     cudaFree(h->st.n_samples); cudaFree(h->st.tail); cudaFree(h->st.ring); cudaFree(h->st.trig);
     cudaFree(h->d_wcat); cudaFree(h->d_bias); cudaFree(h->d_wd); cudaFree(h->d_count);
-    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_bfrag); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd); cudaFree(h->d_proj_w); cudaFree(h->d_proj_b); cudaFree(h->d_proj_ring);
+    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd);
     if (h->h_count_pinned) cudaFreeHost(h->h_count_pinned);
     for (int i = 0; i < HOST_PIPE; ++i) {
         cudaFree(h->d_stage_pcm[i]); cudaFree(h->d_stage_ids[i]); cudaFree(h->d_stage_raw[i]);
@@ -321,9 +315,6 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     h->n_out = c.vectorizer == PB_VEC_MELS ? c.n_filt : std::min(c.n_filt, c.n_mfcc);
     h->feat = h->n_out * (c.use_delta ? 2 : 1);
     h->row_stride = (h->n_out + 3) & ~3;
-    // default-sized networks cache the input projection of every frame in a second ring (gru_mma_kernel<.., PROJ>)
-    h->has_proj = c.hidden == 20 && h->n_out == 13 && !c.use_delta && c.vectorizer == PB_VEC_MFCCS &&
-                  c.chunk_samples / c.hop_samples + 2 <= 8;      // long chunks (fed as sub-chunks, launch_stream_mfcc) may add more rows than the cache logic tracks
     // speechpy's stack_frames yields floor((len - window) / hop) frames, one fewer than sonopy's framing: frame k is released one hop later
     h->rel_window = c.window_samples + (c.vectorizer == PB_VEC_SPEECHPY_MFCCS ? c.hop_samples : 0);
     h->ring_rows = c.n_features + (h->rel_window - h->used) / c.hop_samples + 2;
@@ -442,7 +433,6 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     CKH(cudaMemset(h->st.n_samples, 0, S * sizeof(long long)));
     CKH(cudaMemset(h->st.tail, 0, S * h->tail_cap * sizeof(int16_t)));
     CKH(cudaMemset(h->st.ring, 0, S * h->ring_rows * h->row_stride * sizeof(float)));
-    if (h->has_proj) CKH(cudaMalloc((void**)&h->d_proj_ring, ((S + 15) / 16) * h->ring_rows * PROJ_BLOCK * sizeof(float)));
     CKH(cudaMemset(h->st.trig, 0, S * sizeof(int)));
     CKH(cudaMalloc((void**)&h->d_count, sizeof(unsigned long long)));
     CKH(cudaMemset(h->d_count, 0, sizeof(unsigned long long)));
@@ -490,12 +480,12 @@ PB_API int pb_set_cdf(pb_handle* h, const double* cd, int64_t len) {
     return PB_OK;
 }
 
-// Networks gru_bank_kernel scores (and gru_mma16_kernel, for the default one): H <= 24, feature_size <= 16, no deltas.
+// Networks gru_bank_kernel scores: H <= 24, feature_size <= 16, no deltas.
 static bool bank_fused(const pb_handle* h) {
     return h->cfg.hidden <= BANK_MAX_H && h->feat <= BANK_MAX_F && !h->cfg.use_delta;
 }
 
-// fp16 hi / lo weight fragments of the fused family (gru_mma16_kernel, gru_bank_kernel).  Column (nt, g) -> gate nt / 3,
+// fp16 hi / lo weight fragments of the fused family (gru_bank_kernel).  Column (nt, g) -> gate nt / 3,
 // unit 8 (nt % 3) + g.  Recurrent weights: k-tile 0 = hidden units 0..15 as an m16n8k16 B fragment (b0: k = 2t, 2t + 1;
 // b1: k = 2t + 8, 2t + 9), k-tile 1 = units 16..23 as an m16n8k8 one (b0 only).  Input weights: features 0..15 as one k16
 // fragment.  Bias and dense weights padded to 24 units per gate.
@@ -564,46 +554,6 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
     h->small_path = (H == 20 && F == 13 && !h->cfg.use_delta && h->cfg.activation == PB_ACT_LINEAR &&
                      h->cfg.recurrent_activation == PB_RACT_HARD_SIGMOID);
     if (h->small_path) {
-        // tensor-core fragments (gru_mma_kernel): logical k slot (kt, t, j) -> input 8 kt + 2 t + j
-        // (x feature for kt < 2, hidden unit 8 (kt - 2) + 2 t + j otherwise); column (nt, g) -> gate nt / 3,
-        // unit 8 (nt % 3) + g.  Values are split into TF32 hi / lo parts (round to nearest, ties away).
-        auto tf32 = [](float x) { uint32_t u; memcpy(&u, &x, 4); u = (u + 0x1000u) & 0xffffe000u; float r; memcpy(&r, &u, 4); return r; };
-        std::vector<float4> bf((size_t)MMA_KT * MMA_NT * 32);
-        for (int kt = 0; kt < MMA_KT; ++kt)
-            for (int nt = 0; nt < MMA_NT; ++nt)
-                for (int lane = 0; lane < 32; ++lane) {
-                    const int g = lane >> 2, t = lane & 3, gate = nt / 3, unit = 8 * (nt % 3) + g;
-                    float b[2];
-                    for (int j = 0; j < 2; ++j) {
-                        const int k = 8 * kt + 2 * t + j;
-                        float v = 0.f;
-                        if (unit < H) {
-                            if (kt < 2) { if (k < F) v = kernel[(size_t)k * H3 + gate * H + unit]; }
-                            else { const int hu = k - 16; if (hu < H) v = recurrent[(size_t)hu * H3 + gate * H + unit]; }
-                        }
-                        b[j] = v;
-                    }
-                    const float b0h = tf32(b[0]), b1h = tf32(b[1]);
-                    bf[((size_t)kt * MMA_NT + nt) * 32 + lane] = make_float4(b0h, b1h, tf32(b[0] - b0h), tf32(b[1] - b1h));
-                }
-        {   // fp16 fragments (gru_mma16_kernel): built below with the other networks of the fused family
-            CK(ensure_dyn_smem(gru_mma16_kernel<20, 13, 4>, (size_t)K2_STAGED_SMEM));
-            CK(ensure_dyn_smem(gru_mma16_kernel<20, 13, 5>, (size_t)K2_STAGED_SMEM));
-            CK(ensure_dyn_smem(gru_mma_kernel<20, 13, true, true, 1, true>, (size_t)K2_STAGED_SMEM));
-        }
-        {   // input projection table: wx[f][col], col = gate * 24 + unit (same column order as the accumulator tiles)
-            std::vector<float> pw((size_t)F * PROJ_COLS, 0.f), pbias(PROJ_COLS, 0.f);
-            for (int gate = 0; gate < 3; ++gate)
-                for (int u = 0; u < H; ++u) {
-                    pbias[gate * 24 + u] = bias[gate * H + u];
-                    for (int f = 0; f < F; ++f) pw[(size_t)f * PROJ_COLS + gate * 24 + u] = kernel[(size_t)f * H3 + gate * H + u];
-                }
-            cudaFree(h->d_proj_w); cudaFree(h->d_proj_b); h->d_proj_w = h->d_proj_b = nullptr;
-            CK(upload(&h->d_proj_w, pw));
-            CK(upload(&h->d_proj_b, pbias));
-        }
-        cudaFree(h->d_bfrag); h->d_bfrag = nullptr;
-        CK(upload(&h->d_bfrag, bf));
         memcpy(h->w_small.W, kernel, sizeof(h->w_small.W));
         memcpy(h->w_small.U, recurrent, sizeof(h->w_small.U));
         memcpy(h->w_small.b, bias, sizeof(h->w_small.b));
@@ -660,7 +610,6 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
         if (rc != PB_OK) return rc;
     }
     h->have_weights = true;
-    h->proj_dirty = true;
     return PB_OK;
 }
 
@@ -688,7 +637,12 @@ struct ProfScope {
     ~ProfScope() { if (idx >= 0) cudaEventRecord(h->prof[slot].ev[idx + 1], s); }
 };
 
-PB_API int pb_debug_gru_mode(pb_handle* h, int mode) { if (!h) return fail(PB_ERR_INVALID, "null handle"); h->gru_mode = mode; return PB_OK; }
+PB_API int pb_debug_gru_mode(pb_handle* h, int mode) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (mode < 0 || mode > 2) return fail(PB_ERR_INVALID, "gru mode must be 0 (automatic), 1 (CUDA-core kernel) or 2 (tensor-core kernel)");
+    h->gru_mode = mode;
+    return PB_OK;
+}
 
 PB_API int pb_debug_k1_mode(pb_handle* h, int mode) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
@@ -874,36 +828,34 @@ PB_API int pb_mfcc_f32(pb_handle* h, const float* d_audio, int64_t n_streams, in
     return mfcc_impl<float>(h, d_audio, n_streams, L, d_out, (cudaStream_t)stream, 1.0f / (float)h->cfg.n_fft);
 }
 
+// Model slot `slot` of a gru_bank_kernel launch: network hm, scored with decoder dp into o.
+static void set_bank_slot(BankParams& P, int slot, const pb_handle* hm, const DecodeParams& dp, const K2Out& o) {
+    BankModelW& w = P.w[slot];
+    w.bfrag = hm->d_bfrag16; w.xfrag = hm->d_xfrag16; w.bias = hm->d_mma_bias; w.wd = hm->d_mma_wd; w.bd = hm->bd;
+    w.act = hm->cfg.activation; w.ract = hm->cfg.recurrent_activation;
+    P.dp[slot] = dp;
+    P.o[slot] = o;
+}
+
+template <int NM, bool RING>
+static int launch_bank_nm(const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
+    constexpr size_t smem = (size_t)NM * BANK_MODEL_SMEM;
+    if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(gru_bank_kernel<NM, RING>, smem));      // above the default limit
+    const int per_cta = (MMA_THREADS / 32) * 16;
+    gru_bank_kernel<NM, RING><<<(int)((n + per_cta - 1) / per_cta), MMA_THREADS, smem, s>>>(P, in, n);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
 static int launch_gru_kernels(pb_handle* h, const K2In& in, bool ring, int64_t n, const DecodeParams& dp, const K2Out& o, cudaStream_t s) {
     if (h->small_path && n <= K2_WARP_PATH_MAX && h->gru_mode == 0) {                 // latency path: a warp per stream
         const int grid = (int)((n + 3) / 4);
         if (ring) gru_warp_kernel<20, 13, true><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
         else gru_warp_kernel<20, 13, false><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
-    } else if (h->small_path && h->gru_mode != 1) {               // tensor-core scan (mma.sync TF32 x3)
-        GruMmaW w;
-        w.bfrag = h->d_bfrag; w.bias = h->d_mma_bias; w.wd = h->d_mma_wd; w.bd = h->bd;
-        const int per_cta = (MMA_THREADS / 32) * 16 * MMA_MB;
-        const int grid = (int)((n + per_cta - 1) / per_cta);
-        // Steady-state stream scan: 16-stream tiles (MB = 1) unless forced (gru_mode 7).  With 32-stream tiles 131 072 streams
-        // are 2.3 rounds of 3 CTAs/SM and the last, 31 % full round still costs most of a round (each warp's step is a
-        // dependent chain); 16-stream tiles fit 5 CTAs/SM and leave a much shorter tail.
-        if (ring && in.proj != nullptr && h->gru_mode != 7) {
-            const int per1 = (MMA_THREADS / 32) * 16;
-            if (h->gru_mode == 9)            // A/B: 3xTF32 scan without bulk-copy staging of the projection blocks
-                gru_mma_kernel<20, 13, true, true, 1><<<(int)((n + per1 - 1) / per1), MMA_THREADS, 0, s>>>(w, in, n, dp, o);
-            else if (h->gru_mode == 10)      // A/B: 3xTF32 scan with staging
-                gru_mma_kernel<20, 13, true, true, 1, true><<<(int)((n + per1 - 1) / per1), MMA_THREADS, K2_STAGED_SMEM, s>>>(w, in, n, dp, o);
-            else {                           // default: fp16x3 recurrent products (half the tensor-pipe time), staged projection blocks
-                GruMma16W w16;
-                w16.bfrag = h->d_bfrag16; w16.xfrag = h->d_xfrag16; w16.bias = h->d_mma_bias; w16.wd = h->d_mma_wd; w16.bd = h->bd;
-                if (h->gru_mode == 11)       // A/B: 5 CTAs per SM (96 registers, a small spill): 215 vs 211 us
-                    gru_mma16_kernel<20, 13, 5><<<(int)((n + per1 - 1) / per1), MMA_THREADS, K2_STAGED_SMEM, s>>>(w16, in, n, dp, o);
-                else                         // 4 CTAs per SM, 128 registers
-                    gru_mma16_kernel<20, 13, 4><<<(int)((n + per1 - 1) / per1), MMA_THREADS, K2_STAGED_SMEM, s>>>(w16, in, n, dp, o);
-            }
-        } else if (ring && in.proj != nullptr) gru_mma_kernel<20, 13, true, true><<<grid, MMA_THREADS, 0, s>>>(w, in, n, dp, o);
-        else if (ring) gru_mma_kernel<20, 13, true, false><<<grid, MMA_THREADS, 0, s>>>(w, in, n, dp, o);
-        else gru_mma_kernel<20, 13, false, false><<<grid, MMA_THREADS, 0, s>>>(w, in, n, dp, o);
+    } else if (h->small_path && h->gru_mode != 1) {               // tensor-core scan (mma.sync fp16 x 3): the bank kernel with one model
+        BankParams P{};
+        set_bank_slot(P, 0, h, dp, o);
+        return ring ? launch_bank_nm<1, true>(P, in, n, s) : launch_bank_nm<1, false>(P, in, n, s);
     } else if (h->small_path) {
         const int per_cta = K2_SMALL_THREADS * K2_NS;
         const int grid = (int)((n + per_cta - 1) / per_cta);
@@ -1057,26 +1009,16 @@ PB_API int pb_update_vectors(pb_handle* h, const int16_t* d_pcm, const int32_t* 
     int rc = check_tick(h, d_pcm, n);
     if (rc != PB_OK || n == 0) return rc;
     CK(cudaSetDevice(h->cfg.device));
-    h->proj_dirty = true;
     return launch_stream_mfcc(h, d_pcm, d_ids, n, (cudaStream_t)stream);
 }
 
-// Does a tick of n streams run the scan that reads cached input projections (gru_mma_kernel<.., PROJ>)?
-static bool wants_projection(const pb_handle* h, int64_t n) {
-    return h->has_proj && h->small_path && n > K2_WARP_PATH_MAX && (h->gru_mode == 0 || h->gru_mode == 2 || h->gru_mode == 7 || h->gru_mode == 9 || h->gru_mode == 10 || h->gru_mode == 11);
-}
-
-// Recompute the projection of every ring row once (all streams), then the cache is maintained incrementally.
-static int rebuild_projections_if_dirty(pb_handle* h, cudaStream_t s) {
-    if (!h->proj_dirty) return PB_OK;
-    ProfScope ps(h, 3, s);
-    const long long rows = (long long)h->cfg.max_streams * h->ring_rows;
-    const int grid = (int)std::min<long long>((rows + PROJ_FRAMES_PER_CTA - 1) / PROJ_FRAMES_PER_CTA, (long long)h->sm_count * 16);
-    input_proj_all_kernel<13><<<grid, 64 * PROJ_FRAMES_PER_CTA, 0, s>>>(h->d_proj_w, h->d_proj_b, rows, h->st.ring, h->ring_rows, h->row_stride, h->d_proj_ring,
-                                                                       (h->cfg.max_streams + 15) / 16);
-    CK(cudaGetLastError());
-    h->proj_dirty = false;
-    return PB_OK;
+// Where a stream tick's network kernels read the window of item i: stream d_ids[i] (i when d_ids is null) of the handle's ring.
+static K2In stream_k2in(const pb_handle* h, const int32_t* d_ids) {
+    K2In in{};
+    in.ring = h->st.ring; in.n_samples = h->st.n_samples; in.ids = d_ids;
+    in.ring_rows = h->ring_rows; in.row_stride = h->row_stride; in.window = h->rel_window; in.hop = h->cfg.hop_samples;
+    in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
+    return in;
 }
 
 PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
@@ -1087,41 +1029,11 @@ PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, i
     if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    // Default network, large batch: the tensor-core scan reads cached input projections.  A stale cache (weights changed,
-    // or ticks that skipped the projection) is rebuilt for every existing row BEFORE this tick's MFCC kernel runs -- the
-    // host-buffer path calls this up front on its first pipe, see pb_update_host -- and the rows the tick adds are projected
-    // right after it, so the rebuild never reads or writes a row that another sub-batch of the same tick is producing.
-    const bool want_proj = wants_projection(h, n);
-    if (want_proj) { rc = rebuild_projections_if_dirty(h, s); if (rc != PB_OK) return rc; }
     rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
-    // The default scan (gru_mma16_kernel, gru_mode 0) projects the frames a tick has added itself, in its prologue; the separate
-    // projection kernel serves the other scans (A/B modes) and short sub-batches of a large host tick (second case below), whose
-    // warp-per-stream kernel does not touch the cache.
-    const bool scan_projects = want_proj && (h->gru_mode == 0 || h->gru_mode == 11);
-    if ((want_proj && !scan_projects) || (!want_proj && h->host_tick_proj && !h->proj_dirty)) {
-        ProfScope ps(h, 3, s);
-        const long long items = (long long)n * h->max_new;
-        const int grid = (int)((items + PROJ_THREADS - 1) / PROJ_THREADS);     // 32 frames per warp
-        input_proj_kernel<13><<<grid, PROJ_THREADS, 0, s>>>(h->d_bfrag, h->d_proj_b, h->st.n_samples, d_ids, (int)n,
-            h->cfg.chunk_samples, h->used, h->cfg.hop_samples, h->max_new, h->st.ring, h->ring_rows, h->row_stride, h->d_proj_ring,
-            (h->cfg.max_streams + 15) / 16);
-        CK(cudaGetLastError());
-    } else if (!scan_projects && h->has_proj && h->small_path) {
-        h->proj_dirty = true;                                  // this tick's frames get no projection
-    }
-    const bool use_proj = want_proj;
-    K2In in{};
-    in.ring = h->st.ring; in.n_samples = h->st.n_samples; in.ids = d_ids;
-    in.ring_rows = h->ring_rows; in.row_stride = h->row_stride; in.window = h->rel_window; in.hop = h->cfg.hop_samples;
-    in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
     K2Out o{};
-    in.proj = use_proj ? h->d_proj_ring : nullptr;
-    in.proj_tiles = (h->cfg.max_streams + 15) / 16;
-    in.used = h->used;
-    in.chunk = h->cfg.chunk_samples;
     o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = h->st.trig;
-    return launch_gru(h, in, true, n, decode_params(h), o, s);
+    return launch_gru(h, stream_k2in(h, d_ids), true, n, decode_params(h), o, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1172,26 +1084,16 @@ PB_API int pb_num_models(const pb_handle* h) {
     return 1 + (int)h->bank.size();
 }
 
-template <int NM>
-static int launch_bank_nm(pb_handle* h, const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
-    const size_t smem = (size_t)NM * BANK_MODEL_SMEM;
-    CK(ensure_dyn_smem(gru_bank_kernel<NM>, smem));
-    const int per_cta = (MMA_THREADS / 32) * 16;
-    gru_bank_kernel<NM><<<(int)((n + per_cta - 1) / per_cta), MMA_THREADS, smem, s>>>(P, in, n);
-    CK(cudaGetLastError());
-    return PB_OK;
-}
-
-static int launch_bank(pb_handle* h, const BankParams& P, int nm, const K2In& in, int64_t n, cudaStream_t s) {
+static int launch_bank(const BankParams& P, int nm, const K2In& in, int64_t n, cudaStream_t s) {
     switch (nm) {
-        case 1: return launch_bank_nm<1>(h, P, in, n, s);
-        case 2: return launch_bank_nm<2>(h, P, in, n, s);
-        case 3: return launch_bank_nm<3>(h, P, in, n, s);
-        case 4: return launch_bank_nm<4>(h, P, in, n, s);
-        case 5: return launch_bank_nm<5>(h, P, in, n, s);
-        case 6: return launch_bank_nm<6>(h, P, in, n, s);
-        case 7: return launch_bank_nm<7>(h, P, in, n, s);
-        case 8: return launch_bank_nm<8>(h, P, in, n, s);
+        case 1: return launch_bank_nm<1, true>(P, in, n, s);
+        case 2: return launch_bank_nm<2, true>(P, in, n, s);
+        case 3: return launch_bank_nm<3, true>(P, in, n, s);
+        case 4: return launch_bank_nm<4, true>(P, in, n, s);
+        case 5: return launch_bank_nm<5, true>(P, in, n, s);
+        case 6: return launch_bank_nm<6, true>(P, in, n, s);
+        case 7: return launch_bank_nm<7, true>(P, in, n, s);
+        case 8: return launch_bank_nm<8, true>(P, in, n, s);
     }
     return fail(PB_ERR_INVALID, "%d fused models", nm);
 }
@@ -1208,15 +1110,7 @@ PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d
     const int M = 1 + (int)h->bank.size();
     rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
-    h->proj_dirty = true;                                      // this tick's frames get no cached projection: pb_update rebuilds it
-    K2In in{};
-    in.ring = h->st.ring; in.n_samples = h->st.n_samples; in.ids = d_ids;
-    in.ring_rows = h->ring_rows; in.row_stride = h->row_stride; in.window = h->rel_window; in.hop = h->cfg.hop_samples;
-    in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
-    in.proj = nullptr;
-    in.proj_tiles = (h->cfg.max_streams + 15) / 16;
-    in.used = h->used;
-    in.chunk = h->cfg.chunk_samples;
+    const K2In in = stream_k2in(h, d_ids);
     ProfScope ps(h, 1, s);
     // the fused family in one gru_bank_kernel launch; other networks one launch each of their own kernel, on the same ring
     BankParams P{};
@@ -1230,18 +1124,13 @@ PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d
         o.count = d_count ? d_count + m : nullptr;
         o.trig = hm->st.trig;
         if (bank_fused(hm)) {
-            BankModelW& w = P.w[nm];
-            w.bfrag = hm->d_bfrag16; w.xfrag = hm->d_xfrag16; w.bias = hm->d_mma_bias; w.wd = hm->d_mma_wd; w.bd = hm->bd;
-            w.act = hm->cfg.activation; w.ract = hm->cfg.recurrent_activation;
-            P.dp[nm] = decode_params(hm);
-            P.o[nm] = o;
-            ++nm;
+            set_bank_slot(P, nm++, hm, decode_params(hm), o);
         } else {
             rc = launch_gru_kernels(hm, in, true, n, decode_params(hm), o, s);
             if (rc != PB_OK) return rc;
         }
     }
-    return nm ? launch_bank(h, P, nm, in, n, s) : PB_OK;
+    return nm ? launch_bank(P, nm, in, n, s) : PB_OK;
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {
@@ -1267,10 +1156,7 @@ PB_API int pb_read_window(pb_handle* h, const int32_t* d_ids, int64_t n, float* 
     if (n == 0) return PB_OK;
     if (!d_out) return fail(PB_ERR_INVALID, "null buffer");
     CK(cudaSetDevice(h->cfg.device));
-    K2In in{};
-    in.ring = h->st.ring; in.n_samples = h->st.n_samples; in.ids = d_ids;
-    in.ring_rows = h->ring_rows; in.row_stride = h->row_stride; in.window = h->rel_window; in.hop = h->cfg.hop_samples;
-    in.T = h->cfg.n_features; in.F_base = h->n_out;
+    const K2In in = stream_k2in(h, d_ids);
     long long total = n * in.T * in.F_base;
     read_window_kernel<<<(int)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(in, d_ids, n, d_out);
     CK(cudaGetLastError());
@@ -1371,16 +1257,11 @@ PB_API int pb_update_host(pb_handle* h, const int16_t* h_pcm, const int32_t* h_i
     // the counter is zeroed on pipe 0; the other pipes wait for that, pipe 0 waits for them at the end,
     // so the whole tick costs one host synchronisation
     CK(cudaMemsetAsync(h->d_count, 0, sizeof(unsigned long long), h->pipe[0]));
-    // equal sub-batches (a short last one would drop below the size at which the tick uses the projection cache and
-    // invalidate it every tick); step <= sb, a multiple of 32 except when one sub-batch takes everything
+    // equal sub-batches: nothing overlaps the first sub-batch's upload (pipeline fill) or the last one's kernels and download
+    // (drain), and for a given number of sub-batches the largest one is smallest when all are equal (16 400 streams: 8 224 +
+    // 8 176 rather than 16 384 + 16); step <= sb, a multiple of 32 except when one sub-batch takes everything
     const int64_t n_sub = (n + sb - 1) / sb;
     const int64_t step = n_sub == 1 ? n : std::min(sb, ((n + n_sub - 1) / n_sub + 31) & ~(int64_t)31);
-    struct TickFlag { bool& f; ~TickFlag() { f = false; } } tick_flag{h->host_tick_proj};
-    if (wants_projection(h, std::min(step, n))) {
-        rc = rebuild_projections_if_dirty(h, h->pipe[0]);
-        if (rc != PB_OK) return rc;
-        h->host_tick_proj = true;
-    }
     const int used_pipes = (int)std::min<int64_t>(HOST_PIPE, (n + step - 1) / step);
     if (used_pipes > 1) {
         CK(cudaEventRecord(h->pipe_ev[0], h->pipe[0]));

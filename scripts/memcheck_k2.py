@@ -1,4 +1,4 @@
-"""Small run of the default large-batch tick (mfcc kernels + gru_mma16_kernel with staged and ragged warps) for compute-sanitizer."""
+"""Small run of the default large-batch tick (MFCC kernels + gru_bank_kernel, a partial last tile, shuffled ids) for compute-sanitizer."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch, mycroft_precise_b200 as m
@@ -10,7 +10,7 @@ ids = torch.from_numpy(rs.permutation(S)[:8500].astype(np.int32)).cuda()
 for k in range(5):
     pcm = torch.from_numpy((rs.randn(S, 1024) * 3000).astype(np.int16)).cuda()
     if k == 3:
-        sb.update(pcm[:8500], ids)          # shuffled ids: every warp takes the ragged (LDG) path
+        sb.update(pcm[:8500], ids)          # shuffled ids: a tile's 16 streams are scattered over the ring
     else:
         sb.update(pcm)
 torch.cuda.synchronize()

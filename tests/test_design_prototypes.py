@@ -84,35 +84,3 @@ def test_tensor_core_tick_state_machine_claims():
             tail, ts_tail, n0 = ch[ts1 - n0:], ts1, n1
         assert produced == _frames_ready(n0, used, hop)
 
-
-def test_projection_cache_layout_is_a_bijection_and_coalesces():
-    """proj_off (csrc/gru_kernels.cuh): position of accumulator columns (2t, 2t + 1) of n-tile nt for row r16 inside a 960-float block
-    of the projection cache.  Restated here: the 60 stored values x 16 rows fill the block exactly once, a warp's LDG.64 for one
-    (n-tile, row half) is one contiguous 256-byte (full n-tile) or 128-byte (half n-tile) run, and the column read by the scan is the
-    (gate, unit) the projection kernels write."""
-    def proj_off(nt, r16, t):
-        return ((nt // 3) * 2 + nt % 3) * 128 + r16 * 8 + 2 * t if nt % 3 != 2 else 768 + (nt // 3) * 64 + r16 * 4 + 2 * t
-    seen = {}
-    for nt in range(9):
-        for r16 in range(16):
-            for t in range(4):
-                if nt % 3 == 2 and t >= 2:
-                    continue                      # units 20..23 of a gate do not exist
-                for j in range(2):
-                    gate, unit = nt // 3, 8 * (nt % 3) + 2 * t + j
-                    assert unit < 20
-                    off = proj_off(nt, r16, t) + j
-                    assert off not in seen
-                    seen[off] = (r16, gate, unit)
-    assert sorted(seen) == list(range(960))
-    for nt in range(9):
-        for hf in range(2):
-            lanes = [(g, t) for g in range(8) for t in range(4) if not (nt % 3 == 2 and t >= 2)]
-            offs = sorted(proj_off(nt, g + 8 * hf, t) for g, t in lanes)
-            assert offs == list(range(offs[0], offs[0] + 2 * len(lanes), 2))        # consecutive float2: one contiguous run
-            assert offs[0] * 4 % 128 == 0                                           # starting on a line boundary
-    # input_proj_all_kernel's inverse map: stored column c = 20 gate + unit
-    for c in range(60):
-        gate, unit = c // 20, c % 20
-        nt, t, j = 3 * gate + unit // 8, (unit & 7) >> 1, unit & 1
-        assert seen[proj_off(nt, 5, t) + j] == (5, gate, unit)

@@ -143,7 +143,7 @@ def test_bank_vs_independent_handles_large():
 
 @gpu
 def test_bank_mixed_with_single_model_api():
-    """update (cached-projection scan, > 8192 streams) and update_models alternate on one handle, with a slot-0 weight reload,
+    """update (tensor-core scan, > 8192 streams) and update_models alternate on one handle, with a slot-0 weight reload,
     a clear of some streams, an ids-permuted tick and a one-stream tick; independent handles driven through the same
     sequence give the same results (the second model's handle only advances its MFCC state on update ticks)."""
     import torch

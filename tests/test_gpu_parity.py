@@ -196,7 +196,7 @@ def test_predict_small_path(core, scale):
 
 @pytest.mark.parametrize('mode', [0, 1, 2])
 def test_default_network_kernel_variants(core, mode):
-    """warp-per-stream (auto, small n), thread-per-stream CUDA-core (1) and tensor-core mma.sync 3xTF32 (2) kernels."""
+    """warp-per-stream (auto, small n), thread-per-stream CUDA-core (1) and tensor-core mma.sync fp16 x 3 (2) kernels."""
     w = og.GruWeights.random(13, 20, seed=11, scale=0.1)
     core.load_weights(w.kernel, w.recurrent, w.bias, w.dense_w, w.dense_b)
     core.gru_mode(mode)
@@ -237,9 +237,10 @@ def test_stream_tick_kernel_variants_agree():
     assert all(abs(o[2] - outs[0][2]) <= 3 for o in outs[1:])
 
 
-def test_cached_projection_path_large_batch():
-    """n > 8192 streams: tensor-core scan reading cached input projections (input_proj_kernel) vs the CUDA-core kernel,
-    including a weight reload and a small-batch tick in between (both invalidate the cache)."""
+def test_large_batch_tensor_core_scan():
+    """n > 8192 streams: the tensor-core scan (gru_bank_kernel with one model) vs the CUDA-core kernel, including a weight
+    reload and a small-batch tick in between.  A one-model update_models arm goes through the same sequence and must score
+    bit for bit like update's scan: a window's score does not depend on the ticks before it."""
     m = _mod()
     S, K, chunk = 9000, 36, 1024
     pcm = noise(64, K * chunk, seed=33)
@@ -247,35 +248,38 @@ def test_cached_projection_path_large_batch():
     pcm[::7] = np.roll(pcm[::7], 123, axis=1)
     model = m.GruModel.random(13, 20, seed=8, scale=0.1)
     model.dense_b = 3.0
-    res = []
-    # 0: default scan over cached projections (fp16x3 recurrent products, bulk-copy staged blocks); 10: 3xTF32 products, staged,
-    # 16-stream warp tiles; 9: the same without staging; 7: 3xTF32 with 32-stream tiles; 1: CUDA cores
-    for mode in (0, 10, 9, 7, 1):
+
+    def run(mode):
+        """mode 0 (automatic) / 1 (CUDA cores) through update, or 'bank' through update_models: raw [K][S], detections."""
         sb = m.StreamBatch(model, S, chunk_samples=chunk)
-        sb.core.gru_mode(mode)
+        if mode == 'bank':
+            tick = lambda c, ids=None: sb.update_models(c, ids)['raw'][0]
+        else:
+            sb.core.gru_mode(mode)
+            tick = lambda c, ids=None: sb.update(c, ids)['raw']
         raws = []
         for k in range(K):
             if k == 20:                                              # reload weights mid-stream
                 sb.core.load_weights(model.kernel, model.recurrent, model.bias, model.dense_w, model.dense_b)
-            if k == 25:                                              # a small tick for a few streams (warp-per-stream kernel)
-                ids = torch.arange(5, dtype=torch.int32, device='cuda')
-                o = sb.update(cuda(pcm[:5, k * chunk:(k + 1) * chunk]), ids)
-                r5 = o['raw'].cpu().numpy().copy()
-                o2 = sb.update(cuda(pcm[5:, k * chunk:(k + 1) * chunk]), torch.arange(5, S, dtype=torch.int32, device='cuda'))
-                raws.append(np.concatenate([r5, o2['raw'].cpu().numpy()]))
+            if k == 25:                                              # a small tick for a few streams (warp-per-stream kernel in update)
+                r5 = tick(cuda(pcm[:5, k * chunk:(k + 1) * chunk]), torch.arange(5, dtype=torch.int32, device='cuda')).cpu().numpy()
+                r = tick(cuda(pcm[5:, k * chunk:(k + 1) * chunk]), torch.arange(5, S, dtype=torch.int32, device='cuda')).cpu().numpy()
+                raws.append(np.concatenate([r5, r]))
                 continue
-            o = sb.update(cuda(pcm[:, k * chunk:(k + 1) * chunk]))
-            raws.append(o['raw'].cpu().numpy().copy())
-        res.append((np.array(raws), int(sb.count.item())))
+            raws.append(tick(cuda(pcm[:, k * chunk:(k + 1) * chunk])).cpu().numpy())
+        count = int(sb.counts[0].item()) if mode == 'bank' else int(sb.count.item())
         sb.core.close()
-    for r, c in res[:-1]:
-        assert np.max(np.abs(r - res[-1][0])) < 1e-5
-        assert c > 0 and abs(c - res[-1][1]) <= 3
-    for i, j in ((1, 2), (1, 3)):                                    # the 3xTF32 variants: same arithmetic per stream, different tiling / staging ...
-        a, b = res[i][0].copy(), res[j][0].copy()
-        a[25, :5] = b[25, :5] = 0                                    # ... except the 5-stream tick (warp-per-stream kernel vs forced MMA)
-        assert np.array_equal(a, b), (i, j)
-    print('max |raw - CUDA-core kernel|: fp16x3 %.3g, 3xTF32 %.3g' % (np.max(np.abs(res[0][0] - res[-1][0])), np.max(np.abs(res[1][0] - res[-1][0]))))
+        return np.array(raws), count
+
+    ref = run(1)
+    res = [run(0), run('bank')]
+    for r, c in res:
+        assert np.max(np.abs(r - ref[0])) < 1e-5
+        assert c > 0 and abs(c - ref[1]) <= 3
+    a, b = res[0][0].copy(), res[1][0].copy()
+    a[25, :5] = b[25, :5] = 0                                        # the 5-stream tick: warp-per-stream kernel in update only
+    assert np.array_equal(a, b)
+    print('max |raw - CUDA-core kernel|: %.3g' % np.max(np.abs(res[0][0] - ref[0])))
 
 
 def _generic_case(pr_kw, H, act='linear', ract='hard_sigmoid', N=200, seed=5, mode=0):
@@ -459,9 +463,9 @@ def test_stream_host_path_equals_device_path():
         assert a[4] == b[4] and a[4] > 0
 
 
-def test_host_path_sub_batches_keep_projection_cache():
-    """pb_update_host on 16 400 streams = two pipelined sub-batches (8 224 + 8 176: the second is below the size at which a
-    tick uses the cached input projections) with a weight reload in between: must equal the single-launch device path."""
+def test_host_path_sub_batches_equal_device_path():
+    """pb_update_host on 16 400 streams = two pipelined sub-batches (8 224 + 8 176: the first runs the tensor-core scan, the
+    second the warp-per-stream kernel) with a weight reload in between: must equal the single-launch device path."""
     m = _mod()
     S, K, chunk = 16400, 32, 1024
     pcm = noise(64, K * chunk, seed=41)
@@ -647,6 +651,18 @@ def test_speechpy_vectorizer(kw):
     w = og.GruWeights(model.kernel, model.recurrent, model.bias, model.dense_w, model.dense_b)
     oraw, oconf, ofired = run_streams(w, pcm, chunk, pr=opr, sensitivity=0.8, trigger_level=1)
     assert np.max(np.abs(raw - oraw)) < 1e-4 and np.array_equal(fired, ofired)
+
+
+def test_gru_mode_accepts_only_existing_kernels(core):
+    """pb_debug_gru_mode: 0 (automatic), 1 (CUDA cores) and 2 (tensor cores) select a kernel; any other mode is refused."""
+    try:
+        for mode in (0, 1, 2):
+            core.gru_mode(mode)
+        for mode in (-1, 3, 7, 9, 10, 11):
+            with pytest.raises(ValueError, match='gru mode'):
+                core.gru_mode(mode)
+    finally:
+        core.gru_mode(0)
 
 
 def test_unsupported_and_errors():
