@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <map>
 #include <cuda_fp16.h>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <utility>
@@ -61,8 +62,74 @@ struct ProfSlot {
     uint64_t launches = 0;
 };
 
+// Device memory of `n` elements of T, freed when the owner goes away.  cudaFree acts on the current device, so every entry
+// point that can destroy or replace one (pb_create on failure, pb_destroy, pb_load_weights, pb_add_model) sets the handle's
+// device first.
+template <typename T>
+class DevArray {
+public:
+    DevArray() = default;
+    DevArray(DevArray&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+    DevArray& operator=(DevArray&& o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }
+    DevArray(const DevArray&) = delete;
+    DevArray& operator=(const DevArray&) = delete;
+    ~DevArray() { if (p_) cudaFree(p_); }
+
+    // Uninitialised memory.  alloc and upload replace (and free) what the array held only when they succeed.
+    cudaError_t alloc(size_t n) {
+        T* p = nullptr;
+        const cudaError_t e = cudaMalloc((void**)&p, std::max<size_t>(n, 1) * sizeof(T));
+        if (e != cudaSuccess) return e;
+        DevArray fresh;
+        fresh.p_ = p; fresh.n_ = n;
+        *this = std::move(fresh);
+        return cudaSuccess;
+    }
+    cudaError_t upload(const std::vector<T>& v) {
+        DevArray fresh;
+        cudaError_t e = fresh.alloc(v.size());
+        if (e == cudaSuccess && !v.empty()) e = cudaMemcpy(fresh.p_, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) *this = std::move(fresh);
+        return e;
+    }
+    T* get() const { return p_; }
+    size_t size() const { return n_; }
+
+private:
+    T* p_ = nullptr;
+    size_t n_ = 0;
+};
+
+// One network's weights in every layout a kernel reads (load_weights builds them all at once; they never change after).
+struct NetWeights {
+    bool small_path = false;         // the default network (H = 20, F = 13, linear / hard_sigmoid): gru_warp / gru_small / gru_bank<1>
+    GruSmallW<20, 13> w_small;       // ... its weights as a kernel parameter
+    DevArray<float> wcat, bias, wd;  // gru_tiled_kernel: [W; U], bias, dense weights (gru_wide_kernel reads wd as well)
+    float bd = 0.f;
+    DevArray<uint4> bfrag16;         // fused family (gru_bank_kernel): recurrent weights as fp16 hi / lo fragments
+    DevArray<uint4> xfrag16;         // ... and the input weights
+    DevArray<float> mma_bias, mma_wd;
+    bool wide_ok = false;            // gru_wide_kernel covers the network (H <= 128, F <= 40)
+    int wg_fp = 0, wg_hp = 0;
+    DevArray<uint4> wg_b1, wg_b2; DevArray<float> wg_bias;
+};
+
+// One model of a handle's bank: its network, ThresholdDecoder table, TriggerDetector state and weights.  It reads the
+// handle's MFCC ring; the front-end fields of its cfg equal the handle's.
+struct Network {
+    pb_config cfg;                   // network (hidden, activations), decoder and trigger fields
+    std::vector<double> cd;          // decoder table (build_cdf, or pb_set_cdf / pb_add_model's cd)
+    int min_out = 0, max_out = 0;
+    DevArray<double> d_cd;
+    DevArray<int> trig;              // [max_streams] TriggerDetector.activation
+    int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core kernel, 2 = force tensor-core kernel (pb_debug_gru_mode, slot 0)
+    std::unique_ptr<NetWeights> w;   // null until weights are loaded
+};
+
+// A handle: the MFCC front end (tables, per-stream sample count, tail and ring), the host pipeline and the profiler, shared
+// by the models[] it scores.  models[0] is the handle's own network (pb_load_weights), 1.. come from pb_add_model.
 struct pb_handle {
-    pb_config cfg;
+    pb_config cfg;                   // the front end; its network fields are models[0]'s
     int sm_count = 132;
     // derived
     int used = 0, n_bins = 0, n_out = 0, feat = 0, ring_rows = 0, row_stride = 0, tail_cap = 0, max_new = 0;
@@ -71,65 +138,67 @@ struct pb_handle {
     bool force_generic = false;      // tests: exercise the generic kernels on the aligned geometry
     int k1_mode = 0;                 // 0 = default (the FFT kernel with 32-bit set-up where the geometry allows it), 2 = always the FFT kernel, 3 = FFT kernel with the original 64-bit set-up, 4 / 5 / 6 = the mma.sync DFT tick (mfcc_mma.cuh): stage 1 on the CUDA cores / on the tensor cores / the latter with a shuffle epilogue
     bool mma_ok = false;             // geometry mfcc_mma_kernel covers (n_fft = frame = 512, hop >= 512, chunk >= hop, MFCC vectorizer)
-    uint2 *d_mm_b1 = nullptr, *d_mm_b2 = nullptr; float2* d_mm_tw = nullptr;
-    MmRec* d_mm_recs = nullptr; unsigned int* d_mm_counters = nullptr;
+    DevArray<uint2> d_mm_b1, d_mm_b2; DevArray<float2> d_mm_tw;
+    DevArray<MmRec> d_mm_recs; DevArray<unsigned int> d_mm_counters;
     int mm_parity = 0;               // which of the two frame counters the next tick's plan kernel fills
-    std::vector<float> h_wrise, h_wfall; std::vector<int> h_grid;      // mel tables of the CPU model of the matrix-product DFT (pb_debug_tc*_mfcc_frame)
     bool fast_ok = false;            // aligned geometry: warp-autonomous kernels (mfcc_fast.cuh)
     int npl = 0, maxc = 0, nol = 0;
-    float4* d_ptab = nullptr;
-    unsigned char* d_ctab = nullptr;
-    float* d_dct_t = nullptr;
-    // host copies of tables
-    std::vector<double> fb;        // [n_filt][n_bins]
-    std::vector<double> cd;
-    int min_out = 0, max_out = 0;
+    DevArray<float4> d_ptab;
+    DevArray<unsigned char> d_ctab;
+    DevArray<float> d_dct_t;
+    std::vector<double> fb;          // [n_filt][n_bins] (pb_get_filterbank)
     // device tables
-    float *d_wrise = nullptr, *d_wfall = nullptr, *d_dct = nullptr;
-    int* d_grid = nullptr;
-    float2 *d_tw_stage = nullptr, *d_tw_post = nullptr, *d_tw_any = nullptr;
-    double* d_cd = nullptr;
-    // state
-    StreamState st{};
-    // weights
-    bool have_weights = false;
-    bool small_path = false;
-    GruSmallW<20, 13> w_small;
-    float *d_wcat = nullptr, *d_bias = nullptr, *d_wd = nullptr;
-    uint4* d_bfrag16 = nullptr;      // fused family (gru_bank_kernel): recurrent weights as fp16 hi / lo fragments
-    uint4* d_xfrag16 = nullptr;      // ... and the input weights
-    float *d_mma_bias = nullptr, *d_mma_wd = nullptr;
-    bool wide_ok = false;            // gru_wide_kernel covers the network (H <= 128, F <= 40)
-    int wg_fp = 0, wg_hp = 0;
-    uint4 *d_wg_b1 = nullptr, *d_wg_b2 = nullptr; float* d_wg_bias = nullptr;
-    int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core kernel, 2 = force tensor-core kernel
-    float bd = 0.f;
+    DevArray<float> d_wrise, d_wfall, d_dct;
+    DevArray<int> d_grid;
+    DevArray<float2> d_tw_stage, d_tw_post, d_tw_any;
+    // per-stream state (stream_state)
+    DevArray<long long> d_n_samples;
+    DevArray<int16_t> d_tail;
+    DevArray<float> d_ring;
+    std::vector<Network> models;
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
     cudaEvent_t pipe_ev[HOST_PIPE] = {nullptr, nullptr, nullptr};
-    int16_t* d_stage_pcm[HOST_PIPE] = {nullptr, nullptr, nullptr};
-    int* d_stage_ids[HOST_PIPE] = {nullptr, nullptr, nullptr};
-    float* d_stage_raw[HOST_PIPE] = {nullptr, nullptr, nullptr};
-    double* d_stage_conf[HOST_PIPE] = {nullptr, nullptr, nullptr};
-    uint8_t* d_stage_fired[HOST_PIPE] = {nullptr, nullptr, nullptr};
-    unsigned long long* d_count = nullptr;
+    DevArray<int16_t> d_stage_pcm[HOST_PIPE];
+    DevArray<int> d_stage_ids[HOST_PIPE];
+    DevArray<float> d_stage_raw[HOST_PIPE];
+    DevArray<double> d_stage_conf[HOST_PIPE];
+    DevArray<uint8_t> d_stage_fired[HOST_PIPE];
+    DevArray<unsigned long long> d_count;
     unsigned long long* h_count_pinned = nullptr;
-    // model bank: slots 1..M-1 (pb_add_model).  Each is a handle without stream state of its own: network, decoder table and
-    // trigger settings, and a [max_streams] trigger array in st.trig; it reads this handle's ring.
-    std::vector<pb_handle*> bank;
     // profiling
     bool profiling = false;
     ProfSlot prof[N_PROFILE_SLOTS];
+
+    pb_handle() = default;
+    pb_handle(const pb_handle&) = delete;
+    pb_handle& operator=(const pb_handle&) = delete;
+    ~pb_handle() {
+        if (h_count_pinned) cudaFreeHost(h_count_pinned);
+        for (int i = 0; i < HOST_PIPE; ++i) {
+            if (pipe[i]) cudaStreamDestroy(pipe[i]);
+            if (pipe_ev[i]) cudaEventDestroy(pipe_ev[i]);
+        }
+        for (auto& p : prof)
+            for (auto e : p.ev) cudaEventDestroy(e);
+    }
 };
 
 // ------------------------------------------------------------------------------------------------
 // table construction (host, float64), restating sonopy.filterbanks as the reference calls it
 // (precise/vectorization.py:36-39): grid up to sample_rate, int() truncation, duplicate bins pushed
 // forward, np.linspace(endpoint=False) edge weights.
-static int build_mel(pb_handle* h, std::vector<float>& wrise, std::vector<float>& wfall, std::vector<int>& grid) {
-    const pb_config& c = h->cfg;
-    const int nb = h->n_bins, nf = c.n_filt;
+struct MelHost {
+    std::vector<int> grid;            // [n_filt + 2] corner bins
+    std::vector<float> wrise, wfall;  // [n_bins] weight of a bin on the rising / falling edge of its triangle
+    std::vector<double> fb;           // [n_filt][n_bins]
+};
+
+static int build_mel(const pb_config& c, int n_bins, MelHost& mel) {
+    const int nb = n_bins, nf = c.n_filt;
     const double top = 1127.0 * log(1.0 + (double)c.sample_rate / 700.0);
+    std::vector<int>& grid = mel.grid;
+    std::vector<double>& fb = mel.fb;
     grid.assign(nf + 2, 0);
     long long shift = 0, prev = -1;
     if (c.vectorizer == PB_VEC_SPEECHPY_MFCCS) {
@@ -155,22 +224,22 @@ static int build_mel(pb_handle* h, std::vector<float>& wrise, std::vector<float>
     }
     if (grid[nf + 1] > nb)
         return fail(PB_ERR_INVALID, "mel grid exceeds the spectrum (%d > %d bins): the reference's sonopy.filterbanks raises here", grid[nf + 1], nb);
-    h->fb.assign((size_t)nf * nb, 0.0);
-    wrise.assign(nb, 0.f);
-    wfall.assign(nb, 0.f);
+    fb.assign((size_t)nf * nb, 0.0);
+    mel.wrise.assign(nb, 0.f);
+    mel.wfall.assign(nb, 0.f);
     for (int i = 0; i < nf; ++i) {
         int lo = grid[i], mid = grid[i + 1], hi = grid[i + 2];
-        for (int k = lo; k < mid; ++k) h->fb[(size_t)i * nb + k] = (double)(k - lo) * (1.0 / (double)(mid - lo));
-        for (int k = mid; k < hi; ++k) h->fb[(size_t)i * nb + k] = (double)(k - mid) * (-1.0 / (double)(hi - mid)) + 1.0;
-        for (int k = lo; k < mid; ++k) wrise[k] = (float)h->fb[(size_t)i * nb + k];
-        for (int k = mid; k < hi; ++k) wfall[k] = (float)h->fb[(size_t)i * nb + k];
+        for (int k = lo; k < mid; ++k) fb[(size_t)i * nb + k] = (double)(k - lo) * (1.0 / (double)(mid - lo));
+        for (int k = mid; k < hi; ++k) fb[(size_t)i * nb + k] = (double)(k - mid) * (-1.0 / (double)(hi - mid)) + 1.0;
+        for (int k = lo; k < mid; ++k) mel.wrise[k] = (float)fb[(size_t)i * nb + k];
+        for (int k = mid; k < hi; ++k) mel.wfall[k] = (float)fb[(size_t)i * nb + k];
     }
     return PB_OK;
 }
 
-static void build_cdf(pb_handle* h) {
+static void build_cdf(Network& net) {
     // precise/threshold_decoder.py:38-43, :68-70 and functions.pdf (:104-108)
-    const pb_config& c = h->cfg;
+    const pb_config& c = net.cfg;
     const int resolution = 200;
     double lo = 0, hi = 0;
     for (int i = 0; i < c.n_thresholds; ++i) {
@@ -178,16 +247,16 @@ static void build_cdf(pb_handle* h) {
         if (i == 0 || a < lo) lo = a;
         if (i == 0 || b > hi) hi = b;
     }
-    h->min_out = (int)lo;
-    h->max_out = (int)hi;
-    const int range = h->max_out - h->min_out;
+    net.min_out = (int)lo;
+    net.max_out = (int)hi;
+    const int range = net.max_out - net.min_out;
     const int num = resolution * range;
-    h->cd.assign(std::max(num, 0), 0.0);
+    net.cd.assign(std::max(num, 0), 0.0);
     if (num <= 0) return;
-    const double step = num > 1 ? (double)(h->max_out - h->min_out) / (double)(num - 1) : 0.0;
+    const double step = num > 1 ? (double)(net.max_out - net.min_out) / (double)(num - 1) : 0.0;
     double run = 0.0;
     for (int j = 0; j < num; ++j) {
-        double x = (j == num - 1 && num > 1) ? (double)h->max_out : (double)j * step + (double)h->min_out;
+        double x = (j == num - 1 && num > 1) ? (double)net.max_out : (double)j * step + (double)net.min_out;
         double s = 0.0;
         for (int i = 0; i < c.n_thresholds; ++i) {
             double mu = c.threshold_mu[i], sd = c.threshold_std[i];
@@ -195,15 +264,24 @@ static void build_cdf(pb_handle* h) {
             s = (i == 0) ? p : s + p;
         }
         run += s / (double)(resolution * c.n_thresholds);
-        h->cd[j] = run;
+        net.cd[j] = run;
     }
 }
 
-template <typename T>
-static cudaError_t upload(T** dst, const std::vector<T>& v) {
-    cudaError_t e = cudaMalloc((void**)dst, std::max<size_t>(v.size(), 1) * sizeof(T));
-    if (e != cudaSuccess) return e;
-    if (!v.empty()) e = cudaMemcpy(*dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+// The network fields of a configuration (pb_create checks hidden earlier, with the other sizes).
+static int check_network(const pb_config& c) {
+    if (c.hidden < 1) return fail(PB_ERR_INVALID, "hidden must be positive");
+    if (c.n_thresholds < 1 || c.n_thresholds > PB_MAX_THRESHOLDS) return fail(PB_ERR_INVALID, "n_thresholds must be in [1, %d]", PB_MAX_THRESHOLDS);
+    if (c.activation < 0 || c.activation > 1 || c.recurrent_activation < 0 || c.recurrent_activation > 1)
+        return fail(PB_ERR_UNSUPPORTED, "unsupported GRU activation");
+    return PB_OK;
+}
+
+// A network's decoder table (net.cd as built or replaced) and zeroed trigger array on the current device.
+static cudaError_t upload_network_state(Network& net, size_t max_streams) {
+    cudaError_t e = net.d_cd.upload(net.cd);
+    if (e == cudaSuccess) e = net.trig.alloc(max_streams);
+    if (e == cudaSuccess) e = cudaMemset(net.trig.get(), 0, max_streams * sizeof(int));
     return e;
 }
 
@@ -264,23 +342,6 @@ PB_API int pb_config_default(pb_config* cfg) {
 PB_API void pb_destroy(pb_handle* h) {
     if (!h) return;
     cudaSetDevice(h->cfg.device);
-    cudaFree(h->d_wrise); cudaFree(h->d_wfall); cudaFree(h->d_dct); cudaFree(h->d_grid);
-    cudaFree(h->d_mm_b1); cudaFree(h->d_mm_b2); cudaFree(h->d_mm_tw); cudaFree(h->d_mm_recs); cudaFree(h->d_mm_counters);
-    cudaFree(h->d_wg_b1); cudaFree(h->d_wg_b2); cudaFree(h->d_wg_bias);
-    cudaFree(h->d_tw_stage); cudaFree(h->d_tw_post); cudaFree(h->d_tw_any); cudaFree(h->d_cd); cudaFree(h->d_ptab); cudaFree(h->d_ctab); cudaFree(h->d_dct_t);
-    cudaFree(h->st.n_samples); cudaFree(h->st.tail); cudaFree(h->st.ring); cudaFree(h->st.trig);
-    cudaFree(h->d_wcat); cudaFree(h->d_bias); cudaFree(h->d_wd); cudaFree(h->d_count);
-    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd);
-    if (h->h_count_pinned) cudaFreeHost(h->h_count_pinned);
-    for (int i = 0; i < HOST_PIPE; ++i) {
-        cudaFree(h->d_stage_pcm[i]); cudaFree(h->d_stage_ids[i]); cudaFree(h->d_stage_raw[i]);
-        cudaFree(h->d_stage_conf[i]); cudaFree(h->d_stage_fired[i]);
-        if (h->pipe[i]) cudaStreamDestroy(h->pipe[i]);
-        if (h->pipe_ev[i]) cudaEventDestroy(h->pipe_ev[i]);
-    }
-    for (auto& p : h->prof)
-        for (auto e : p.ev) cudaEventDestroy(e);
-    for (pb_handle* m : h->bank) pb_destroy(m);
     delete h;
 }
 
@@ -297,15 +358,14 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     if (!is_pow2(c.n_fft) || c.n_fft < 64 || c.n_fft > 1024)
         return fail(PB_ERR_UNSUPPORTED, "n_fft %d: powers of two in [64, 1024] are implemented (512 is the reference default)", c.n_fft);
     if (c.n_filt < 1 || c.n_filt > 64 || c.n_mfcc < 1 || c.n_mfcc > 64) return fail(PB_ERR_UNSUPPORTED, "n_filt and n_mfcc must be in [1, 64]");
-    if (c.n_thresholds < 1 || c.n_thresholds > PB_MAX_THRESHOLDS) return fail(PB_ERR_INVALID, "n_thresholds must be in [1, %d]", PB_MAX_THRESHOLDS);
-    if (c.activation < 0 || c.activation > 1 || c.recurrent_activation < 0 || c.recurrent_activation > 1)
-        return fail(PB_ERR_UNSUPPORTED, "unsupported GRU activation");
+    int rc = check_network(c);
+    if (rc != PB_OK) return rc;
     int ndev = 0;
     CK(cudaGetDeviceCount(&ndev));
     if (c.device < 0 || c.device >= ndev) return fail(PB_ERR_CUDA, "device %d not available (%d visible)", c.device, ndev);
     CK(cudaSetDevice(c.device));
 
-    pb_handle* h = new (std::nothrow) pb_handle();
+    std::unique_ptr<pb_handle> h(new (std::nothrow) pb_handle());      // deleted, with this device current, on every early return
     if (!h) return fail(PB_ERR_CUDA, "out of host memory");
     h->cfg = c;
     cudaDeviceProp prop;
@@ -324,10 +384,10 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     const size_t k1_big = c.n_fft > 512 ? k1_big_smem + 16 : 0;      // n_fft = 1024: power rows and FFT scratch in the dynamic tail
     h->k1_batch_smem = sizeof(K1Smem) + (size_t)h->n_out * c.n_filt * sizeof(float) + k1_big;
     h->k1_stream_smem = sizeof(K1StreamSmem) + (size_t)h->n_out * c.n_filt * sizeof(float) + k1_big;
-    std::vector<float> wrise, wfall;
-    std::vector<int> grid;
-    int rc = build_mel(h, wrise, wfall, grid);
-    if (rc != PB_OK) { delete h; return rc; }
+    MelHost mel;
+    rc = build_mel(c, h->n_bins, mel);
+    if (rc != PB_OK) return rc;
+    const std::vector<int>& grid = mel.grid;
     // piece schedule of the 16-lane mel stage (mfcc_fast.cuh): <= 8 bins each, never across a grid point
     std::vector<int> pieces, seg_first(c.n_filt + 2, 0);
     {
@@ -357,7 +417,7 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
                 float wr = 0.f, wf = 0.f;
                 if (pidx < n_pieces) {
                     const int start = pieces[pidx] & 0xffff, len = pieces[pidx] >> 16;
-                    if (e < len) { bin = start + e; wr = wrise[bin]; wf = wfall[bin]; }
+                    if (e < len) { bin = start + e; wr = mel.wrise[bin]; wf = mel.wfall[bin]; }
                 }
                 const int off = bin * 4;
                 float offf; memcpy(&offf, &off, 4);
@@ -398,55 +458,47 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
         double a = 2.0 * M_PI * (double)k / (double)c.n_fft;
         twa[k] = make_float2((float)cos(a), (float)-sin(a));
     }
-    build_cdf(h);
-
-#define CKH(call)                                                                                 \
-    do {                                                                                          \
-        cudaError_t e_ = (call);                                                                  \
-        if (e_ != cudaSuccess) {                                                                  \
-            pb_destroy(h);                                                                        \
-            return fail(PB_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_));             \
-        }                                                                                         \
-    } while (0)
-    CKH(upload(&h->d_wrise, wrise));
-    CKH(upload(&h->d_wfall, wfall));
-    CKH(upload(&h->d_grid, grid));
-    CKH(upload(&h->d_dct, dct));
-    CKH(upload(&h->d_tw_stage, tws));
-    CKH(upload(&h->d_tw_post, twp));
-    CKH(upload(&h->d_tw_any, twa));
-    CKH(upload(&h->d_cd, h->cd));
+    CK(h->d_wrise.upload(mel.wrise));
+    CK(h->d_wfall.upload(mel.wfall));
+    CK(h->d_grid.upload(grid));
+    h->fb = std::move(mel.fb);
+    CK(h->d_dct.upload(dct));
+    CK(h->d_tw_stage.upload(tws));
+    CK(h->d_tw_post.upload(twp));
+    CK(h->d_tw_any.upload(twa));
     {
         std::vector<float> dct_t((size_t)c.n_filt * 16 * h->nol, 0.f);
         for (int k = 0; k < h->n_out; ++k)
             for (int n = 0; n < c.n_filt; ++n) dct_t[(size_t)n * 16 * h->nol + k] = dct[(size_t)k * c.n_filt + n];
-        CKH(upload(&h->d_dct_t, dct_t));
+        CK(h->d_dct_t.upload(dct_t));
     }
-    CKH(upload(&h->d_ptab, ptab));
-    CKH(upload(&h->d_ctab, ctab));
+    CK(h->d_ptab.upload(ptab));
+    CK(h->d_ctab.upload(ctab));
     const size_t S = (size_t)c.max_streams;
-    h->st.tail_cap = h->tail_cap; h->st.ring_rows = h->ring_rows; h->st.row_stride = h->row_stride;
-    CKH(cudaMalloc((void**)&h->st.n_samples, S * sizeof(long long)));
-    CKH(cudaMalloc((void**)&h->st.tail, S * h->tail_cap * sizeof(int16_t)));
-    CKH(cudaMalloc((void**)&h->st.ring, S * h->ring_rows * h->row_stride * sizeof(float)));
-    CKH(cudaMalloc((void**)&h->st.trig, S * sizeof(int)));
-    CKH(cudaMemset(h->st.n_samples, 0, S * sizeof(long long)));
-    CKH(cudaMemset(h->st.tail, 0, S * h->tail_cap * sizeof(int16_t)));
-    CKH(cudaMemset(h->st.ring, 0, S * h->ring_rows * h->row_stride * sizeof(float)));
-    CKH(cudaMemset(h->st.trig, 0, S * sizeof(int)));
-    CKH(cudaMalloc((void**)&h->d_count, sizeof(unsigned long long)));
-    CKH(cudaMemset(h->d_count, 0, sizeof(unsigned long long)));
-    CKH(ensure_dyn_smem(mfcc_batch_kernel<int16_t, true>, (size_t)(h->k1_batch_smem)));
-    CKH(ensure_dyn_smem(mfcc_batch_kernel<int16_t, false>, (size_t)(h->k1_batch_smem)));
-    CKH(ensure_dyn_smem(mfcc_batch_kernel<float, true>, (size_t)(h->k1_batch_smem)));
-    CKH(ensure_dyn_smem(mfcc_batch_kernel<float, false>, (size_t)(h->k1_batch_smem)));
-    CKH(ensure_dyn_smem(mfcc_fast_batch_kernel, (size_t)(h->k1_fast_smem)));
-    CKH(ensure_dyn_smem(mfcc_fast_stream_kernel<false>, (size_t)(h->k1_fast_smem)));
-    CKH(ensure_dyn_smem(mfcc_fast_stream_kernel<true>, (size_t)(h->k1_fast_smem)));
-    CKH(ensure_dyn_smem(mfcc_stream_kernel<true>, (size_t)(h->k1_stream_smem)));
-    CKH(ensure_dyn_smem(mfcc_stream_kernel<false>, (size_t)(h->k1_stream_smem)));
-#undef CKH
-    *out = h;
+    CK(h->d_n_samples.alloc(S));
+    CK(h->d_tail.alloc(S * h->tail_cap));
+    CK(h->d_ring.alloc(S * h->ring_rows * h->row_stride));
+    CK(cudaMemset(h->d_n_samples.get(), 0, S * sizeof(long long)));
+    CK(cudaMemset(h->d_tail.get(), 0, S * h->tail_cap * sizeof(int16_t)));
+    CK(cudaMemset(h->d_ring.get(), 0, S * h->ring_rows * h->row_stride * sizeof(float)));
+    CK(h->d_count.alloc(1));
+    CK(cudaMemset(h->d_count.get(), 0, sizeof(unsigned long long)));
+    CK(ensure_dyn_smem(mfcc_batch_kernel<int16_t, true>, (size_t)(h->k1_batch_smem)));
+    CK(ensure_dyn_smem(mfcc_batch_kernel<int16_t, false>, (size_t)(h->k1_batch_smem)));
+    CK(ensure_dyn_smem(mfcc_batch_kernel<float, true>, (size_t)(h->k1_batch_smem)));
+    CK(ensure_dyn_smem(mfcc_batch_kernel<float, false>, (size_t)(h->k1_batch_smem)));
+    CK(ensure_dyn_smem(mfcc_fast_batch_kernel, (size_t)(h->k1_fast_smem)));
+    CK(ensure_dyn_smem(mfcc_fast_stream_kernel<false>, (size_t)(h->k1_fast_smem)));
+    CK(ensure_dyn_smem(mfcc_fast_stream_kernel<true>, (size_t)(h->k1_fast_smem)));
+    CK(ensure_dyn_smem(mfcc_stream_kernel<true>, (size_t)(h->k1_stream_smem)));
+    CK(ensure_dyn_smem(mfcc_stream_kernel<false>, (size_t)(h->k1_stream_smem)));
+
+    Network net;                     // slot 0: weights come with pb_load_weights
+    net.cfg = c;
+    build_cdf(net);
+    CK(upload_network_state(net, S));
+    h->models.push_back(std::move(net));
+    *out = h.release();
     return PB_OK;
 }
 
@@ -465,32 +517,34 @@ PB_API int pb_get_filterbank(const pb_handle* h, double* out) {
 
 PB_API int64_t pb_get_cdf(const pb_handle* h, double* out, int64_t capacity, int32_t* min_out, int32_t* max_out) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
-    if (min_out) *min_out = h->min_out;
-    if (max_out) *max_out = h->max_out;
-    if (out) memcpy(out, h->cd.data(), std::min<int64_t>(capacity, (int64_t)h->cd.size()) * sizeof(double));
-    return (int64_t)h->cd.size();
+    const Network& net = h->models[0];
+    if (min_out) *min_out = net.min_out;
+    if (max_out) *max_out = net.max_out;
+    if (out) memcpy(out, net.cd.data(), std::min<int64_t>(capacity, (int64_t)net.cd.size()) * sizeof(double));
+    return (int64_t)net.cd.size();
 }
 
 PB_API int pb_set_cdf(pb_handle* h, const double* cd, int64_t len) {
     if (!h || !cd) return fail(PB_ERR_INVALID, "null argument");
-    if (len != (int64_t)h->cd.size()) return fail(PB_ERR_INVALID, "cdf length %lld != %zu", (long long)len, h->cd.size());
+    Network& net = h->models[0];
+    if (len != (int64_t)net.cd.size()) return fail(PB_ERR_INVALID, "cdf length %lld != %zu", (long long)len, net.cd.size());
     CK(cudaSetDevice(h->cfg.device));
-    memcpy(h->cd.data(), cd, len * sizeof(double));
-    if (len) CK(cudaMemcpy(h->d_cd, cd, len * sizeof(double), cudaMemcpyHostToDevice));
+    memcpy(net.cd.data(), cd, len * sizeof(double));
+    if (len) CK(cudaMemcpy(net.d_cd.get(), cd, len * sizeof(double), cudaMemcpyHostToDevice));
     return PB_OK;
 }
 
-// Networks gru_bank_kernel scores: H <= 24, feature_size <= 16, no deltas.
-static bool bank_fused(const pb_handle* h) {
-    return h->cfg.hidden <= BANK_MAX_H && h->feat <= BANK_MAX_F && !h->cfg.use_delta;
+// Networks gru_bank_kernel scores: H <= 24, feature_size F <= 16, no deltas.
+static bool bank_fused(const Network& net, int F) {
+    return net.cfg.hidden <= BANK_MAX_H && F <= BANK_MAX_F && !net.cfg.use_delta;
 }
 
 // fp16 hi / lo weight fragments of the fused family (gru_bank_kernel).  Column (nt, g) -> gate nt / 3,
 // unit 8 (nt % 3) + g.  Recurrent weights: k-tile 0 = hidden units 0..15 as an m16n8k16 B fragment (b0: k = 2t, 2t + 1;
 // b1: k = 2t + 8, 2t + 9), k-tile 1 = units 16..23 as an m16n8k8 one (b0 only).  Input weights: features 0..15 as one k16
 // fragment.  Bias and dense weights padded to 24 units per gate.
-static int upload_frag16(pb_handle* h, const float* kernel, const float* recurrent, const float* bias, const float* dense_w) {
-    const int H = h->cfg.hidden, F = h->feat, H3 = 3 * H;
+static int upload_frag16(NetWeights& w, int H, int F, const float* kernel, const float* recurrent, const float* bias, const float* dense_w) {
+    const int H3 = 3 * H;
     auto h2 = [](float lo16, float hi16) {
         const __half a = __float2half_rn(lo16), b = __float2half_rn(hi16);
         uint16_t ua, ub; memcpy(&ua, &a, 2); memcpy(&ub, &b, 2);
@@ -528,12 +582,97 @@ static int upload_frag16(pb_handle* h, const float* kernel, const float* recurre
     for (int gate = 0; gate < 3; ++gate)
         for (int u = 0; u < H; ++u) mb[gate * 24 + u] = bias[gate * H + u];
     for (int u = 0; u < H; ++u) mw[u] = dense_w[u];
-    cudaFree(h->d_bfrag16); cudaFree(h->d_xfrag16); cudaFree(h->d_mma_bias); cudaFree(h->d_mma_wd);
-    h->d_bfrag16 = nullptr; h->d_xfrag16 = nullptr; h->d_mma_bias = h->d_mma_wd = nullptr;
-    CK(upload(&h->d_bfrag16, bf16));
-    CK(upload(&h->d_xfrag16, xf16));
-    CK(upload(&h->d_mma_bias, mb));
-    CK(upload(&h->d_mma_wd, mw));
+    CK(w.bfrag16.upload(bf16));
+    CK(w.xfrag16.upload(xf16));
+    CK(w.mma_bias.upload(mb));
+    CK(w.mma_wd.upload(mw));
+    return PB_OK;
+}
+
+// Fragment-ordered, TF32-split weights of gru_wide_kernel: k = 8 s + t (+ 4) is x feature k (k < FP) or hidden unit k - FP;
+// phase-1 column n = 8 nt + g is z unit n (n < HP) or r unit n - HP, phase-2 column n is candidate unit n.
+static int upload_wide(NetWeights& w, int H, int F, const float* kernel, const float* recurrent, const float* bias) {
+    const int H3 = 3 * H;
+    auto tf32 = [](float x) { uint32_t u; memcpy(&u, &x, 4); u = (u + 0x1000u) & 0xffffe000u; float r; memcpy(&r, &u, 4); return r; };
+    const int FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
+    w.wg_fp = FP; w.wg_hp = HP;
+    auto wv = [&](int k, int gate, int unit) -> float {
+        if (unit >= H) return 0.f;
+        if (k < FP) return k < F ? kernel[(size_t)k * H3 + gate * H + unit] : 0.f;
+        const int hu = k - FP;
+        return hu < H ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
+    };
+    auto frag = [&](int s, int lane, int gate, int unit) {
+        const int t = lane & 3;
+        const float v0 = wv(8 * s + t, gate, unit), v1 = wv(8 * s + t + 4, gate, unit);
+        const float h0 = tf32(v0), h1 = tf32(v1), l0 = tf32(v0 - h0), l1 = tf32(v1 - h1);
+        uint4 r; memcpy(&r.x, &h0, 4); memcpy(&r.y, &h1, 4); memcpy(&r.z, &l0, 4); memcpy(&r.w, &l1, 4);
+        return r;
+    };
+    std::vector<uint4> b1((size_t)KS * (HP / 4) * 32), b2((size_t)KS * (HP / 8) * 32);
+    for (int s = 0; s < KS; ++s)
+        for (int lane = 0; lane < 32; ++lane) {
+            for (int nt = 0; nt < HP / 4; ++nt) {
+                const int c = 8 * nt + (lane >> 2);
+                b1[((size_t)s * (HP / 4) + nt) * 32 + lane] = frag(s, lane, c < HP ? 0 : 1, c % HP);
+            }
+            for (int nt = 0; nt < HP / 8; ++nt) b2[((size_t)s * (HP / 8) + nt) * 32 + lane] = frag(s, lane, 2, 8 * nt + (lane >> 2));
+        }
+    std::vector<float> wb((size_t)3 * HP, 0.f);
+    for (int g3 = 0; g3 < 3; ++g3)
+        for (int u = 0; u < H; ++u) wb[(size_t)g3 * HP + u] = bias[g3 * H + u];
+    CK(w.wg_b1.upload(b1));
+    CK(w.wg_b2.upload(b2));
+    CK(w.wg_bias.upload(wb));
+    return PB_OK;
+}
+
+// [W; U] of gru_tiled_kernel, its bias and the dense weights.
+static int upload_tiled(NetWeights& w, int H, int F, const float* kernel, const float* recurrent, const float* bias, const float* dense_w) {
+    const int H3 = 3 * H;
+    std::vector<float> wcat((size_t)(F + H) * H3);
+    memcpy(wcat.data(), kernel, (size_t)F * H3 * sizeof(float));
+    memcpy(wcat.data() + (size_t)F * H3, recurrent, (size_t)H * H3 * sizeof(float));
+    CK(w.wcat.upload(wcat));
+    CK(w.bias.upload(std::vector<float>(bias, bias + H3)));
+    CK(w.wd.upload(std::vector<float>(dense_w, dense_w + H)));
+    return PB_OK;
+}
+
+// Builds every layout of net's new weights (F = the front end's feature size) and raises the kernels' shared-memory limits;
+// only when all of that succeeded do they replace net's weights.  On failure net keeps what it had, weights or none.
+// The current device is the handle's: the replaced weights are freed on it.
+static int load_weights(Network& net, int F, const float* kernel, const float* recurrent, const float* bias,
+                        const float* dense_w, float dense_b) {
+    const pb_config& c = net.cfg;
+    const int H = c.hidden;
+    const size_t tiled_smem = (size_t)(F + 3 * H) * K2_TILE_STREAMS * sizeof(float);
+    if (tiled_smem > 200 * 1024) return fail(PB_ERR_UNSUPPORTED, "feature_size + 3*hidden = %d is too large for the tiled GRU kernel", F + 3 * H);
+    std::unique_ptr<NetWeights> w(new (std::nothrow) NetWeights());
+    if (!w) return fail(PB_ERR_CUDA, "out of host memory");
+    w->bd = dense_b;
+    w->small_path = H == 20 && F == 13 && !c.use_delta && c.activation == PB_ACT_LINEAR && c.recurrent_activation == PB_RACT_HARD_SIGMOID;
+    if (w->small_path) {
+        memcpy(w->w_small.W, kernel, sizeof(w->w_small.W));
+        memcpy(w->w_small.U, recurrent, sizeof(w->w_small.U));
+        memcpy(w->w_small.b, bias, sizeof(w->w_small.b));
+        memcpy(w->w_small.wd, dense_w, sizeof(w->w_small.wd));
+        w->w_small.bd = dense_b;
+    }
+    w->wide_ok = !w->small_path && H <= WG_MAX_H && F <= WG_MAX_F;
+    int rc = upload_tiled(*w, H, F, kernel, recurrent, bias, dense_w);
+    if (rc == PB_OK && w->wide_ok) rc = upload_wide(*w, H, F, kernel, recurrent, bias);
+    if (rc == PB_OK && bank_fused(net, F)) rc = upload_frag16(*w, H, F, kernel, recurrent, bias, dense_w);
+    if (rc != PB_OK) return rc;
+    if (w->wide_ok) {
+        CK(ensure_dyn_smem(gru_wide_kernel<true>, wg_smem(w->wg_fp, w->wg_hp)));
+        CK(ensure_dyn_smem(gru_wide_kernel<false>, wg_smem(w->wg_fp, w->wg_hp)));
+    }
+    if (!w->small_path) {
+        CK(ensure_dyn_smem(gru_tiled_kernel<true>, tiled_smem));
+        CK(ensure_dyn_smem(gru_tiled_kernel<false>, tiled_smem));
+    }
+    net.w = std::move(w);
     return PB_OK;
 }
 
@@ -541,76 +680,7 @@ PB_API int pb_load_weights(pb_handle* h, const float* kernel, const float* recur
                     const float* dense_w, float dense_b) {
     if (!h || !kernel || !recurrent || !bias || !dense_w) return fail(PB_ERR_INVALID, "null argument");
     CK(cudaSetDevice(h->cfg.device));
-    const int H = h->cfg.hidden, F = h->feat, H3 = 3 * H;
-    std::vector<float> wcat((size_t)(F + H) * H3);
-    memcpy(wcat.data(), kernel, (size_t)F * H3 * sizeof(float));
-    memcpy(wcat.data() + (size_t)F * H3, recurrent, (size_t)H * H3 * sizeof(float));
-    cudaFree(h->d_wcat); cudaFree(h->d_bias); cudaFree(h->d_wd);
-    h->d_wcat = h->d_bias = h->d_wd = nullptr;
-    CK(upload(&h->d_wcat, wcat));
-    CK(upload(&h->d_bias, std::vector<float>(bias, bias + H3)));
-    CK(upload(&h->d_wd, std::vector<float>(dense_w, dense_w + H)));
-    h->bd = dense_b;
-    h->small_path = (H == 20 && F == 13 && !h->cfg.use_delta && h->cfg.activation == PB_ACT_LINEAR &&
-                     h->cfg.recurrent_activation == PB_RACT_HARD_SIGMOID);
-    if (h->small_path) {
-        memcpy(h->w_small.W, kernel, sizeof(h->w_small.W));
-        memcpy(h->w_small.U, recurrent, sizeof(h->w_small.U));
-        memcpy(h->w_small.b, bias, sizeof(h->w_small.b));
-        memcpy(h->w_small.wd, dense_w, sizeof(h->w_small.wd));
-        h->w_small.bd = dense_b;
-    } else {
-        h->wide_ok = H <= WG_MAX_H && F <= WG_MAX_F;
-        if (h->wide_ok) {
-            // fragment-ordered, TF32-split weights of gru_wide_kernel: k = 8 s + t (+ 4) is x feature k (k < FP) or hidden unit k - FP;
-            // phase-1 column n = 8 nt + g is z unit n (n < HP) or r unit n - HP, phase-2 column n is candidate unit n
-            auto tf32 = [](float x) { uint32_t u; memcpy(&u, &x, 4); u = (u + 0x1000u) & 0xffffe000u; float r; memcpy(&r, &u, 4); return r; };
-            const int FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
-            h->wg_fp = FP; h->wg_hp = HP;
-            auto wv = [&](int k, int gate, int unit) -> float {
-                if (unit >= H) return 0.f;
-                if (k < FP) return k < F ? kernel[(size_t)k * H3 + gate * H + unit] : 0.f;
-                const int hu = k - FP;
-                return hu < H ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
-            };
-            auto frag = [&](int s, int lane, int gate, int unit) {
-                const int t = lane & 3;
-                const float v0 = wv(8 * s + t, gate, unit), v1 = wv(8 * s + t + 4, gate, unit);
-                const float h0 = tf32(v0), h1 = tf32(v1), l0 = tf32(v0 - h0), l1 = tf32(v1 - h1);
-                uint4 r; memcpy(&r.x, &h0, 4); memcpy(&r.y, &h1, 4); memcpy(&r.z, &l0, 4); memcpy(&r.w, &l1, 4);
-                return r;
-            };
-            std::vector<uint4> b1((size_t)KS * (HP / 4) * 32), b2((size_t)KS * (HP / 8) * 32);
-            for (int s = 0; s < KS; ++s)
-                for (int lane = 0; lane < 32; ++lane) {
-                    for (int nt = 0; nt < HP / 4; ++nt) {
-                        const int c = 8 * nt + (lane >> 2);
-                        b1[((size_t)s * (HP / 4) + nt) * 32 + lane] = frag(s, lane, c < HP ? 0 : 1, c % HP);
-                    }
-                    for (int nt = 0; nt < HP / 8; ++nt) b2[((size_t)s * (HP / 8) + nt) * 32 + lane] = frag(s, lane, 2, 8 * nt + (lane >> 2));
-                }
-            std::vector<float> wb((size_t)3 * HP, 0.f);
-            for (int g3 = 0; g3 < 3; ++g3)
-                for (int u = 0; u < H; ++u) wb[(size_t)g3 * HP + u] = bias[g3 * H + u];
-            cudaFree(h->d_wg_b1); cudaFree(h->d_wg_b2); cudaFree(h->d_wg_bias);
-            h->d_wg_b1 = h->d_wg_b2 = nullptr; h->d_wg_bias = nullptr;
-            CK(upload(&h->d_wg_b1, b1));
-            CK(upload(&h->d_wg_b2, b2));
-            CK(upload(&h->d_wg_bias, wb));
-            CK(ensure_dyn_smem(gru_wide_kernel<true>, wg_smem(FP, HP)));
-            CK(ensure_dyn_smem(gru_wide_kernel<false>, wg_smem(FP, HP)));
-        }
-        size_t smem = (size_t)(F + 3 * H) * K2_TILE_STREAMS * sizeof(float);
-        if (smem > 200 * 1024) return fail(PB_ERR_UNSUPPORTED, "feature_size + 3*hidden = %d is too large for the tiled GRU kernel", F + 3 * H);
-        CK(ensure_dyn_smem(gru_tiled_kernel<true>, (size_t)(smem)));
-        CK(ensure_dyn_smem(gru_tiled_kernel<false>, (size_t)(smem)));
-    }
-    if (bank_fused(h)) {
-        const int rc = upload_frag16(h, kernel, recurrent, bias, dense_w);
-        if (rc != PB_OK) return rc;
-    }
-    h->have_weights = true;
-    return PB_OK;
+    return load_weights(h->models[0], h->feat, kernel, recurrent, bias, dense_w, dense_b);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -640,7 +710,7 @@ struct ProfScope {
 PB_API int pb_debug_gru_mode(pb_handle* h, int mode) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (mode < 0 || mode > 2) return fail(PB_ERR_INVALID, "gru mode must be 0 (automatic), 1 (CUDA-core kernel) or 2 (tensor-core kernel)");
-    h->gru_mode = mode;
+    h->models[0].gru_mode = mode;
     return PB_OK;
 }
 
@@ -661,31 +731,40 @@ PB_API int pb_debug_tc_dft_power(const int16_t* x512, double* power257) {
     return PB_OK;
 }
 
-static void tcd_host_tables(const pb_handle* h, std::vector<float4>& etab, std::vector<float>& dct, float* tot_scale);
+// tables of the CPU model of the matrix-product MFCC, from the mel tables of configuration c (n_out MFCCs)
+static void tcd_host_tables(const pb_config& c, int n_out, const MelHost& mel, std::vector<float4>& etab, std::vector<float>& dct,
+                            float* tot_scale) {
+    const float inv = 1.0f / 32768.0f, scale = inv * inv / (float)c.n_fft, pscale = scale / (TCD_A_SCALE * TCD_A_SCALE);
+    tcd_build_etab(etab, mel.wrise, mel.wfall, mel.grid, c.n_filt, pscale);
+    dct.assign((size_t)TCD_MAX_OUT * 24, 0.f);
+    for (int k = 0; k < n_out; ++k)
+        for (int j = 0; j < c.n_filt; ++j) {
+            double v = cos(M_PI * k * (2 * j + 1) / (2.0 * c.n_filt)) * sqrt(2.0 / c.n_filt);
+            if (k == 0) v *= sqrt(0.5);
+            dct[(size_t)k * 24 + j] = (float)v;
+        }
+    *tot_scale = pscale;
+}
 
 // CPU model of the whole matrix-product MFCC for one frame: accumulator row (as above) + the epilogue (mel, log, DCT, c0) with
-// the tables of a handle of this configuration.  Needs no device: only the mel-table part of pb_create runs.
+// the tables a handle of this configuration builds.  Needs no device.
 PB_API int pb_debug_tc_mfcc_frame(const pb_config* cfg, const int16_t* x512, float* out) {
     if (!cfg || !x512 || !out) return fail(PB_ERR_INVALID, "null argument");
     if (cfg->n_fft != 512 || cfg->n_filt < 1 || cfg->n_filt > TCD_MAX_FILT || cfg->vectorizer != PB_VEC_MFCCS)
         return fail(PB_ERR_UNSUPPORTED, "the tensor-core MFCC model covers n_fft 512, n_filt <= %d, MFCC vectorizer", TCD_MAX_FILT);
-    pb_handle* h = new (std::nothrow) pb_handle();
-    if (!h) return fail(PB_ERR_CUDA, "out of host memory");
-    h->cfg = *cfg;
-    h->n_bins = cfg->n_fft / 2 + 1;
-    h->n_out = std::min(cfg->n_filt, cfg->n_mfcc);
-    int rc = h->n_out > TCD_MAX_OUT ? fail(PB_ERR_UNSUPPORTED, "n_mfcc > %d", TCD_MAX_OUT) : build_mel(h, h->h_wrise, h->h_wfall, h->h_grid);
-    if (rc == PB_OK) {
-        std::vector<float4> etab;
-        std::vector<float> dct;
-        float tot_scale = 0.f;
-        tcd_host_tables(h, etab, dct, &tot_scale);
-        float d[TCD_BLOCKS][64];
-        tcd_host_accumulators(x512, d);
-        tcd_host_epilogue(d, etab.data(), dct.data(), cfg->n_filt, h->n_out, tot_scale, out);
-    }
-    delete h;
-    return rc;
+    const int n_out = std::min(cfg->n_filt, cfg->n_mfcc);
+    if (n_out > TCD_MAX_OUT) return fail(PB_ERR_UNSUPPORTED, "n_mfcc > %d", TCD_MAX_OUT);
+    MelHost mel;
+    const int rc = build_mel(*cfg, cfg->n_fft / 2 + 1, mel);
+    if (rc != PB_OK) return rc;
+    std::vector<float4> etab;
+    std::vector<float> dct;
+    float tot_scale = 0.f;
+    tcd_host_tables(*cfg, n_out, mel, etab, dct, &tot_scale);
+    float d[TCD_BLOCKS][64];
+    tcd_host_accumulators(x512, d);
+    tcd_host_epilogue(d, etab.data(), dct.data(), cfg->n_filt, n_out, tot_scale, out);
+    return PB_OK;
 }
 
 // ... and of the formulation with both DFT stages as matrix products (mfcc_tc3.cuh): exact int16 split, stage-1 matrix passes, twiddle,
@@ -694,34 +773,30 @@ PB_API int pb_debug_tc3_mfcc_frame(const pb_config* cfg, const int16_t* x512, fl
     if (!cfg || !x512 || !out) return fail(PB_ERR_INVALID, "null argument");
     if (cfg->n_fft != 512 || cfg->n_filt < 1 || cfg->n_filt > TCD_MAX_FILT || cfg->vectorizer != PB_VEC_MFCCS)
         return fail(PB_ERR_UNSUPPORTED, "the tensor-core MFCC model covers n_fft 512, n_filt <= %d, MFCC vectorizer", TCD_MAX_FILT);
-    pb_handle* h = new (std::nothrow) pb_handle();
-    if (!h) return fail(PB_ERR_CUDA, "out of host memory");
-    h->cfg = *cfg;
-    h->n_bins = cfg->n_fft / 2 + 1;
-    h->n_out = std::min(cfg->n_filt, cfg->n_mfcc);
-    int rc = h->n_out > TCD_MAX_OUT ? fail(PB_ERR_UNSUPPORTED, "n_mfcc > %d", TCD_MAX_OUT) : build_mel(h, h->h_wrise, h->h_wfall, h->h_grid);
-    if (rc == PB_OK) {
-        std::vector<float4> etab;
-        std::vector<float> dct;
-        float tot_scale = 0.f;
-        tcd_host_tables(h, etab, dct, &tot_scale);
-        float d[TCD_BLOCKS][64];
-        tc3_host_accumulators(x512, d);
-        tc3_host_epilogue(d, h->h_wrise, h->h_wfall, h->h_grid, dct.data(), cfg->n_filt, h->n_out, tot_scale, out);
-        if (power257) {
-            const double inv = 1.0 / ((double)TCD_A_SCALE * (double)TCD_A_SCALE);
-            for (int b = 0; b < TCD_BLOCKS; ++b)
-                for (int half = 0; half < 2; ++half)
-                    for (int m = 0; m < 16; ++m) {
-                        const int k = tcd_col_bin(b, 32 * half + m);
-                        if (k < 0) continue;
-                        const double re = d[b][32 * half + m], im = d[b][32 * half + 16 + m];
-                        power257[k] = (k == 0 || k == 256) ? re * re * inv : (re * re + im * im) * inv;
-                    }
-        }
+    const int n_out = std::min(cfg->n_filt, cfg->n_mfcc);
+    if (n_out > TCD_MAX_OUT) return fail(PB_ERR_UNSUPPORTED, "n_mfcc > %d", TCD_MAX_OUT);
+    MelHost mel;
+    const int rc = build_mel(*cfg, cfg->n_fft / 2 + 1, mel);
+    if (rc != PB_OK) return rc;
+    std::vector<float4> etab;
+    std::vector<float> dct;
+    float tot_scale = 0.f;
+    tcd_host_tables(*cfg, n_out, mel, etab, dct, &tot_scale);
+    float d[TCD_BLOCKS][64];
+    tc3_host_accumulators(x512, d);
+    tc3_host_epilogue(d, mel.wrise, mel.wfall, mel.grid, dct.data(), cfg->n_filt, n_out, tot_scale, out);
+    if (power257) {
+        const double inv = 1.0 / ((double)TCD_A_SCALE * (double)TCD_A_SCALE);
+        for (int b = 0; b < TCD_BLOCKS; ++b)
+            for (int half = 0; half < 2; ++half)
+                for (int m = 0; m < 16; ++m) {
+                    const int k = tcd_col_bin(b, 32 * half + m);
+                    if (k < 0) continue;
+                    const double re = d[b][32 * half + m], im = d[b][32 * half + 16 + m];
+                    power257[k] = (k == 0 || k == 256) ? re * re * inv : (re * re + im * im) * inv;
+                }
     }
-    delete h;
-    return rc;
+    return PB_OK;
 }
 
 // CPU model of the mma.sync MFCC tick's DFT (mfcc_mma.cuh: its fragment tables, splits and bin assembly) for one frame.  Test hook.
@@ -760,33 +835,41 @@ PB_API int pb_profile_read(pb_handle* h, double ms[4], uint64_t launches[4]) {
 // ------------------------------------------------------------------------------------------------
 static MelTables mel_tables(const pb_handle* h) {
     MelTables t;
-    t.w_rise = h->d_wrise; t.w_fall = h->d_wfall; t.grid = h->d_grid; t.dct = h->d_dct;
-    t.tw_stage = h->d_tw_stage; t.tw_post = h->d_tw_post;
+    t.w_rise = h->d_wrise.get(); t.w_fall = h->d_wfall.get(); t.grid = h->d_grid.get(); t.dct = h->d_dct.get();
+    t.tw_stage = h->d_tw_stage.get(); t.tw_post = h->d_tw_post.get();
     t.n_bins = h->n_bins; t.n_filt = h->cfg.n_filt; t.n_out = h->n_out;
     t.mels_only = h->cfg.vectorizer == PB_VEC_MELS;
-    t.n_fft = h->cfg.n_fft; t.tw_any = h->d_tw_any;
+    t.n_fft = h->cfg.n_fft; t.tw_any = h->d_tw_any.get();
     return t;
 }
 
 static FastTables fast_tables(const pb_handle* h) {
     FastTables f;
-    f.ptab = h->d_ptab; f.ctab = h->d_ctab; f.dct_t = h->d_dct_t;
+    f.ptab = h->d_ptab.get(); f.ctab = h->d_ctab.get(); f.dct_t = h->d_dct_t.get();
     f.npl = h->npl; f.maxc = h->maxc; f.nol = h->nol;
     return f;
 }
 
-static DecodeParams decode_params(const pb_handle* h) {
+static StreamState stream_state(const pb_handle* h) {
+    StreamState st;
+    st.n_samples = h->d_n_samples.get(); st.tail = h->d_tail.get(); st.ring = h->d_ring.get();
+    st.tail_cap = h->tail_cap; st.ring_rows = h->ring_rows; st.row_stride = h->row_stride;
+    return st;
+}
+
+static DecodeParams decode_params(const Network& net) {
+    const pb_config& c = net.cfg;
     DecodeParams d;
-    d.cd = h->d_cd; d.cd_len = (int)h->cd.size();
-    d.min_out = h->min_out; d.out_range = h->max_out - h->min_out;
-    d.center = h->cfg.threshold_center;
-    d.hot_threshold = 1.0 - h->cfg.sensitivity;
-    d.trigger_level = h->cfg.trigger_level;
-    const long long bytes = 2LL * h->cfg.chunk_samples;          // TriggerDetector.chunk_size is in bytes
+    d.cd = net.d_cd.get(); d.cd_len = (int)net.cd.size();
+    d.min_out = net.min_out; d.out_range = net.max_out - net.min_out;
+    d.center = c.threshold_center;
+    d.hot_threshold = 1.0 - c.sensitivity;
+    d.trigger_level = c.trigger_level;
+    const long long bytes = 2LL * c.chunk_samples;                // TriggerDetector.chunk_size is in bytes
     long long q = -(8 * 2048) / bytes;                            // C truncates toward zero ...
     if ((-(8 * 2048)) % bytes != 0) q -= 1;                       // ... python floors
     d.trigger_reset = (int)q;
-    d.legacy_f64 = h->cfg.decode_legacy_f64 != 0;
+    d.legacy_f64 = c.decode_legacy_f64 != 0;
     return d;
 }
 
@@ -828,12 +911,13 @@ PB_API int pb_mfcc_f32(pb_handle* h, const float* d_audio, int64_t n_streams, in
     return mfcc_impl<float>(h, d_audio, n_streams, L, d_out, (cudaStream_t)stream, 1.0f / (float)h->cfg.n_fft);
 }
 
-// Model slot `slot` of a gru_bank_kernel launch: network hm, scored with decoder dp into o.
-static void set_bank_slot(BankParams& P, int slot, const pb_handle* hm, const DecodeParams& dp, const K2Out& o) {
+// Model slot `slot` of a gru_bank_kernel launch: network net, scored with its decoder into o.
+static void set_bank_slot(BankParams& P, int slot, const Network& net, const K2Out& o) {
+    const NetWeights& nw = *net.w;
     BankModelW& w = P.w[slot];
-    w.bfrag = hm->d_bfrag16; w.xfrag = hm->d_xfrag16; w.bias = hm->d_mma_bias; w.wd = hm->d_mma_wd; w.bd = hm->bd;
-    w.act = hm->cfg.activation; w.ract = hm->cfg.recurrent_activation;
-    P.dp[slot] = dp;
+    w.bfrag = nw.bfrag16.get(); w.xfrag = nw.xfrag16.get(); w.bias = nw.mma_bias.get(); w.wd = nw.mma_wd.get(); w.bd = nw.bd;
+    w.act = net.cfg.activation; w.ract = net.cfg.recurrent_activation;
+    P.dp[slot] = decode_params(net);
     P.o[slot] = o;
 }
 
@@ -847,32 +931,36 @@ static int launch_bank_nm(const BankParams& P, const K2In& in, int64_t n, cudaSt
     return PB_OK;
 }
 
-static int launch_gru_kernels(pb_handle* h, const K2In& in, bool ring, int64_t n, const DecodeParams& dp, const K2Out& o, cudaStream_t s) {
-    if (h->small_path && n <= K2_WARP_PATH_MAX && h->gru_mode == 0) {                 // latency path: a warp per stream
+// Scores network net (which has weights; F = the front end's feature size) with its decoder into o.
+static int launch_gru_kernels(const Network& net, int F, const K2In& in, bool ring, int64_t n, const K2Out& o, cudaStream_t s) {
+    const NetWeights& nw = *net.w;
+    const pb_config& c = net.cfg;
+    const DecodeParams dp = decode_params(net);
+    if (nw.small_path && n <= K2_WARP_PATH_MAX && net.gru_mode == 0) {                 // latency path: a warp per stream
         const int grid = (int)((n + 3) / 4);
-        if (ring) gru_warp_kernel<20, 13, true><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
-        else gru_warp_kernel<20, 13, false><<<grid, 128, 0, s>>>(h->w_small, in, n, dp, o);
-    } else if (h->small_path && h->gru_mode != 1) {               // tensor-core scan (mma.sync fp16 x 3): the bank kernel with one model
+        if (ring) gru_warp_kernel<20, 13, true><<<grid, 128, 0, s>>>(nw.w_small, in, n, dp, o);
+        else gru_warp_kernel<20, 13, false><<<grid, 128, 0, s>>>(nw.w_small, in, n, dp, o);
+    } else if (nw.small_path && net.gru_mode != 1) {              // tensor-core scan (mma.sync fp16 x 3): the bank kernel with one model
         BankParams P{};
-        set_bank_slot(P, 0, h, dp, o);
+        set_bank_slot(P, 0, net, o);
         return ring ? launch_bank_nm<1, true>(P, in, n, s) : launch_bank_nm<1, false>(P, in, n, s);
-    } else if (h->small_path) {
+    } else if (nw.small_path) {
         const int per_cta = K2_SMALL_THREADS * K2_NS;
         const int grid = (int)((n + per_cta - 1) / per_cta);
-        if (ring) gru_small_kernel<20, 13, true><<<grid, K2_SMALL_THREADS, 0, s>>>(h->w_small, in, n, dp, o);
-        else gru_small_kernel<20, 13, false><<<grid, K2_SMALL_THREADS, 0, s>>>(h->w_small, in, n, dp, o);
-    } else if (h->wide_ok && h->gru_mode != 1) {                  // tensor-core scan (mma.sync 3xTF32) for other networks
+        if (ring) gru_small_kernel<20, 13, true><<<grid, K2_SMALL_THREADS, 0, s>>>(nw.w_small, in, n, dp, o);
+        else gru_small_kernel<20, 13, false><<<grid, K2_SMALL_THREADS, 0, s>>>(nw.w_small, in, n, dp, o);
+    } else if (nw.wide_ok && net.gru_mode != 1) {                 // tensor-core scan (mma.sync 3xTF32) for other networks
         GruWideW w;
-        w.b1 = h->d_wg_b1; w.b2 = h->d_wg_b2; w.bias = h->d_wg_bias; w.wd = h->d_wd; w.bd = h->bd;
-        w.H = h->cfg.hidden; w.F = h->feat; w.FP = h->wg_fp; w.HP = h->wg_hp; w.act = h->cfg.activation; w.ract = h->cfg.recurrent_activation;
+        w.b1 = nw.wg_b1.get(); w.b2 = nw.wg_b2.get(); w.bias = nw.wg_bias.get(); w.wd = nw.wd.get(); w.bd = nw.bd;
+        w.H = c.hidden; w.F = F; w.FP = nw.wg_fp; w.HP = nw.wg_hp; w.act = c.activation; w.ract = c.recurrent_activation;
         const int grid = (int)((n + WG_STREAMS - 1) / WG_STREAMS);
         const size_t smem = wg_smem(w.FP, w.HP);
         if (ring) gru_wide_kernel<true><<<grid, WG_THREADS, smem, s>>>(w, in, n, dp, o);
         else gru_wide_kernel<false><<<grid, WG_THREADS, smem, s>>>(w, in, n, dp, o);
     } else {
         GruTiledW w;
-        w.wcat = h->d_wcat; w.bias = h->d_bias; w.wd = h->d_wd; w.bd = h->bd;
-        w.H = h->cfg.hidden; w.F_in = h->feat; w.act = h->cfg.activation; w.ract = h->cfg.recurrent_activation;
+        w.wcat = nw.wcat.get(); w.bias = nw.bias.get(); w.wd = nw.wd.get(); w.bd = nw.bd;
+        w.H = c.hidden; w.F_in = F; w.act = c.activation; w.ract = c.recurrent_activation;
         const size_t smem = (size_t)(w.F_in + 3 * w.H) * K2_TILE_STREAMS * sizeof(float);
         const int grid = (int)((n + K2_TILE_STREAMS - 1) / K2_TILE_STREAMS);
         if (ring) gru_tiled_kernel<true><<<grid, K2_TILE_THREADS, smem, s>>>(w, in, n, dp, o);
@@ -882,14 +970,14 @@ static int launch_gru_kernels(pb_handle* h, const K2In& in, bool ring, int64_t n
     return PB_OK;
 }
 
-static int launch_gru(pb_handle* h, const K2In& in, bool ring, int64_t n, const DecodeParams& dp, const K2Out& o, cudaStream_t s) {
+static int launch_gru(pb_handle* h, const Network& net, const K2In& in, bool ring, int64_t n, const K2Out& o, cudaStream_t s) {
     ProfScope ps(h, 1, s);
-    return launch_gru_kernels(h, in, ring, n, dp, o, s);
+    return launch_gru_kernels(net, h->feat, in, ring, n, o, s);
 }
 
 PB_API int pb_predict(pb_handle* h, const float* d_inputs, int64_t n, float* d_out, float* d_logit, void* stream) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
-    if (!h->have_weights) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
     if (n < 0) return fail(PB_ERR_INVALID, "negative n");
     if (n == 0) return PB_OK;
     if (!d_inputs || !d_out) return fail(PB_ERR_INVALID, "null buffer");
@@ -898,7 +986,7 @@ PB_API int pb_predict(pb_handle* h, const float* d_inputs, int64_t n, float* d_o
     in.inputs = d_inputs; in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = 0;
     K2Out o{};
     o.raw = d_out; o.logit = d_logit;
-    return launch_gru(h, in, false, n, decode_params(h), o, (cudaStream_t)stream);
+    return launch_gru(h, h->models[0], in, false, n, o, (cudaStream_t)stream);
 }
 
 PB_API int pb_decode(pb_handle* h, const float* d_raw, int64_t n, double* d_conf, void* stream) {
@@ -909,7 +997,7 @@ PB_API int pb_decode(pb_handle* h, const float* d_raw, int64_t n, double* d_conf
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     ProfScope ps(h, 2, s);
-    decode_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(d_raw, n, decode_params(h), d_conf);
+    decode_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(d_raw, n, decode_params(h->models[0]), d_conf);
     CK(cudaGetLastError());
     return PB_OK;
 }
@@ -921,34 +1009,20 @@ static int check_tick(pb_handle* h, const void* pcm, int64_t n) {
     return PB_OK;
 }
 
-// tables of the CPU model of the matrix-product MFCC
-static void tcd_host_tables(const pb_handle* h, std::vector<float4>& etab, std::vector<float>& dct, float* tot_scale) {
-    const float inv = 1.0f / 32768.0f, scale = inv * inv / (float)h->cfg.n_fft, pscale = scale / (TCD_A_SCALE * TCD_A_SCALE);
-    tcd_build_etab(etab, h->h_wrise, h->h_wfall, h->h_grid, h->cfg.n_filt, pscale);
-    dct.assign((size_t)TCD_MAX_OUT * 24, 0.f);
-    for (int k = 0; k < h->n_out; ++k)
-        for (int j = 0; j < h->cfg.n_filt; ++j) {
-            double v = cos(M_PI * k * (2 * j + 1) / (2.0 * h->cfg.n_filt)) * sqrt(2.0 / h->cfg.n_filt);
-            if (k == 0) v *= sqrt(0.5);
-            dct[(size_t)k * 24 + j] = (float)v;
-        }
-    *tot_scale = pscale;
-}
-
 static int ensure_mma_tables(pb_handle* h) {
-    if (h->d_mm_b1) return PB_OK;
+    if (h->d_mm_b1.get()) return PB_OK;
     std::vector<uint2> b1, b2;
     std::vector<float2> tw;
     mm_build_tables(b1, b2, tw);
-    CK(upload(&h->d_mm_b2, b2));
-    CK(upload(&h->d_mm_tw, tw));
-    CK(cudaMalloc((void**)&h->d_mm_recs, (size_t)h->cfg.max_streams * (size_t)std::max(1, h->max_new) * sizeof(MmRec)));
-    CK(cudaMalloc((void**)&h->d_mm_counters, 2 * sizeof(unsigned int)));
-    CK(cudaMemset(h->d_mm_counters, 0, 2 * sizeof(unsigned int)));
+    CK(h->d_mm_b2.upload(b2));
+    CK(h->d_mm_tw.upload(tw));
+    CK(h->d_mm_recs.alloc((size_t)h->cfg.max_streams * (size_t)std::max(1, h->max_new)));
+    CK(h->d_mm_counters.alloc(2));
+    CK(cudaMemset(h->d_mm_counters.get(), 0, 2 * sizeof(unsigned int)));
     CK(ensure_dyn_smem(mfcc_mma_kernel<false, false>, sizeof(MmSmem)));
     CK(ensure_dyn_smem(mfcc_mma_kernel<true, false>, sizeof(MmSmem)));
     CK(ensure_dyn_smem(mfcc_mma_kernel<true, true>, sizeof(MmSmem)));
-    CK(upload(&h->d_mm_b1, b1));                         // last: its presence marks the set as complete
+    CK(h->d_mm_b1.upload(b1));                           // last: its presence marks the set as complete
     return PB_OK;
 }
 
@@ -958,25 +1032,28 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
     const int64_t tiles = (n + K1_STREAMS_PER_CTA - 1) / K1_STREAMS_PER_CTA;
     const int grid = (int)std::min<int64_t>(tiles, (int64_t)h->sm_count * 4);
     const float inv = 1.0f / 32768.0f, scale = inv * inv / (float)h->cfg.n_fft;
+    const StreamState st = stream_state(h);
     ProfScope ps(h, 0, s);
     if (h->k1_mode >= 4 && h->mma_ok && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
         int rc = ensure_mma_tables(h);
         if (rc != PB_OK) return rc;
         MmTables t;
-        t.b1 = h->d_mm_b1; t.b2 = h->d_mm_b2; t.tw = h->d_mm_tw;
+        t.b1 = h->d_mm_b1.get(); t.b2 = h->d_mm_b2.get(); t.tw = h->d_mm_tw.get();
         t.pscale = inv * inv / (float)h->cfg.n_fft * 1024.f;             // the accumulators hold 2^-5 X
         const int par = h->mm_parity;
         h->mm_parity ^= 1;
+        MmRec* recs = h->d_mm_recs.get();
+        unsigned int* counters = h->d_mm_counters.get();
         mfcc_mma_plan_kernel<<<(int)((n + MM_PLAN_THREADS - 1) / MM_PLAN_THREADS), MM_PLAN_THREADS, 0, s>>>(
-            d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, h->st, h->d_mm_recs, h->d_mm_counters, par);
+            d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, st, recs, counters, par);
         const int64_t max_tiles = (n * std::max(1, h->max_new) + MM_FRAMES - 1) / MM_FRAMES;
         const int gm = (int)std::min<int64_t>((max_tiles + MM_WARPS - 1) / MM_WARPS, h->sm_count);
         if (h->k1_mode == 4)
-            mfcc_mma_kernel<false, false><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), h->d_mm_recs, h->d_mm_counters, par);
+            mfcc_mma_kernel<false, false><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), recs, counters, par);
         else if (h->k1_mode == 5)
-            mfcc_mma_kernel<true, false><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), h->d_mm_recs, h->d_mm_counters, par);
+            mfcc_mma_kernel<true, false><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), recs, counters, par);
         else
-            mfcc_mma_kernel<true, true><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), h->d_mm_recs, h->d_mm_counters, par);
+            mfcc_mma_kernel<true, true><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), recs, counters, par);
     } else if (h->fast_ok && h->max_new <= 8 && h->cfg.chunk_samples % 8 == 0 && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
         // streams per warp tile: 16 at scale; fewer when the batch cannot fill the machine's warps
         const int64_t warps_total = (int64_t)h->sm_count * 4 * K1F_WARPS;
@@ -985,10 +1062,10 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
         const int gridf = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
         if (h->k1_mode != 3)                     // default: the 32-bit per-pass set-up (bit-identical rows); 3 = the 64-bit original
             mfcc_fast_stream_kernel<true><<<gridf, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
-                                                                                      mel_tables(h), fast_tables(h), h->st);
+                                                                                      mel_tables(h), fast_tables(h), st);
         else
             mfcc_fast_stream_kernel<false><<<gridf, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
-                                                                                       mel_tables(h), fast_tables(h), h->st);
+                                                                                       mel_tables(h), fast_tables(h), st);
     } else if (h->max_new > 8) {
         // A chunk that completes more than 8 frames per stream: consecutive sub-chunks of at most 6 hops (<= 8 frames each) through the
         // generic kernel -- to the state machine they are separate ticks (Listener.update_vectors is chunking-independent); the network
@@ -996,11 +1073,11 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
         const int sub = std::max(1, 6 * h->cfg.hop_samples);
         for (int off = 0; off < h->cfg.chunk_samples; off += sub)
             mfcc_stream_kernel<false><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm + off, d_ids, (int)n, std::min(sub, h->cfg.chunk_samples - off),
-                                                                                    h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), h->st);
+                                                                                    h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st);
     } else if (pairs)
-        mfcc_stream_kernel<true><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), h->st);
+        mfcc_stream_kernel<true><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st);
     else
-        mfcc_stream_kernel<false><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), h->st);
+        mfcc_stream_kernel<false><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st);
     CK(cudaGetLastError());
     return PB_OK;
 }
@@ -1015,7 +1092,7 @@ PB_API int pb_update_vectors(pb_handle* h, const int16_t* d_pcm, const int32_t* 
 // Where a stream tick's network kernels read the window of item i: stream d_ids[i] (i when d_ids is null) of the handle's ring.
 static K2In stream_k2in(const pb_handle* h, const int32_t* d_ids) {
     K2In in{};
-    in.ring = h->st.ring; in.n_samples = h->st.n_samples; in.ids = d_ids;
+    in.ring = h->d_ring.get(); in.n_samples = h->d_n_samples.get(); in.ids = d_ids;
     in.ring_rows = h->ring_rows; in.row_stride = h->row_stride; in.window = h->rel_window; in.hop = h->cfg.hop_samples;
     in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
     return in;
@@ -1025,15 +1102,16 @@ PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, i
               uint8_t* d_fired, unsigned long long* d_count, void* stream) {
     int rc = check_tick(h, d_pcm, n);
     if (rc != PB_OK || n == 0) return rc;
-    if (!h->have_weights) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    const Network& net = h->models[0];
+    if (!net.w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
     if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
     K2Out o{};
-    o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = h->st.trig;
-    return launch_gru(h, stream_k2in(h, d_ids), true, n, decode_params(h), o, s);
+    o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = net.trig.get();
+    return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1051,37 +1129,29 @@ PB_API int pb_add_model(pb_handle* h, const pb_config* cfg, const float* kernel,
     PB_SAME_FRONT_END(n_filt); PB_SAME_FRONT_END(n_mfcc); PB_SAME_FRONT_END(n_features); PB_SAME_FRONT_END(use_delta);
     PB_SAME_FRONT_END(vectorizer); PB_SAME_FRONT_END(chunk_samples); PB_SAME_FRONT_END(device);
 #undef PB_SAME_FRONT_END
-    if ((int)h->bank.size() + 1 >= PB_MAX_MODELS) return fail(PB_ERR_INVALID, "a bank holds at most %d models", PB_MAX_MODELS);
-    if (c.hidden < 1) return fail(PB_ERR_INVALID, "hidden must be positive");
-    if (c.n_thresholds < 1 || c.n_thresholds > PB_MAX_THRESHOLDS) return fail(PB_ERR_INVALID, "n_thresholds must be in [1, %d]", PB_MAX_THRESHOLDS);
-    if (c.activation < 0 || c.activation > 1 || c.recurrent_activation < 0 || c.recurrent_activation > 1)
-        return fail(PB_ERR_UNSUPPORTED, "unsupported GRU activation");
+    if (h->models.size() >= PB_MAX_MODELS) return fail(PB_ERR_INVALID, "a bank holds at most %d models", PB_MAX_MODELS);
+    int rc = check_network(c);
+    if (rc != PB_OK) return rc;
     CK(cudaSetDevice(c.device));
-    pb_handle* m = new (std::nothrow) pb_handle();
-    if (!m) return fail(PB_ERR_CUDA, "out of host memory");
-    m->cfg = c;
-    m->cfg.max_streams = h->cfg.max_streams;
-    m->sm_count = h->sm_count; m->used = h->used; m->n_bins = h->n_bins; m->n_out = h->n_out; m->feat = h->feat;
-    m->ring_rows = h->ring_rows; m->row_stride = h->row_stride; m->rel_window = h->rel_window; m->tail_cap = h->tail_cap; m->max_new = h->max_new;
-    build_cdf(m);
-    int rc = PB_OK;
-    if (cd && cd_len != (int64_t)m->cd.size()) rc = fail(PB_ERR_INVALID, "cdf length %lld != %zu", (long long)cd_len, m->cd.size());
-    else if (cd) memcpy(m->cd.data(), cd, cd_len * sizeof(double));
-    const size_t S = (size_t)h->cfg.max_streams;
-    cudaError_t e = cudaSuccess;
-    if (rc == PB_OK && (e = upload(&m->d_cd, m->cd)) == cudaSuccess && (e = cudaMalloc((void**)&m->st.trig, S * sizeof(int))) == cudaSuccess)
-        e = cudaMemset(m->st.trig, 0, S * sizeof(int));
-    if (rc == PB_OK && e != cudaSuccess) rc = fail(PB_ERR_CUDA, "model bank allocation failed: %s", cudaGetErrorString(e));
-    if (rc == PB_OK) rc = pb_load_weights(m, kernel, recurrent, bias, dense_w, dense_b);
-    if (rc != PB_OK) { pb_destroy(m); return rc; }
-    h->bank.push_back(m);
-    if (slot) *slot = (int32_t)h->bank.size();
+    // built aside and appended only when complete: a failure leaves the bank as it was
+    Network net;
+    net.cfg = c;
+    net.cfg.max_streams = h->cfg.max_streams;
+    build_cdf(net);
+    if (cd && cd_len != (int64_t)net.cd.size()) return fail(PB_ERR_INVALID, "cdf length %lld != %zu", (long long)cd_len, net.cd.size());
+    if (cd) memcpy(net.cd.data(), cd, cd_len * sizeof(double));
+    const cudaError_t e = upload_network_state(net, (size_t)h->cfg.max_streams);
+    if (e != cudaSuccess) return fail(PB_ERR_CUDA, "model bank allocation failed: %s", cudaGetErrorString(e));
+    rc = load_weights(net, h->feat, kernel, recurrent, bias, dense_w, dense_b);
+    if (rc != PB_OK) return rc;
+    h->models.push_back(std::move(net));
+    if (slot) *slot = (int32_t)h->models.size() - 1;
     return PB_OK;
 }
 
 PB_API int pb_num_models(const pb_handle* h) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
-    return 1 + (int)h->bank.size();
+    return (int)h->models.size();
 }
 
 static int launch_bank(const BankParams& P, int nm, const K2In& in, int64_t n, cudaStream_t s) {
@@ -1102,12 +1172,12 @@ PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d
                             uint8_t* d_fired, unsigned long long* d_count, void* stream) {
     int rc = check_tick(h, d_pcm, n);
     if (rc != PB_OK) return rc;
-    if (!h->have_weights) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
     if (n == 0) return PB_OK;
     if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    const int M = 1 + (int)h->bank.size();
+    const int M = (int)h->models.size();
     rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
     const K2In in = stream_k2in(h, d_ids);
@@ -1116,17 +1186,17 @@ PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d
     BankParams P{};
     int nm = 0;
     for (int m = 0; m < M; ++m) {
-        pb_handle* hm = m == 0 ? h : h->bank[m - 1];
+        const Network& net = h->models[m];
         K2Out o{};
         o.raw = d_raw ? d_raw + (int64_t)m * n : nullptr;
         o.conf = d_conf + (int64_t)m * n;
         o.fired = d_fired ? d_fired + (int64_t)m * n : nullptr;
         o.count = d_count ? d_count + m : nullptr;
-        o.trig = hm->st.trig;
-        if (bank_fused(hm)) {
-            set_bank_slot(P, nm++, hm, decode_params(hm), o);
+        o.trig = net.trig.get();
+        if (bank_fused(net, h->feat)) {
+            set_bank_slot(P, nm++, net, o);
         } else {
-            rc = launch_gru_kernels(hm, in, true, n, decode_params(hm), o, s);
+            rc = launch_gru_kernels(net, h->feat, in, true, n, o, s);
             if (rc != PB_OK) return rc;
         }
     }
@@ -1163,17 +1233,19 @@ PB_API int pb_read_window(pb_handle* h, const int32_t* d_ids, int64_t n, float* 
     return PB_OK;
 }
 
-__global__ void clear_kernel(StreamState st, const int* ids, long long n) {
+struct TrigArrays {
+    int* trig[PB_MAX_MODELS];        // each bank model's TriggerDetector.activation; null past the last model
+};
+
+// Stream ids[i] (or i) starts over: no samples consumed, every model's trigger re-armed.
+__global__ void clear_kernel(long long* n_samples, TrigArrays t, const int* ids, long long n) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int sid = ids ? ids[i] : (int)i;
-    st.n_samples[sid] = 0;
-    st.trig[sid] = 0;
-}
-
-__global__ void clear_trig_kernel(int* trig, const int* ids, long long n) {
-    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) trig[ids ? ids[i] : (int)i] = 0;
+    n_samples[sid] = 0;
+#pragma unroll
+    for (int m = 0; m < PB_MAX_MODELS; ++m)
+        if (t.trig[m]) t.trig[m][sid] = 0;
 }
 
 PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream) {
@@ -1181,12 +1253,10 @@ PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream)
     if (n < 0 || n > h->cfg.max_streams) return fail(PB_ERR_INVALID, "bad n");
     if (n == 0) return PB_OK;
     CK(cudaSetDevice(h->cfg.device));
-    clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->st, d_ids, n);
+    TrigArrays t{};
+    for (size_t m = 0; m < h->models.size(); ++m) t.trig[m] = h->models[m].trig.get();
+    clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->d_n_samples.get(), t, d_ids, n);
     CK(cudaGetLastError());
-    for (pb_handle* m : h->bank) {                             // the other models of the bank: their trigger counters
-        clear_trig_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(m->st.trig, d_ids, n);
-        CK(cudaGetLastError());
-    }
     return PB_OK;
 }
 
@@ -1208,11 +1278,11 @@ static int ensure_pipe(pb_handle* h) {
     for (int i = 0; i < HOST_PIPE; ++i) {
         CK(cudaStreamCreateWithFlags(&h->pipe[i], cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&h->pipe_ev[i], cudaEventDisableTiming));
-        CK(cudaMalloc((void**)&h->d_stage_pcm[i], sb * h->cfg.chunk_samples * sizeof(int16_t)));
-        CK(cudaMalloc((void**)&h->d_stage_ids[i], sb * sizeof(int)));
-        CK(cudaMalloc((void**)&h->d_stage_raw[i], sb * sizeof(float)));
-        CK(cudaMalloc((void**)&h->d_stage_conf[i], sb * sizeof(double)));
-        CK(cudaMalloc((void**)&h->d_stage_fired[i], sb * sizeof(uint8_t)));
+        CK(h->d_stage_pcm[i].alloc(sb * h->cfg.chunk_samples));
+        CK(h->d_stage_ids[i].alloc(sb));
+        CK(h->d_stage_raw[i].alloc(sb));
+        CK(h->d_stage_conf[i].alloc(sb));
+        CK(h->d_stage_fired[i].alloc(sb));
     }
     CK(cudaHostAlloc((void**)&h->h_count_pinned, sizeof(unsigned long long), cudaHostAllocDefault));
     return PB_OK;
@@ -1228,7 +1298,7 @@ PB_API int pb_update_host(pb_handle* h, const int16_t* h_pcm, const int32_t* h_i
     int rc = check_tick(h, h_pcm, n);
     if (rc != PB_OK) return rc;
     if (n == 0) { if (h_count) *h_count = 0; return PB_OK; }
-    if (!h->have_weights) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
     if (!h_conf) return fail(PB_ERR_INVALID, "null h_conf");
     CK(cudaSetDevice(h->cfg.device));
     rc = ensure_pipe(h);
@@ -1256,7 +1326,8 @@ PB_API int pb_update_host(pb_handle* h, const int16_t* h_pcm, const int32_t* h_i
     }
     // the counter is zeroed on pipe 0; the other pipes wait for that, pipe 0 waits for them at the end,
     // so the whole tick costs one host synchronisation
-    CK(cudaMemsetAsync(h->d_count, 0, sizeof(unsigned long long), h->pipe[0]));
+    unsigned long long* d_count = h->d_count.get();
+    CK(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), h->pipe[0]));
     // equal sub-batches: nothing overlaps the first sub-batch's upload (pipeline fill) or the last one's kernels and download
     // (drain), and for a given number of sub-batches the largest one is smallest when all are equal (16 400 streams: 8 224 +
     // 8 176 rather than 16 384 + 16); step <= sb, a multiple of 32 except when one sub-batch takes everything
@@ -1271,21 +1342,25 @@ PB_API int pb_update_host(pb_handle* h, const int16_t* h_pcm, const int32_t* h_i
     for (int64_t off = 0; off < n; off += step, p = (p + 1) % HOST_PIPE) {
         const int64_t m = std::min(step, n - off);
         cudaStream_t s = h->pipe[p];
-        CK(cudaMemcpyAsync(h->d_stage_pcm[p], h_pcm + off * chunk, m * chunk * sizeof(int16_t), cudaMemcpyHostToDevice, s));
-        if (h_ids) CK(cudaMemcpyAsync(h->d_stage_ids[p], h_ids + off, m * sizeof(int), cudaMemcpyHostToDevice, s));
-        else { iota_kernel<<<(int)((m + 255) / 256), 256, 0, s>>>(h->d_stage_ids[p], (int)off, (int)m); CK(cudaGetLastError()); }
-        rc = pb_update(h, h->d_stage_pcm[p], h->d_stage_ids[p], m, h_raw ? h->d_stage_raw[p] : nullptr, h->d_stage_conf[p],
-                       h_fired ? h->d_stage_fired[p] : nullptr, h->d_count, s);
+        int16_t* pcm = h->d_stage_pcm[p].get();
+        int* ids = h->d_stage_ids[p].get();
+        float* raw = h->d_stage_raw[p].get();
+        double* conf = h->d_stage_conf[p].get();
+        uint8_t* fired = h->d_stage_fired[p].get();
+        CK(cudaMemcpyAsync(pcm, h_pcm + off * chunk, m * chunk * sizeof(int16_t), cudaMemcpyHostToDevice, s));
+        if (h_ids) CK(cudaMemcpyAsync(ids, h_ids + off, m * sizeof(int), cudaMemcpyHostToDevice, s));
+        else { iota_kernel<<<(int)((m + 255) / 256), 256, 0, s>>>(ids, (int)off, (int)m); CK(cudaGetLastError()); }
+        rc = pb_update(h, pcm, ids, m, h_raw ? raw : nullptr, conf, h_fired ? fired : nullptr, d_count, s);
         if (rc != PB_OK) return rc;
-        CK(cudaMemcpyAsync(h_conf + off, h->d_stage_conf[p], m * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (h_raw) CK(cudaMemcpyAsync(h_raw + off, h->d_stage_raw[p], m * sizeof(float), cudaMemcpyDeviceToHost, s));
-        if (h_fired) CK(cudaMemcpyAsync(h_fired + off, h->d_stage_fired[p], m * sizeof(uint8_t), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(h_conf + off, conf, m * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (h_raw) CK(cudaMemcpyAsync(h_raw + off, raw, m * sizeof(float), cudaMemcpyDeviceToHost, s));
+        if (h_fired) CK(cudaMemcpyAsync(h_fired + off, fired, m * sizeof(uint8_t), cudaMemcpyDeviceToHost, s));
     }
     for (int i = 1; i < used_pipes; ++i) {
         CK(cudaEventRecord(h->pipe_ev[i], h->pipe[i]));
         CK(cudaStreamWaitEvent(h->pipe[0], h->pipe_ev[i], 0));
     }
-    CK(cudaMemcpyAsync(h->h_count_pinned, h->d_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->pipe[0]));
+    CK(cudaMemcpyAsync(h->h_count_pinned, d_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->pipe[0]));
     CK(cudaStreamSynchronize(h->pipe[0]));
     if (h_count) *h_count = *h->h_count_pinned;
     return PB_OK;

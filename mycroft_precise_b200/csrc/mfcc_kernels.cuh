@@ -270,7 +270,6 @@ struct StreamState {
     long long* n_samples;     // [max_streams] samples consumed so far
     int16_t* tail;            // [max_streams][tail_cap] unconsumed samples a later frame still needs
     float* ring;              // [max_streams][ring_rows][row_stride] MFCC rows, slot = frame index % ring_rows
-    int* trig;                // [max_streams] TriggerDetector.activation
     int tail_cap, ring_rows, row_stride;
 };
 
