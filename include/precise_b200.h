@@ -176,6 +176,28 @@ int pb_num_models(const pb_handle* h);
 int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, int64_t n,
                      float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_count, void* stream);
 
+/* Ragged tick: the pb_update_models tick, but stream i brings its own number of samples, as Listener.update takes a chunk of
+ * any length (network_runner.py:125-153).  For every stream and bank model: Listener.update(chunk) then TriggerDetector.update.
+ *   d_pcm        packed int16 samples; item i's chunk is d_pcm[d_offsets[i] .. d_offsets[i+1])
+ *   d_offsets    [n+1] int64, DEVICE, non-decreasing; any alignment (odd offsets allowed); d_pcm holds at least
+ *                d_offsets[n] samples
+ *   max_len      host-side upper bound on every d_offsets[i+1] - d_offsets[i] (>= 1)
+ *   d_stream_ids as pb_update; outputs model-major as pb_update_models ([M][n], d_count [M]).  A one-model handle scores
+ *                as pb_update does ([1][n] is its layout), a bank as pb_update_models does.
+ * Every length must lie in [1, max_len].  The kernels clamp lengths to [0, max_len] and never read outside
+ * [d_pcm + d_offsets[0], d_pcm + d_offsets[n]), so a caller's mistake gives wrong answers for that stream, never an
+ * out-of-bounds access.  A chunk may complete any number of MFCC frames (long chunks run as several MFCC launches).
+ * TriggerDetector's refractory count still uses the handle's chunk_samples: the reference fixes chunk_size when it builds the
+ * detector (runner/precise_runner/runner.py:121, :140), whatever the lengths of later reads.
+ * After a handle's first ragged tick, its uniform ticks (pb_update, pb_update_models, pb_update_vectors, pb_update_host) run
+ * the ragged tick's MFCC kernel too (a stream's sample count is then no longer a multiple of 8), and pb_debug_k1_mode accepts
+ * only 0.
+ * PB_ERR_INVALID: null handle, d_offsets or d_conf, n outside [0, max_streams], max_len < 1.  PB_ERR_STATE: slot 0 has no
+ * weights, or pb_debug_k1_mode is non-zero. */
+int pb_update_ragged(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len,
+                     const int32_t* d_stream_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
+                     unsigned long long* d_count, void* stream);
+
 /* Listener.update_vectors only (network_runner.py:125-146): advance stream state, no network. */
 int pb_update_vectors(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream_ids, int64_t n,
                       void* stream);

@@ -20,7 +20,7 @@ class StreamBatch:
         self.core.load_weights(model.kernel, model.recurrent, model.bias, model.dense_w, model.dense_b)
         torch = self.core.torch
         self.count = torch.zeros(1, dtype=torch.int64, device=self.core.device)
-        self.counts = torch.zeros(1, dtype=torch.int64, device=self.core.device)    # per bank model, update_models only
+        self.counts = torch.zeros(1, dtype=torch.int64, device=self.core.device)    # per bank model, update_models / update_ragged
         self._out = None
         self._bank_out = None
 
@@ -33,17 +33,27 @@ class StreamBatch:
         self._bank_out = None
         return slot
 
-    def update_models(self, pcm, ids=None):
-        """One tick for every bank model: pcm int16 CUDA [n, chunk_samples] -> dict(raw f32, conf f64, fired u8), each
-        [M, n].  ``self.counts`` (int64[M], device) accumulates each model's fired streams until reset_count()."""
-        n, M = pcm.shape[0], self.core.num_models
+    def _bank_buffers(self, n):
+        """The cached [M, n] outputs of a bank tick."""
+        M = self.core.num_models
         if self._bank_out is None or tuple(self._bank_out['conf'].shape) != (M, n):
             torch = self.core.torch
             dev = self.core.device
             self._bank_out = dict(raw=torch.empty((M, n), dtype=torch.float32, device=dev),
                                   conf=torch.empty((M, n), dtype=torch.float64, device=dev),
                                   fired=torch.empty((M, n), dtype=torch.uint8, device=dev))
-        return self.core.update_models(pcm, ids, self._bank_out, self.counts)
+        return self._bank_out
+
+    def update_models(self, pcm, ids=None):
+        """One tick for every bank model: pcm int16 CUDA [n, chunk_samples] -> dict(raw f32, conf f64, fired u8), each
+        [M, n].  ``self.counts`` (int64[M], device) accumulates each model's fired streams until reset_count()."""
+        return self.core.update_models(pcm, ids, self._bank_buffers(pcm.shape[0]), self.counts)
+
+    def update_ragged(self, pcm, offsets, ids=None, max_len=None):
+        """Ragged tick for every bank model: stream item i brings pcm[offsets[i]:offsets[i + 1]] (1-D int16 CUDA pcm, int64
+        CUDA offsets [n + 1]) -> dict(raw, conf, fired), each [M, n], accumulating ``self.counts``.  See
+        PreciseB200.update_ragged."""
+        return self.core.update_ragged(pcm, offsets, ids, max_len, self._bank_buffers(offsets.numel() - 1), self.counts)
 
     def update(self, pcm, ids=None):
         """pcm: int16 CUDA tensor [n, chunk_samples] -> dict(raw f32[n], conf f64[n], fired u8[n]).

@@ -56,6 +56,7 @@ SYMBOLS = {
     'pb_add_model': (C.c_int, [_VP, C.POINTER(pb_config), _VP, _VP, _VP, _VP, C.c_float, _VP, _I64, C.POINTER(_I32)]),
     'pb_num_models': (C.c_int, [_VP]),
     'pb_update_models': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
+    'pb_update_ragged': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
     'pb_update_vectors': (C.c_int, [_VP, _VP, _VP, _I64, _VP]),
     'pb_update_host': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP]),
     'pb_read_window': (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
@@ -389,6 +390,50 @@ class PreciseB200:
                        fired=torch.empty((M, n), dtype=torch.uint8, device=self.device))
         check(self.lib.pb_update_models(self._h, _ptr(pcm), _ptr(ids), n, _ptr(out.get('raw')), _ptr(out['conf']),
                                         _ptr(out.get('fired')), _ptr(counts), self._stream()))
+        return out
+
+    def update_ragged(self, pcm, offsets, ids=None, max_len=None, out=None, counts=None):
+        """Ragged bank tick: stream item i brings pcm[offsets[i]:offsets[i + 1]] (any length >= 1, any alignment) this tick.
+        pcm is a 1-D int16 CUDA tensor, offsets an int64 CUDA tensor [n + 1].  ``max_len`` bounds every length (None: computed
+        here, one device sync).  Returns dict(raw f32, conf f64, fired u8), each [M, n], as update_models; ``counts`` (int64
+        [M]) accumulates.  With check_ids, offsets must also be non-decreasing, within pcm, with every length in [1, max_len]."""
+        torch = self.torch
+        if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
+                or pcm.device != self.device):
+            raise ValueError('pcm must be a contiguous 1-D int16 tensor on %s' % self.device)
+        if (not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1
+                or not offsets.is_contiguous() or offsets.device != self.device):
+            raise ValueError('offsets must be a contiguous 1-D int64 [n + 1] tensor on %s' % self.device)
+        n = offsets.numel() - 1
+        if n > self.max_streams:
+            raise ValueError('n = %d exceeds max_streams = %d' % (n, self.max_streams))
+        self._check_ids(ids, n)
+        lens = offsets[1:] - offsets[:-1]
+        if max_len is None:
+            max_len = max(1, int(lens.max())) if n else 1
+        max_len = int(max_len)
+        if max_len < 1:
+            raise ValueError('max_len must be >= 1, got %d' % max_len)
+        if self.check_ids and n:
+            lo, hi = int(lens.min()), int(lens.max())
+            if lo < 1 or hi > max_len:
+                raise ValueError('chunk lengths must lie in [1, max_len = %d], got [%d, %d] (offsets must be non-decreasing)'
+                                 % (max_len, lo, hi))
+            first, last = int(offsets[0]), int(offsets[-1])
+            if first < 0 or last > pcm.numel():
+                raise ValueError('offsets [%d, %d] outside pcm of %d samples' % (first, last, pcm.numel()))
+        M = self.num_models
+        if out is not None:
+            self._check_t("out['raw']", out.get('raw'), torch.float32, M * n)
+            self._check_t("out['conf']", out.get('conf'), torch.float64, M * n, optional=False)
+            self._check_t("out['fired']", out.get('fired'), torch.uint8, M * n)
+        self._check_t('counts', counts, torch.int64, M)
+        if out is None:
+            out = dict(raw=torch.empty((M, n), dtype=torch.float32, device=self.device),
+                       conf=torch.empty((M, n), dtype=torch.float64, device=self.device),
+                       fired=torch.empty((M, n), dtype=torch.uint8, device=self.device))
+        check(self.lib.pb_update_ragged(self._h, _ptr(pcm), _ptr(offsets), max_len, _ptr(ids), n, _ptr(out.get('raw')),
+                                        _ptr(out['conf']), _ptr(out.get('fired')), _ptr(counts), self._stream()))
         return out
 
     def update_vectors(self, pcm, ids=None):

@@ -24,6 +24,7 @@
 #include "gru_wide.cuh"
 #include "mfcc_kernels.cuh"
 #include "mfcc_fast.cuh"
+#include "mfcc_ragged.cuh"
 #include "mfcc_tc.cuh"
 #include "mfcc_tc3.cuh"
 #include "mfcc_mma.cuh"
@@ -134,7 +135,9 @@ struct pb_handle {
     // derived
     int used = 0, n_bins = 0, n_out = 0, feat = 0, ring_rows = 0, row_stride = 0, tail_cap = 0, max_new = 0;
     int rel_window = 0;              // samples before frame 0 is released: window_samples (sonopy), window_samples + hop_samples (speechpy drops the last complete frame)
-    size_t k1_batch_smem = 0, k1_stream_smem = 0, k1_fast_smem = 0;
+    size_t k1_batch_smem = 0, k1_stream_smem = 0, k1_fast_smem = 0, k1_ragged_smem = 0;
+    bool ragged = false;             // set by the first pb_update_ragged: n_samples may no longer be a multiple of 8, so every later tick's
+                                     // K1 runs launch_ragged_mfcc (the aligned-only kernels would mis-stage it)
     bool force_generic = false;      // tests: exercise the generic kernels on the aligned geometry
     int k1_mode = 0;                 // 0 = default (the FFT kernel with 32-bit set-up where the geometry allows it), 2 = always the FFT kernel, 3 = FFT kernel with the original 64-bit set-up, 4 / 5 / 6 = the mma.sync DFT tick (mfcc_mma.cuh): stage 1 on the CUDA cores / on the tensor cores / the latter with a shuffle epilogue
     bool mma_ok = false;             // geometry mfcc_mma_kernel covers (n_fft = frame = 512, hop >= 512, chunk >= hop, MFCC vectorizer)
@@ -433,8 +436,10 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     h->fast_ok = c.n_fft == 512 && h->used == 512 && c.hop_samples % 8 == 0 && n_pieces <= 64 && h->npl <= 4;
     h->mma_ok = h->fast_ok && c.vectorizer == PB_VEC_MFCCS && c.n_filt <= MM_MAX_FILT && h->n_out <= MM_MAX_FILT && !c.use_delta &&
                 c.chunk_samples % 8 == 0 && c.hop_samples >= 512 && c.chunk_samples >= c.hop_samples && c.chunk_samples <= 32760;
-    h->k1_fast_smem = K1F_WARPS * sizeof(K1FWarp) + (size_t)h->npl * 128 * sizeof(float4) +
-                      (size_t)c.n_filt * 16 * h->nol * sizeof(float) + (((size_t)c.n_filt * h->maxc + 15) & ~(size_t)15);
+    const size_t k1_fast_tables = (size_t)h->npl * 128 * sizeof(float4) + (size_t)c.n_filt * 16 * h->nol * sizeof(float) +
+                                  (((size_t)c.n_filt * h->maxc + 15) & ~(size_t)15);
+    h->k1_fast_smem = K1F_WARPS * sizeof(K1FWarp) + k1_fast_tables;
+    h->k1_ragged_smem = K1F_WARPS * sizeof(K1RWarp) + k1_fast_tables;
     // DCT-II, norm='ortho' (scipy.fftpack.dct as sonopy.mfcc_spec calls it), first n_out rows
     std::vector<float> dct((size_t)h->n_out * c.n_filt);
     for (int k = 0; k < h->n_out; ++k)
@@ -492,6 +497,8 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     CK(ensure_dyn_smem(mfcc_fast_stream_kernel<true>, (size_t)(h->k1_fast_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<true>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<false>, (size_t)(h->k1_stream_smem)));
+    CK(ensure_dyn_smem(mfcc_stream_kernel<false, true>, (size_t)(h->k1_stream_smem)));
+    CK(ensure_dyn_smem(mfcc_ragged_stream_kernel, (size_t)(h->k1_ragged_smem)));
 
     Network net;                     // slot 0: weights come with pb_load_weights
     net.cfg = c;
@@ -717,6 +724,7 @@ PB_API int pb_debug_gru_mode(pb_handle* h, int mode) {
 PB_API int pb_debug_k1_mode(pb_handle* h, int mode) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (mode < 0 || mode > 6 || mode == 1) return fail(PB_ERR_INVALID, "k1 mode must be 0 (automatic), 2 (FFT kernel, lean set-up), 3 (FFT kernel), 4 (tensor-core DFT stage 2), 5 (both DFT stages on the tensor cores) or 6 (5 with a shuffle epilogue)");
+    if (mode != 0 && h->ragged) return fail(PB_ERR_STATE, "k1 modes 2-6 need 16-byte-aligned stream state, which a handle loses with its first pb_update_ragged");
     if (mode >= 4 && !h->mma_ok) return fail(PB_ERR_UNSUPPORTED, "the tensor-core MFCC tick needs n_fft = 512 = frame length, hop >= 512 (a multiple of 8), chunk >= hop (a multiple of 8), n_filt <= 32, MFCC vectorizer");
     if ((mode == 2 || mode == 3) && !h->fast_ok) return fail(PB_ERR_UNSUPPORTED, "k1 mode 2 needs the aligned geometry of the fast MFCC kernels");
     h->k1_mode = mode;
@@ -1026,7 +1034,41 @@ static int ensure_mma_tables(pb_handle* h) {
     return PB_OK;
 }
 
+// K1 of a ragged tick: item i's chunk is d_pcm[d_offsets[i] .. d_offsets[i + 1]) (d_offsets null: the uniform tick's
+// d_pcm[i * chunk_samples ..), max_len = chunk_samples), lengths clamped to [0, max_len].  The tick runs as rounds of at most 6 hops
+// per stream, so no stream completes more than 8 frames in one launch; to the state machine the rounds are separate ticks
+// (Listener.update_vectors is chunking-independent).  Any alignment of offsets, lengths and sample counts.
+static int launch_ragged_mfcc(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len, const int32_t* d_ids,
+                              int64_t n, cudaStream_t s) {
+    const float inv = 1.0f / 32768.0f, scale = inv * inv / (float)h->cfg.n_fft;
+    const StreamState st = stream_state(h);
+    RaggedIn rg;
+    rg.offsets = reinterpret_cast<const long long*>(d_offsets);
+    rg.max_len = max_len;
+    rg.chunk = h->cfg.chunk_samples;
+    rg.sub = 6 * h->cfg.hop_samples;
+    const bool fast = h->fast_ok && !h->force_generic;
+    const int64_t warps_total = (int64_t)h->sm_count * 4 * K1F_WARPS;
+    const int spw = (int)std::max<int64_t>(1, std::min<int64_t>(K1F_STREAMS_PER_WARP, (n + warps_total - 1) / warps_total));
+    const int64_t tilesf = (n + spw - 1) / spw;
+    const int gridf = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
+    const int grid = (int)std::min<int64_t>((n + K1_STREAMS_PER_CTA - 1) / K1_STREAMS_PER_CTA, (int64_t)h->sm_count * 4);
+    ProfScope ps(h, 0, s);
+    for (int64_t off = 0; off < max_len; off += rg.sub) {
+        rg.round_off = off;
+        if (fast)
+            mfcc_ragged_stream_kernel<<<gridf, K1F_THREADS, h->k1_ragged_smem, s>>>(d_pcm, rg, d_ids, (int)n, h->cfg.hop_samples, spw, scale,
+                                                                                   mel_tables(h), fast_tables(h), st);
+        else
+            mfcc_stream_kernel<false, true><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, 0, 0, h->cfg.hop_samples, h->used,
+                                                                                       scale, mel_tables(h), st, rg);
+        CK(cudaGetLastError());
+    }
+    return PB_OK;
+}
+
 static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, cudaStream_t s) {
+    if (h->ragged) return launch_ragged_mfcc(h, d_pcm, nullptr, h->cfg.chunk_samples, d_ids, n, s);
     const bool pairs = (h->cfg.chunk_samples % 2 == 0) && (h->cfg.hop_samples % 2 == 0) && (h->used % 2 == 0) &&
                        ((uintptr_t)d_pcm % 4 == 0);
     const int64_t tiles = (n + K1_STREAMS_PER_CTA - 1) / K1_STREAMS_PER_CTA;
@@ -1073,11 +1115,11 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
         const int sub = std::max(1, 6 * h->cfg.hop_samples);
         for (int off = 0; off < h->cfg.chunk_samples; off += sub)
             mfcc_stream_kernel<false><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm + off, d_ids, (int)n, std::min(sub, h->cfg.chunk_samples - off),
-                                                                                    h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st);
+                                                                                    h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st, RaggedIn{});
     } else if (pairs)
-        mfcc_stream_kernel<true><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st);
+        mfcc_stream_kernel<true><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st, RaggedIn{});
     else
-        mfcc_stream_kernel<false><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st);
+        mfcc_stream_kernel<false><<<grid, K1_THREADS, h->k1_stream_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.chunk_samples, h->cfg.hop_samples, h->used, scale, mel_tables(h), st, RaggedIn{});
     CK(cudaGetLastError());
     return PB_OK;
 }
@@ -1098,6 +1140,15 @@ static K2In stream_k2in(const pb_handle* h, const int32_t* d_ids) {
     return in;
 }
 
+// The network half of pb_update: slot 0 scores the windows of the n streams (its warp-per-stream kernel up to 8 192 streams).
+static int score_model0(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
+                        unsigned long long* d_count, cudaStream_t s) {
+    const Network& net = h->models[0];
+    K2Out o{};
+    o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = net.trig.get();
+    return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
+}
+
 PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
               uint8_t* d_fired, unsigned long long* d_count, void* stream) {
     int rc = check_tick(h, d_pcm, n);
@@ -1109,9 +1160,7 @@ PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, i
     cudaStream_t s = (cudaStream_t)stream;
     rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
-    K2Out o{};
-    o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = net.trig.get();
-    return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
+    return score_model0(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1168,18 +1217,12 @@ static int launch_bank(const BankParams& P, int nm, const K2In& in, int64_t n, c
     return fail(PB_ERR_INVALID, "%d fused models", nm);
 }
 
-PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
-                            uint8_t* d_fired, unsigned long long* d_count, void* stream) {
-    int rc = check_tick(h, d_pcm, n);
-    if (rc != PB_OK) return rc;
-    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
-    if (n == 0) return PB_OK;
-    if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
-    CK(cudaSetDevice(h->cfg.device));
-    cudaStream_t s = (cudaStream_t)stream;
+// The network half of a bank tick (pb_update_models, pb_update_ragged): every model scores the windows of the n streams, outputs
+// model-major.
+static int score_bank(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
+                      unsigned long long* d_count, cudaStream_t s) {
+    int rc = PB_OK;
     const int M = (int)h->models.size();
-    rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
-    if (rc != PB_OK) return rc;
     const K2In in = stream_k2in(h, d_ids);
     ProfScope ps(h, 1, s);
     // the fused family in one gru_bank_kernel launch; other networks one launch each of their own kernel, on the same ring
@@ -1201,6 +1244,41 @@ PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d
         }
     }
     return nm ? launch_bank(P, nm, in, n, s) : PB_OK;
+}
+
+PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
+                            uint8_t* d_fired, unsigned long long* d_count, void* stream) {
+    int rc = check_tick(h, d_pcm, n);
+    if (rc != PB_OK) return rc;
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (n == 0) return PB_OK;
+    if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
+    if (rc != PB_OK) return rc;
+    return score_bank(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
+}
+
+PB_API int pb_update_ragged(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len, const int32_t* d_ids,
+                            int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_count, void* stream) {
+    int rc = check_tick(h, d_pcm, n);
+    if (rc != PB_OK) return rc;
+    if (!d_offsets) return fail(PB_ERR_INVALID, "null d_offsets");
+    if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
+    if (max_len < 1) return fail(PB_ERR_INVALID, "max_len = %lld must be >= 1", (long long)max_len);
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (h->k1_mode != 0) return fail(PB_ERR_STATE, "ragged ticks run only with k1 mode 0");
+    if (n == 0) return PB_OK;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    h->ragged = true;
+    rc = launch_ragged_mfcc(h, d_pcm, d_offsets, max_len, d_ids, n, s);
+    if (rc != PB_OK) return rc;
+    // one model: pb_update's network path, so a ragged tick of uniform chunks equals pb_update bit for bit; a bank:
+    // pb_update_models's
+    if (h->models.size() == 1) return score_model0(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
+    return score_bank(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {

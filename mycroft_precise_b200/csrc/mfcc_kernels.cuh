@@ -277,6 +277,34 @@ __host__ __device__ __forceinline__ long long frames_ready(long long n, int need
     return n >= need ? (n - need) / hop + 1 : 0;
 }
 
+// Ragged tick (pb_update_ragged): where item i's samples of one launch lie.  The host runs a tick as rounds of at most `sub`
+// samples per stream (<= 6 hops, so no stream completes more than 8 frames per launch); round r starts at round_off = r * sub.
+struct RaggedIn {
+    const long long* offsets;  // [n + 1]: item i's chunk is pcm[offsets[i] .. offsets[i + 1]); null: pcm[i * chunk .. (i + 1) * chunk)
+    long long max_len;         // chunk lengths are clamped to [0, max_len]
+    long long round_off;
+    int chunk;                 // uniform chunk length (offsets null)
+    int sub;
+};
+
+// Item i's part of this launch: pcm[src .. src + len).  Offsets are clamped so that nothing outside
+// [pcm + offsets[0], pcm + offsets[n]) is ever read, whatever the caller passed.
+__device__ __forceinline__ void ragged_chunk(const RaggedIn& r, int i, int n, long long& src, int& len) {
+    long long b, L;
+    if (r.offsets) {
+        const long long lo = __ldg(r.offsets), hi = max(lo, __ldg(r.offsets + n));
+        b = min(max(__ldg(r.offsets + i), lo), hi);
+        const long long e = min(max(__ldg(r.offsets + i + 1), b), hi);
+        L = min(e - b, r.max_len);
+    } else {
+        b = (long long)i * r.chunk;
+        L = r.chunk;
+    }
+    L = min(max(L - r.round_off, 0ll), (long long)r.sub);
+    src = b + r.round_off;
+    len = (int)L;
+}
+
 struct K1StreamSmem {
     K1Smem k1;
     // frame work list for this tile
@@ -288,15 +316,20 @@ struct K1StreamSmem {
     long long st_n0[K1_STREAMS_PER_CTA];
     long long st_ts0[K1_STREAMS_PER_CTA];
     long long st_c0[K1_STREAMS_PER_CTA];
+    long long st_src[K1_STREAMS_PER_CTA];        // RAGGED: first sample of the stream's part of this launch, in pcm
+    int st_len[K1_STREAMS_PER_CTA];              // RAGGED: its length
 };
 
 // One tick: stream ids[i] (or i) receives pcm[i * pcm_stride + 0 .. chunk).  A stream completes at most 8 frames per launch: the
 // host feeds longer chunks as consecutive sub-chunks of the same rows (pcm_stride = the full chunk length), which the state machine
 // cannot tell from separate ticks (Listener.update_vectors is chunking-independent).
-template <bool PAIRS>
+// RAGGED: stream ids[i] receives its own part of the launch instead, pcm[src .. src + len) from ragged_chunk(rg, i) (chunk and
+// pcm_stride are unused); any alignment, so only with PAIRS = false.
+template <bool PAIRS, bool RAGGED = false>
 __global__ void __launch_bounds__(K1_THREADS, 4)
 mfcc_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids, int n, int chunk, int pcm_stride,
-                   int hop, int used, float scale, MelTables tab, StreamState st) {
+                   int hop, int used, float scale, MelTables tab, StreamState st, RaggedIn rg) {
+    static_assert(!(PAIRS && RAGGED), "ragged chunks have any alignment");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     K1StreamSmem& sm = *reinterpret_cast<K1StreamSmem*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, l16 = lane & 15, half = lane >> 4;
@@ -321,7 +354,13 @@ mfcc_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids,
                 sid = ids ? ids[i] : i;
                 n0 = st.n_samples[sid];
                 c0 = frames_ready(n0, used, hop);
-                cnt = (int)(frames_ready(n0 + chunk, used, hop) - c0);
+                int len = chunk;
+                if (RAGGED) {
+                    long long src;
+                    ragged_chunk(rg, i, n, src, len);
+                    sm.st_src[lane] = src; sm.st_len[lane] = len;
+                }
+                cnt = (int)(frames_ready(n0 + len, used, hop) - c0);
                 ts0 = c0 * hop < n0 ? c0 * hop : n0;        // first absolute sample held in the tail
             }
             sm.st_id[lane] = sid; sm.st_n0[lane] = n0; sm.st_ts0[lane] = ts0; sm.st_cnt[lane] = cnt; sm.st_c0[lane] = c0;
@@ -342,7 +381,7 @@ mfcc_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids,
                 for (int slot = warp; slot < nr; slot += K1_WARPS) {               // generic n_fft: one frame per warp at a time
                     const int t = sm.fr_stream[r0 + slot];
                     const long long a0 = (sm.st_c0[t] + sm.fr_sub[r0 + slot]) * hop, n0 = sm.st_n0[t];
-                    const int16_t* chunk_p = pcm + (long long)(base + t) * pcm_stride;
+                    const int16_t* chunk_p = pcm + (RAGGED ? sm.st_src[t] : (long long)(base + t) * pcm_stride);
                     FrameSrc<int16_t> src;
                     src.used = used;
                     if (a0 >= n0) { src.len0 = 0; src.p0 = chunk_p; src.p1 = chunk_p + (a0 - n0); }
@@ -363,7 +402,7 @@ mfcc_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids,
                     const int t = sm.fr_stream[r0 + slot];
                     const long long a0 = (sm.st_c0[t] + sm.fr_sub[r0 + slot]) * hop;     // absolute first sample
                     const long long n0 = sm.st_n0[t];
-                    const int16_t* chunk_p = pcm + (long long)(base + t) * pcm_stride;
+                    const int16_t* chunk_p = pcm + (RAGGED ? sm.st_src[t] : (long long)(base + t) * pcm_stride);
                     FrameSrc<int16_t> src;
                     src.used = used;
                     if (a0 >= n0) { src.len0 = 0; src.p0 = chunk_p; src.p1 = chunk_p + (a0 - n0); }
@@ -394,13 +433,13 @@ mfcc_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids,
         for (int t = warp; t < K1_STREAMS_PER_CTA; t += K1_WARPS) {
             const int sid = sm.st_id[t];
             if (sid < 0) continue;
-            const long long n0 = sm.st_n0[t], n1 = n0 + chunk, ts0 = sm.st_ts0[t];
+            const long long n0 = sm.st_n0[t], n1 = n0 + (RAGGED ? sm.st_len[t] : chunk), ts0 = sm.st_ts0[t];
             const long long c1 = sm.st_c0[t] + sm.st_cnt[t];
             const long long ts1 = c1 * hop < n1 ? c1 * hop : n1;
             const int len1 = (int)(n1 - ts1);
             const int n_old = ts1 < n0 ? (int)(n0 - ts1) : 0;       // part that comes from the old tail
             int16_t* tl = st.tail + (long long)sid * st.tail_cap;
-            const int16_t* chunk_p = pcm + (long long)(base + t) * pcm_stride;
+            const int16_t* chunk_p = pcm + (RAGGED ? sm.st_src[t] : (long long)(base + t) * pcm_stride);
             if (n_old > 0) {
                 int16_t keep[64];                                    // tail_cap <= 2048 = 64 * 32
                 const int off = (int)(ts1 - ts0);
