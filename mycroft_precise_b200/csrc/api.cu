@@ -929,14 +929,24 @@ static void set_bank_slot(BankParams& P, int slot, const Network& net, const K2O
     P.o[slot] = o;
 }
 
-template <int NM, bool RING>
-static int launch_bank_nm(const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
-    constexpr size_t smem = (size_t)NM * BANK_MODEL_SMEM;
-    if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(gru_bank_kernel<NM, RING>, smem));      // above the default limit
+template <int NM, bool RING, bool KERAS_ACT>
+static int launch_bank_act(const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
+    constexpr size_t smem = (size_t)NM * BANK_MODEL_SMEM + (bank_stages(NM, RING) ? BANK_STAGE_SMEM : 0);
+    if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(gru_bank_kernel<NM, RING, KERAS_ACT>, smem));      // above the default limit
     const int per_cta = (MMA_THREADS / 32) * 16;
-    gru_bank_kernel<NM, RING><<<(int)((n + per_cta - 1) / per_cta), MMA_THREADS, smem, s>>>(P, in, n);
+    gru_bank_kernel<NM, RING, KERAS_ACT><<<(int)((n + per_cta - 1) / per_cta), MMA_THREADS, smem, s>>>(P, in, n);
     CK(cudaGetLastError());
     return PB_OK;
+}
+
+// One model with Keras's GRU defaults (the networks Precise trains) runs with its activation pair compiled in.  Banks keep
+// the run-time dispatch: with compiled-in activations ptxas interleaves the models' chains and needs up to 255 registers,
+// spilling from NM = 4 on.
+template <int NM, bool RING>
+static int launch_bank_nm(const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
+    if constexpr (NM == 1)
+        if (P.w[0].act == PB_ACT_LINEAR && P.w[0].ract == PB_RACT_HARD_SIGMOID) return launch_bank_act<1, RING, true>(P, in, n, s);
+    return launch_bank_act<NM, RING, false>(P, in, n, s);
 }
 
 // Scores network net (which has weights; F = the front end's feature size) with its decoder into o.

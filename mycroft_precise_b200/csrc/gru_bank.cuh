@@ -8,7 +8,7 @@
 // its accumulators = the (2t, 2t + 1) and (2t + 8, 2t + 9) k pairs of the A fragment), so h turns into the next step's A
 // operand with two F2FP packs per n-tile and no data movement.
 //
-// A warp owns a 16-stream tile.  At each of the T steps it loads the tile's MFCC rows once, splits them into fp16 hi / lo A
+// A warp owns a 16-stream tile.  At each of the T steps it reads the tile's MFCC rows once, splits them into fp16 hi / lo A
 // fragments once, and then runs, model after model, the x.W products (one k16 MMA per n-tile and pass) and the h.U products
 // (mma3_f16).  Each model's h stays in registers, so the M models give the warp M independent dependency chains per step
 // while the window's rows are read once per tick for all of them.  Per model the accumulation order is bias, x part, h part.
@@ -82,8 +82,46 @@ struct BankParams {
     K2Out o[BANK_MAX_MODELS];        // each model's outputs, trigger array and count slot
 };
 
-// RING: rows from the stream ring (a tick); otherwise from in.inputs, [n][T][F_base] contiguous (pb_predict).
-template <int NM, bool RING>
+// Ring rows are staged per warp through shared memory, BANK_STAGE_STEPS steps at a time, two buffers: while the warp scans
+// the steps of one buffer, 16-byte cp.async copies fill the other with the tile's rows of the next steps.  A lane pair owns one
+// stream of the tile and copies its rows (32 B per lane pair and copy, 256 B per stream and buffer); zero rows (before a
+// young stream's first frame, padding streams past n) are zero-filled by the copy itself (src-size 0).
+constexpr int BANK_STAGE_STEPS = 4;
+constexpr int BANK_STAGE_ROW = 16;                                   // floats per staged row: feature_size <= 16
+constexpr int BANK_STAGE_BUF = BANK_STAGE_STEPS * 16 * BANK_STAGE_ROW;                   // floats: [step][stream][feature]
+constexpr int BANK_STAGE_SMEM = (MMA_THREADS / 32) * 2 * BANK_STAGE_BUF * 4;             // 32 768 B per CTA
+// Banks of up to two models stage; larger ones load ring rows directly, because the staging buffers would cost them a CTA
+// per SM (shared memory: NM = 3, 4 drop from 3 CTAs to 2, NM = 6 .. 8 from 2 to 1) and that costs more than staging gains.
+constexpr bool bank_stages(int nm, bool ring) { return ring && nm <= 2; }
+
+__device__ __forceinline__ void cp_async16(float* dst, const float* src, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;"
+                 :: "r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" :: "n"(PENDING) : "memory"); }
+
+// This lane's share of steps t0 .. t0 + BANK_STAGE_STEPS - 1 of stream `cs` of the tile into buf: 16-byte pieces q = lane & 1 and
+// 2 + (lane & 1) of each row.  cur is null-rowed for a padding stream (ok = false).
+__device__ __forceinline__ void bank_stage(float* buf, const RingCursor& cur, bool ok, int cs, int t0, int T, const float* any, int lane) {
+#pragma unroll
+    for (int r = 0; r < BANK_STAGE_STEPS; ++r) {
+        const float* row = ok && t0 + r < T ? cur.at(t0 + r) : nullptr;
+        float* dst = buf + (r * 16 + cs) * BANK_STAGE_ROW;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int q = 2 * h + (lane & 1);
+            const bool copy = row != nullptr && 4 * q < cur.stride;
+            cp_async16(dst + 4 * q, copy ? row + 4 * q : any, copy ? 16u : 0u);
+        }
+    }
+}
+
+// RING: rows from the stream ring (a tick), staged through shared memory up to NM = 2; otherwise from in.inputs,
+// [n][T][F_base] contiguous (pb_predict), loaded directly.  KERAS_ACT: every model uses Keras's GRU defaults (recurrent hard_sigmoid, activation
+// linear), compiled in; otherwise each model's pair is dispatched at run time.  Both compute the same expressions.
+template <int NM, bool RING, bool KERAS_ACT>
 __global__ void __launch_bounds__(MMA_THREADS, NM == 1 ? 4 : 1)      // NM = 1: 128 registers (ptxas alone picks 96 and spills)
 gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
     extern __shared__ __align__(16) unsigned char bank_smem[];
@@ -100,10 +138,11 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const long long base = ((long long)blockIdx.x * (MMA_THREADS / 32) + warp) * 16;
     if (base >= n) return;
+    constexpr bool STAGE = bank_stages(NM, RING);
     const int F = in.F_base;
     long long idx[2];
     int sid[2];
-    RingCursor cur[2];
+    RingCursor rc[2];                                        // direct ring loads (RING && !STAGE)
     bool ok[2];
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
@@ -112,10 +151,30 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
         sid[hf] = 0;
         if (RING && ok[hf]) {
             sid[hf] = in.ids ? in.ids[idx[hf]] : (int)idx[hf];
-            const long long ns = in.n_samples[sid[hf]];
-            cur[hf].init(in, sid[hf], ns >= in.window ? (ns - in.window) / in.hop + 1 : 0);
+            if (!STAGE) {
+                const long long ns = in.n_samples[sid[hf]];
+                rc[hf].init(in, sid[hf], ns >= in.window ? (ns - in.window) / in.hop + 1 : 0);
+            }
         }
     }
+    // staging: this lane copies rows of stream cs = lane / 2 of the tile; chunk c of the window goes to buffer c & 1
+    float* stage = reinterpret_cast<float*>(bank_smem + NM * BANK_MODEL_SMEM) + warp * 2 * BANK_STAGE_BUF;
+    const int cs = lane >> 1;
+    const bool cok = STAGE && base + cs < n;
+    RingCursor cur;
+    cur.stride = 0;
+    if (cok) {
+        const int csid = in.ids ? in.ids[base + cs] : (int)(base + cs);
+        const long long ns = in.n_samples[csid];
+        cur.init(in, csid, ns >= in.window ? (ns - in.window) / in.hop + 1 : 0);
+    }
+    if (STAGE) {
+        bank_stage(stage, cur, cok, cs, 0, in.T, in.ring, lane);
+        cp_async_commit();
+        bank_stage(stage + BANK_STAGE_BUF, cur, cok, cs, BANK_STAGE_STEPS, in.T, in.ring, lane);
+        cp_async_commit();
+    }
+    int chunk = 0, cr = 0;                                   // step = chunk * BANK_STAGE_STEPS + cr
     float hreg[NM][3][4];
 #pragma unroll
     for (int m = 0; m < NM; ++m)
@@ -128,14 +187,40 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
     for (int step = 0; step < in.T; ++step) {
         // ---- the tile's MFCC row as a k16 A fragment: a0 / a1 = rows g / g + 8 at k 2t, 2t + 1; a2 / a3 at k 2t + 8, 2t + 9
         float xv[2][4];
+        if (STAGE) {
+            if (cr == 0) {                                                  // chunk `chunk` has landed (the next may be in flight)
+                cp_async_wait<1>();
+                __syncwarp();
+            }
+            const float* xs = stage + (chunk & 1) * BANK_STAGE_BUF + cr * 16 * BANK_STAGE_ROW;
 #pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-            const float* row = nullptr;                                     // stays nullptr: a row before the stream's first frame
-            if (ok[hf]) row = RING ? cur[hf].next(step) : in.inputs + (idx[hf] * in.T + step) * F;
-            xv[hf][0] = (row != nullptr && 2 * t < F) ? __ldg(row + 2 * t) : 0.f;
-            xv[hf][1] = (row != nullptr && 2 * t + 1 < F) ? __ldg(row + 2 * t + 1) : 0.f;
-            xv[hf][2] = (row != nullptr && 2 * t + 8 < F) ? __ldg(row + 2 * t + 8) : 0.f;
-            xv[hf][3] = (row != nullptr && 2 * t + 9 < F) ? __ldg(row + 2 * t + 9) : 0.f;
+            for (int hf = 0; hf < 2; ++hf) {
+                const float* row = xs + (g + 8 * hf) * BANK_STAGE_ROW;
+                const float2 lo = *reinterpret_cast<const float2*>(row + 2 * t), hi = *reinterpret_cast<const float2*>(row + 2 * t + 8);
+                xv[hf][0] = 2 * t < F ? lo.x : 0.f;
+                xv[hf][1] = 2 * t + 1 < F ? lo.y : 0.f;
+                xv[hf][2] = 2 * t + 8 < F ? hi.x : 0.f;
+                xv[hf][3] = 2 * t + 9 < F ? hi.y : 0.f;
+            }
+            if (cr + 1 == BANK_STAGE_STEPS) {                               // last step of the chunk: refill its buffer with chunk + 2
+                __syncwarp();
+                bank_stage(stage + (chunk & 1) * BANK_STAGE_BUF, cur, cok, cs, (chunk + 2) * BANK_STAGE_STEPS, in.T, in.ring, lane);
+                cp_async_commit();
+                cr = 0;
+                ++chunk;
+            } else {
+                ++cr;
+            }
+        } else {
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                const float* row = nullptr;                                 // stays nullptr: a row before the stream's first frame
+                if (ok[hf]) row = RING ? rc[hf].next(step) : in.inputs + (idx[hf] * in.T + step) * F;
+                xv[hf][0] = (row != nullptr && 2 * t < F) ? __ldg(row + 2 * t) : 0.f;
+                xv[hf][1] = (row != nullptr && 2 * t + 1 < F) ? __ldg(row + 2 * t + 1) : 0.f;
+                xv[hf][2] = (row != nullptr && 2 * t + 8 < F) ? __ldg(row + 2 * t + 8) : 0.f;
+                xv[hf][3] = (row != nullptr && 2 * t + 9 < F) ? __ldg(row + 2 * t + 9) : 0.f;
+            }
         }
         uint32_t xh[4], xl[4];
         split_f16(xv[0][0], xv[0][1], xh[0], xl[0]);
@@ -180,20 +265,26 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
 #pragma unroll
                 for (int nt = 0; nt < 3; ++nt)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) rh[nt][e] = apply_ract(acc[3 + nt][e], ra) * hreg[m][nt][e];
+                    for (int e = 0; e < 4; ++e) {
+                        const float r = KERAS_ACT ? hard_sigmoid(acc[3 + nt][e]) : apply_ract(acc[3 + nt][e], ra);
+                        rh[nt][e] = __fmul_rn(r, hreg[m][nt][e]);
+                    }
                 uint32_t ah[4], al[4], ch[2], cl[2];
                 frag_f16(rh, ah, al, ch, cl);
                 mma3_f16(acc, 6, ah, al, ch, cl, sB, lane);
             }
+            // h = z h + (1 - z) a, rounded as fma(z, h, (1 - z) a) in every specialisation
 #pragma unroll
             for (int nt = 0; nt < 3; ++nt)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    const float z = apply_ract(acc[nt][e], ra);
-                    hreg[m][nt][e] = z * hreg[m][nt][e] + (1.f - z) * apply_act(acc[6 + nt][e], ac);
+                    const float z = KERAS_ACT ? hard_sigmoid(acc[nt][e]) : apply_ract(acc[nt][e], ra);
+                    const float a = KERAS_ACT ? acc[6 + nt][e] : apply_act(acc[6 + nt][e], ac);
+                    hreg[m][nt][e] = __fmaf_rn(z, hreg[m][nt][e], __fmul_rn(__fsub_rn(1.f, z), a));
                 }
         }
     }
+    if (STAGE) cp_async_wait<0>();                                    // copies of chunks past the window
     // ---- per model: Dense(1) (per-thread partial over its 6 units per row, reduced over the quad) and the epilogue
 #pragma unroll
     for (int m = 0; m < NM; ++m) {

@@ -141,6 +141,12 @@ struct RingCursor {
         slot = slot + 1 == rows ? 0 : slot + 1;
         return r;
     }
+    // row of step t in any order (t < T <= rows: the window wraps the ring at most once), nullptr for a zero row
+    __device__ __forceinline__ const float* at(int t) const {
+        if (t < lead) return nullptr;
+        const int s = slot + t;
+        return base + (long long)(s >= rows ? s - rows : s) * stride;
+    }
 };
 
 // ------------------------------------------------------------------------------------------------
