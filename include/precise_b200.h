@@ -217,6 +217,25 @@ int pb_read_window(pb_handle* h, const int32_t* d_stream_ids, int64_t n, float* 
  * d_stream_ids NULL => streams 0..n-1. */
 int pb_clear(pb_handle* h, const int32_t* d_stream_ids, int64_t n, void* stream);
 
+/* Per-stream model subscriptions, as a device of a many-streams server runs a Listener only for its own wake word(s).
+ * Bit m of a stream's mask = bank slot m scores that stream.  Every stream starts with mask 0xFF: every model, including
+ * models added later.  Bits at or above pb_num_models are stored and take effect when such a model is added.  HOST arrays;
+ * h_stream_ids NULL => 0..n-1.  Synchronous: work already queued on the device finishes under the old masks.  A bit that goes
+ * from 0 to 1 re-arms that model's TriggerDetector for that stream, as a new detector would start.  PB_ERR_INVALID (and
+ * nothing changes): null handle, n outside [0, max_streams], an id outside [0, max_streams), a duplicate id.
+ *
+ * pb_update, pb_update_host (bit 0), pb_update_models and pb_update_ragged honour the masks.  For a (stream item, model) pair
+ * whose bit is clear: raw and conf are NaN, fired is 0, the model's trigger state for that stream does not change and nothing
+ * is added to its count.  A stream with mask 0 still advances its MFCC state (pb_read_window sees its real window).
+ * pb_clear leaves masks as they are.  A bank tick costs one window scan per subscribed (stream, model) pair; K1 and the ring
+ * stay shared.  A handle that never calls pb_set_stream_models runs exactly as before; the first call allocates
+ * [max_streams] mask bytes and 64 B per stream of route-list scratch.  Two bank ticks of one routed handle on different CUDA
+ * streams are ordered by the library (they share that scratch). */
+int pb_set_stream_models(pb_handle* h, const int32_t* h_stream_ids, const uint8_t* h_masks, int64_t n);
+/* The masks of the given streams (h_stream_ids NULL => 0..n-1) into h_masks [n] (HOST).  PB_ERR_INVALID: null handle, n outside
+ * [0, max_streams], an id outside [0, max_streams). */
+int pb_get_stream_models(const pb_handle* h, const int32_t* h_stream_ids, int64_t n, uint8_t* h_masks);
+
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);

@@ -33,6 +33,11 @@ class StreamBatch:
         self._bank_out = None
         return slot
 
+    def set_stream_models(self, masks, ids=None):
+        """Which bank models score which streams: bit m of masks[i] (host uint8) = slot m scores stream ids[i] (host int32;
+        None: stream i).  Unsubscribed pairs come back as NaN / NaN / 0.  See PreciseB200.set_stream_models."""
+        self.core.set_stream_models(masks, ids)
+
     def _bank_buffers(self, n):
         """The cached [M, n] outputs of a bank tick."""
         M = self.core.num_models

@@ -61,6 +61,8 @@ SYMBOLS = {
     'pb_update_host': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP]),
     'pb_read_window': (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
     'pb_clear': (C.c_int, [_VP, _VP, _I64, _VP]),
+    'pb_set_stream_models': (C.c_int, [_VP, _VP, _VP, _I64]),
+    'pb_get_stream_models': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -453,6 +455,26 @@ class PreciseB200:
         n = (ids.numel() if ids is not None else (self.max_streams if n is None else n))
         self._check_ids(ids, n)
         check(self.lib.pb_clear(self._h, _ptr(ids), n, self._stream()))
+
+    # ---- per-stream model subscriptions
+    def set_stream_models(self, masks, ids=None):
+        """Bit m of masks[i] = bank slot m scores stream ids[i] (ids None: stream i).  Host numpy arrays: uint8 masks [n],
+        int32 ids [n].  Unsubscribed (item, model) pairs of later ticks come back as raw NaN, conf NaN, fired 0, with that
+        model's trigger and count untouched; a bit going from 0 to 1 re-arms the model's trigger for the stream.  Streams
+        start at 0xFF (every model, including models added later).  Synchronous; bad ids raise ValueError and change nothing."""
+        masks = np.asarray(masks)
+        n = masks.shape[0] if masks.ndim == 1 else -1
+        _check_np('masks', masks, np.uint8, (n,), optional=False)
+        _check_np('ids', ids, np.int32, (n,))
+        check(self.lib.pb_set_stream_models(self._h, _np_ptr(ids), _np_ptr(masks), n))
+
+    def stream_models(self, ids=None) -> np.ndarray:
+        """uint8 masks of streams ids (host int32 array), or of every stream."""
+        n = self.max_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
+        _check_np('ids', ids, np.int32, (n,))
+        out = np.zeros(n, np.uint8)
+        check(self.lib.pb_get_stream_models(self._h, _np_ptr(ids), n, _np_ptr(out)))
+        return out
 
     def update_host(self, pcm_np, conf_np, raw_np=None, fired_np=None, ids_np=None) -> int:
         """Host-buffer tick (numpy arrays, ideally backed by pinned memory).  Returns this tick's count."""

@@ -159,6 +159,14 @@ struct pb_handle {
     DevArray<int16_t> d_tail;
     DevArray<float> d_ring;
     std::vector<Network> models;
+    // per-stream model subscriptions (pb_set_stream_models); a handle that never sets them keeps routed = false and none of this
+    bool routed = false;             // sticky, set by the first pb_set_stream_models
+    std::vector<uint8_t> route_mask; // host mirror of d_route
+    int64_t subs[PB_MAX_MODELS] = {};  // streams with bit m set, for all PB_MAX_MODELS bits (a model added later finds its count)
+    DevArray<uint8_t> d_route;       // [max_streams] masks, bit m = bank slot m scores the stream
+    DevArray<int2> d_route_list;     // [PB_MAX_MODELS][max_streams] route_kernel's (item, stream) lists: scratch of bank ticks
+    DevArray<unsigned> d_route_count;  // [PB_MAX_MODELS] their lengths
+    cudaEvent_t route_ev = nullptr;  // recorded after each routed bank tick; the next one waits on it before reusing the scratch
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
     cudaEvent_t pipe_ev[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -184,6 +192,7 @@ struct pb_handle {
         }
         for (auto& p : prof)
             for (auto e : p.ev) cudaEventDestroy(e);
+        if (route_ev) cudaEventDestroy(route_ev);
     }
 };
 
@@ -965,7 +974,8 @@ static int launch_gru_kernels(const Network& net, int F, const K2In& in, bool ri
     } else if (nw.small_path) {
         const int per_cta = K2_SMALL_THREADS * K2_NS;
         const int grid = (int)((n + per_cta - 1) / per_cta);
-        if (ring) gru_small_kernel<20, 13, true><<<grid, K2_SMALL_THREADS, 0, s>>>(nw.w_small, in, n, dp, o);
+        if (ring && o.route) gru_small_kernel<20, 13, true, true><<<grid, K2_SMALL_THREADS, 0, s>>>(nw.w_small, in, n, dp, o);
+        else if (ring) gru_small_kernel<20, 13, true><<<grid, K2_SMALL_THREADS, 0, s>>>(nw.w_small, in, n, dp, o);
         else gru_small_kernel<20, 13, false><<<grid, K2_SMALL_THREADS, 0, s>>>(nw.w_small, in, n, dp, o);
     } else if (nw.wide_ok && net.gru_mode != 1) {                 // tensor-core scan (mma.sync 3xTF32) for other networks
         GruWideW w;
@@ -1156,7 +1166,17 @@ static int score_model0(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_
     const Network& net = h->models[0];
     K2Out o{};
     o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = net.trig.get();
-    return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
+    if (!h->routed) return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
+    // routed: NaN fill of the items whose stream lacks bit 0, then the usual kernel with the epilogue's mask.  No list scratch:
+    // pb_update_host runs this on three streams at once.
+    ProfScope ps(h, 1, s);
+    RouteOut r{};
+    r.raw = d_raw; r.conf = d_conf; r.fired = d_fired; r.M = 1;
+    route_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(h->d_route.get(), d_ids, n, r);
+    CK(cudaGetLastError());
+    if (h->subs[0] == 0) return PB_OK;
+    o.route = h->d_route.get(); o.route_bit = 1;
+    return launch_gru_kernels(net, h->feat, stream_k2in(h, d_ids), true, n, o, s);
 }
 
 PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
@@ -1227,10 +1247,75 @@ static int launch_bank(const BankParams& P, int nm, const K2In& in, int64_t n, c
     return fail(PB_ERR_INVALID, "%d fused models", nm);
 }
 
+static bool keras_act(const Network& net) {
+    return net.cfg.activation == PB_ACT_LINEAR && net.cfg.recurrent_activation == PB_RACT_HARD_SIGMOID;
+}
+
+// The network half of a bank tick on a routed handle.  route_kernel writes NaN / NaN / 0 for every unsubscribed (item, model)
+// pair and lists the subscribed pairs of each fused model; gru_bank_routed_kernel scans only those (one launch for the models
+// with Keras's default activations, one for the others), other networks run their own kernel with the epilogue's mask.  A model
+// without subscribers launches nothing.  Grids are sized from the host's subscriber counts: min(n, subs[m]) / 64 tiles each.
+static int score_bank_routed(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
+                             unsigned long long* d_count, cudaStream_t s) {
+    const int M = (int)h->models.size();
+    const K2In in = stream_k2in(h, d_ids);
+    const int64_t stride = h->cfg.max_streams;
+    int2* lists = h->d_route_list.get();
+    unsigned* counts = h->d_route_count.get();
+    ProfScope ps(h, 1, s);
+    // the lists are the handle's: a routed bank tick on another stream may still be reading them
+    CK(cudaStreamWaitEvent(s, h->route_ev, 0));
+    CK(cudaMemsetAsync(counts, 0, PB_MAX_MODELS * sizeof(unsigned), s));
+    RouteOut r{};
+    r.raw = d_raw; r.conf = d_conf; r.fired = d_fired; r.M = M;
+    r.lists = lists; r.list_stride = stride; r.count = counts;
+    K2Out o[PB_MAX_MODELS];
+    for (int m = 0; m < M; ++m) {
+        o[m] = K2Out{};
+        o[m].raw = d_raw ? d_raw + (int64_t)m * n : nullptr;
+        o[m].conf = d_conf + (int64_t)m * n;
+        o[m].fired = d_fired ? d_fired + (int64_t)m * n : nullptr;
+        o[m].count = d_count ? d_count + m : nullptr;
+        o[m].trig = h->models[m].trig.get();
+        if (bank_fused(h->models[m], h->feat)) r.listed |= 1u << m;
+    }
+    route_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(h->d_route.get(), d_ids, n, r);
+    CK(cudaGetLastError());
+    for (int m = 0; m < M; ++m) {
+        if ((r.listed >> m & 1) || h->subs[m] == 0) continue;
+        o[m].route = h->d_route.get();
+        o[m].route_bit = 1u << m;
+        const int rc = launch_gru_kernels(h->models[m], h->feat, in, true, n, o[m], s);
+        if (rc != PB_OK) return rc;
+    }
+    for (int ka = 0; ka < 2; ++ka) {
+        BankParams P{};
+        BankRoute R{};
+        int tiles = 0;
+        for (int m = 0; m < M; ++m) {
+            const Network& net = h->models[m];
+            if (!(r.listed >> m & 1) || h->subs[m] == 0 || keras_act(net) != (ka == 1)) continue;
+            set_bank_slot(P, R.nm, net, o[m]);
+            R.list[R.nm] = lists + m * stride;
+            R.count[R.nm] = counts + m;
+            R.tile0[R.nm++] = tiles;
+            tiles += (int)((std::min<int64_t>(n, h->subs[m]) + 63) / 64);
+        }
+        R.tile0[R.nm] = tiles;
+        if (R.nm == 0) continue;
+        if (ka) gru_bank_routed_kernel<true><<<tiles, MMA_THREADS, BANK_MODEL_SMEM + BANK_STAGE_SMEM, s>>>(P, R, in);
+        else gru_bank_routed_kernel<false><<<tiles, MMA_THREADS, BANK_MODEL_SMEM + BANK_STAGE_SMEM, s>>>(P, R, in);
+        CK(cudaGetLastError());
+    }
+    CK(cudaEventRecord(h->route_ev, s));
+    return PB_OK;
+}
+
 // The network half of a bank tick (pb_update_models, pb_update_ragged): every model scores the windows of the n streams, outputs
 // model-major.
 static int score_bank(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
                       unsigned long long* d_count, cudaStream_t s) {
+    if (h->routed) return score_bank_routed(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
     int rc = PB_OK;
     const int M = (int)h->models.size();
     const K2In in = stream_k2in(h, d_ids);
@@ -1345,6 +1430,101 @@ PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream)
     for (size_t m = 0; m < h->models.size(); ++m) t.trig[m] = h->models[m].trig.get();
     clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->d_n_samples.get(), t, d_ids, n);
     CK(cudaGetLastError());
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// per-stream model subscriptions
+
+// Stream sids[j] gets mask masks[j]; every model m whose bit rearm[j] sets has its trigger re-armed for it.
+__global__ void set_route_kernel(uint8_t* route, TrigArrays t, const int* sids, const uint8_t* masks, const uint8_t* rearm, long long k) {
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= k) return;
+    const int sid = sids[j];
+    route[sid] = masks[j];
+#pragma unroll
+    for (int m = 0; m < PB_MAX_MODELS; ++m)
+        if (t.trig[m] && (rearm[j] >> m & 1)) t.trig[m][sid] = 0;
+}
+
+// The first pb_set_stream_models: device masks (every stream 0xFF), list scratch and its event.  Only then is the handle routed.
+static int ensure_routed(pb_handle* h) {
+    if (h->routed) return PB_OK;
+    const size_t S = (size_t)h->cfg.max_streams;
+    DevArray<uint8_t> route;
+    DevArray<int2> lists;
+    DevArray<unsigned> count;
+    CK(route.alloc(S));
+    CK(cudaMemset(route.get(), 0xFF, S));
+    CK(lists.alloc(PB_MAX_MODELS * S));
+    CK(count.alloc(PB_MAX_MODELS));
+    CK(cudaEventCreateWithFlags(&h->route_ev, cudaEventDisableTiming));
+    h->d_route = std::move(route);
+    h->d_route_list = std::move(lists);
+    h->d_route_count = std::move(count);
+    h->route_mask.assign(S, 0xFF);
+    for (int m = 0; m < PB_MAX_MODELS; ++m) h->subs[m] = (int64_t)S;
+    h->routed = true;
+    return PB_OK;
+}
+
+// Validates stream ids (h_ids null: 0..n-1) before anything changes: range and, for a set, uniqueness.
+static int check_route_ids(const pb_handle* h, const int32_t* h_ids, int64_t n, bool unique) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (n < 0 || n > h->cfg.max_streams) return fail(PB_ERR_INVALID, "n = %lld outside [0, max_streams = %d]", (long long)n, h->cfg.max_streams);
+    if (!h_ids) return PB_OK;
+    std::vector<char> seen(unique ? h->cfg.max_streams : 0, 0);
+    for (int64_t i = 0; i < n; ++i) {
+        const int32_t sid = h_ids[i];
+        if (sid < 0 || sid >= h->cfg.max_streams) return fail(PB_ERR_INVALID, "stream id %d outside [0, %d)", sid, h->cfg.max_streams);
+        if (unique && seen[sid]++) return fail(PB_ERR_INVALID, "stream id %d appears twice", sid);
+    }
+    return PB_OK;
+}
+
+PB_API int pb_set_stream_models(pb_handle* h, const int32_t* h_ids, const uint8_t* h_masks, int64_t n) {
+    int rc = check_route_ids(h, h_ids, n, true);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && !h_masks) return fail(PB_ERR_INVALID, "null masks");
+    CK(cudaSetDevice(h->cfg.device));
+    rc = ensure_routed(h);
+    if (rc != PB_OK) return rc;
+    CK(cudaDeviceSynchronize());                     // queued work finishes under the old masks
+    std::vector<int> sids;
+    std::vector<uint8_t> masks, rearm;
+    for (int64_t i = 0; i < n; ++i) {
+        const int sid = h_ids ? h_ids[i] : (int)i;
+        const uint8_t old = h->route_mask[sid], nw = h_masks[i];
+        if (old == nw) continue;
+        sids.push_back(sid);
+        masks.push_back(nw);
+        rearm.push_back((uint8_t)(nw & ~old));
+    }
+    if (sids.empty()) return PB_OK;
+    DevArray<int> d_sids;
+    DevArray<uint8_t> d_masks, d_rearm;
+    CK(d_sids.upload(sids));
+    CK(d_masks.upload(masks));
+    CK(d_rearm.upload(rearm));
+    TrigArrays t{};
+    for (size_t m = 0; m < h->models.size(); ++m) t.trig[m] = h->models[m].trig.get();
+    const long long k = (long long)sids.size();
+    set_route_kernel<<<(int)((k + 255) / 256), 256>>>(h->d_route.get(), t, d_sids.get(), d_masks.get(), d_rearm.get(), k);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    for (size_t j = 0; j < sids.size(); ++j) {
+        const uint8_t old = h->route_mask[sids[j]];
+        for (int m = 0; m < PB_MAX_MODELS; ++m) h->subs[m] += (int)(masks[j] >> m & 1) - (int)(old >> m & 1);
+        h->route_mask[sids[j]] = masks[j];
+    }
+    return PB_OK;
+}
+
+PB_API int pb_get_stream_models(const pb_handle* h, const int32_t* h_ids, int64_t n, uint8_t* h_masks) {
+    const int rc = check_route_ids(h, h_ids, n, false);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && !h_masks) return fail(PB_ERR_INVALID, "null masks");
+    for (int64_t i = 0; i < n; ++i) h_masks[i] = h->routed ? h->route_mask[h_ids ? h_ids[i] : i] : 0xFF;
     return PB_OK;
 }
 

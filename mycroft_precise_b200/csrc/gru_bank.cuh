@@ -118,25 +118,27 @@ __device__ __forceinline__ void bank_stage(float* buf, const RingCursor& cur, bo
     }
 }
 
+// The scan of one CTA: models m0 .. m0 + NM - 1 of P over the CTA's 64 entries, entries tile * 64 .. of n.  An entry is
+// item e of the tick (stream in.ids[e], or e), or with a route list, list[e] = (item, stream).
 // RING: rows from the stream ring (a tick), staged through shared memory up to NM = 2; otherwise from in.inputs,
 // [n][T][F_base] contiguous (pb_predict), loaded directly.  KERAS_ACT: every model uses Keras's GRU defaults (recurrent hard_sigmoid, activation
 // linear), compiled in; otherwise each model's pair is dispatched at run time.  Both compute the same expressions.
 template <int NM, bool RING, bool KERAS_ACT>
-__global__ void __launch_bounds__(MMA_THREADS, NM == 1 ? 4 : 1)      // NM = 1: 128 registers (ptxas alone picks 96 and spills)
-gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
+__device__ __forceinline__ void bank_scan(const BankParams& P, int m0, const int2* list, long long tile, const K2In& in, long long n) {
     extern __shared__ __align__(16) unsigned char bank_smem[];
 #pragma unroll 1
     for (int m = 0; m < NM; ++m) {
+        const BankModelW& w = P.w[m0 + m];
         uint4* sf = reinterpret_cast<uint4*>(bank_smem + m * BANK_MODEL_SMEM);
         float* sb = reinterpret_cast<float*>(sf + BANK_FRAG_U4);
-        for (int e = threadIdx.x; e < 2 * MMA_NT * 32; e += blockDim.x) sf[e] = __ldg(P.w[m].bfrag + e);
-        for (int e = threadIdx.x; e < MMA_NT * 32; e += blockDim.x) sf[2 * MMA_NT * 32 + e] = __ldg(P.w[m].xfrag + e);
-        for (int e = threadIdx.x; e < 72; e += blockDim.x) sb[e] = __ldg(P.w[m].bias + e);
-        for (int e = threadIdx.x; e < 24; e += blockDim.x) sb[72 + e] = __ldg(P.w[m].wd + e);
+        for (int e = threadIdx.x; e < 2 * MMA_NT * 32; e += blockDim.x) sf[e] = __ldg(w.bfrag + e);
+        for (int e = threadIdx.x; e < MMA_NT * 32; e += blockDim.x) sf[2 * MMA_NT * 32 + e] = __ldg(w.xfrag + e);
+        for (int e = threadIdx.x; e < 72; e += blockDim.x) sb[e] = __ldg(w.bias + e);
+        for (int e = threadIdx.x; e < 24; e += blockDim.x) sb[72 + e] = __ldg(w.wd + e);
     }
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
-    const long long base = ((long long)blockIdx.x * (MMA_THREADS / 32) + warp) * 16;
+    const long long base = (tile * (MMA_THREADS / 32) + warp) * 16;
     if (base >= n) return;
     constexpr bool STAGE = bank_stages(NM, RING);
     const int F = in.F_base;
@@ -149,8 +151,14 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
         idx[hf] = base + g + 8 * hf;
         ok[hf] = idx[hf] < n;
         sid[hf] = 0;
-        if (RING && ok[hf]) {
+        if (list != nullptr && ok[hf]) {
+            const int2 p = list[idx[hf]];
+            idx[hf] = p.x;
+            sid[hf] = p.y;
+        } else if (RING && ok[hf]) {
             sid[hf] = in.ids ? in.ids[idx[hf]] : (int)idx[hf];
+        }
+        if (RING && ok[hf]) {
             if (!STAGE) {
                 const long long ns = in.n_samples[sid[hf]];
                 rc[hf].init(in, sid[hf], ns >= in.window ? (ns - in.window) / in.hop + 1 : 0);
@@ -164,7 +172,7 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
     RingCursor cur;
     cur.stride = 0;
     if (cok) {
-        const int csid = in.ids ? in.ids[base + cs] : (int)(base + cs);
+        const int csid = list != nullptr ? list[base + cs].y : in.ids ? in.ids[base + cs] : (int)(base + cs);
         const long long ns = in.n_samples[csid];
         cur.init(in, csid, ns >= in.window ? (ns - in.window) / in.hop + 1 : 0);
     }
@@ -232,7 +240,7 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
             const uint4* sB = reinterpret_cast<const uint4*>(bank_smem + m * BANK_MODEL_SMEM);
             const uint4* sX = sB + 2 * MMA_NT * 32;
             const float* sBias = reinterpret_cast<const float*>(sB + BANK_FRAG_U4);
-            const int ra = P.w[m].ract, ac = P.w[m].act;
+            const int ra = P.w[m0 + m].ract, ac = P.w[m0 + m].act;
             float acc[MMA_NT][4];
 #pragma unroll
             for (int nt = 0; nt < MMA_NT; ++nt) {
@@ -299,9 +307,81 @@ gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
             }
             part += __shfl_xor_sync(0xffffffffu, part, 1);
             part += __shfl_xor_sync(0xffffffffu, part, 2);
-            epilogue(part + P.w[m].bd, t == 0 && ok[hf], idx[hf], sid[hf], P.dp[m], P.o[m]);
+            epilogue(part + P.w[m0 + m].bd, t == 0 && ok[hf], idx[hf], sid[hf], P.dp[m0 + m], P.o[m0 + m]);
         }
     }
+}
+
+// Every model of P over the n items of a tick (or of pb_predict's inputs), 64 items per CTA.
+template <int NM, bool RING, bool KERAS_ACT>
+__global__ void __launch_bounds__(MMA_THREADS, NM == 1 ? 4 : 1)      // NM = 1: 128 registers (ptxas alone picks 96 and spills)
+gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
+    bank_scan<NM, RING, KERAS_ACT>(P, 0, nullptr, blockIdx.x, in, n);
+}
+
+// Per-stream model subscriptions: route_kernel has listed, for each model m, the (item, stream) pairs of the tick whose
+// stream subscribes to m (count[m] of them).  A routed launch scans models 0 .. nm - 1 of P; model k takes CTAs
+// tile0[k] .. tile0[k + 1] - 1, 64 list entries each, sized on the host from the model's subscriber count.
+struct BankRoute {
+    const int2* list[BANK_MAX_MODELS];           // model k's list
+    const unsigned* count[BANK_MAX_MODELS];      // ... and its length (device)
+    int tile0[BANK_MAX_MODELS + 1];
+    int nm;
+};
+
+// Outputs and lists of route_kernel.  Outputs are model-major [M][n] (M = 1: pb_update's [n]); raw and fired may be null.
+struct RouteOut {
+    float* raw;
+    double* conf;
+    uint8_t* fired;
+    int M;
+    int2* lists;                     // [BANK_MAX_MODELS][list_stride] (item, stream) pairs, or null: NaN fill only
+    long long list_stride;
+    unsigned* count;                 // [BANK_MAX_MODELS] list lengths, zeroed before the launch
+    unsigned listed;                 // bit m: model m is scanned from its list
+};
+
+// One thread per tick item.  For every model m < M whose bit the item's stream lacks: raw = conf = NaN, fired = 0 (the only
+// place that writes them).  For every listed model whose bit it has: appends (item, stream) to m's list, one atomicAdd per
+// warp and model.  The order within a list varies; a window's score does not depend on its tile.
+__global__ void __launch_bounds__(256) route_kernel(const uint8_t* route, const int* ids, long long n, RouteOut r) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool ok = i < n;
+    const int sid = ok ? (ids ? ids[i] : (int)i) : 0;
+    const unsigned mask = ok ? route[sid] : 0u;
+    const int lane = threadIdx.x & 31;
+    for (int m = 0; m < r.M; ++m) {
+        const unsigned bit = 1u << m;
+        const long long o = (long long)m * n + i;
+        if (ok && !(mask & bit)) {
+            if (r.raw) r.raw[o] = __int_as_float(0x7fc00000);
+            r.conf[o] = __longlong_as_double(0x7ff8000000000000LL);
+            if (r.fired) r.fired[o] = 0;
+        }
+        if (r.lists != nullptr && (r.listed & bit)) {                 // uniform over the grid
+            const bool sub = ok && (mask & bit);
+            const unsigned b = __ballot_sync(0xffffffffu, sub);
+            if (b == 0) continue;
+            unsigned at = 0;
+            if (lane == 0) at = atomicAdd(r.count + m, (unsigned)__popc(b));
+            at = __shfl_sync(0xffffffffu, at, 0);
+            if (sub) r.lists[m * r.list_stride + at + __popc(b & ((1u << lane) - 1u))] = make_int2((int)i, sid);
+        }
+    }
+}
+
+// One model per CTA (NM = 1, with its staging and, for KERAS_ACT, the compiled-in activations); a CTA past its model's
+// list exits before it loads any weights.  Outputs go to item list[e].x, the trigger update to stream list[e].y; per model
+// the accumulation order is the bank's, so a pair scores bit-identically routed and unrouted.
+template <bool KERAS_ACT>
+__global__ void __launch_bounds__(MMA_THREADS, 4)
+gru_bank_routed_kernel(const __grid_constant__ BankParams P, const __grid_constant__ BankRoute R, K2In in) {
+    int k = 0;
+    while (k + 1 < R.nm && (int)blockIdx.x >= R.tile0[k + 1]) ++k;
+    const long long tile = (long long)blockIdx.x - R.tile0[k];
+    const long long n = *R.count[k];
+    if (tile * (MMA_THREADS / 32) * 16 >= n) return;
+    bank_scan<1, true, KERAS_ACT>(P, k, R.list[k], tile, in, n);
 }
 
 }  // namespace pb

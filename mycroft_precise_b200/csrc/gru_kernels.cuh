@@ -36,6 +36,8 @@ struct K2Out {
     uint8_t* fired;                  // [n] or null
     unsigned long long* count;       // [1] or null
     int* trig;                       // [max_streams] or null => no trigger update
+    const uint8_t* route;            // [max_streams] per-stream model masks (pb_set_stream_models) or null => every stream scored
+    unsigned route_bit;              // this model's bit of route[sid]
 };
 
 // Where row t of item i comes from.
@@ -80,9 +82,13 @@ __device__ __forceinline__ double decode_one(float raw, const DecodeParams& d) {
 }
 
 // Sigmoid + decode + trigger + count for item i (stream sid).  Called by every thread of the
-// warp (valid = false for padding lanes) because the count is warp-aggregated.
+// warp (valid = false for padding lanes) because the count is warp-aggregated.  ROUTE: a stream whose route mask lacks the
+// model's bit is not scored: no output written (route_kernel fills its NaN), no trigger update, not counted.  The check leaves
+// every kernel's registers as they were except gru_small_kernel's spills, so that kernel alone has instantiations without it.
+template <bool ROUTE = true>
 __device__ __forceinline__ void epilogue(float logit, bool valid, long long i, int sid,
                                          const DecodeParams& d, const K2Out& o) {
+    if (ROUTE && valid && o.route && !(o.route[sid] & o.route_bit)) valid = false;
     bool fired = false;
     if (valid) {
         float raw = sigmoid32(logit);
@@ -196,7 +202,7 @@ __device__ __forceinline__ void gate_dot(const float (*Wt)[KP], int j, float bia
 // memory transposed -- column j of [W;U] is one contiguous row of KP = roundup4(F + H) floats -- and are
 // fetched with warp-uniform (broadcast) 16-byte loads: with 2-way register blocking that is 9 LDS.128
 // per 66 FFMA.
-template <int H, int F, bool RING>
+template <int H, int F, bool RING, bool ROUTE = false>
 __global__ void __launch_bounds__(K2_SMALL_THREADS, 3)
 gru_small_kernel(const __grid_constant__ GruSmallW<H, F> P, K2In in, long long n, DecodeParams dp, K2Out out) {
     constexpr int K = F + H, KP = (K + 3) & ~3;
@@ -286,7 +292,7 @@ gru_small_kernel(const __grid_constant__ GruSmallW<H, F> P, K2In in, long long n
         float logit = P.bd;
 #pragma unroll
         for (int j = 0; j < H; ++j) logit = fmaf(h[s][j], P.wd[j], logit);
-        epilogue(logit, valid[s], i0 + s, sid[s], dp, out);
+        epilogue<ROUTE>(logit, valid[s], i0 + s, sid[s], dp, out);
     }
 }
 
