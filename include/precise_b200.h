@@ -187,8 +187,9 @@ int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_stream
  * Every length must lie in [1, max_len].  The kernels clamp lengths to [0, max_len] and never read outside
  * [d_pcm + d_offsets[0], d_pcm + d_offsets[n]), so a caller's mistake gives wrong answers for that stream, never an
  * out-of-bounds access.  A chunk may complete any number of MFCC frames (long chunks run as several MFCC launches).
- * TriggerDetector's refractory count still uses the handle's chunk_samples: the reference fixes chunk_size when it builds the
- * detector (runner/precise_runner/runner.py:121, :140), whatever the lengths of later reads.
+ * TriggerDetector's refractory count does not follow the lengths: the reference fixes chunk_size when it builds the detector
+ * (runner/precise_runner/runner.py:121, :140), whatever the lengths of later reads.  It comes from the handle's chunk_samples
+ * unless pb_set_stream_trigger gives the stream the chunk size of its own runner.
  * After a handle's first ragged tick, its uniform ticks (pb_update, pb_update_models, pb_update_vectors, pb_update_host) run
  * the ragged tick's MFCC kernel too (a stream's sample count is then no longer a multiple of 8), and pb_debug_k1_mode accepts
  * only 0.
@@ -235,6 +236,37 @@ int pb_set_stream_models(pb_handle* h, const int32_t* h_stream_ids, const uint8_
 /* The masks of the given streams (h_stream_ids NULL => 0..n-1) into h_masks [n] (HOST).  PB_ERR_INVALID: null handle, n outside
  * [0, max_streams], an id outside [0, max_streams). */
 int pb_get_stream_models(const pb_handle* h, const int32_t* h_stream_ids, int64_t n, uint8_t* h_masks);
+
+/* Per-stream TriggerDetector settings of bank slot `slot`, as TriggerDetector(chunk_size, sensitivity, trigger_level)
+ * (runner/precise_runner/runner.py:121) with each device's own values: Mycroft sets sensitivity and trigger_level per wake
+ * word in each device's configuration, and each runner reads its own chunk_size.  HOST arrays of n entries; h_stream_ids
+ * NULL => 0..n-1.  chunk_bytes is the runner's chunk_size in BYTES (refractory = -(8*2048) // chunk_bytes, Python floor
+ * division).
+ *   - Defaults: a stream never set uses the model's cfg.sensitivity, cfg.trigger_level and 2 * chunk_samples;
+ *     pb_get_stream_trigger returns those for it, and exactly what was set (the sensitivity bit for bit) for a stream set.
+ *   - Comparison: a tick compares conf > 1.0 - sensitivity in double (runner.py:130).  Any double is accepted (NaN and
+ *     values outside [0, 1] included, as Python accepts them), any int32 trigger_level; chunk_bytes must be >= 1 (the
+ *     reference would raise ZeroDivisionError).
+ *   - Re-arming: an entry whose values change re-arms that model's detector for that stream (activation 0), as Mycroft
+ *     builds a new runner when a setting changes; an entry set to the values it already has keeps its state.
+ *   - PB_ERR_INVALID, and nothing changes: null handle, slot outside [0, pb_num_models), n outside [0, max_streams], an id
+ *     outside [0, max_streams), a duplicate id, chunk_bytes < 1, a null array with n > 0.
+ *   - Synchronous: work already queued on the device finishes under the old settings.
+ *   - pb_clear re-arms a stream's detectors and keeps its settings; subscription changes (pb_set_stream_models) keep them
+ *     too, and a mask bit going from 0 to 1 still re-arms.
+ *   - pb_update, pb_update_host (zero-copy and pipelined), pb_update_models and pb_update_ragged honour the settings, with
+ *     or without subscriptions; unsubscribed pairs stay NaN / NaN / 0 and their detector does not move.
+ *   - Storage: the first call on a slot allocates that model's records, 16 B per stream on the device (initialised to the
+ *     model's defaults) and a 16 B host mirror, and flags the model for good: its ticks then scan without the trigger and
+ *     run one trigger kernel afterwards.  A model never set runs as before.  pb_destroy releases the records.
+ *   - pb_add_model after settings exist: the new slot starts on its own defaults. */
+int pb_set_stream_trigger(pb_handle* h, int32_t slot, const int32_t* h_stream_ids, const double* h_sensitivity,
+                          const int32_t* h_trigger_level, const int32_t* h_chunk_bytes, int64_t n);
+/* The settings of the given streams (h_stream_ids NULL => 0..n-1) of slot `slot` into h_sensitivity / h_trigger_level /
+ * h_chunk_bytes [n] (HOST).  PB_ERR_INVALID: null handle or output with n > 0, bad slot, n outside [0, max_streams], an id
+ * outside [0, max_streams). */
+int pb_get_stream_trigger(const pb_handle* h, int32_t slot, const int32_t* h_stream_ids, int64_t n,
+                          double* h_sensitivity, int32_t* h_trigger_level, int32_t* h_chunk_bytes);
 
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);

@@ -38,6 +38,15 @@ class StreamBatch:
         None: stream i).  Unsubscribed pairs come back as NaN / NaN / 0.  See PreciseB200.set_stream_models."""
         self.core.set_stream_models(masks, ids)
 
+    def set_stream_trigger(self, slot, sensitivity, trigger_level, chunk_size, ids=None):
+        """Each stream's TriggerDetector(chunk_size in bytes, sensitivity, trigger_level) for bank slot ``slot``; scalars
+        broadcast.  See PreciseB200.set_stream_trigger."""
+        self.core.set_stream_trigger(slot, sensitivity, trigger_level, chunk_size, ids)
+
+    def stream_trigger(self, slot, ids=None):
+        """(sensitivity, trigger_level, chunk_size) host arrays of bank slot ``slot``.  See PreciseB200.stream_trigger."""
+        return self.core.stream_trigger(slot, ids)
+
     def _bank_buffers(self, n):
         """The cached [M, n] outputs of a bank tick."""
         M = self.core.num_models

@@ -63,6 +63,8 @@ SYMBOLS = {
     'pb_clear': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_set_stream_models': (C.c_int, [_VP, _VP, _VP, _I64]),
     'pb_get_stream_models': (C.c_int, [_VP, _VP, _I64, _VP]),
+    'pb_set_stream_trigger': (C.c_int, [_VP, _I32, _VP, _VP, _VP, _VP, _I64]),
+    'pb_get_stream_trigger': (C.c_int, [_VP, _I32, _VP, _I64, _VP, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -475,6 +477,61 @@ class PreciseB200:
         out = np.zeros(n, np.uint8)
         check(self.lib.pb_get_stream_models(self._h, _np_ptr(ids), n, _np_ptr(out)))
         return out
+
+    # ---- per-stream TriggerDetector settings
+    @staticmethod
+    def _slot(slot):
+        if isinstance(slot, (bool, np.bool_)) or not isinstance(slot, (int, np.integer)) or not -2 ** 31 <= slot < 2 ** 31:
+            raise ValueError('slot must be an int32, got %r' % (slot,))
+        return int(slot)
+
+    def set_stream_trigger(self, slot, sensitivity, trigger_level, chunk_size, ids=None):
+        """Bank slot ``slot`` scores stream ids[i] as TriggerDetector(chunk_size[i], sensitivity[i], trigger_level[i]) would
+        (runner.py:121).  ``chunk_size`` is in BYTES, as the reference's TriggerDetector takes it.  Scalars broadcast to the
+        ids; ids (host int32 array) None: streams 0..n-1, n = the length of the array arguments, or every stream when all three
+        are scalars.  A stream whose values change gets a fresh detector; unchanged values keep its state.  Synchronous; bad
+        input raises ValueError and changes nothing."""
+        slot = self._slot(slot)
+        vals = [np.asarray(sensitivity), np.asarray(trigger_level), np.asarray(chunk_size)]
+        if any(v.ndim > 1 for v in vals):
+            raise ValueError('sensitivity, trigger_level and chunk_size must be scalars or 1-D arrays')
+        if ids is not None:
+            if not isinstance(ids, np.ndarray) or ids.ndim != 1:
+                raise ValueError('ids must be a 1-D int32 array')
+            n = ids.shape[0]
+        else:
+            lens = {v.shape[0] for v in vals if v.ndim == 1}
+            if len(lens) > 1:
+                raise ValueError('sensitivity, trigger_level and chunk_size have different lengths %s' % sorted(lens))
+            n = lens.pop() if lens else self.max_streams
+        _check_np('ids', ids, np.int32, (n,))
+        for name, v in zip(('sensitivity', 'trigger_level', 'chunk_size'), vals):
+            if v.ndim == 1 and v.shape[0] != n:
+                raise ValueError('%s has %d entries for %d streams' % (name, v.shape[0], n))
+        sens, level, chunk = vals
+        if sens.dtype.kind not in 'biuf':
+            raise ValueError('sensitivity must be real numbers, got %s' % sens.dtype)
+        for name, v in (('trigger_level', level), ('chunk_size', chunk)):
+            if v.dtype.kind not in 'iu':
+                raise ValueError('%s must be integers, got %s' % (name, v.dtype))
+            if v.size and (int(v.min()) < -2 ** 31 or int(v.max()) >= 2 ** 31):
+                raise ValueError('%s must fit in int32' % name)
+        if chunk.size and int(chunk.min()) < 1:
+            raise ValueError('chunk_size must be >= 1 byte (TriggerDetector divides by it), got %d' % int(chunk.min()))
+        sens = np.ascontiguousarray(np.broadcast_to(sens, (n,)), dtype=np.float64)
+        level = np.ascontiguousarray(np.broadcast_to(level, (n,)), dtype=np.int32)
+        chunk = np.ascontiguousarray(np.broadcast_to(chunk, (n,)), dtype=np.int32)
+        check(self.lib.pb_set_stream_trigger(self._h, slot, _np_ptr(ids), _np_ptr(sens), _np_ptr(level), _np_ptr(chunk), n))
+
+    def stream_trigger(self, slot, ids=None):
+        """(sensitivity f64[n], trigger_level i32[n], chunk_size i32[n], in bytes) of bank slot ``slot`` for streams ids
+        (host int32 array), or for every stream.  Streams never set report the model's own values."""
+        slot = self._slot(slot)
+        n = self.max_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
+        _check_np('ids', ids, np.int32, (n,))
+        sens, level, chunk = np.zeros(n, np.float64), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        check(self.lib.pb_get_stream_trigger(self._h, slot, _np_ptr(ids), n, _np_ptr(sens), _np_ptr(level), _np_ptr(chunk)))
+        return sens, level, chunk
 
     def update_host(self, pcm_np, conf_np, raw_np=None, fired_np=None, ids_np=None) -> int:
         """Host-buffer tick (numpy arrays, ideally backed by pinned memory).  Returns this tick's count."""

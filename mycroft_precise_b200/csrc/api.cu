@@ -28,6 +28,7 @@
 #include "mfcc_tc.cuh"
 #include "mfcc_tc3.cuh"
 #include "mfcc_mma.cuh"
+#include "trigger.cuh"
 
 using namespace pb;
 
@@ -115,6 +116,13 @@ struct NetWeights {
     DevArray<uint4> wg_b1, wg_b2; DevArray<float> wg_bias;
 };
 
+// A stream's TriggerDetector arguments as pb_set_stream_trigger took them (the host mirror of a TrigRec).
+struct StreamTrig {
+    double sensitivity;
+    int32_t trigger_level;
+    int32_t chunk_bytes;
+};
+
 // One model of a handle's bank: its network, ThresholdDecoder table, TriggerDetector state and weights.  It reads the
 // handle's MFCC ring; the front-end fields of its cfg equal the handle's.
 struct Network {
@@ -125,6 +133,11 @@ struct Network {
     DevArray<int> trig;              // [max_streams] TriggerDetector.activation
     int gru_mode = 0;                // 0 = auto, 1 = force CUDA-core kernel, 2 = force tensor-core kernel (pb_debug_gru_mode, slot 0)
     std::unique_ptr<NetWeights> w;   // null until weights are loaded
+    // per-stream TriggerDetector settings (pb_set_stream_trigger); a model that never gets them keeps trig_set = false and
+    // its scan updates the trigger in epilogue, as before
+    bool trig_set = false;           // sticky, set by the first pb_set_stream_trigger on this slot
+    std::vector<StreamTrig> trig_host;  // [max_streams] the settings as set (defaults until then)
+    DevArray<TrigRec> trig_rec;      // [max_streams] their records, read by trigger_kernel
 };
 
 // A handle: the MFCC front end (tables, per-stream sample count, tail and ring), the host pipeline and the profiler, shared
@@ -874,6 +887,13 @@ static StreamState stream_state(const pb_handle* h) {
     return st;
 }
 
+// TriggerDetector's refractory count -(8 * 2048) // chunk_size for chunk_size in bytes (>= 1), Python floor division.
+static int trigger_reset(long long bytes) {
+    long long q = -(8 * 2048) / bytes;                            // C truncates toward zero ...
+    if ((-(8 * 2048)) % bytes != 0) q -= 1;                       // ... python floors
+    return (int)q;
+}
+
 static DecodeParams decode_params(const Network& net) {
     const pb_config& c = net.cfg;
     DecodeParams d;
@@ -882,12 +902,36 @@ static DecodeParams decode_params(const Network& net) {
     d.center = c.threshold_center;
     d.hot_threshold = 1.0 - c.sensitivity;
     d.trigger_level = c.trigger_level;
-    const long long bytes = 2LL * c.chunk_samples;                // TriggerDetector.chunk_size is in bytes
-    long long q = -(8 * 2048) / bytes;                            // C truncates toward zero ...
-    if ((-(8 * 2048)) % bytes != 0) q -= 1;                       // ... python floors
-    d.trigger_reset = (int)q;
+    d.trigger_reset = trigger_reset(2LL * c.chunk_samples);        // TriggerDetector.chunk_size is in bytes
     d.legacy_f64 = c.decode_legacy_f64 != 0;
     return d;
+}
+
+// What a stream of net uses until pb_set_stream_trigger sets it: the model's own sensitivity and trigger_level, and the
+// handle's chunk in bytes (capped at INT32_MAX, where the refractory count is -1 as for any chunk above 16 384 B).
+static StreamTrig default_trig(const Network& net) {
+    return StreamTrig{net.cfg.sensitivity, net.cfg.trigger_level, (int32_t)std::min<long long>(2LL * net.cfg.chunk_samples, INT32_MAX)};
+}
+
+static TrigRec trig_record(const StreamTrig& v) {
+    return TrigRec{1.0 - v.sensitivity, v.trigger_level, trigger_reset(v.chunk_bytes)};
+}
+
+// A model with per-stream settings: its scan (K2Out o) writes raw and conf only, and trigger_kernel's slot nt, filled here from
+// o, updates the trigger, fired and count afterwards.
+static void defer_trigger(TrigTick& t, int& nt, const Network& net, unsigned route_bit, K2Out& o) {
+    t.conf[nt] = o.conf; t.fired[nt] = o.fired; t.count[nt] = o.count; t.trig[nt] = o.trig;
+    t.rec[nt] = net.trig_rec.get(); t.route_bit[nt] = route_bit;
+    ++nt;
+    o.trig = nullptr; o.fired = nullptr; o.count = nullptr;
+}
+
+// trigger_kernel over the nt deferred models of a tick; runs after their scans, on the same stream.
+static int launch_trigger(const TrigTick& t, int nt, cudaStream_t s) {
+    if (nt == 0 || t.n == 0) return PB_OK;
+    trigger_kernel<<<dim3((unsigned)((t.n + 255) / 256), (unsigned)nt), 256, 0, s>>>(t);
+    CK(cudaGetLastError());
+    return PB_OK;
 }
 
 template <typename T>
@@ -1166,17 +1210,25 @@ static int score_model0(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_
     const Network& net = h->models[0];
     K2Out o{};
     o.raw = d_raw; o.conf = d_conf; o.fired = d_fired; o.count = d_count; o.trig = net.trig.get();
-    if (!h->routed) return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
-    // routed: NaN fill of the items whose stream lacks bit 0, then the usual kernel with the epilogue's mask.  No list scratch:
-    // pb_update_host runs this on three streams at once.
+    if (!h->routed && !net.trig_set) return launch_gru(h, net, stream_k2in(h, d_ids), true, n, o, s);
+    TrigTick t{};
+    t.ids = d_ids; t.n = n;
+    int nt = 0;
+    if (net.trig_set) defer_trigger(t, nt, net, 1u, o);
     ProfScope ps(h, 1, s);
-    RouteOut r{};
-    r.raw = d_raw; r.conf = d_conf; r.fired = d_fired; r.M = 1;
-    route_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(h->d_route.get(), d_ids, n, r);
-    CK(cudaGetLastError());
-    if (h->subs[0] == 0) return PB_OK;
-    o.route = h->d_route.get(); o.route_bit = 1;
-    return launch_gru_kernels(net, h->feat, stream_k2in(h, d_ids), true, n, o, s);
+    if (h->routed) {
+        // NaN fill of the items whose stream lacks bit 0, then the usual kernel with the epilogue's mask.  No list scratch:
+        // pb_update_host runs this on three streams at once.
+        RouteOut r{};
+        r.raw = d_raw; r.conf = d_conf; r.fired = d_fired; r.M = 1;
+        route_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(h->d_route.get(), d_ids, n, r);
+        CK(cudaGetLastError());
+        if (h->subs[0] == 0) return PB_OK;
+        o.route = h->d_route.get(); o.route_bit = 1;
+        t.route = h->d_route.get();
+    }
+    const int rc = launch_gru_kernels(net, h->feat, stream_k2in(h, d_ids), true, n, o, s);
+    return rc != PB_OK ? rc : launch_trigger(t, nt, s);
 }
 
 PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
@@ -1270,6 +1322,9 @@ static int score_bank_routed(pb_handle* h, const int32_t* d_ids, int64_t n, floa
     r.raw = d_raw; r.conf = d_conf; r.fired = d_fired; r.M = M;
     r.lists = lists; r.list_stride = stride; r.count = counts;
     K2Out o[PB_MAX_MODELS];
+    TrigTick t{};
+    t.route = h->d_route.get(); t.ids = d_ids; t.n = n;
+    int nt = 0;
     for (int m = 0; m < M; ++m) {
         o[m] = K2Out{};
         o[m].raw = d_raw ? d_raw + (int64_t)m * n : nullptr;
@@ -1277,6 +1332,7 @@ static int score_bank_routed(pb_handle* h, const int32_t* d_ids, int64_t n, floa
         o[m].fired = d_fired ? d_fired + (int64_t)m * n : nullptr;
         o[m].count = d_count ? d_count + m : nullptr;
         o[m].trig = h->models[m].trig.get();
+        if (h->models[m].trig_set && h->subs[m] > 0) defer_trigger(t, nt, h->models[m], 1u << m, o[m]);
         if (bank_fused(h->models[m], h->feat)) r.listed |= 1u << m;
     }
     route_kernel<<<(int)((n + 255) / 256), 256, 0, s>>>(h->d_route.get(), d_ids, n, r);
@@ -1307,6 +1363,8 @@ static int score_bank_routed(pb_handle* h, const int32_t* d_ids, int64_t n, floa
         else gru_bank_routed_kernel<false><<<tiles, MMA_THREADS, BANK_MODEL_SMEM + BANK_STAGE_SMEM, s>>>(P, R, in);
         CK(cudaGetLastError());
     }
+    const int rc = launch_trigger(t, nt, s);
+    if (rc != PB_OK) return rc;
     CK(cudaEventRecord(h->route_ev, s));
     return PB_OK;
 }
@@ -1322,7 +1380,9 @@ static int score_bank(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_ra
     ProfScope ps(h, 1, s);
     // the fused family in one gru_bank_kernel launch; other networks one launch each of their own kernel, on the same ring
     BankParams P{};
-    int nm = 0;
+    TrigTick t{};
+    t.ids = d_ids; t.n = n;
+    int nm = 0, nt = 0;
     for (int m = 0; m < M; ++m) {
         const Network& net = h->models[m];
         K2Out o{};
@@ -1331,6 +1391,7 @@ static int score_bank(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_ra
         o.fired = d_fired ? d_fired + (int64_t)m * n : nullptr;
         o.count = d_count ? d_count + m : nullptr;
         o.trig = net.trig.get();
+        if (net.trig_set) defer_trigger(t, nt, net, 1u << m, o);
         if (bank_fused(net, h->feat)) {
             set_bank_slot(P, nm++, net, o);
         } else {
@@ -1338,7 +1399,11 @@ static int score_bank(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_ra
             if (rc != PB_OK) return rc;
         }
     }
-    return nm ? launch_bank(P, nm, in, n, s) : PB_OK;
+    if (nm) {
+        rc = launch_bank(P, nm, in, n, s);
+        if (rc != PB_OK) return rc;
+    }
+    return launch_trigger(t, nt, s);
 }
 
 PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf,
@@ -1525,6 +1590,84 @@ PB_API int pb_get_stream_models(const pb_handle* h, const int32_t* h_ids, int64_
     if (rc != PB_OK) return rc;
     if (n > 0 && !h_masks) return fail(PB_ERR_INVALID, "null masks");
     for (int64_t i = 0; i < n; ++i) h_masks[i] = h->routed ? h->route_mask[h_ids ? h_ids[i] : i] : 0xFF;
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// per-stream TriggerDetector settings
+
+static bool same_trig(const StreamTrig& a, const StreamTrig& b) {
+    uint64_t x, y;
+    memcpy(&x, &a.sensitivity, 8);
+    memcpy(&y, &b.sensitivity, 8);
+    return x == y && a.trigger_level == b.trigger_level && a.chunk_bytes == b.chunk_bytes;
+}
+
+// The first pb_set_stream_trigger on a model: its records, every stream on the model's defaults.  Only then is it flagged.
+static int ensure_trig_records(pb_handle* h, Network& net) {
+    if (net.trig_set) return PB_OK;
+    const size_t S = (size_t)h->cfg.max_streams;
+    const StreamTrig d = default_trig(net);
+    DevArray<TrigRec> rec;
+    CK(rec.upload(std::vector<TrigRec>(S, trig_record(d))));
+    net.trig_rec = std::move(rec);
+    net.trig_host.assign(S, d);
+    net.trig_set = true;
+    return PB_OK;
+}
+
+PB_API int pb_set_stream_trigger(pb_handle* h, int32_t slot, const int32_t* h_ids, const double* h_sensitivity,
+                                 const int32_t* h_trigger_level, const int32_t* h_chunk_bytes, int64_t n) {
+    int rc = check_route_ids(h, h_ids, n, true);
+    if (rc != PB_OK) return rc;
+    if (slot < 0 || slot >= (int)h->models.size()) return fail(PB_ERR_INVALID, "slot %d outside [0, %d)", slot, (int)h->models.size());
+    if (n > 0 && (!h_sensitivity || !h_trigger_level || !h_chunk_bytes)) return fail(PB_ERR_INVALID, "null settings");
+    for (int64_t i = 0; i < n; ++i)
+        if (h_chunk_bytes[i] < 1)
+            return fail(PB_ERR_INVALID, "chunk_bytes = %d (entry %lld) must be >= 1: TriggerDetector divides by it", h_chunk_bytes[i], (long long)i);
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued work finishes under the old settings
+    Network& net = h->models[slot];
+    rc = ensure_trig_records(h, net);
+    if (rc != PB_OK) return rc;
+    std::vector<int> sids;
+    std::vector<StreamTrig> vals;
+    std::vector<TrigRec> recs;
+    for (int64_t i = 0; i < n; ++i) {
+        const int sid = h_ids ? h_ids[i] : (int)i;
+        const StreamTrig v{h_sensitivity[i], h_trigger_level[i], h_chunk_bytes[i]};
+        if (same_trig(v, net.trig_host[sid])) continue;      // unchanged: the detector keeps its state
+        sids.push_back(sid);
+        vals.push_back(v);
+        recs.push_back(trig_record(v));
+    }
+    if (sids.empty()) return PB_OK;
+    DevArray<int> d_sids;
+    DevArray<TrigRec> d_recs;
+    CK(d_sids.upload(sids));
+    CK(d_recs.upload(recs));
+    const long long k = (long long)sids.size();
+    set_trigger_kernel<<<(int)((k + 255) / 256), 256>>>(net.trig_rec.get(), net.trig.get(), d_sids.get(), d_recs.get(), k);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    for (size_t j = 0; j < sids.size(); ++j) net.trig_host[sids[j]] = vals[j];
+    return PB_OK;
+}
+
+PB_API int pb_get_stream_trigger(const pb_handle* h, int32_t slot, const int32_t* h_ids, int64_t n, double* h_sensitivity,
+                                 int32_t* h_trigger_level, int32_t* h_chunk_bytes) {
+    const int rc = check_route_ids(h, h_ids, n, false);
+    if (rc != PB_OK) return rc;
+    if (slot < 0 || slot >= (int)h->models.size()) return fail(PB_ERR_INVALID, "slot %d outside [0, %d)", slot, (int)h->models.size());
+    if (n > 0 && (!h_sensitivity || !h_trigger_level || !h_chunk_bytes)) return fail(PB_ERR_INVALID, "null output");
+    const Network& net = h->models[slot];
+    const StreamTrig d = default_trig(net);
+    for (int64_t i = 0; i < n; ++i) {
+        const StreamTrig& v = net.trig_set ? net.trig_host[h_ids ? h_ids[i] : i] : d;
+        h_sensitivity[i] = v.sensitivity;
+        h_trigger_level[i] = v.trigger_level;
+        h_chunk_bytes[i] = v.chunk_bytes;
+    }
     return PB_OK;
 }
 
