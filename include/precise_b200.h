@@ -268,6 +268,52 @@ int pb_set_stream_trigger(pb_handle* h, int32_t slot, const int32_t* h_stream_id
 int pb_get_stream_trigger(const pb_handle* h, int32_t slot, const int32_t* h_stream_ids, int64_t n,
                           double* h_sensitivity, int32_t* h_trigger_level, int32_t* h_chunk_bytes);
 
+/* Stream state export / import: a stream's listener state (Listener's window_audio and mfccs, network_runner.py:101-109,
+ * and each bank model's TriggerDetector.activation, runner.py:125) as a self-describing record, so a stream can be
+ * checkpointed to host memory or disk, or moved to another handle (a larger max_streams, another GPU, a new process).
+ *
+ * Record layout, pb_stream_state_bytes(h) bytes, every section 16-byte aligned:
+ *   [0, 96)                      pb_stream_state_header below
+ *   [96, 96 + 2 tail_cap)        the tail, tail_cap int16 copied whole; tail_cap = round_up(min(n_fft, window_samples), 8)
+ *   [96 + 2 tail_cap, end)       the MFCC ring, ring_rows x row_stride float32 copied whole, padding columns included;
+ *                                row_stride = round_up(mfcc width, 4), ring_rows = n_features + (release window - min(n_fft,
+ *                                window_samples)) / hop_samples + 2, release window = window_samples (+ hop_samples for the
+ *                                speechpy vectoriser)
+ * The size depends only on the front-end fields, so two handles with the same front end agree on it (1024 + 2048 + 96 =
+ * 3168 B at the defaults).  Not in the record: subscription masks and per-stream trigger settings (pb_get_stream_models /
+ * pb_get_stream_trigger read them), and the handle's chunk_samples (a record imports into a handle with another chunk). */
+#define PB_STATE_MAGIC 0x53534250u    /* "PBSS" in little-endian bytes */
+#define PB_STATE_VERSION 1
+typedef struct pb_stream_state_header {
+    uint32_t magic;                   /* PB_STATE_MAGIC                                                     */
+    uint32_t version;                 /* PB_STATE_VERSION                                                   */
+    int32_t num_models;               /* pb_num_models of the exporting handle                              */
+    int32_t sample_rate, window_samples, hop_samples, n_fft, n_filt, n_mfcc, n_features, use_delta, vectorizer;
+    int64_t n_samples;                /* samples the stream has consumed                                    */
+    int32_t reserved[2];              /* 0                                                                  */
+    int32_t activation[PB_MAX_MODELS];  /* TriggerDetector.activation of bank slot m; 0 from num_models on  */
+} pb_stream_state_header;
+
+/* Bytes of one stream's record (a multiple of 16), or a negative pb_status. */
+int64_t pb_stream_state_bytes(const pb_handle* h);
+/* Writes the records of streams d_stream_ids[i] (DEVICE; NULL => 0..n-1) to d_out [n][pb_stream_state_bytes] (DEVICE,
+ * 16-byte aligned).  Asynchronous on `stream`, like pb_read_window: the caller orders it after the ticks whose state it
+ * wants.  Reads state only: ticks after an export compute what they would have computed without it.  PB_ERR_INVALID: null
+ * handle, n outside [0, max_streams], a null or unaligned d_out with n > 0. */
+int pb_export_streams(pb_handle* h, const int32_t* d_stream_ids, int64_t n, void* d_out, void* stream);
+/* Overwrites the state of streams h_stream_ids[i] (HOST; NULL => 0..n-1; unique, in [0, max_streams)) with record i of d_in
+ * [n][pb_stream_state_bytes] (DEVICE, 16-byte aligned).  Slot m's activation goes to slot m: the caller makes sure the banks
+ * correspond (the library does not fingerprint weights).  Synchronous: work already queued on the device finishes first.
+ * Every record is validated before anything is written; on an error the handle is unchanged.
+ *   PB_ERR_INVALID: null handle, n outside [0, max_streams], a bad or duplicate id, a null or unaligned d_in with n > 0, or a
+ *   record with the wrong magic or version, a front-end field or model count that differs from this handle's, or
+ *   n_samples < 0 (the message names the first bad record and the field).
+ *   A record whose n_samples is not a multiple of 8 (a stream that took ragged ticks) makes the handle ragged, as its first
+ *   pb_update_ragged does; PB_ERR_STATE if pb_debug_k1_mode is then non-zero.  Records that are all multiples of 8 leave
+ *   the handle as it was, so its uniform ticks keep the fast MFCC kernel.
+ * The imported streams keep this handle's masks and trigger settings. */
+int pb_import_streams(pb_handle* h, const int32_t* h_stream_ids, int64_t n, const void* d_in);
+
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);

@@ -4,9 +4,11 @@ TriggerDetector.update] per tick, all state device-resident.
 """
 import numpy as np
 
-from .core import PreciseB200
+from .core import FRONT_END_FIELDS, PreciseB200, _check_np
 from .model_io import GruModel
 from .params import ListenerParams
+
+STATE_FIELDS = ('magic', 'version', 'num_models') + FRONT_END_FIELDS    # the first 12 int32 words of a state record
 
 
 class StreamBatch:
@@ -46,6 +48,63 @@ class StreamBatch:
     def stream_trigger(self, slot, ids=None):
         """(sensitivity, trigger_level, chunk_size) host arrays of bank slot ``slot``.  See PreciseB200.stream_trigger."""
         return self.core.stream_trigger(slot, ids)
+
+    def _host_ids(self, ids, n):
+        _check_np('ids', ids, np.int32, (n,))
+        if ids is None:
+            return np.arange(n, dtype=np.int32)
+        if n and (ids.min() < 0 or ids.max() >= self.n_streams or len(np.unique(ids)) != n):
+            raise ValueError('stream ids must be unique and lie in [0, %d)' % self.n_streams)
+        return ids
+
+    def export_streams(self, ids=None):
+        """A snapshot of streams ids (host int32 array; None: every stream): dict(state = their state records, a uint8 CUDA
+        tensor [n, stream_state_bytes]; stream_models = their masks; stream_trigger = each bank slot's (sensitivity,
+        trigger_level, chunk_size)).  The tensor may go through .cpu() or .to(another device) and come back.  See
+        PreciseB200.export_streams."""
+        core = self.core
+        n = self.n_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
+        sids = self._host_ids(ids, n)
+        state = core.export_streams(core.torch.from_numpy(sids).to(core.device))
+        return dict(state=state, stream_models=core.stream_models(sids),
+                    stream_trigger=[core.stream_trigger(m, sids) for m in range(core.num_models)])
+
+    def import_streams(self, snapshot, ids=None):
+        """Continue the snapshot's streams (export_streams of a batch with the same front end and bank) as streams ids (host
+        int32 array; None: 0..n-1) of this batch.  Their masks, then each slot's trigger settings are set where they differ
+        from this batch's, so a batch never becomes routed or trigger-flagged for nothing; then the state is imported, which
+        overwrites the activations those two steps may have re-armed.  A snapshot that does not match raises ValueError
+        before anything changes."""
+        core = self.core
+        torch = core.torch
+        state = snapshot['state'].to(core.device)
+        masks = np.asarray(snapshot['stream_models'], np.uint8)
+        trig = snapshot['stream_trigger']
+        n = state.shape[0] if state.dim() == 2 else -1
+        core._check_state('state', state, n)
+        sids = self._host_ids(ids, n)
+        _check_np('stream_models', masks, np.uint8, (n,), optional=False)
+        if len(trig) != core.num_models:
+            raise ValueError('snapshot has trigger settings of %d bank models, this batch has %d' % (len(trig), core.num_models))
+        # the record headers against this batch's own, so that the steps below never run for a snapshot import would refuse
+        ref = core.export_streams(n=1)[0, :48]
+        bad = (state[:, :48] != ref).any(1) | (state[:, 48:56].contiguous().view(torch.int64)[:, 0] < 0)
+        if n and bool(bad.any()):
+            i = int(bad.nonzero()[0, 0])
+            got, want = state[i, :48].cpu().numpy().view(np.int32), ref.cpu().numpy().view(np.int32)
+            k = np.nonzero(got != want)[0]
+            what = ('%s = %d, this batch has %d' % (STATE_FIELDS[k[0]], got[k[0]], want[k[0]])) if k.size else 'n_samples < 0'
+            raise ValueError('snapshot record %d does not match this batch: %s; nothing was changed' % (i, what))
+        differ = core.stream_models(sids) != masks
+        if differ.any():
+            core.set_stream_models(masks[differ], sids[differ])
+        for slot, (sens, lvl, chunk) in enumerate(trig):
+            sens, lvl, chunk = np.asarray(sens, np.float64), np.asarray(lvl, np.int32), np.asarray(chunk, np.int32)
+            cs, cl, cc = core.stream_trigger(slot, sids)
+            differ = (cs.view(np.uint64) != sens.view(np.uint64)) | (cl != lvl) | (cc != chunk)
+            if differ.any():
+                core.set_stream_trigger(slot, sens[differ], lvl[differ], chunk[differ], ids=sids[differ])
+        core.import_streams(state, sids)
 
     def _bank_buffers(self, n):
         """The cached [M, n] outputs of a bank tick."""

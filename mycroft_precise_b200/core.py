@@ -65,6 +65,9 @@ SYMBOLS = {
     'pb_get_stream_models': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_set_stream_trigger': (C.c_int, [_VP, _I32, _VP, _VP, _VP, _VP, _I64]),
     'pb_get_stream_trigger': (C.c_int, [_VP, _I32, _VP, _I64, _VP, _VP, _VP]),
+    'pb_stream_state_bytes': (_I64, [_VP]),
+    'pb_export_streams': (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
+    'pb_import_streams': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -532,6 +535,46 @@ class PreciseB200:
         sens, level, chunk = np.zeros(n, np.float64), np.zeros(n, np.int32), np.zeros(n, np.int32)
         check(self.lib.pb_get_stream_trigger(self._h, slot, _np_ptr(ids), n, _np_ptr(sens), _np_ptr(level), _np_ptr(chunk)))
         return sens, level, chunk
+
+    # ---- stream state export / import
+    @property
+    def stream_state_bytes(self) -> int:
+        """Bytes of one stream's state record (layout: include/precise_b200.h); equal on every handle with this front end."""
+        b = int(self.lib.pb_stream_state_bytes(self._h))
+        if b < 0:
+            check(b)
+        return b
+
+    def _check_state(self, name, t, n):
+        B = self.stream_state_bytes
+        if not isinstance(t, self.torch.Tensor) or tuple(t.shape) != (n, B):
+            raise ValueError('%s must be a [n, %d] uint8 tensor of stream state records, got shape %s'
+                             % (name, B, tuple(getattr(t, 'shape', ()))))
+        self._check_t(name, t, self.torch.uint8, n * B, optional=False)
+
+    def export_streams(self, ids=None, n=None, out=None):
+        """The state records of streams ids (int32 CUDA tensor; None: streams 0..n-1, n defaulting to max_streams): a uint8
+        CUDA tensor [n, stream_state_bytes], written into ``out`` when given.  Asynchronous on the current stream, after the
+        ticks queued before it; reads state only."""
+        torch = self.torch
+        n = ids.numel() if ids is not None else (self.max_streams if n is None else n)
+        self._check_ids(ids, n)
+        if out is None:
+            out = torch.empty((n, self.stream_state_bytes), dtype=torch.uint8, device=self.device)
+        else:
+            self._check_state('out', out, n)
+        check(self.lib.pb_export_streams(self._h, _ptr(ids), n, _ptr(out), self._stream()))
+        return out
+
+    def import_streams(self, state, ids=None):
+        """Overwrite streams ids[i] (host int32 array, unique; None: streams 0..n-1) with record i of ``state``, a uint8 tensor
+        [n, stream_state_bytes] on this handle's device from export_streams of a handle with the same front end and bank
+        size (its chunk_samples may differ).  Bank slot m's trigger state goes to slot m.  The streams keep this handle's
+        masks and trigger settings.  Synchronous; a bad record or id raises ValueError and changes nothing."""
+        n = state.shape[0] if isinstance(state, self.torch.Tensor) and state.dim() == 2 else -1
+        self._check_state('state', state, n)
+        _check_np('ids', ids, np.int32, (n,))
+        check(self.lib.pb_import_streams(self._h, _np_ptr(ids), n, _ptr(state)))
 
     def update_host(self, pcm_np, conf_np, raw_np=None, fired_np=None, ids_np=None) -> int:
         """Host-buffer tick (numpy arrays, ideally backed by pinned memory).  Returns this tick's count."""

@@ -29,6 +29,7 @@
 #include "mfcc_tc3.cuh"
 #include "mfcc_mma.cuh"
 #include "trigger.cuh"
+#include "stream_state.cuh"
 
 using namespace pb;
 
@@ -1668,6 +1669,95 @@ PB_API int pb_get_stream_trigger(const pb_handle* h, int32_t slot, const int32_t
         h_trigger_level[i] = v.trigger_level;
         h_chunk_bytes[i] = v.chunk_bytes;
     }
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// stream state export / import (stream_state.cuh)
+
+static const char* const STATE_FIELD[] = {"magic", "version", "num_models", "sample_rate", "window_samples", "hop_samples",
+                                          "n_fft", "n_filt", "n_mfcc", "n_features", "use_delta", "vectorizer"};
+static_assert(sizeof(STATE_FIELD) / sizeof(STATE_FIELD[0]) == STATE_HEAD_WORDS, "one name per header word");
+
+static StateLayout state_layout(const pb_handle* h) {
+    const pb_config& c = h->cfg;
+    const int32_t fe[] = {c.sample_rate, c.window_samples, c.hop_samples, c.n_fft, c.n_filt, c.n_mfcc, c.n_features,
+                          c.use_delta, c.vectorizer};
+    StateLayout L{};
+    L.head[0] = PB_STATE_MAGIC;
+    L.head[1] = PB_STATE_VERSION;
+    L.head[2] = (unsigned)h->models.size();
+    for (int i = 0; i < 9; ++i) L.head[3 + i] = (unsigned)fe[i];
+    for (size_t m = 0; m < h->models.size(); ++m) L.trig[m] = h->models[m].trig.get();
+    L.tail_vecs = h->tail_cap / 8;                                   // tail_cap is a multiple of 8 int16
+    L.ring_vecs = h->ring_rows * h->row_stride / 4;                  // row_stride is a multiple of 4 floats
+    L.rec_vecs = STATE_HEADER_VECS + L.tail_vecs + L.ring_vecs;
+    return L;
+}
+
+PB_API int64_t pb_stream_state_bytes(const pb_handle* h) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    return state_layout(h).rec_vecs * 16;
+}
+
+PB_API int pb_export_streams(pb_handle* h, const int32_t* d_ids, int64_t n, void* d_out, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (n < 0 || n > h->cfg.max_streams) return fail(PB_ERR_INVALID, "n = %lld outside [0, max_streams = %d]", (long long)n, h->cfg.max_streams);
+    if (n == 0) return PB_OK;
+    if (!d_out) return fail(PB_ERR_INVALID, "null d_out");
+    if ((uintptr_t)d_out % 16 != 0) return fail(PB_ERR_INVALID, "d_out must be 16-byte aligned");
+    CK(cudaSetDevice(h->cfg.device));
+    const int per = STATE_THREADS / 32;
+    export_state_kernel<<<(unsigned)((n + per - 1) / per), STATE_THREADS, 0, (cudaStream_t)stream>>>(
+        state_layout(h), stream_state(h), d_ids, n, static_cast<uint4*>(d_out));
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+PB_API int pb_import_streams(pb_handle* h, const int32_t* h_ids, int64_t n, const void* d_in) {
+    int rc = check_route_ids(h, h_ids, n, true);
+    if (rc != PB_OK) return rc;
+    if (n == 0) return PB_OK;
+    if (!d_in) return fail(PB_ERR_INVALID, "null d_in");
+    if ((uintptr_t)d_in % 16 != 0) return fail(PB_ERR_INVALID, "d_in must be 16-byte aligned");
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued work finishes on the old state
+    const StateLayout L = state_layout(h);
+    const uint4* in = static_cast<const uint4*>(d_in);
+    DevArray<StateCheck> d_check;
+    const StateCheck init{~0ull, 0u, 0u};
+    CK(d_check.upload(std::vector<StateCheck>(1, init)));
+    validate_state_kernel<<<(unsigned)((n + STATE_THREADS - 1) / STATE_THREADS), STATE_THREADS>>>(L, in, n, d_check.get());
+    CK(cudaGetLastError());
+    StateCheck chk;
+    CK(cudaMemcpy(&chk, d_check.get(), sizeof(chk), cudaMemcpyDeviceToHost));
+    if (chk.bad) {
+        const long long i = (long long)(chk.first >> 8);
+        const int reason = (int)(chk.first & 0xff);
+        pb_stream_state_header hd;
+        CK(cudaMemcpy(&hd, in + i * L.rec_vecs, sizeof(hd), cudaMemcpyDeviceToHost));
+        if (reason == STATE_BAD_N_SAMPLES)
+            return fail(PB_ERR_INVALID, "record %lld: n_samples = %lld < 0 (%u bad records; nothing imported)", i, (long long)hd.n_samples, chk.bad);
+        unsigned got[STATE_HEAD_WORDS];
+        memcpy(got, &hd, sizeof(got));
+        const int k = reason - 1;
+        if (k < 2)
+            return fail(PB_ERR_INVALID, "record %lld: %s = 0x%x, expected 0x%x: not a stream state record of this format (%u bad records; nothing imported)",
+                        i, STATE_FIELD[k], got[k], L.head[k], chk.bad);
+        return fail(PB_ERR_INVALID, "record %lld: %s = %d, this handle has %d (%u bad records; nothing imported)", i, STATE_FIELD[k],
+                    (int)got[k], (int)L.head[k], chk.bad);
+    }
+    // K1's aligned-only kernels (and k1 modes 2-6) need n_samples % 8 == 0 (§3 "Sticky routing"): an unaligned record makes the
+    // handle ragged, as its first pb_update_ragged does
+    if (chk.unaligned && h->k1_mode != 0)
+        return fail(PB_ERR_STATE, "a record's n_samples is not a multiple of 8 (the stream took ragged ticks): it needs k1 mode 0; nothing imported");
+    DevArray<int> d_sids;
+    if (h_ids) CK(d_sids.upload(std::vector<int>(h_ids, h_ids + n)));
+    const int per = STATE_THREADS / 32;
+    import_state_kernel<<<(unsigned)((n + per - 1) / per), STATE_THREADS>>>(L, stream_state(h), d_sids.get(), n, in);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    if (chk.unaligned) h->ragged = true;
     return PB_OK;
 }
 

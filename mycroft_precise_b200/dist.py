@@ -6,7 +6,8 @@ import os
 
 
 def shard_range(n_streams: int, rank: int, world: int):
-    """Contiguous block sharding: stream s lives on rank s // ceil(n/world); state never migrates."""
+    """Contiguous block sharding: stream s lives on rank s // ceil(n/world).  A stream's state can move to another handle or
+    rank with StreamBatch.export_streams / import_streams; carrying the snapshot between ranks is the caller's."""
     per = -(-n_streams // world)
     lo = min(rank * per, n_streams)
     hi = min(lo + per, n_streams)
