@@ -314,13 +314,47 @@ int pb_export_streams(pb_handle* h, const int32_t* d_stream_ids, int64_t n, void
  * The imported streams keep this handle's masks and trigger settings. */
 int pb_import_streams(pb_handle* h, const int32_t* h_stream_ids, int64_t n, const void* d_in);
 
+/* Stream audio history: the recent int16 audio of chosen streams, kept on the device, so that a server can save the clip
+ * behind an activation (the reference's listen.py keeps `audio_buffer`, buffer_samples long, and saves it on every
+ * activation: precise/scripts/listen.py:59, :88-90).  Opt-in per stream: 2 B per sample and stream that has it.
+ *   - Invariant: sample k of a stream's audio, counted as n_samples counts, lives at position k mod cap of the stream's row;
+ *     cap is history_samples rounded up to a multiple of 8.  A chunk longer than cap keeps its last cap samples.
+ *   - Which ticks append: every tick that consumes audio -- pb_update, pb_update_models, pb_update_ragged (each item's chunk
+ *     exactly as K1 takes it, offsets clamped the same way), pb_update_vectors and pb_update_host (pipelined and zero-copy) --
+ *     masks or not.  The stateless calls (pb_mfcc*, pb_predict) do not.
+ *   - History start: a stream's n_samples when it was switched on, cleared (pb_clear: 0) or imported into (the record's
+ *     n_samples), whichever came last.  Positions before it read as 0, so a read never returns audio of a previous life.
+ *   - Not in state records (pb_export_streams): an imported stream that has history starts empty at the record's n_samples.
+ *   - A handle without a pool runs exactly as before.
+ *
+ * pb_set_history: a pool of max_rows rows (max_rows in [1, max_streams]) of the last history_samples (>= 1) samples each.
+ * Synchronous.  Calling it again replaces the pool and switches every stream off; (0, 0) frees it (pb_destroy frees it too).
+ * PB_ERR_INVALID: null handle, a value out of range.  PB_ERR_CUDA: the allocation failed (the handle then has no pool). */
+int pb_set_history(pb_handle* h, int64_t history_samples, int32_t max_rows);
+/* Switches streams h_stream_ids[i] (HOST; NULL => 0..n-1) on (h_on[i] != 0) or off.  A stream that goes on starts empty at
+ * its n_samples; one already on keeps its audio; one that goes off returns its row to the pool.  Validates everything before
+ * it changes anything, then synchronises the device.  PB_ERR_INVALID, and nothing changes: null handle, n outside
+ * [0, max_streams], an id outside [0, max_streams), a duplicate id, a null array with n > 0, more streams on than max_rows
+ * after the call.  PB_ERR_STATE: no pool. */
+int pb_set_stream_history(pb_handle* h, const int32_t* h_stream_ids, const uint8_t* h_on, int64_t n);
+/* 1 if stream h_stream_ids[i] (HOST; NULL => 0..n-1) has history, else 0 (all 0 without a pool), into h_on [n] (HOST).
+ * PB_ERR_INVALID: null handle or h_on with n > 0, n outside [0, max_streams], an id outside [0, max_streams). */
+int pb_get_stream_history(const pb_handle* h, const int32_t* h_stream_ids, int64_t n, uint8_t* h_on);
+/* d_out [n][samples] int16 (DEVICE): row i = samples [N - samples, N) of stream d_stream_ids[i] (DEVICE; NULL => 0..n-1),
+ * oldest first, N = its n_samples at that point in stream order; 0 before its history start, all 0 for a stream that is off.
+ * samples in [1, history_samples].  Asynchronous on `stream`, like pb_read_window; writes nothing but d_out.
+ * PB_ERR_INVALID: null handle or d_out with n > 0, n outside [0, max_streams], samples out of range.  PB_ERR_STATE: no
+ * pool. */
+int pb_read_history(pb_handle* h, const int32_t* d_stream_ids, int64_t n, int64_t samples, int16_t* d_out, void* stream);
+
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);
 
 /* Per-kernel device timing (CUDA events on the launching stream), for bench.py's roofline.
  * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel (a bank tick: all its network kernels), 2 = decode-only kernel,
- * 3 = unused (always 0).
+ * 3 = stream audio history kernels (the append of each tick, pb_read_history, switching and restarts; always 0 on a handle
+ * without a history pool).
  * pb_profile_read synchronises the recorded events, returns accumulated ms and launch counts
  * since the last pb_profile_reset. */
 int pb_profile_enable(pb_handle* h, int on);

@@ -49,6 +49,46 @@ class StreamBatch:
         """(sensitivity, trigger_level, chunk_size) host arrays of bank slot ``slot``.  See PreciseB200.stream_trigger."""
         return self.core.stream_trigger(slot, ids)
 
+    def set_history(self, samples=None, max_rows=None):
+        """A device pool for the recent audio of up to ``max_rows`` streams, ``samples`` each (default buffer_samples, the
+        reference's clip).  See PreciseB200.set_history."""
+        self.core.set_history(samples, max_rows)
+
+    def set_stream_history(self, on, ids=None):
+        """Switch each stream's history on or off; a scalar broadcasts.  See PreciseB200.set_stream_history."""
+        self.core.set_stream_history(on, ids)
+
+    def stream_history(self, ids=None):
+        """Host bool array: which streams have history.  See PreciseB200.stream_history."""
+        return self.core.stream_history(ids)
+
+    def read_history(self, ids=None, samples=None, out=None):
+        """int16 CUDA [n, samples]: each stream's last samples, oldest first.  See PreciseB200.read_history."""
+        return self.core.read_history(ids, samples, out)
+
+    def activation_audio(self, fired, ids=None, samples=None):
+        """The clip behind every activation of the tick just run, as listen.py saves it in on_activation: ``fired`` and ``ids``
+        are that tick's output ([n] or [M, n]) and ids (int32 CUDA tensor; None: items are streams 0..n-1).  Returns dict(slot =
+        bank slot, stream = stream id, audio = int16 [k, samples] ending with that tick's chunk) for every fired (model, item)
+        pair whose stream has history, in torch.nonzero order (model-major).  Call it before the next tick on those streams."""
+        core = self.core
+        torch = core.torch
+        f = fired if fired.dim() == 2 else fired.reshape(1, -1)
+        n = f.shape[1]
+        if ids is None:
+            ids = torch.arange(n, dtype=torch.int32, device=core.device)
+        core._check_t('ids', ids, torch.int32, n, optional=False)
+        pairs = torch.nonzero(f)
+        streams = ids[pairs[:, 1]]
+        keep = torch.from_numpy(core.stream_history(streams.cpu().numpy().astype(np.int32))).to(core.device)
+        pairs, streams = pairs[keep], streams[keep].contiguous()
+        if streams.numel() == 0:
+            s = core.history_samples if samples is None else int(samples)
+            audio = torch.empty((0, s), dtype=torch.int16, device=core.device)
+        else:
+            audio = core.read_history(streams, samples)
+        return dict(slot=pairs[:, 0], stream=streams, audio=audio)
+
     def _host_ids(self, ids, n):
         _check_np('ids', ids, np.int32, (n,))
         if ids is None:
@@ -60,8 +100,8 @@ class StreamBatch:
     def export_streams(self, ids=None):
         """A snapshot of streams ids (host int32 array; None: every stream): dict(state = their state records, a uint8 CUDA
         tensor [n, stream_state_bytes]; stream_models = their masks; stream_trigger = each bank slot's (sensitivity,
-        trigger_level, chunk_size)).  The tensor may go through .cpu() or .to(another device) and come back.  See
-        PreciseB200.export_streams."""
+        trigger_level, chunk_size)).  The tensor may go through .cpu() or .to(another device) and come back.  Whether a
+        stream has audio history, and that audio, are not part of a snapshot.  See PreciseB200.export_streams."""
         core = self.core
         n = self.n_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
         sids = self._host_ids(ids, n)
@@ -74,7 +114,8 @@ class StreamBatch:
         int32 array; None: 0..n-1) of this batch.  Their masks, then each slot's trigger settings are set where they differ
         from this batch's, so a batch never becomes routed or trigger-flagged for nothing; then the state is imported, which
         overwrites the activations those two steps may have re-armed.  A snapshot that does not match raises ValueError
-        before anything changes."""
+        before anything changes.  History on / off is not carried: the streams keep this batch's setting, and one that has
+        history starts empty at the imported sample count."""
         core = self.core
         torch = core.torch
         state = snapshot['state'].to(core.device)

@@ -68,6 +68,10 @@ SYMBOLS = {
     'pb_stream_state_bytes': (_I64, [_VP]),
     'pb_export_streams': (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
     'pb_import_streams': (C.c_int, [_VP, _VP, _I64, _VP]),
+    'pb_set_history': (C.c_int, [_VP, _I64, _I32]),
+    'pb_set_stream_history': (C.c_int, [_VP, _VP, _VP, _I64]),
+    'pb_get_stream_history': (C.c_int, [_VP, _VP, _I64, _VP]),
+    'pb_read_history': (C.c_int, [_VP, _VP, _I64, _I64, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -229,6 +233,7 @@ class PreciseB200:
         if hi > lo:                      # out_range 0 (threshold_decoder.py:48-49): the table is never indexed
             check(self.lib.pb_set_cdf(h, cd.ctypes.data_as(C.c_void_p), len(cd)))
         self._count = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self.history_samples = 0             # set_history's samples; 0 = no history pool
 
     def close(self):
         if getattr(self, '_h', None):
@@ -575,6 +580,72 @@ class PreciseB200:
         self._check_state('state', state, n)
         _check_np('ids', ids, np.int32, (n,))
         check(self.lib.pb_import_streams(self._h, _np_ptr(ids), n, _ptr(state)))
+
+    # ---- stream audio history
+    @staticmethod
+    def _int(name, v):
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+            raise ValueError('%s must be an integer, got %r' % (name, v))
+        return int(v)
+
+    def set_history(self, samples=None, max_rows=None):
+        """A device pool of ``max_rows`` rows (default max_streams), each holding the last ``samples`` int16 samples (default
+        params.buffer_samples, the clip the reference's listen.py saves) of one stream that has history.  Every stream starts
+        off (set_stream_history switches them on); calling it again replaces the pool, (0, 0) frees it.  Synchronous."""
+        samples = self._int('samples', self.params.buffer_samples if samples is None else samples)
+        max_rows = self._int('max_rows', self.max_streams if max_rows is None else max_rows)
+        if not -2 ** 31 <= max_rows < 2 ** 31:
+            raise ValueError('max_rows must fit in int32, got %d' % max_rows)
+        rc = self.lib.pb_set_history(self._h, samples, max_rows)
+        if rc != -1:                         # anything but a refused argument replaced the pool
+            self.history_samples = samples if rc == 0 else 0
+        check(rc)
+
+    def set_stream_history(self, on, ids=None):
+        """Switch history on (true) or off for streams ids (host int32 array; None: streams 0..n-1, n = len(on), or every
+        stream when ``on`` is a scalar, which broadcasts).  A stream that goes on starts empty; one already on keeps its audio.
+        Synchronous; bad input, or more streams on than the pool's rows, raises ValueError and changes nothing."""
+        on = np.asarray(on)
+        if on.ndim > 1 or on.dtype.kind not in 'biu':
+            raise ValueError('on must be a bool / integer scalar or 1-D array')
+        if ids is not None:
+            if not isinstance(ids, np.ndarray) or ids.ndim != 1:
+                raise ValueError('ids must be a 1-D int32 array')
+            n = ids.shape[0]
+        else:
+            n = on.shape[0] if on.ndim == 1 else self.max_streams
+        _check_np('ids', ids, np.int32, (n,))
+        if on.ndim == 1 and on.shape[0] != n:
+            raise ValueError('on has %d entries for %d streams' % (on.shape[0], n))
+        flags = np.ascontiguousarray(np.broadcast_to(on != 0, (n,)), dtype=np.uint8)
+        check(self.lib.pb_set_stream_history(self._h, _np_ptr(ids), _np_ptr(flags), n))
+
+    def stream_history(self, ids=None) -> np.ndarray:
+        """bool array: which of streams ids (host int32 array), or of every stream, have history."""
+        n = self.max_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
+        _check_np('ids', ids, np.int32, (n,))
+        out = np.zeros(n, np.uint8)
+        check(self.lib.pb_get_stream_history(self._h, _np_ptr(ids), n, _np_ptr(out)))
+        return out.astype(bool)
+
+    def read_history(self, ids=None, samples=None, out=None):
+        """The last ``samples`` (default: all set_history kept) samples of streams ids, as of the work queued before this call:
+        an int16 CUDA tensor [n, samples], oldest first, 0 before the stream's history start and for streams without history.
+        ids: int32 CUDA tensor (repeats allowed); None: every stream.  Asynchronous on the current stream."""
+        torch = self.torch
+        n = ids.numel() if ids is not None else self.max_streams
+        self._check_t('ids', ids, torch.int32, n)
+        if ids is not None and self.check_ids and n:
+            lo, hi = int(ids.min()), int(ids.max())
+            if lo < 0 or hi >= self.max_streams:
+                raise ValueError('stream ids must lie in [0, %d), got [%d, %d]' % (self.max_streams, lo, hi))
+        samples = self._int('samples', self.history_samples if samples is None else samples)
+        if out is None:
+            out = torch.empty((n, max(samples, 0)), dtype=torch.int16, device=self.device)
+        else:
+            self._check_t('out', out, torch.int16, n * samples, optional=False)
+        check(self.lib.pb_read_history(self._h, _ptr(ids), n, samples, _ptr(out), self._stream()))
+        return out
 
     def update_host(self, pcm_np, conf_np, raw_np=None, fired_np=None, ids_np=None) -> int:
         """Host-buffer tick (numpy arrays, ideally backed by pinned memory).  Returns this tick's count."""

@@ -30,6 +30,7 @@
 #include "mfcc_mma.cuh"
 #include "trigger.cuh"
 #include "stream_state.cuh"
+#include "history.cuh"
 
 using namespace pb;
 
@@ -181,6 +182,16 @@ struct pb_handle {
     DevArray<int2> d_route_list;     // [PB_MAX_MODELS][max_streams] route_kernel's (item, stream) lists: scratch of bank ticks
     DevArray<unsigned> d_route_count;  // [PB_MAX_MODELS] their lengths
     cudaEvent_t route_ev = nullptr;  // recorded after each routed bank tick; the next one waits on it before reusing the scratch
+    // stream audio history (pb_set_history); a handle without a pool keeps history = false and launches none of this
+    bool history = false;            // a pool exists
+    int64_t hist_samples = 0;        // history_samples as set
+    int hist_cap = 0;                // row length: hist_samples rounded up to a multiple of 8
+    int hist_rows = 0;               // max_rows
+    DevArray<int16_t> d_hist;        // [hist_rows][hist_cap] the pool
+    DevArray<int> d_hist_row;        // [max_streams] row of each stream, -1 = off
+    DevArray<long long> d_hist_start;  // [max_streams] history start
+    std::vector<int> hist_row;       // host mirror of d_hist_row
+    std::vector<int> hist_free;      // rows no stream owns
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
     cudaEvent_t pipe_ev[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -1189,11 +1200,41 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
     return PB_OK;
 }
 
+static HistPool hist_pool(const pb_handle* h) {
+    HistPool P;
+    P.rows = h->d_hist.get(); P.row_of = h->d_hist_row.get(); P.start = h->d_hist_start.get(); P.cap = h->hist_cap;
+    return P;
+}
+
+// History half of a tick, before its K1 (the pre-tick n_samples): item i's chunk as K1 takes it (d_offsets null: the uniform
+// tick's d_pcm[i * chunk_samples ..)) goes to the row of its stream.  Nothing without a pool.
+static int append_history(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len, const int32_t* d_ids,
+                          int64_t n, cudaStream_t s) {
+    if (!h->history) return PB_OK;
+    RaggedIn rg{};
+    rg.offsets = reinterpret_cast<const long long*>(d_offsets);
+    rg.max_len = max_len;
+    rg.chunk = h->cfg.chunk_samples;
+    rg.sub = (int)std::min<int64_t>(max_len, INT32_MAX);
+    const int per = HIST_THREADS / 32;
+    ProfScope ps(h, 3, s);
+    history_append_kernel<<<(unsigned)((n + per - 1) / per), HIST_THREADS, 0, s>>>(d_pcm, rg, d_ids, (int)n, h->d_n_samples.get(),
+                                                                                  hist_pool(h));
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+// A uniform tick's K1 with its history append first.
+static int tick_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, cudaStream_t s) {
+    const int rc = append_history(h, d_pcm, nullptr, h->cfg.chunk_samples, d_ids, n, s);
+    return rc != PB_OK ? rc : launch_stream_mfcc(h, d_pcm, d_ids, n, s);
+}
+
 PB_API int pb_update_vectors(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, int64_t n, void* stream) {
     int rc = check_tick(h, d_pcm, n);
     if (rc != PB_OK || n == 0) return rc;
     CK(cudaSetDevice(h->cfg.device));
-    return launch_stream_mfcc(h, d_pcm, d_ids, n, (cudaStream_t)stream);
+    return tick_mfcc(h, d_pcm, d_ids, n, (cudaStream_t)stream);
 }
 
 // Where a stream tick's network kernels read the window of item i: stream d_ids[i] (i when d_ids is null) of the handle's ring.
@@ -1241,7 +1282,7 @@ PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, i
     if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
+    rc = tick_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
     return score_model0(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
 }
@@ -1416,7 +1457,7 @@ PB_API int pb_update_models(pb_handle* h, const int16_t* d_pcm, const int32_t* d
     if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    rc = launch_stream_mfcc(h, d_pcm, d_ids, n, s);
+    rc = tick_mfcc(h, d_pcm, d_ids, n, s);
     if (rc != PB_OK) return rc;
     return score_bank(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
 }
@@ -1434,6 +1475,8 @@ PB_API int pb_update_ragged(pb_handle* h, const int16_t* d_pcm, const int64_t* d
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     h->ragged = true;
+    rc = append_history(h, d_pcm, d_offsets, max_len, d_ids, n, s);
+    if (rc != PB_OK) return rc;
     rc = launch_ragged_mfcc(h, d_pcm, d_offsets, max_len, d_ids, n, s);
     if (rc != PB_OK) return rc;
     // one model: pb_update's network path, so a ragged tick of uniform chunks equals pb_update bit for bit; a bank:
@@ -1476,6 +1519,16 @@ struct TrigArrays {
     int* trig[PB_MAX_MODELS];        // each bank model's TriggerDetector.activation; null past the last model
 };
 
+// With a history pool: the history of streams ids[i] (or i) restarts at their n_samples, so that no read returns audio of a
+// stream's previous life.  Runs after whatever reset n_samples, on the same stream.
+static int restart_history(pb_handle* h, const int32_t* d_ids, int64_t n, cudaStream_t s) {
+    if (!h->history) return PB_OK;
+    ProfScope ps(h, 3, s);
+    history_restart_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(hist_pool(h), h->d_n_samples.get(), d_ids, n);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
 // Stream ids[i] (or i) starts over: no samples consumed, every model's trigger re-armed.
 __global__ void clear_kernel(long long* n_samples, TrigArrays t, const int* ids, long long n) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1496,7 +1549,7 @@ PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream)
     for (size_t m = 0; m < h->models.size(); ++m) t.trig[m] = h->models[m].trig.get();
     clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->d_n_samples.get(), t, d_ids, n);
     CK(cudaGetLastError());
-    return PB_OK;
+    return restart_history(h, d_ids, n, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1756,8 +1809,127 @@ PB_API int pb_import_streams(pb_handle* h, const int32_t* h_ids, int64_t n, cons
     const int per = STATE_THREADS / 32;
     import_state_kernel<<<(unsigned)((n + per - 1) / per), STATE_THREADS>>>(L, stream_state(h), d_sids.get(), n, in);
     CK(cudaGetLastError());
+    rc = restart_history(h, d_sids.get(), n, 0);                   // history restarts at the record's n_samples
+    if (rc != PB_OK) return rc;
     CK(cudaDeviceSynchronize());
     if (chk.unaligned) h->ragged = true;
+    return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// stream audio history (history.cuh)
+
+PB_API int pb_set_history(pb_handle* h, int64_t history_samples, int32_t max_rows) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    const bool drop = history_samples == 0 && max_rows == 0;
+    if (!drop) {
+        if (history_samples < 1 || history_samples > INT32_MAX - 7)
+            return fail(PB_ERR_INVALID, "history_samples = %lld outside [1, %d]", (long long)history_samples, INT32_MAX - 7);
+        if (max_rows < 1 || max_rows > h->cfg.max_streams)
+            return fail(PB_ERR_INVALID, "max_rows = %d outside [1, max_streams = %d]", max_rows, h->cfg.max_streams);
+    }
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued ticks finish with the old pool
+    h->history = false;                              // the old pool goes first, so a failed allocation leaves none
+    h->d_hist = DevArray<int16_t>();
+    h->d_hist_row = DevArray<int>();
+    h->d_hist_start = DevArray<long long>();
+    h->hist_row.clear();
+    h->hist_free.clear();
+    h->hist_samples = 0;
+    h->hist_cap = h->hist_rows = 0;
+    if (drop) return PB_OK;
+    const size_t S = (size_t)h->cfg.max_streams;
+    const int cap = (int)((history_samples + 7) & ~7LL);
+    DevArray<int16_t> pool;
+    DevArray<int> row_of;
+    DevArray<long long> start;
+    CK(pool.alloc((size_t)max_rows * cap));
+    CK(row_of.alloc(S));
+    CK(start.alloc(S));
+    CK(cudaMemset(row_of.get(), 0xFF, S * sizeof(int)));
+    CK(cudaMemset(start.get(), 0, S * sizeof(long long)));
+    h->d_hist = std::move(pool);
+    h->d_hist_row = std::move(row_of);
+    h->d_hist_start = std::move(start);
+    h->hist_row.assign(S, -1);
+    for (int r = max_rows - 1; r >= 0; --r) h->hist_free.push_back(r);
+    h->hist_samples = history_samples;
+    h->hist_cap = cap;
+    h->hist_rows = max_rows;
+    h->history = true;
+    return PB_OK;
+}
+
+PB_API int pb_set_stream_history(pb_handle* h, const int32_t* h_ids, const uint8_t* h_on, int64_t n) {
+    int rc = check_route_ids(h, h_ids, n, true);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && !h_on) return fail(PB_ERR_INVALID, "null h_on");
+    if (!h->history) return fail(PB_ERR_STATE, "no history pool: call pb_set_history first");
+    int64_t on_after = h->hist_rows - (int64_t)h->hist_free.size();
+    for (int64_t i = 0; i < n; ++i) {
+        const int sid = h_ids ? h_ids[i] : (int)i;
+        on_after += (int)(h_on[i] != 0) - (int)(h->hist_row[sid] >= 0);
+    }
+    if (on_after > h->hist_rows)
+        return fail(PB_ERR_INVALID, "%lld streams would have history, the pool has max_rows = %d; nothing changed", (long long)on_after,
+                    h->hist_rows);
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued ticks finish with the old rows
+    // rows of the streams that go off first, then one for each stream that goes on
+    std::vector<int> free_rows = h->hist_free, sids, rows;
+    for (int pass = 0; pass < 2; ++pass)
+        for (int64_t i = 0; i < n; ++i) {
+            const int sid = h_ids ? h_ids[i] : (int)i;
+            const bool was = h->hist_row[sid] >= 0, on = h_on[i] != 0;
+            if (pass == 0 && was && !on) {
+                free_rows.push_back(h->hist_row[sid]);
+                sids.push_back(sid);
+                rows.push_back(-1);
+            } else if (pass == 1 && !was && on) {
+                sids.push_back(sid);
+                rows.push_back(free_rows.back());
+                free_rows.pop_back();
+            }
+        }
+    if (sids.empty()) return PB_OK;
+    DevArray<int> d_sids, d_rows;
+    CK(d_sids.upload(sids));
+    CK(d_rows.upload(rows));
+    const long long k = (long long)sids.size();
+    {
+        ProfScope ps(h, 3, 0);
+        history_set_kernel<<<(unsigned)((k + 255) / 256), 256>>>(hist_pool(h), h->d_n_samples.get(), d_sids.get(), d_rows.get(), k);
+        CK(cudaGetLastError());
+    }
+    CK(cudaDeviceSynchronize());
+    for (size_t j = 0; j < sids.size(); ++j) h->hist_row[sids[j]] = rows[j];
+    h->hist_free = std::move(free_rows);
+    return PB_OK;
+}
+
+PB_API int pb_get_stream_history(const pb_handle* h, const int32_t* h_ids, int64_t n, uint8_t* h_on) {
+    const int rc = check_route_ids(h, h_ids, n, false);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && !h_on) return fail(PB_ERR_INVALID, "null h_on");
+    for (int64_t i = 0; i < n; ++i) h_on[i] = h->history && h->hist_row[h_ids ? h_ids[i] : i] >= 0;
+    return PB_OK;
+}
+
+PB_API int pb_read_history(pb_handle* h, const int32_t* d_ids, int64_t n, int64_t samples, int16_t* d_out, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (n < 0 || n > h->cfg.max_streams) return fail(PB_ERR_INVALID, "n = %lld outside [0, max_streams = %d]", (long long)n, h->cfg.max_streams);
+    if (!h->history) return fail(PB_ERR_STATE, "no history pool: call pb_set_history first");
+    if (samples < 1 || samples > h->hist_samples)
+        return fail(PB_ERR_INVALID, "samples = %lld outside [1, history_samples = %lld]", (long long)samples, (long long)h->hist_samples);
+    if (n == 0) return PB_OK;
+    if (!d_out) return fail(PB_ERR_INVALID, "null d_out");
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    ProfScope ps(h, 3, s);
+    history_read_kernel<<<(unsigned)n, HIST_THREADS, 0, s>>>(hist_pool(h), h->d_n_samples.get(), d_ids, h->cfg.max_streams,
+                                                              (int)samples, d_out);
+    CK(cudaGetLastError());
     return PB_OK;
 }
 
