@@ -378,9 +378,9 @@ int pb_debug_force_generic(pb_handle* h, int on);
  * the fp16x3 mma.sync scan of csrc/gru_bank.cuh with one model), 1 = CUDA-core thread-per-stream kernel, 2 = the tensor-core scan
  * also for small batches.  Any other mode: PB_ERR_INVALID.  All variants are parity-tested (tests/test_gpu_parity.py). */
 int pb_debug_gru_mode(pb_handle* h, int mode);
-/* Test / A-B hook for the stateful tick's MFCC kernel (aligned default geometry).  0 = automatic: the FFT kernel on the CUDA
- * cores (csrc/mfcc_fast.cuh) where the geometry allows it, else the generic kernel; 2 = always the FFT kernel; 3 = the FFT kernel
- * with its original 64-bit set-up; 4 / 5 / 6 = csrc/mfcc_mma.cuh, the DFT on mma.sync (stage 2 / both stages / both with a
+/* Test / A-B hook for the stateful tick's MFCC kernel (aligned default geometry).  0 = automatic: the pipelined FFT kernel on
+ * the CUDA cores (csrc/mfcc_fast.cuh, mfcc_pipe_stream_kernel) where the geometry allows it, else the generic kernel; 2 = always
+ * the FFT kernel it replaced (mfcc_fast_stream_kernel, bit-identical results); 3 = that kernel with its original 64-bit set-up; 4 / 5 / 6 = csrc/mfcc_mma.cuh, the DFT on mma.sync (stage 2 / both stages / both with a
  * shuffle epilogue; hop >= 512, chunk >= hop).  All variants are parity-tested (tests/test_gpu_parity.py). */
 int pb_debug_k1_mode(pb_handle* h, int mode);
 /* CPU model of a tensor-core formulation of the DFT (csrc/mfcc_tc.cuh: radix-16 butterflies, second stage as an fp16 hi / lo

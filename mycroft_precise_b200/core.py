@@ -673,7 +673,8 @@ class PreciseB200:
         check(self.lib.pb_debug_force_generic(self._h, int(on)))
 
     def k1_mode(self, mode):
-        """0 = default MFCC kernel choice, 2 = the FFT kernel, 3 = the FFT kernel with its 64-bit set-up, 4 / 5 / 6 = the DFT on
+        """0 = default MFCC kernel choice (the pipelined FFT kernel on the aligned geometry), 2 = the FFT kernel it replaced
+        (bit-identical results), 3 = that kernel with its 64-bit set-up, 4 / 5 / 6 = the DFT on
         mma.sync (stage 2 only / both stages / both stages with a shuffle epilogue)."""
         check(self.lib.pb_debug_k1_mode(self._h, int(mode)))
 

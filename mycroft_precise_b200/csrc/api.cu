@@ -150,11 +150,11 @@ struct pb_handle {
     // derived
     int used = 0, n_bins = 0, n_out = 0, feat = 0, ring_rows = 0, row_stride = 0, tail_cap = 0, max_new = 0;
     int rel_window = 0;              // samples before frame 0 is released: window_samples (sonopy), window_samples + hop_samples (speechpy drops the last complete frame)
-    size_t k1_batch_smem = 0, k1_stream_smem = 0, k1_fast_smem = 0, k1_ragged_smem = 0;
+    size_t k1_batch_smem = 0, k1_stream_smem = 0, k1_fast_smem = 0, k1_pipe_smem = 0, k1_ragged_smem = 0;
     bool ragged = false;             // set by the first pb_update_ragged: n_samples may no longer be a multiple of 8, so every later tick's
                                      // K1 runs launch_ragged_mfcc (the aligned-only kernels would mis-stage it)
     bool force_generic = false;      // tests: exercise the generic kernels on the aligned geometry
-    int k1_mode = 0;                 // 0 = default (the FFT kernel with 32-bit set-up where the geometry allows it), 2 = always the FFT kernel, 3 = FFT kernel with the original 64-bit set-up, 4 / 5 / 6 = the mma.sync DFT tick (mfcc_mma.cuh): stage 1 on the CUDA cores / on the tensor cores / the latter with a shuffle epilogue
+    int k1_mode = 0;                 // 0 = default (the pipelined FFT kernel where the geometry allows it), 2 = always the FFT kernel it replaced, 3 = FFT kernel with the original 64-bit set-up, 4 / 5 / 6 = the mma.sync DFT tick (mfcc_mma.cuh): stage 1 on the CUDA cores / on the tensor cores / the latter with a shuffle epilogue
     bool mma_ok = false;             // geometry mfcc_mma_kernel covers (n_fft = frame = 512, hop >= 512, chunk >= hop, MFCC vectorizer)
     DevArray<uint2> d_mm_b1, d_mm_b2; DevArray<float2> d_mm_tw;
     DevArray<MmRec> d_mm_recs; DevArray<unsigned int> d_mm_counters;
@@ -473,6 +473,7 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     const size_t k1_fast_tables = (size_t)h->npl * 128 * sizeof(float4) + (size_t)c.n_filt * 16 * h->nol * sizeof(float) +
                                   (((size_t)c.n_filt * h->maxc + 15) & ~(size_t)15);
     h->k1_fast_smem = K1F_WARPS * sizeof(K1FWarp) + k1_fast_tables;
+    h->k1_pipe_smem = K1F_WARPS * sizeof(K1PWarp) + 256 * sizeof(float2) + k1_fast_tables;
     h->k1_ragged_smem = K1F_WARPS * sizeof(K1RWarp) + k1_fast_tables;
     // DCT-II, norm='ortho' (scipy.fftpack.dct as sonopy.mfcc_spec calls it), first n_out rows
     std::vector<float> dct((size_t)h->n_out * c.n_filt);
@@ -529,6 +530,9 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     CK(ensure_dyn_smem(mfcc_fast_batch_kernel, (size_t)(h->k1_fast_smem)));
     CK(ensure_dyn_smem(mfcc_fast_stream_kernel<false>, (size_t)(h->k1_fast_smem)));
     CK(ensure_dyn_smem(mfcc_fast_stream_kernel<true>, (size_t)(h->k1_fast_smem)));
+    CK(ensure_dyn_smem(mfcc_pipe_stream_kernel, (size_t)(h->k1_pipe_smem)));
+    // K1P_CTAS_PER_SM CTAs of k1_pipe_smem each need the largest shared-memory carveout
+    CK(cudaFuncSetAttribute(mfcc_pipe_stream_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     CK(ensure_dyn_smem(mfcc_stream_kernel<true>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<false>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<false, true>, (size_t)(h->k1_stream_smem)));
@@ -757,10 +761,10 @@ PB_API int pb_debug_gru_mode(pb_handle* h, int mode) {
 
 PB_API int pb_debug_k1_mode(pb_handle* h, int mode) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
-    if (mode < 0 || mode > 6 || mode == 1) return fail(PB_ERR_INVALID, "k1 mode must be 0 (automatic), 2 (FFT kernel, lean set-up), 3 (FFT kernel), 4 (tensor-core DFT stage 2), 5 (both DFT stages on the tensor cores) or 6 (5 with a shuffle epilogue)");
+    if (mode < 0 || mode > 6 || mode == 1) return fail(PB_ERR_INVALID, "k1 mode must be 0 (automatic), 2 (FFT kernel, lean set-up, not pipelined), 3 (FFT kernel, 64-bit set-up), 4 (tensor-core DFT stage 2), 5 (both DFT stages on the tensor cores) or 6 (5 with a shuffle epilogue)");
     if (mode != 0 && h->ragged) return fail(PB_ERR_STATE, "k1 modes 2-6 need 16-byte-aligned stream state, which a handle loses with its first pb_update_ragged");
     if (mode >= 4 && !h->mma_ok) return fail(PB_ERR_UNSUPPORTED, "the tensor-core MFCC tick needs n_fft = 512 = frame length, hop >= 512 (a multiple of 8), chunk >= hop (a multiple of 8), n_filt <= 32, MFCC vectorizer");
-    if ((mode == 2 || mode == 3) && !h->fast_ok) return fail(PB_ERR_UNSUPPORTED, "k1 mode 2 needs the aligned geometry of the fast MFCC kernels");
+    if ((mode == 2 || mode == 3) && !h->fast_ok) return fail(PB_ERR_UNSUPPORTED, "k1 modes 2 and 3 need the aligned geometry of the fast MFCC kernels");
     h->k1_mode = mode;
     return PB_OK;
 }
@@ -1173,12 +1177,17 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
         else
             mfcc_mma_kernel<true, true><<<gm, MM_THREADS, sizeof(MmSmem), s>>>(t, mel_tables(h), recs, counters, par);
     } else if (h->fast_ok && h->max_new <= 8 && h->cfg.chunk_samples % 8 == 0 && (uintptr_t)d_pcm % 16 == 0 && !h->force_generic) {
-        // streams per warp tile: 16 at scale; fewer when the batch cannot fill the machine's warps
+        // streams per warp tile: 16 at scale; fewer when the batch cannot fill the machine's warps.  Every mode keeps this
+        // tiling: a frame's half-warp, and with it the order of its mel16 sums, follows from its place in the tile
         const int64_t warps_total = (int64_t)h->sm_count * 4 * K1F_WARPS;
         const int spw = (int)std::max<int64_t>(1, std::min<int64_t>(K1F_STREAMS_PER_WARP, (n + warps_total - 1) / warps_total));
         const int64_t tilesf = (n + spw - 1) / spw;
         const int gridf = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
-        if (h->k1_mode != 3)                     // default: the 32-bit per-pass set-up (bit-identical rows); 3 = the 64-bit original
+        if (h->k1_mode == 0) {                   // default: the pipelined kernel (bit-identical rows, tails and counts to mode 2)
+            const int gridp = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * K1P_CTAS_PER_SM);
+            mfcc_pipe_stream_kernel<<<gridp, K1F_THREADS, h->k1_pipe_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
+                                                                              mel_tables(h), fast_tables(h), st);
+        } else if (h->k1_mode != 3)              // the kernel mode 0 replaced: 32-bit per-pass set-up; 3 = its 64-bit original
             mfcc_fast_stream_kernel<true><<<gridf, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
                                                                                       mel_tables(h), fast_tables(h), st);
         else

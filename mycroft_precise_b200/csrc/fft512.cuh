@@ -76,6 +76,18 @@ constexpr int NBINS512 = 257;
 struct FftLaneConst {
     float twr[16], twi[16];   // W256^(n2 k1), k1 = 0..15 (lane = n2)
     float pcr, psi;           // cos/sin(2 pi k1 / 512)            (lane = k1)
+    static constexpr bool kSplitXch = false;
+    __device__ __forceinline__ float2 tw(int k) const { return make_float2(twr[k], twi[k]); }
+};
+
+// The same constants with the stage twiddles read from shared memory instead of 32 registers: tws = a [k1][16] float2
+// table (W256^(n2 k1) at tws[16 k1 + n2]) plus this lane's n2, so the 16 lanes of a half-warp read 16 consecutive float2.
+// Its exchange goes through a float [16][XCH_STRIDE] scratch, one component at a time (half the shared memory).
+struct FftSmemConst {
+    const float2* tws;
+    float pcr, psi;
+    static constexpr bool kSplitXch = true;
+    __device__ __forceinline__ float2 tw(int k) const { return tws[16 * k]; }
 };
 
 __device__ __forceinline__ void load_lane_const(FftLaneConst& c, const float2* __restrict__ tw_stage,
@@ -99,19 +111,36 @@ __device__ __forceinline__ void w32(int k2, float& c, float& s) {
 
 // One frame per half-warp.  z[n1] = packed complex element 16 n1 + l16 of this lane's frame
 // (inactive half-warps pass zeros and `active` = false; all 32 lanes must call).
-// xch: this half-warp's XCH_ELEMS float2 scratch.  P: this frame's power row (>= 257 floats).
-// scale multiplies |X|^2 (1/512 and the int16 -> float normalisation folded together).
-__device__ __forceinline__ void fft512_power(cpx (&z)[16], const FftLaneConst& c, float2* xch,
+// xch: this half-warp's scratch, XCH_ELEMS float2 (FftLaneConst) or XCH_ELEMS floats (FftSmemConst).  P: this frame's power
+// row (>= 257 floats).  scale multiplies |X|^2 (1/512 and the int16 -> float normalisation folded together).
+template <class Const>
+__device__ __forceinline__ void fft512_power(cpx (&z)[16], const Const& c, void* xch,
                                              float* P, float scale, int l16, bool active) {
     const unsigned FULL = 0xffffffffu;
     fft16(z);
 #pragma unroll
-    for (int k = 1; k < 16; ++k) z[k] = cmul(z[k], c.twr[k], c.twi[k]);
+    for (int k = 1; k < 16; ++k) { const float2 w = c.tw(k); z[k] = cmul(z[k], w.x, w.y); }
+    if (Const::kSplitXch) {
+        float* x = static_cast<float*>(xch);
 #pragma unroll
-    for (int k = 0; k < 16; ++k) xch[k * XCH_STRIDE + l16] = make_float2(z[k].x, z[k].y);
-    __syncwarp();
+        for (int k = 0; k < 16; ++k) x[k * XCH_STRIDE + l16] = z[k].x;
+        __syncwarp();
 #pragma unroll
-    for (int n = 0; n < 16; ++n) { float2 t = xch[l16 * XCH_STRIDE + n]; z[n].x = t.x; z[n].y = t.y; }
+        for (int n = 0; n < 16; ++n) z[n].x = x[l16 * XCH_STRIDE + n];
+        __syncwarp();
+#pragma unroll
+        for (int k = 0; k < 16; ++k) x[k * XCH_STRIDE + l16] = z[k].y;
+        __syncwarp();
+#pragma unroll
+        for (int n = 0; n < 16; ++n) z[n].y = x[l16 * XCH_STRIDE + n];
+    } else {
+        float2* x = static_cast<float2*>(xch);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) x[k * XCH_STRIDE + l16] = make_float2(z[k].x, z[k].y);
+        __syncwarp();
+#pragma unroll
+        for (int n = 0; n < 16; ++n) { float2 t = x[l16 * XCH_STRIDE + n]; z[n].x = t.x; z[n].y = t.y; }
+    }
     __syncwarp();
     fft16(z);                                  // z[k2] = Z[l16 + 16 k2]
     const int lane = threadIdx.x & 31;

@@ -105,12 +105,15 @@ __device__ __forceinline__ K1FTab load_fast_tables(unsigned char* smem, const Me
 //   part  : K1F_PART floats of scratch; part[128] must read 0
 //   eoff  : this lane's 8 entry offsets (in float4 units) into a piece-table block: ((i + rot) & 7) * 16 + l16
 // All 32 lanes of the warp call this (the other half works on its own frame); `active` gates the store.
+// UQ / UC unroll the piece and filter-slot loops: above 1, the shared loads of several iterations are in flight at once
+// (piece entries, then the bins they select; slot indices, then the partials they select); every sum keeps its order.
+template <int UQ = 1, int UC = 1>
 __device__ __forceinline__ void mel16(const float* P, const K1FTab& tb, const FastTables& ft, const MelTables& t,
                                       float* part, float* mel, const int (&eoff)[8], int l16, bool active,
                                       float* __restrict__ out) {
     const char* Pb = reinterpret_cast<const char*>(P);
     float tot = 0.f;
-#pragma unroll 1
+#pragma unroll UQ
     for (int q = 0; q < ft.npl; ++q) {
         const float4* blk = tb.ptab + q * 128;
         float r = 0.f, f = 0.f;
@@ -132,7 +135,7 @@ __device__ __forceinline__ void mel16(const float* P, const K1FTab& tb, const Fa
     for (int j = l16; j < t.n_filt; j += 16) {
         const unsigned char* ci = tb.ctab + j * ft.maxc;
         float m0 = 0.f, m1 = 0.f;
-#pragma unroll 1
+#pragma unroll UC
         for (int c = 0; c + 1 < ft.maxc; c += 2) { m0 += part[ci[c]]; m1 += part[ci[c + 1]]; }
         if (ft.maxc & 1) m0 += part[ci[ft.maxc - 1]];
         mel[j] = logf(fmaxf(m0 + m1, K1_EPS));
@@ -401,6 +404,223 @@ mfcc_fast_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__
                 if (dst[u] != nullptr) *dst[u] = v[u];
         }
         __syncwarp();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Stateful tick, pipelined (pb_update / pb_update_vectors on the aligned geometry; k1 mode 2 runs mfcc_fast_stream_kernel<true>
+// above instead).  Every frame's arithmetic, the tiling and the frame -> half-warp assignment are mfcc_fast_stream_kernel<true>'s,
+// so rows, tails and sample counts are bit-identical to it.  What differs is how the warp waits (DESIGN.md §3 K1):
+//   - 5 CTAs of 4 warps per SM instead of 4.  The stage twiddles live in one shared [k1][n2] table per CTA instead of 32
+//     registers per lane, the FFT exchange goes through a float scratch one component at a time, the 1 KB input stages are
+//     separate from that scratch, and mel16's partials and log-mels live in the input stage the pass has just read.
+//   - A tile's stream ids are loaded one tile ahead (their latency hides under the passes) and its sample counts during the
+//     previous tile's tail update.
+constexpr int K1P_CTAS_PER_SM = 5;
+constexpr int K1P_TAIL_INFLIGHT = 4;
+constexpr int K1P_MEL_UQ = 1, K1P_MEL_UC = 4;   // mel16's unroll factors
+constexpr int K1P_IN_WORDS = 256 + 16;         // 1 KB frame +64 B: the two half-warps' input reads fall in disjoint bank halves
+static_assert(K1F_PART + K1_MAX_FILT <= K1P_IN_WORDS, "mel16's part | mel must fit in an input stage");
+static_assert(K1F_ZERO_BIN < XCH_ELEMS, "the zero bin must lie in the exchange scratch");
+
+struct K1PWarp {               // per warp
+    int in[2][2][K1P_IN_WORDS];                // [stage][half]: 1 KB input frame (int16 pairs); once read: mel16's part | mel
+    float xch[2][XCH_ELEMS];                   // [half]: FFT exchange scratch -> power bins (272 words apart: disjoint bank halves)
+    unsigned long long bar[2];
+    long long st_n0[K1F_STREAMS_PER_WARP], st_ts0[K1F_STREAMS_PER_WARP], st_c0[K1F_STREAMS_PER_WARP];
+    int st_id[K1F_STREAMS_PER_WARP], st_cnt[K1F_STREAMS_PER_WARP];
+    int st_vbeg[K1F_STREAMS_PER_WARP];         // tail update: first vector of stream t in the tile's packed vector list
+    short fr_stream[K1F_STREAMS_PER_WARP * K1F_MAX_NEW], fr_sub[K1F_STREAMS_PER_WARP * K1F_MAX_NEW];
+};
+static_assert(sizeof(K1PWarp) % 16 == 0, "every warp's input stages start 16-byte aligned (bulk copy destinations)");
+
+// fast_pass for K1PWarp: the same conversion, FFT and mel16, with the scratch and mel16's arrays placed as above.  mel16's entry
+// offsets are rebuilt from `rot` per pass (the same values) rather than held in 8 registers across the tile.
+__device__ __forceinline__ void pipe_pass(K1PWarp& ws, int stage, uint32_t parity, const FftSmemConst& lc, const K1FTab& tb,
+                                          const FastTables& ft, const MelTables& t, float scale, int rot,
+                                          int l16, int half, bool active, float* __restrict__ out) {
+    mbar_wait(&ws.bar[stage], parity);
+    const int* in = ws.in[stage][half];
+    cpx z[16];
+#pragma unroll
+    for (int n1 = 0; n1 < 16; ++n1) {              // int16 pair -> two floats, exactly as fast_pass
+        const unsigned v = (active ? (unsigned)in[16 * n1 + l16] : 0u) ^ 0x80008000u;
+        z[n1].x = __uint_as_float(__byte_perm(v, 0x4b000000u, 0x7610)) - 8421376.f;
+        z[n1].y = __uint_as_float(__byte_perm(v, 0x4b000000u, 0x7632)) - 8421376.f;
+    }
+    __syncwarp();                                  // all lanes have read the staged samples: the stage becomes mel16's scratch
+    float* P = ws.xch[half];
+    fft512_power(z, lc, P, P, scale, l16, active); // P aliases the scratch: written after the last scratch read
+    float* part = reinterpret_cast<float*>(ws.in[stage][half]);
+    if (l16 == 0) { P[K1F_ZERO_BIN] = 0.f; part[128] = 0.f; }
+    int eoff[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) eoff[i] = ((i + rot) & 7) * 16 + l16;
+    __syncwarp();
+    mel16<K1P_MEL_UQ, K1P_MEL_UC>(P, tb, ft, t, part, part + K1F_PART, eoff, l16, active, out);
+}
+
+__global__ void __launch_bounds__(K1F_THREADS, K1P_CTAS_PER_SM)
+mfcc_pipe_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids, int n, int chunk, int hop, int spw,
+                        float scale, MelTables tab, FastTables ft, StreamState st) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    K1PWarp* wsm = reinterpret_cast<K1PWarp*>(smem_raw);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, l16 = lane & 15, half = lane >> 4;
+    K1PWarp& ws = wsm[warp];
+    float2* tws = reinterpret_cast<float2*>(smem_raw + K1F_WARPS * sizeof(K1PWarp));
+    const K1FTab tb = load_fast_tables(reinterpret_cast<unsigned char*>(tws + 256), tab, ft);
+    for (int k = threadIdx.x; k < 256; k += blockDim.x) tws[k] = tab.tw_stage[(k & 15) * 16 + (k >> 4)];   // [n2][k1] -> [k1][n2]
+    if (lane == 0) { mbar_init(&ws.bar[0], 1); mbar_init(&ws.bar[1], 1); fence_mbar_init(); }
+    const int rot = ((l16 >> 2) + (half << 2)) & 7;   // rotated walk through a piece: see mel16
+    FftSmemConst lc;
+    lc.tws = tws + l16;
+    {
+        const float2 p = tab.tw_post[l16];
+        lc.pcr = p.x; lc.psi = p.y;
+    }
+    __syncthreads();
+
+    constexpr int used = 512;
+    const int gwarp = blockIdx.x * K1F_WARPS + warp, nwarps = gridDim.x * K1F_WARPS;
+    // lane i < spw: id of stream base + i, -1 past the batch
+    auto stream_id = [&](int base) {
+        const int i = base + lane;
+        return (lane < spw && i < n) ? (ids ? ids[i] : i) : -1;
+    };
+    int sid = stream_id(gwarp * spw);
+    long long n0 = sid >= 0 ? st.n_samples[sid] : 0;
+    uint32_t uses0 = 0, uses1 = 0;                          // completed uses of each staging buffer (mbarrier phase)
+    for (int base = gwarp * spw; base < n; base += nwarps * spw) {
+        const int sid_next = stream_id(base + nwarps * spw);   // in flight across this tile's passes
+        // ---- bookkeeping: lane i < spw <-> stream base + i (mfcc_fast_stream_kernel<true>'s encoding of st_ts0)
+        int cnt = 0;
+        {
+            long long c0 = 0, ts0 = 0;
+            if (sid >= 0) {
+                c0 = frames_ready(n0, used, hop);
+                cnt = (int)(frames_ready(n0 + chunk, used, hop) - c0);
+                ts0 = ((long long)(int)(c0 % st.ring_rows) << 32) | (long long)(unsigned)(int)(c0 * hop - n0);
+            }
+            if (lane < spw) {
+                ws.st_id[lane] = sid; ws.st_n0[lane] = n0; ws.st_ts0[lane] = ts0; ws.st_cnt[lane] = cnt; ws.st_c0[lane] = c0;
+            }
+        }
+        int incl = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += v; }
+        const int nf = __shfl_sync(0xffffffffu, incl, 31);
+        for (int j = 0; j < cnt; ++j) { ws.fr_stream[incl - cnt + j] = (short)lane; ws.fr_sub[incl - cnt + j] = (short)j; }
+        __syncwarp();
+
+        auto issue = [&](int f0, int stage) {               // lane 0: bulk copies for frames f0, f0+1 of the list
+            const int nfr = min(2, nf - f0);
+            fence_proxy_async();
+            mbar_expect_tx(&ws.bar[stage], 1024u * nfr);
+            for (int hf = 0; hf < nfr; ++hf) {
+                const int t = ws.fr_stream[f0 + hf];
+                const int16_t* chunk_p = pcm + (long long)(base + t) * chunk;
+                char* dst = reinterpret_cast<char*>(ws.in[stage][hf]);
+                const int sub_off = ws.fr_sub[f0 + hf] * hop;
+                const int rel = (int)(unsigned)(ws.st_ts0[t] & 0xffffffffll) + sub_off;        // first sample of the frame, relative to the chunk
+                if (rel >= 0) {
+                    bulk_g2s(dst, chunk_p + rel, 1024u, &ws.bar[stage]);
+                } else {                                  // rel < 0 implies the tail starts at frame c0: offset in the tail = sub * hop
+                    const int len0 = min(used, -rel);
+                    bulk_g2s(dst, st.tail + (long long)ws.st_id[t] * st.tail_cap + sub_off, 2u * len0, &ws.bar[stage]);
+                    if (len0 < used) bulk_g2s(dst + 2 * len0, chunk_p, 2u * (used - len0), &ws.bar[stage]);
+                }
+            }
+        };
+        int stage = 0;
+        if (nf > 0 && lane == 0) issue(0, 0);
+        for (int f0 = 0; f0 < nf; f0 += 2, stage ^= 1) {
+            if (f0 + 2 < nf && lane == 0) issue(f0 + 2, stage ^ 1);
+            const bool active = f0 + half < nf;
+            float* row = st.ring;
+            if (active) {
+                const int t = ws.fr_stream[f0 + half];
+                int slot = (int)(ws.st_ts0[t] >> 32) + ws.fr_sub[f0 + half];                 // fr_sub < ring_rows
+                if (slot >= st.ring_rows) slot -= st.ring_rows;
+                row = st.ring + ((long long)ws.st_id[t] * st.ring_rows + slot) * st.row_stride;
+            }
+            const uint32_t parity = (stage == 0 ? uses0 : uses1) & 1;
+            pipe_pass(ws, stage, parity, lc, tb, ft, tab, scale, rot, l16, half, active, row);
+            if (stage == 0) ++uses0; else ++uses1;
+        }
+        // the next tile's sample counts: its ids have landed during the passes, the loads overlap the tail update below
+        // (stream ids are unique, so no stream of this tile is among them)
+        const long long n0_next = sid_next >= 0 ? st.n_samples[sid_next] : 0;
+        // ---- tail + sample counter: mfcc_fast_stream_kernel's plan, with the copy over a packed list of the tile's vectors
+        int my_nv = 0, my_nold = 0;
+        if (lane < spw && ws.st_id[lane] >= 0) {
+            const long long n0 = ws.st_n0[lane], n1 = n0 + chunk;
+            const long long c1 = ws.st_c0[lane] + ws.st_cnt[lane];
+            const long long ts1 = c1 * hop < n1 ? c1 * hop : n1;
+            my_nold = ts1 < n0 ? (int)(n0 - ts1) : 0;
+            my_nv = ((int)(n1 - ts1) - my_nold) >> 3;
+            ws.st_ts0[lane] = ts1 > n0 ? ts1 - n0 : 0;      // reuse: offset of the copied part inside the chunk
+            ws.st_cnt[lane] = my_nv | (my_nold << 16);
+            st.n_samples[ws.st_id[lane]] = n1;
+        }
+        int vend = my_nv;                                     // inclusive prefix of the streams' vector counts
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { int v = __shfl_up_sync(0xffffffffu, vend, d); if (lane >= d) vend += v; }
+        const int n_vec = __shfl_sync(0xffffffffu, vend, 31);
+        if (lane < spw) ws.st_vbeg[lane] = vend - my_nv;
+        const unsigned any_old = __ballot_sync(0xffffffffu, my_nold > 0);
+        __syncwarp();
+        if (any_old) {                                        // chunk shorter than the FFT window: shift inside the tail first
+            for (int t = 0; t < spw; ++t) {
+                const int sid = ws.st_id[t];
+                if (sid < 0) continue;
+                const int n_old = ws.st_cnt[t] >> 16;
+                if (n_old == 0) continue;
+                const long long n0 = ws.st_n0[t];
+                int16_t* tl = st.tail + (long long)sid * st.tail_cap;
+                // old tail held [n0 - len0, n0); the part that survives is its last n_old samples
+                const long long c0 = frames_ready(n0, used, hop);
+                const long long ts0 = c0 * hop < n0 ? c0 * hop : n0;
+                const int len0 = (int)(n0 - ts0);
+                int4 keep[2];
+                const int4* srcv = reinterpret_cast<const int4*>(tl + (len0 - n_old));
+                const int nv = n_old >> 3;
+#pragma unroll
+                for (int j = 0; j < 2; ++j) if (j * 32 + lane < nv) keep[j] = srcv[j * 32 + lane];
+                __syncwarp();
+#pragma unroll
+                for (int j = 0; j < 2; ++j) if (j * 32 + lane < nv) reinterpret_cast<int4*>(tl)[j * 32 + lane] = keep[j];
+            }
+            __syncwarp();
+        }
+        // flat loop over the tile's n_vec vectors (stream t owns [st_vbeg[t], st_vbeg[t] + its count)), K1P_TAIL_INFLIGHT
+        // loads in flight per lane before the first store: ceil(n_vec / 128) round trips, not one per 64 * 2 slots of
+        // mfcc_fast_stream_kernel's (stream, vector) grid, most of which are empty
+#pragma unroll 1
+        for (int e0 = lane; e0 < n_vec; e0 += 32 * K1P_TAIL_INFLIGHT) {
+            int4 v[K1P_TAIL_INFLIGHT];
+            int4* dst[K1P_TAIL_INFLIGHT];
+#pragma unroll
+            for (int u = 0; u < K1P_TAIL_INFLIGHT; ++u) {
+                const int e = e0 + 32 * u;
+                dst[u] = nullptr;
+                if (e < n_vec) {
+                    int t = 0;                                // the last stream whose first vector is <= e
+#pragma unroll
+                    for (int b = 8; b >= 1; b >>= 1)
+                        if (t + b < spw && ws.st_vbeg[t + b] <= e) t += b;
+                    const int vi = e - ws.st_vbeg[t];
+                    const int cn = ws.st_cnt[t];
+                    v[u] = __ldg(reinterpret_cast<const int4*>(pcm + (long long)(base + t) * chunk + ws.st_ts0[t]) + vi);
+                    dst[u] = reinterpret_cast<int4*>(st.tail + (long long)ws.st_id[t] * st.tail_cap + (cn >> 16)) + vi;
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < K1P_TAIL_INFLIGHT; ++u)
+                if (dst[u] != nullptr) *dst[u] = v[u];
+        }
+        __syncwarp();
+        sid = sid_next;
+        n0 = n0_next;
     }
 }
 
