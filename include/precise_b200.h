@@ -347,12 +347,62 @@ int pb_get_stream_history(const pb_handle* h, const int32_t* h_stream_ids, int64
  * pool. */
 int pb_read_history(pb_handle* h, const int32_t* d_stream_ids, int64_t n, int64_t samples, int16_t* d_out, void* stream);
 
+/* Recorded corpora: whole recordings scored on the device in one call, the hot path of precise-simulate
+ * (precise/scripts/simulate.py:92-129) and of false-activation mining (precise/scripts/train_incremental.py:113-137).
+ * No stream state is read or written (n_samples, tails, rings, trigger state, history); subscriptions and per-stream trigger
+ * settings do not apply.
+ *
+ * Schedules, for chunk c:
+ *   PB_CORPUS_LISTENER  window k (k < floor(L / c)) is what Listener.update returns after samples [0, (k + 1) c) were fed in
+ *                       chunks of c to a fresh listener (network_runner.py:125-153: the 29 rows ending at the last released
+ *                       frame, zero rows before the first; deltas within the window).  conf = the model's decode; fired = the
+ *                       model's TriggerDetector(2c bytes, cfg.sensitivity, cfg.trigger_level) over conf, in order
+ *                       (runner.py:121-142); activations = fired count.  Equals one pb_update_ragged tick per chunk of a
+ *                       fresh stream.  d_above and d_sum must be NULL.
+ *   PB_CORPUS_SIMULATE  c = simulate's -c (samples between tests), c / hop_samples >= 1.  Windows end at frames
+ *                       n_features + j (c / hop) < pb_mfcc_frames(L) (simulate.py:96-99's range).  fired =
+ *                       TriggerDetector(c, sensitivity = threshold, trigger_level = 0) over raw (simulate.py:114-120,
+ *                       refractory -(8 * 2048) // c); above = #(raw > threshold); sum = sum of raw in double (the reference
+ *                       sums float32: the last bits differ).  Both comparisons are float32 against the threshold rounded to
+ *                       float32, as numpy compares a float32 array with a Python float: raw > (float)(1 - threshold) and
+ *                       raw > (float)threshold.  A recording with fewer than n_features + 1 frames yields 0 windows (the
+ *                       reference's Runner.predict fails on its empty input). */
+enum { PB_CORPUS_LISTENER = 0, PB_CORPUS_SIMULATE = 1 };
+
+/* Windows one recording of n_samples yields under `schedule` (no device needed; cfg gives the front end), or a negative
+ * pb_status: PB_ERR_INVALID for a null cfg, non-positive window / hop / n_features, a bad schedule or chunk, n_samples < 0. */
+int64_t pb_corpus_windows(const pb_config* cfg, int32_t schedule, int64_t chunk, int64_t n_samples);
+
+/* Scores n_rec recordings: recording r is d_pcm[h_offsets[r] .. h_offsets[r + 1]) (HOST offsets [n_rec + 1], non-decreasing,
+ * any alignment; empty recordings yield 0 windows).  divisor: 32768 (buffer_to_audio, util.py:37) or 32767 (load_audio,
+ * util.py:65), folded into the power scale as pb_mfcc folds 2^-15.  Window w of recording r is entry W_r + w, W_r the
+ * exclusive prefix of pb_corpus_windows over the recordings.  Outputs are model-major over every bank model,
+ * M = pb_num_models:
+ *   d_raw [M][W_total] float32 (required), d_conf [M][W_total] float64, d_fired [M][W_total] uint8,
+ *   d_activations, d_above [M][n_rec] int64, d_sum [M][n_rec] float64 -- all but d_raw optional (NULL).
+ * Asynchronous on `stream`; h_offsets may be reused once the call returns.  The frames, window table and device offsets live
+ * in a handle-owned workspace that grows on demand (about one row_stride-float row per hop of audio, 4 % of the int16
+ * bytes at the defaults) and is freed by pb_destroy.  Two corpus calls on different CUDA streams are ordered by the library
+ * (an event recorded after every call, failed ones included); the host waits for the previous call only when the workspace
+ * must grow.
+ * Profile slot 0 counts the MFCC kernels, slot 1 the network and trigger kernels.
+ * At the aligned default geometry, recordings whose offset is a multiple of 8 samples (and d_pcm 16-byte aligned) take the
+ * per-frame arithmetic of pb_mfcc's fast kernel, the others its generic kernel: frames are bit-identical to pb_mfcc of the
+ * recording alone wherever both take the same kernel.
+ * PB_ERR_INVALID: null handle, h_offsets or d_raw, a null d_pcm with samples, n_rec < 0, decreasing or negative offsets, a
+ * bad divisor, schedule or chunk, d_above / d_sum with the listener schedule.  PB_ERR_STATE: slot 0 has no weights.
+ * PB_ERR_CUDA: the workspace cannot be allocated (the handle is then unchanged). */
+int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                    int32_t divisor, int32_t schedule, int64_t chunk, double threshold,
+                    float* d_raw, double* d_conf, uint8_t* d_fired,
+                    int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream);
+
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);
 
 /* Per-kernel device timing (CUDA events on the launching stream), for bench.py's roofline.
- * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel (a bank tick: all its network kernels), 2 = decode-only kernel,
+ * slot 0 = MFCC kernel, 1 = GRU(+decode+trigger) kernel (a bank tick or a corpus call: all its network kernels), 2 = decode-only kernel,
  * 3 = stream audio history kernels (the append of each tick, pb_read_history, switching and restarts; always 0 on a handle
  * without a history pool).
  * pb_profile_read synchronises the recorded events, returns accumulated ms and launch counts

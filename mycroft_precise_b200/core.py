@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 PB_MAX_THRESHOLDS = 8
 PB_MAX_MODELS = 8
 PB_ABI_VERSION = 2
+CORPUS_SCHEDULES = {'listener': 0, 'simulate': 1}   # PB_CORPUS_LISTENER, PB_CORPUS_SIMULATE
 # ListenerParams fields of the MFCC front end: the models of one handle's bank must agree on all of them
 FRONT_END_FIELDS = ('sample_rate', 'window_samples', 'hop_samples', 'n_fft', 'n_filt', 'n_mfcc', 'n_features',
                     'use_delta', 'vectorizer')
@@ -72,6 +73,8 @@ SYMBOLS = {
     'pb_set_stream_history': (C.c_int, [_VP, _VP, _VP, _I64]),
     'pb_get_stream_history': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_read_history': (C.c_int, [_VP, _VP, _I64, _I64, _VP, _VP]),
+    'pb_corpus_windows': (_I64, [C.POINTER(pb_config), _I32, _I64, _I64]),
+    'pb_score_corpus': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -179,6 +182,14 @@ def numpy_cdf(threshold_config, resolution=200, min_z=-4, max_z=4):
 
     pd = np.sum([pdf(points, mu, std) for mu, std in mu_stds], axis=0) / (resolution * len(mu_stds))
     return np.ascontiguousarray(np.cumsum(pd), dtype=np.float64), min_out, max_out
+
+
+def _schedule(schedule) -> int:
+    if schedule in CORPUS_SCHEDULES:
+        return CORPUS_SCHEDULES[schedule]
+    if isinstance(schedule, (int, np.integer)) and not isinstance(schedule, bool) and int(schedule) in CORPUS_SCHEDULES.values():
+        return int(schedule)
+    raise ValueError('schedule must be one of %s, got %r' % (sorted(CORPUS_SCHEDULES), schedule))
 
 
 def _ptr(t):
@@ -645,6 +656,47 @@ class PreciseB200:
         else:
             self._check_t('out', out, torch.int16, n * samples, optional=False)
         check(self.lib.pb_read_history(self._h, _ptr(ids), n, samples, _ptr(out), self._stream()))
+        return out
+
+    # ---- recorded corpora
+    def corpus_windows(self, n_samples, schedule='listener', chunk=1024) -> int:
+        """Windows one recording of n_samples yields under ``schedule`` ('listener' or 'simulate') with chunk ``chunk``."""
+        n = int(self.lib.pb_corpus_windows(C.byref(self.cfg), _schedule(schedule), int(chunk), int(n_samples)))
+        if n < 0:
+            check(n)
+        return n
+
+    def score_corpus(self, pcm, offsets, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
+        """Every bank model over recordings pcm[offsets[r]:offsets[r + 1]] (pcm a 1-D int16 CUDA tensor, offsets a host int64
+        array [n_rec + 1]).  Returns dict(raw f32 [M, W], conf f64 [M, W], fired u8 [M, W], activations i64 [M, n_rec], and
+        for the simulate schedule above i64 [M, n_rec] and sum f64 [M, n_rec]; None otherwise), W the total window count.
+        Asynchronous on the current stream.  Schedules and outputs: pb_score_corpus in include/precise_b200.h."""
+        torch = self.torch
+        sched = _schedule(schedule)
+        if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
+                or pcm.device != self.device):
+            raise ValueError('pcm must be a contiguous 1-D int16 tensor on %s' % self.device)
+        offsets = np.asarray(offsets)
+        if offsets.ndim != 1 or offsets.shape[0] < 1 or offsets.dtype.kind not in 'iu':
+            raise ValueError('offsets must be a 1-D integer array [n_rec + 1]')
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        n_rec = offsets.shape[0] - 1
+        if n_rec and int(offsets[-1]) > pcm.numel():
+            raise ValueError('offsets end at %d, past pcm of %d samples' % (int(offsets[-1]), pcm.numel()))
+        lens = np.diff(offsets)
+        if lens.size and lens.min() < 0:
+            raise ValueError('offsets must be non-decreasing')
+        W = sum(self.corpus_windows(int(L), schedule, chunk) for L in lens)
+        M = self.num_models
+        f = lambda shape, dt: torch.empty(shape, dtype=dt, device=self.device)
+        out = dict(raw=f((M, W), torch.float32), conf=f((M, W), torch.float64), fired=f((M, W), torch.uint8),
+                   activations=f((M, n_rec), torch.int64), above=None, sum=None)
+        if sched == 1:
+            out['above'] = f((M, n_rec), torch.int64)
+            out['sum'] = f((M, n_rec), torch.float64)
+        check(self.lib.pb_score_corpus(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, int(divisor), sched, int(chunk),
+                                       float(threshold), _ptr(out['raw']), _ptr(out['conf']), _ptr(out['fired']),
+                                       _ptr(out['activations']), _ptr(out['above']), _ptr(out['sum']), self._stream()))
         return out
 
     def update_host(self, pcm_np, conf_np, raw_np=None, fired_np=None, ids_np=None) -> int:

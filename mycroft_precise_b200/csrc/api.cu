@@ -31,6 +31,7 @@
 #include "trigger.cuh"
 #include "stream_state.cuh"
 #include "history.cuh"
+#include "corpus.cuh"
 
 using namespace pb;
 
@@ -192,6 +193,14 @@ struct pb_handle {
     DevArray<long long> d_hist_start;  // [max_streams] history start
     std::vector<int> hist_row;       // host mirror of d_hist_row
     std::vector<int> hist_free;      // rows no stream owns
+    // recorded corpora (pb_score_corpus): a workspace that grows on demand and never shrinks
+    DevArray<float> d_cw_rows;       // the frame buffer (corpus.cuh)
+    DevArray<CorpusPair> d_cw_pairs; // K1's pair list
+    DevArray<long long> d_cw_starts; // [windows] first row of each window
+    DevArray<long long> d_cw_win0;   // [n_rec + 1] window prefix
+    DevArray<long long> d_cw_frow;   // [n_rec] row of each recording's frame 0
+    DevArray<CorpusRec> d_cw_recs;   // [n_rec + 1] recordings in pair-list order
+    cudaEvent_t corpus_ev = nullptr; // recorded after each corpus call; the next one waits on it before reusing the workspace
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
     cudaEvent_t pipe_ev[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -218,6 +227,7 @@ struct pb_handle {
         for (auto& p : prof)
             for (auto e : p.ev) cudaEventDestroy(e);
         if (route_ev) cudaEventDestroy(route_ev);
+        if (corpus_ev) cudaEventDestroy(corpus_ev);
     }
 };
 
@@ -537,6 +547,8 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     CK(ensure_dyn_smem(mfcc_stream_kernel<false>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<false, true>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_ragged_stream_kernel, (size_t)(h->k1_ragged_smem)));
+    CK(ensure_dyn_smem(mfcc_fast_corpus_kernel, (size_t)(h->k1_fast_smem)));
+    CK(ensure_dyn_smem(mfcc_corpus_kernel, (size_t)(h->k1_batch_smem)));
 
     Network net;                     // slot 0: weights come with pb_load_weights
     net.cfg = c;
@@ -1071,7 +1083,7 @@ PB_API int pb_predict(pb_handle* h, const float* d_inputs, int64_t n, float* d_o
     if (!d_inputs || !d_out) return fail(PB_ERR_INVALID, "null buffer");
     CK(cudaSetDevice(h->cfg.device));
     K2In in{};
-    in.inputs = d_inputs; in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = 0;
+    in.inputs = d_inputs; in.row_stride = h->feat; in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = 0;
     K2Out o{};
     o.raw = d_out; o.logit = d_logit;
     return launch_gru(h, h->models[0], in, false, n, o, (cudaStream_t)stream);
@@ -1336,16 +1348,18 @@ PB_API int pb_num_models(const pb_handle* h) {
     return (int)h->models.size();
 }
 
+// RING: a tick's bank over the stream ring; otherwise over predict-mode windows (a recorded corpus's frame rows).
+template <bool RING>
 static int launch_bank(const BankParams& P, int nm, const K2In& in, int64_t n, cudaStream_t s) {
     switch (nm) {
-        case 1: return launch_bank_nm<1, true>(P, in, n, s);
-        case 2: return launch_bank_nm<2, true>(P, in, n, s);
-        case 3: return launch_bank_nm<3, true>(P, in, n, s);
-        case 4: return launch_bank_nm<4, true>(P, in, n, s);
-        case 5: return launch_bank_nm<5, true>(P, in, n, s);
-        case 6: return launch_bank_nm<6, true>(P, in, n, s);
-        case 7: return launch_bank_nm<7, true>(P, in, n, s);
-        case 8: return launch_bank_nm<8, true>(P, in, n, s);
+        case 1: return launch_bank_nm<1, RING>(P, in, n, s);
+        case 2: return launch_bank_nm<2, RING>(P, in, n, s);
+        case 3: return launch_bank_nm<3, RING>(P, in, n, s);
+        case 4: return launch_bank_nm<4, RING>(P, in, n, s);
+        case 5: return launch_bank_nm<5, RING>(P, in, n, s);
+        case 6: return launch_bank_nm<6, RING>(P, in, n, s);
+        case 7: return launch_bank_nm<7, RING>(P, in, n, s);
+        case 8: return launch_bank_nm<8, RING>(P, in, n, s);
     }
     return fail(PB_ERR_INVALID, "%d fused models", nm);
 }
@@ -1451,7 +1465,7 @@ static int score_bank(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_ra
         }
     }
     if (nm) {
-        rc = launch_bank(P, nm, in, n, s);
+        rc = launch_bank<true>(P, nm, in, n, s);
         if (rc != PB_OK) return rc;
     }
     return launch_trigger(t, nt, s);
@@ -1492,6 +1506,202 @@ PB_API int pb_update_ragged(pb_handle* h, const int16_t* d_pcm, const int64_t* d
     // pb_update_models's
     if (h->models.size() == 1) return score_model0(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
     return score_bank(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
+}
+
+// ------------------------------------------------------------------------------------------------
+// recorded corpora (corpus.cuh)
+
+// Frames vectorize_raw yields for n samples under front end c (pb_mfcc_frames without a handle).
+static int64_t corpus_frames(const pb_config& c, int64_t n) {
+    const int64_t rel = c.window_samples + (c.vectorizer == PB_VEC_SPEECHPY_MFCCS ? c.hop_samples : 0);
+    return n < rel ? 0 : (n - rel) / c.hop_samples + 1;
+}
+
+static int check_corpus_schedule(const pb_config& c, int32_t schedule, int64_t chunk) {
+    if (schedule != PB_CORPUS_LISTENER && schedule != PB_CORPUS_SIMULATE) return fail(PB_ERR_INVALID, "unknown corpus schedule %d", schedule);
+    if (chunk < 1) return fail(PB_ERR_INVALID, "chunk = %lld must be >= 1", (long long)chunk);
+    if (schedule == PB_CORPUS_SIMULATE && chunk / c.hop_samples < 1)
+        return fail(PB_ERR_INVALID, "simulate chunk %lld is shorter than one hop (%d samples)", (long long)chunk, c.hop_samples);
+    return PB_OK;
+}
+
+// Windows of one recording of n samples (arguments checked).  LISTENER: one per complete chunk.  SIMULATE:
+// len(range(n_features, n_frames, chunk // hop)) (simulate.py:96-99).
+static int64_t corpus_windows(const pb_config& c, int32_t schedule, int64_t chunk, int64_t n) {
+    if (schedule == PB_CORPUS_LISTENER) return n / chunk;
+    const int64_t nf = corpus_frames(c, n), hops = chunk / c.hop_samples;
+    return nf > c.n_features ? (nf - c.n_features + hops - 1) / hops : 0;
+}
+
+PB_API int64_t pb_corpus_windows(const pb_config* cfg, int32_t schedule, int64_t chunk, int64_t n_samples) {
+    if (!cfg) return fail(PB_ERR_INVALID, "cfg is null");
+    if (cfg->window_samples < 1 || cfg->hop_samples < 1 || cfg->n_features < 1)
+        return fail(PB_ERR_INVALID, "window_samples, hop_samples and n_features must be positive");
+    if (n_samples < 0) return fail(PB_ERR_INVALID, "n_samples = %lld is negative", (long long)n_samples);
+    const int rc = check_corpus_schedule(*cfg, schedule, chunk);
+    return rc != PB_OK ? rc : corpus_windows(*cfg, schedule, chunk, n_samples);
+}
+
+// Grows a workspace array to n elements.  The replaced array is freed only after the previous corpus call is done with it.
+template <typename T>
+static cudaError_t corpus_grow(const DevArray<T>& a, size_t n, DevArray<T>& fresh) {
+    if (a.size() >= n) return cudaSuccess;
+    return fresh.alloc(n + n / 4);
+}
+
+PB_API int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
+                           int32_t schedule, int64_t chunk, double threshold, float* d_raw, double* d_conf, uint8_t* d_fired,
+                           int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    const pb_config& c = h->cfg;
+    if (n_rec < 0 || n_rec > INT32_MAX) return fail(PB_ERR_INVALID, "n_rec = %lld outside [0, 2^31)", (long long)n_rec);
+    if (!h_offsets) return fail(PB_ERR_INVALID, "null h_offsets");
+    if (!d_raw) return fail(PB_ERR_INVALID, "null d_raw");
+    if (divisor != 32768 && divisor != 32767) return fail(PB_ERR_INVALID, "divisor %d: 32768 (buffer_to_audio) or 32767 (load_audio)", divisor);
+    int rc = check_corpus_schedule(c, schedule, chunk);
+    if (rc != PB_OK) return rc;
+    if (schedule == PB_CORPUS_LISTENER && (d_above || d_sum)) return fail(PB_ERR_INVALID, "d_above and d_sum belong to the simulate schedule");
+    if (h_offsets[0] < 0) return fail(PB_ERR_INVALID, "offset 0 = %lld is negative", (long long)h_offsets[0]);
+    for (int64_t r = 0; r < n_rec; ++r)
+        if (h_offsets[r + 1] < h_offsets[r]) return fail(PB_ERR_INVALID, "offsets decrease at recording %lld", (long long)r);
+    if (h_offsets[n_rec] > h_offsets[0] && !d_pcm) return fail(PB_ERR_INVALID, "null d_pcm");
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (n_rec == 0) return PB_OK;
+    CK(cudaSetDevice(c.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int M = (int)h->models.size(), T = c.n_features;
+    // host plan: window prefix, frame rows, and the recordings in pair-list order (aligned geometry first)
+    const bool fast = h->fast_ok && !h->force_generic && (uintptr_t)d_pcm % 16 == 0;
+    std::vector<long long> win0((size_t)n_rec + 1), frow((size_t)n_rec);
+    std::vector<CorpusRec> recs;
+    recs.reserve((size_t)n_rec + 1);
+    long long rows = 1, n_fast_pairs = 0, n_pairs = 0;
+    win0[0] = 0;
+    for (int pass = 0; pass < 2; ++pass)
+        for (int64_t r = 0; r < n_rec; ++r) {
+            const int64_t L = h_offsets[r + 1] - h_offsets[r], nf = corpus_frames(c, L);
+            const bool fr = fast && h_offsets[r] % 8 == 0;
+            if (pass == 0) {
+                win0[r + 1] = win0[r] + corpus_windows(c, schedule, chunk, L);
+                frow[r] = rows + T - 1;
+                rows += T - 1 + nf;
+            }
+            if (fr != (pass == 0)) continue;
+            recs.push_back(CorpusRec{h_offsets[r], frow[r], nf, n_pairs});
+            n_pairs += (nf + 1) / 2;
+            if (fr) n_fast_pairs = n_pairs;
+        }
+    recs.push_back(CorpusRec{0, 0, 0, n_pairs});
+    const long long W = win0[n_rec];
+    // the workspace: grown all at once, so that a failed allocation leaves the handle as it was
+    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
+    {
+        DevArray<float> f_rows; DevArray<CorpusPair> f_pairs; DevArray<long long> f_starts, f_win0, f_frow; DevArray<CorpusRec> f_recs;
+        cudaError_t e = corpus_grow(h->d_cw_rows, (size_t)rows * h->row_stride, f_rows);
+        if (e == cudaSuccess) e = corpus_grow(h->d_cw_pairs, (size_t)n_pairs, f_pairs);
+        if (e == cudaSuccess) e = corpus_grow(h->d_cw_starts, (size_t)W, f_starts);
+        if (e == cudaSuccess) e = corpus_grow(h->d_cw_win0, (size_t)n_rec + 1, f_win0);
+        if (e == cudaSuccess) e = corpus_grow(h->d_cw_frow, (size_t)n_rec, f_frow);
+        if (e == cudaSuccess) e = corpus_grow(h->d_cw_recs, recs.size(), f_recs);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(PB_ERR_CUDA, "corpus workspace allocation failed (%lld frame rows, %lld windows): %s", rows, W, cudaGetErrorString(e));
+        }
+        const bool grows = f_rows.get() || f_pairs.get() || f_starts.get() || f_win0.get() || f_frow.get() || f_recs.get();
+        if (grows) CK(cudaEventSynchronize(h->corpus_ev));            // the previous call may still read what is replaced
+        if (f_rows.get()) h->d_cw_rows = std::move(f_rows);
+        if (f_pairs.get()) h->d_cw_pairs = std::move(f_pairs);
+        if (f_starts.get()) h->d_cw_starts = std::move(f_starts);
+        if (f_win0.get()) h->d_cw_win0 = std::move(f_win0);
+        if (f_frow.get()) h->d_cw_frow = std::move(f_frow);
+        if (f_recs.get()) h->d_cw_recs = std::move(f_recs);
+    }
+    CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));                      // a corpus call on another stream may still use it
+    // the call's work on s; the event is recorded after it even when a launch fails, so the next call orders itself after
+    // whatever this one queued
+    auto launch = [&]() -> int {
+        CK(cudaMemcpyAsync(h->d_cw_win0.get(), win0.data(), win0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_cw_frow.get(), frow.data(), frow.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_cw_recs.get(), recs.data(), recs.size() * sizeof(CorpusRec), cudaMemcpyHostToDevice, s));
+        float* frames = h->d_cw_rows.get();
+        if (n_pairs > 0 || W > 0) {
+            ProfScope ps(h, 0, s);
+            CK(cudaMemsetAsync(frames, 0, (size_t)rows * h->row_stride * sizeof(float), s));
+            const float inv = 1.0f / (float)divisor, scale = inv * inv / (float)c.n_fft;
+            if (n_pairs > 0) {
+                corpus_pairs_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, s>>>(h->d_cw_recs.get(), (int)recs.size() - 1, n_pairs,
+                                                                                    c.hop_samples, h->d_cw_pairs.get());
+                CK(cudaGetLastError());
+            }
+            if (n_fast_pairs > 0) {
+                const int grid = (int)std::min<int64_t>((n_fast_pairs + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
+                mfcc_fast_corpus_kernel<<<grid, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, h->d_cw_pairs.get(), n_fast_pairs, c.hop_samples, scale,
+                                                                                  mel_tables(h), fast_tables(h), frames, h->row_stride);
+                CK(cudaGetLastError());
+            }
+            if (n_pairs > n_fast_pairs) {
+                const int64_t tiles = (n_pairs - n_fast_pairs + K1_TILE / 2 - 1) / (K1_TILE / 2);
+                const int grid = (int)std::min<int64_t>(tiles, (int64_t)h->sm_count * 4);
+                mfcc_corpus_kernel<<<grid, K1_THREADS, h->k1_batch_smem, s>>>(d_pcm, h->d_cw_pairs.get() + n_fast_pairs, n_pairs - n_fast_pairs,
+                                                                             c.hop_samples, h->used, scale, mel_tables(h), frames, h->row_stride);
+                CK(cudaGetLastError());
+            }
+            if (W > 0) {
+                corpus_windows_kernel<<<(unsigned)((W + 255) / 256), 256, 0, s>>>(h->d_cw_win0.get(), h->d_cw_frow.get(), (int)n_rec, W, schedule, chunk,
+                                                                                h->rel_window, c.hop_samples, T, h->d_cw_starts.get());
+                CK(cudaGetLastError());
+            }
+        }
+        {
+            ProfScope ps(h, 1, s);
+            if (W > 0) {
+                // every model scans the windows in place.  One model runs pb_predict's dispatch (the warp-per-window kernel up to
+                // 8 192 windows for the default network); a bank runs its fused family in one predict-mode bank launch, the others
+                // one launch each
+                K2In in{};
+                in.inputs = frames; in.starts = h->d_cw_starts.get(); in.row_stride = h->row_stride;
+                in.T = T; in.F_base = h->n_out; in.use_delta = c.use_delta;
+                BankParams P{};
+                int nm = 0;
+                for (int m = 0; m < M; ++m) {
+                    const Network& net = h->models[m];
+                    K2Out o{};
+                    o.raw = d_raw + (int64_t)m * W;
+                    o.conf = d_conf ? d_conf + (int64_t)m * W : nullptr;
+                    if (M > 1 && bank_fused(net, h->feat)) {
+                        set_bank_slot(P, nm++, net, o);
+                    } else {
+                        rc = launch_gru_kernels(net, h->feat, in, false, W, o, s);
+                        if (rc != PB_OK) return rc;
+                    }
+                }
+                if (nm) {
+                    rc = launch_bank<false>(P, nm, in, W, s);
+                    if (rc != PB_OK) return rc;
+                }
+            }
+            if (d_fired || d_activations || d_above || d_sum) {
+                CorpusTrig t{};
+                t.raw = d_raw; t.conf = d_conf; t.fired = d_fired; t.activations = d_activations; t.above = d_above; t.sum = d_sum;
+                t.win0 = h->d_cw_win0.get(); t.W = W; t.n_rec = (int)n_rec; t.schedule = schedule;
+                t.hot_f = (float)(1.0 - threshold); t.above_f = (float)threshold;
+                t.sim_reset = trigger_reset(chunk);
+                for (int m = 0; m < M; ++m) {
+                    t.dp[m] = decode_params(h->models[m]);
+                    t.dp[m].trigger_reset = trigger_reset(2 * chunk);            // TriggerDetector(2c bytes, ...) of a chunk-c listener
+                }
+                const unsigned per = CORPUS_TRIG_THREADS / 32;
+                corpus_trigger_kernel<<<dim3((unsigned)((n_rec + per - 1) / per), (unsigned)M), CORPUS_TRIG_THREADS, 0, s>>>(t);
+                CK(cudaGetLastError());
+            }
+        }
+        return PB_OK;
+    };
+    rc = launch();
+    const cudaError_t er = cudaEventRecord(h->corpus_ev, s);
+    if (rc != PB_OK) return rc;
+    if (er != cudaSuccess) return fail(PB_ERR_CUDA, "cudaEventRecord failed: %s", cudaGetErrorString(er));
+    return PB_OK;
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {

@@ -223,7 +223,7 @@ __device__ __forceinline__ void bank_scan(const BankParams& P, int m0, const int
 #pragma unroll
             for (int hf = 0; hf < 2; ++hf) {
                 const float* row = nullptr;                                 // stays nullptr: a row before the stream's first frame
-                if (ok[hf]) row = RING ? rc[hf].next(step) : in.inputs + (idx[hf] * in.T + step) * F;
+                if (ok[hf]) row = RING ? rc[hf].next(step) : input_row(in, idx[hf], step);
                 xv[hf][0] = (row != nullptr && 2 * t < F) ? __ldg(row + 2 * t) : 0.f;
                 xv[hf][1] = (row != nullptr && 2 * t + 1 < F) ? __ldg(row + 2 * t + 1) : 0.f;
                 xv[hf][2] = (row != nullptr && 2 * t + 8 < F) ? __ldg(row + 2 * t + 8) : 0.f;

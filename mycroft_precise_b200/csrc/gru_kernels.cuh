@@ -40,16 +40,36 @@ struct K2Out {
     unsigned route_bit;              // this model's bit of route[sid]
 };
 
-// Where row t of item i comes from.
+// Where row t of item i comes from.  Predict mode (!RING) reads row starts[i] + t of `inputs`, rows row_stride floats apart:
+// pb_predict's [n][T][F_in] windows (starts null: item i starts at row i * T, row_stride = F_in), or a recorded corpus's
+// frame rows (pb_score_corpus: one start row per window, rows of the MFCC width padded to 4, use_delta taken within the
+// window).  The union keeps K2In, and with it every stream-tick kernel's parameter block, the size it had.
 struct K2In {
-    const float* inputs;             // predict mode: [n][T][F_in] contiguous
+    const float* inputs;             // predict mode: window rows (see above)
     const float* ring;               // stream mode: [max_streams][ring_rows][row_stride]
-    const long long* n_samples;      // stream mode: samples consumed (after this tick)
+    union {
+        const long long* n_samples;  // stream mode: samples consumed (after this tick)
+        const long long* starts;     // predict mode: first row of item i's window, or null
+    };
     const int* ids;                  // stream mode: item -> stream id (null = identity)
     int ring_rows, row_stride, window, hop;
     int T, F_base;                   // F_base = MFCC width (without deltas)
     int use_delta;
 };
+
+// Predict mode: row t of item i's window.
+__device__ __forceinline__ const float* input_row(const K2In& in, long long i, int t) {
+    return in.inputs + ((in.starts ? in.starts[i] : i * in.T) + t) * (long long)in.row_stride;
+}
+
+// Predict mode, column f of row t of item i: with use_delta (corpus windows of F_base columns) column f >= F_base is the
+// delta of column f - F_base against row t - 1, 0 on row 0 (add_deltas within the window, network_runner.py:150-151).
+__device__ __forceinline__ float input_value(const K2In& in, long long i, int t, int f) {
+    const float* row = input_row(in, i, t);
+    if (!in.use_delta || f < in.F_base) return __ldg(row + f);
+    const int fb = f - in.F_base;
+    return t > 0 ? __ldg(row + fb) - __ldg(row + fb - in.row_stride) : 0.f;
+}
 
 __device__ __forceinline__ float hard_sigmoid(float x) { return fminf(fmaxf(fmaf(0.2f, x, 0.5f), 0.f), 1.f); }
 __device__ __forceinline__ float sigmoid32(float x) { return 1.f / (1.f + expf(-x)); }
@@ -257,7 +277,7 @@ gru_small_kernel(const __grid_constant__ GruSmallW<H, F> P, K2In in, long long n
                         }
                     }
                 } else {
-                    const float* row = in.inputs + ((i0 + s) * in.T + t) * F;
+                    const float* row = input_row(in, i0 + s, t);
 #pragma unroll
                     for (int f = 0; f < F; ++f) x[s][f] = __ldg(row + f);
                 }
@@ -337,7 +357,7 @@ gru_warp_kernel(const __grid_constant__ GruSmallW<H, F> P, K2In in, long long n,
                 const int t = lane;
                 if (t >= cur.lead) { int sl = cur.slot + t; sl = sl >= cur.rows ? sl - cur.rows : sl; row = cur.base + sl * cur.stride; }
             } else {
-                row = in.inputs + (i * in.T + lane) * F;
+                row = input_row(in, i, lane);
             }
         }
         if (row != nullptr) {
@@ -353,7 +373,7 @@ gru_warp_kernel(const __grid_constant__ GruSmallW<H, F> P, K2In in, long long n,
 #pragma unroll
             for (int f = 0; f < F; ++f) x[f] = __shfl_sync(0xffffffffu, xrow[f], t);
         } else {
-            const float* row = RING ? cur.next(t) : in.inputs + (i * in.T + t) * F;
+            const float* row = RING ? cur.next(t) : input_row(in, i, t);
 #pragma unroll
             for (int f = 0; f < F; ++f) x[f] = row ? __ldg(row + f) : 0.f;          // same address in every lane: broadcast
         }
@@ -488,7 +508,7 @@ gru_tiled_kernel(GruTiledW W, K2In in, long long n, DecodeParams dp, K2Out out) 
                         v = cur - (prow ? prow[fb] : 0.f);
                     }
                 } else {
-                    v = __ldg(in.inputs + (i * in.T + t) * F + f);
+                    v = input_value(in, i, t, f);
                 }
             }
             X[f * K2_TILE_STREAMS + b] = v;

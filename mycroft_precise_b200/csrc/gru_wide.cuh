@@ -82,7 +82,7 @@ gru_wide_kernel(GruWideW W, K2In in, long long n, DecodeParams dp, K2Out out) {
                         v = cur - (prow ? prow[fb] : 0.f);
                     }
                 } else {
-                    v = __ldg(in.inputs + (i * in.T + step) * F + f);
+                    v = input_value(in, i, step, f);
                 }
             }
             A[b * AS + f] = v;

@@ -8,7 +8,14 @@
 
 The gather of overlapping windows is a strided view on the device tensor (torch, plumbing); MFCC and
 the network run in the CUDA library.
+
+Recorded corpora (many recordings per device call, no window materialised: pb_score_corpus):
+  score_corpus      every bank model over a list of recordings, listener or simulate schedule
+  Metric, simulate  ~ precise/scripts/simulate.py:45-80, :106-129 (SimulateScript.run's per-file metrics and total)
+  false_activations ~ precise/scripts/train_incremental.py:113-137 (train_on_audio's selection of clips, fixed weights)
 """
+from dataclasses import dataclass
+
 import numpy as np
 
 from .core import PreciseB200
@@ -89,3 +96,160 @@ def evaluate(core: PreciseB200, audio, chunk_size_bytes: int = 2048):
     if win.shape[0] == 0:
         return win.new_zeros((0,))
     return core.predict(win)
+
+
+# Samples per library call of score_corpus: larger lists are scored in several calls (a single longer recording alone).
+CORPUS_CALL_SAMPLES = 1 << 30
+
+
+def _pack(core: PreciseB200, recs):
+    """Recordings -> (1-D int16 device tensor, host int64 offsets [entries + 1], entry index of each recording).  Every
+    recording starts at a multiple of 8 samples, so that at the default geometry all its frames take the fast MFCC kernel;
+    where the previous one ends elsewhere, an entry of the 1..7 padding samples sits between them (its outputs are dropped)."""
+    torch = core.torch
+    bounds, entry, pos = [0], [], 0
+    for r in recs:
+        if pos % 8:
+            pos += 8 - pos % 8
+            bounds.append(pos)
+        entry.append(len(bounds) - 1)
+        pos += int(r.shape[0])
+        bounds.append(pos)
+    offsets = np.asarray(bounds, np.int64)
+    pcm = torch.zeros(max(pos, 1), dtype=torch.int16, device=core.device)
+    for r, e in zip(recs, entry):
+        if r.shape[0]:
+            pcm[offsets[e]:offsets[e + 1]].copy_(torch.from_numpy(r) if isinstance(r, np.ndarray) else r)
+    return pcm, offsets, np.asarray(entry, np.int64)
+
+
+def _check_recording(core: PreciseB200, r):
+    torch = core.torch
+    if isinstance(r, np.ndarray):
+        ok = r.dtype == np.int16 and r.ndim == 1
+    else:
+        ok = isinstance(r, torch.Tensor) and r.dtype == torch.int16 and r.dim() == 1 and r.device == core.device
+    if not ok:
+        raise ValueError('recordings must be 1-D int16 numpy arrays or CUDA tensors on %s' % core.device)
+    return r if isinstance(r, np.ndarray) else r.contiguous()
+
+
+def score_corpus(core: PreciseB200, recordings, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
+    """Every bank model of ``core`` over ``recordings`` (a list of 1-D int16 numpy arrays or CUDA tensors of any lengths).
+    Returns dict(raw f32 [M, W], conf f64 [M, W], fired u8 [M, W], window_offsets (host int64 [n + 1]: recording r's windows
+    are columns window_offsets[r] .. window_offsets[r + 1] - 1), activations i64 [M, n], and for the simulate schedule
+    above i64 [M, n] and sum f64 [M, n], else None).  Schedules: include/precise_b200.h, pb_score_corpus.  divisor: 32768 for
+    audio as the stream path reads it (buffer_to_audio), 32767 for audio as load_audio reads wav files."""
+    torch = core.torch
+    recs = [_check_recording(core, r) for r in recordings]
+    groups, cur, size = [], [], 0
+    for r in recs:
+        L = int(r.shape[0])
+        if cur and size + L + 8 > CORPUS_CALL_SAMPLES:
+            groups.append(cur)
+            cur, size = [], 0
+        cur.append(r)
+        size += L + 8
+    groups.append(cur)
+    parts = []
+    for g in groups:
+        pcm, offsets, entry = _pack(core, g)
+        res = core.score_corpus(pcm, offsets, schedule, chunk, threshold, divisor)
+        if len(entry) < len(offsets) - 1:                     # drop the padding entries
+            counts = np.array([core.corpus_windows(int(L), schedule, chunk) for L in np.diff(offsets)], np.int64)
+            w0 = np.concatenate([[0], np.cumsum(counts)])
+            cols = torch.from_numpy(np.concatenate([np.arange(w0[e], w0[e + 1]) for e in entry] + [np.zeros(0, np.int64)])).to(core.device)
+            rows = torch.from_numpy(entry).to(core.device)
+            res = {k: None if v is None else v.index_select(1, cols if k in ('raw', 'conf', 'fired') else rows)
+                   for k, v in res.items()}
+        parts.append(res)
+    cat = lambda k: None if parts[0][k] is None else torch.cat([p[k] for p in parts], 1)
+    out = {k: cat(k) for k in ('raw', 'conf', 'fired', 'activations', 'above', 'sum')}
+    counts = [core.corpus_windows(int(r.shape[0]), schedule, chunk) for r in recs]
+    out['window_offsets'] = np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)
+    return out
+
+
+@dataclass
+class Metric:
+    """precise-simulate's false-activation metric of one recording or of a whole folder (simulate.py:45-80)."""
+    chunk_size: int
+    seconds: float = 0.0
+    activated_chunks: int = 0
+    activations: int = 0
+    activation_sum: float = 0.0
+    sample_rate: int = 16000
+
+    @property
+    def days(self) -> float:
+        return self.seconds / 86400.0
+
+    @property
+    def chunks(self) -> float:
+        return self.seconds * self.sample_rate / self.chunk_size
+
+    def add(self, other: 'Metric'):
+        self.seconds += other.seconds
+        self.activated_chunks += other.activated_chunks
+        self.activations += other.activations
+        self.activation_sum += other.activation_sum
+
+    def info_string(self, title: str) -> str:
+        lines = ['=== %s ===' % title,
+                 'Hours: {:.2f}'.format(self.days * 24),
+                 'Activations / Day: {:.2f}'.format(self.activations / self.days),
+                 'Activated Chunks / Day: {:.2f}'.format(self.activated_chunks / self.days),
+                 'Average Activation (*100): {:.2f}'.format(100.0 * self.activation_sum / self.chunks)]
+        return '\n'.join(lines)
+
+
+def simulate(core: PreciseB200, recordings, chunk_size=4096, threshold=0.5):
+    """SimulateScript.run's numbers for bank slot 0 over int16 recordings read as load_audio reads them (samples / 32767):
+    (one Metric per recording, their total).  An empty recording is skipped, as the reference skips it: its entry is None.
+    A recording too short for one window (fewer than n_features + 1 frames) counts its seconds with no windows, where the
+    reference's Runner.predict fails on an empty input."""
+    res = score_corpus(core, recordings, 'simulate', chunk_size, threshold, divisor=32767)
+    above = res['above'][0].cpu().numpy()
+    acts = res['activations'][0].cpu().numpy()
+    sums = res['sum'][0].cpu().numpy()
+    sr = core.params.sample_rate
+    total = Metric(chunk_size, sample_rate=sr)
+    metrics = []
+    for i, r in enumerate(recordings):
+        L = int(r.shape[0])
+        if L == 0:
+            metrics.append(None)
+            continue
+        m = Metric(chunk_size, L / sr, int(above[i]), int(acts[i]), float(sums[i]), sr)
+        total.add(m)
+        metrics.append(m)
+    return metrics, total
+
+
+def false_activations(core: PreciseB200, recordings, chunk_size=2048, threshold=0.5):
+    """train_on_audio's selection (train_incremental.py:113-137) with fixed weights, bank slot 0, recordings read as
+    load_audio reads them (samples / 32767).  Each recording is cut as chunk_audio cuts it (util.py:30-32: chunks end at
+    range(c, L, c), floor((L - 1) / c) of them) and fed to a fresh listener of chunk c.  Returns a list of (recording index,
+    chunk index, clip) for every chunk whose confidence is above ``threshold``; the clip is the float32 audio of the last
+    buffer_samples samples up to the end of that chunk, zeros before the recording's start.
+    Deliberate differences: the reference's audio_buffer carries the previous file's tail into the next file (glob order),
+    here every recording starts from zeros; and it retrains between chunks, which is out of scope here."""
+    c = int(chunk_size)
+    recs = [r[:((int(r.shape[0]) - 1) // c) * c] if int(r.shape[0]) else r for r in recordings]
+    res = score_corpus(core, recs, 'listener', c, divisor=32767)
+    conf = res['conf'][0].cpu().numpy()
+    wo = res['window_offsets']
+    bs = core.params.buffer_samples
+    out = []
+    for i, r in enumerate(recs):
+        hits = np.nonzero(conf[wo[i]:wo[i + 1]] > threshold)[0]
+        if hits.size == 0:
+            continue
+        a = r if isinstance(r, np.ndarray) else r.cpu().numpy()
+        for k in hits:
+            end = (int(k) + 1) * c
+            clip = np.zeros(bs, np.float32)
+            seg = a[max(0, end - bs):end].astype(np.float32) / np.float32(32767)
+            clip[bs - seg.shape[0]:] = seg
+            out.append((i, int(k), clip))
+    return out
