@@ -214,7 +214,8 @@ int pb_update_host(pb_handle* h, const int16_t* h_pcm, const int32_t* h_stream_i
  * given streams: d_out [n][n_features][pb_mfcc_width()] float32, oldest row first. */
 int pb_read_window(pb_handle* h, const int32_t* d_stream_ids, int64_t n, float* d_out, void* stream);
 
-/* Replaces Listener.clear (network_runner.py:121-123) and re-arms the stream's trigger counter (of every bank model).
+/* Replaces Listener.clear (network_runner.py:121-123) and re-arms the stream's trigger counter (of every bank model, and its
+ * pool detector).
  * d_stream_ids NULL => streams 0..n-1. */
 int pb_clear(pb_handle* h, const int32_t* d_stream_ids, int64_t n, void* stream);
 
@@ -281,7 +282,9 @@ int pb_get_stream_trigger(const pb_handle* h, int32_t slot, const int32_t* h_str
  *                                speechpy vectoriser)
  * The size depends only on the front-end fields, so two handles with the same front end agree on it (1024 + 2048 + 96 =
  * 3168 B at the defaults).  Not in the record: subscription masks and per-stream trigger settings (pb_get_stream_models /
- * pb_get_stream_trigger read them), and the handle's chunk_samples (a record imports into a handle with another chunk). */
+ * pb_get_stream_trigger read them), the stream's pool model (pb_get_stream_pool), and the handle's chunk_samples (a record
+ * imports into a handle with another chunk).  A handle with a model pool writes the stream's pool detector into pool_activation
+ * and reads it back on import; a handle without one writes 0 and ignores it. */
 #define PB_STATE_MAGIC 0x53534250u    /* "PBSS" in little-endian bytes */
 #define PB_STATE_VERSION 1
 typedef struct pb_stream_state_header {
@@ -290,7 +293,8 @@ typedef struct pb_stream_state_header {
     int32_t num_models;               /* pb_num_models of the exporting handle                              */
     int32_t sample_rate, window_samples, hop_samples, n_fft, n_filt, n_mfcc, n_features, use_delta, vectorizer;
     int64_t n_samples;                /* samples the stream has consumed                                    */
-    int32_t reserved[2];              /* 0                                                                  */
+    int32_t pool_activation;          /* TriggerDetector.activation of the stream's pool model; 0 without a pool */
+    int32_t reserved;                 /* 0                                                                  */
     int32_t activation[PB_MAX_MODELS];  /* TriggerDetector.activation of bank slot m; 0 from num_models on  */
 } pb_stream_state_header;
 
@@ -346,6 +350,55 @@ int pb_get_stream_history(const pb_handle* h, const int32_t* h_stream_ids, int64
  * PB_ERR_INVALID: null handle or d_out with n > 0, n outside [0, max_streams], samples out of range.  PB_ERR_STATE: no
  * pool. */
 int pb_read_history(pb_handle* h, const int32_t* d_stream_ids, int64_t n, int64_t samples, int16_t* d_out, void* stream);
+
+/* Model pool: a second, large set of networks on a handle, beside the bank, for a server whose devices each bring their own
+ * wake word (custom models trained with precise-train, each used by one or a few devices).  Each stream points at at most one
+ * pool model, or at none.  A pool tick runs K1 once, as every tick does, then scores every item whose stream has a pool model
+ * with that model's network, ThresholdDecoder and TriggerDetector (the model's sensitivity and trigger_level; the refractory
+ * count from the handle's chunk_samples).  One window scan per item, whatever the number of models: the scan of a model
+ * costs one 14 208 B weight load per tile of 64 (or of at most 16) of its streams.
+ *   - Networks: the fused family only (hidden <= 24, feature size <= 16, no deltas), which every network precise-train builds
+ *     at its defaults is in.  A pool stream's raw and conf are bit-identical to the same network's in a bank.
+ *   - Memory: about 14.3 KB per slot, 51 200 B per distinct decoder table at the default thresholds (models whose tables
+ *     are bit-identical share one copy), 16 B per stream.
+ *   - The bank, its masks and trigger settings are independent of the pool; pb_update_models does not score pool models and
+ *     pb_update_pool scores no bank model.  Not covered: pb_update_host, pb_score_corpus, per-stream trigger settings.
+ *   - A handle that never calls pb_set_pool runs exactly as before.
+ *
+ * pb_set_pool: a pool of max_models slots (max_models in [1, 2^24]), every slot empty and every stream on none.  Synchronous.
+ * Calling it again replaces the pool and unassigns every stream; 0 frees it (pb_destroy frees it too).  PB_ERR_INVALID: null
+ * handle, max_models out of range.  PB_ERR_CUDA: an allocation failed (the handle then has no pool). */
+int pb_set_pool(pb_handle* h, int32_t max_models);
+/* Loads a network into slot model_id in [0, max_models): cfg, weights, h_cd and cd_len as pb_add_model takes them (front-end
+ * fields equal to the handle's).  A slot that holds a model is replaced; its streams keep the slot and get fresh detectors, as
+ * Mycroft builds a new runner for a new model, and score the new weights from the next tick.  Synchronous (queued work
+ * finishes with the old model); on an error the slot is as it was.  PB_ERR_INVALID: a null argument, model_id out of range, a
+ * front-end field that differs, a bad network field or cd_len.  PB_ERR_UNSUPPORTED: a network outside the fused family.
+ * PB_ERR_STATE: no pool. */
+int pb_pool_load(pb_handle* h, int32_t model_id, const pb_config* cfg, const float* h_kernel, const float* h_recurrent,
+                 const float* h_bias, const float* h_dense_w, float dense_b, const double* h_cd, int64_t cd_len);
+/* Stream h_stream_ids[i] (HOST; NULL => 0..n-1) goes to pool slot h_model_ids[i] (HOST), -1 = none.  Validates everything
+ * before it changes anything, then synchronises the device.  A stream whose model changes gets a fresh detector; one set to
+ * the model it has keeps its state.  pb_clear re-arms a stream's pool detector and keeps its model.  PB_ERR_INVALID, and
+ * nothing changes: null handle, n outside [0, max_streams], an id outside [0, max_streams), a duplicate id, a null array with
+ * n > 0, a model id outside [-1, max_models) or a slot that holds no model.  PB_ERR_STATE: no pool. */
+int pb_set_stream_pool(pb_handle* h, const int32_t* h_stream_ids, const int32_t* h_model_ids, int64_t n);
+/* The pool models of the given streams (h_stream_ids NULL => 0..n-1; -1 = none, and -1 for every stream without a pool) into
+ * h_model_ids [n] (HOST).  PB_ERR_INVALID: null handle or output with n > 0, n outside [0, max_streams], an id outside
+ * [0, max_streams). */
+int pb_get_stream_pool(const pb_handle* h, const int32_t* h_stream_ids, int64_t n, int32_t* h_model_ids);
+/* Pool tick.  d_offsets NULL: pb_update's uniform tick (d_pcm [n][chunk_samples], max_len ignored); otherwise pb_update_ragged's
+ * (d_offsets [n+1] DEVICE, max_len >= 1, and the handle becomes ragged).  History is appended as on every tick.  Outputs are
+ * [n]: d_raw (optional), d_conf, d_fired (optional), d_count [1] (optional, += the tick's pool fires).  An item whose stream
+ * has no pool model gets NaN / NaN / 0; its detector does not move and it is not counted.  Needs no slot-0 weights.
+ * d_stream_ids must be unique, as for pb_update; ids that repeat a stream give wrong answers for it but never a write outside
+ * the pool's buffers (items past a model's stream count are not scored and get NaN / NaN / 0).
+ * Asynchronous on `stream`; pool ticks on different CUDA streams are ordered by the library (they share list scratch).
+ * PB_ERR_INVALID: null handle or d_conf, n outside [0, max_streams], max_len < 1 with offsets.  PB_ERR_STATE: no pool, or
+ * offsets with a non-zero pb_debug_k1_mode. */
+int pb_update_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len,
+                   const int32_t* d_stream_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
+                   unsigned long long* d_count, void* stream);
 
 /* Recorded corpora: whole recordings scored on the device in one call, the hot path of precise-simulate
  * (precise/scripts/simulate.py:92-129) and of false-activation mining (precise/scripts/train_incremental.py:113-137).
@@ -433,6 +486,9 @@ int pb_debug_gru_mode(pb_handle* h, int mode);
  * the FFT kernel it replaced (mfcc_fast_stream_kernel, bit-identical results); 3 = that kernel with its original 64-bit set-up; 4 / 5 / 6 = csrc/mfcc_mma.cuh, the DFT on mma.sync (stage 2 / both stages / both with a
  * shuffle epilogue; hop >= 512, chunk >= hop).  All variants are parity-tested (tests/test_gpu_parity.py). */
 int pb_debug_k1_mode(pb_handle* h, int mode);
+/* Test / A-B hook for the model pool's tiles: 0 = block tiles of 64 for each model's full groups, warp tiles of 16 for the
+ * rest; 1 = warp tiles of 16 for every position.  Both score bit-identical outputs.  PB_ERR_STATE without a pool. */
+int pb_debug_pool_tiles(pb_handle* h, int warp_only);
 /* CPU model of a tensor-core formulation of the DFT (csrc/mfcc_tc.cuh: radix-16 butterflies, second stage as an fp16 hi / lo
  * matrix product) for one frame of 512 int16 samples -> |X[k]|^2, k = 0..256.  No device needed.  Test hook. */
 int pb_debug_tc_dft_power(const int16_t* x512, double* power257);

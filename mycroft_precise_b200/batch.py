@@ -23,6 +23,7 @@ class StreamBatch:
         torch = self.core.torch
         self.count = torch.zeros(1, dtype=torch.int64, device=self.core.device)
         self.counts = torch.zeros(1, dtype=torch.int64, device=self.core.device)    # per bank model, update_models / update_ragged
+        self.pool_count = torch.zeros(1, dtype=torch.int64, device=self.core.device)   # pool fires, update_pool
         self._out = None
         self._bank_out = None
 
@@ -48,6 +49,29 @@ class StreamBatch:
     def stream_trigger(self, slot, ids=None):
         """(sensitivity, trigger_level, chunk_size) host arrays of bank slot ``slot``.  See PreciseB200.stream_trigger."""
         return self.core.stream_trigger(slot, ids)
+
+    def set_pool(self, max_models):
+        """A model pool of ``max_models`` slots beside the bank; each stream is scored by at most one pool model.  See
+        PreciseB200.set_pool."""
+        self.core.set_pool(max_models)
+
+    def pool_load(self, model_id, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False):
+        """Load a network (GruModel or weights path) into pool slot ``model_id``.  See PreciseB200.pool_load."""
+        self.core.pool_load(model_id, model, params, sensitivity, trigger_level, decode_legacy_f64)
+
+    def set_stream_pool(self, model_ids, ids=None):
+        """Each stream's pool model (host int32, -1 = none).  See PreciseB200.set_stream_pool."""
+        self.core.set_stream_pool(model_ids, ids)
+
+    def stream_pool(self, ids=None):
+        """Host int32 array: each stream's pool model, -1 = none.  See PreciseB200.stream_pool."""
+        return self.core.stream_pool(ids)
+
+    def update_pool(self, pcm, ids=None, offsets=None, max_len=None):
+        """One pool tick (update's with pcm [n, chunk_samples]; update_ragged's with 1-D pcm and ``offsets``) -> dict(raw,
+        conf, fired), each [n].  ``self.pool_count`` accumulates pool fires until reset_count().  See
+        PreciseB200.update_pool."""
+        return self.core.update_pool(pcm, ids, offsets, max_len, count=self.pool_count)
 
     def set_history(self, samples=None, max_rows=None):
         """A device pool for the recent audio of up to ``max_rows`` streams, ``samples`` each (default buffer_samples, the
@@ -100,22 +124,26 @@ class StreamBatch:
     def export_streams(self, ids=None):
         """A snapshot of streams ids (host int32 array; None: every stream): dict(state = their state records, a uint8 CUDA
         tensor [n, stream_state_bytes]; stream_models = their masks; stream_trigger = each bank slot's (sensitivity,
-        trigger_level, chunk_size)).  The tensor may go through .cpu() or .to(another device) and come back.  Whether a
-        stream has audio history, and that audio, are not part of a snapshot.  See PreciseB200.export_streams."""
+        trigger_level, chunk_size); with a model pool, stream_pool = their pool models).  The tensor may go through .cpu() or
+        .to(another device) and come back.  Whether a stream has audio history, and that audio, are not part of a snapshot.
+        See PreciseB200.export_streams."""
         core = self.core
         n = self.n_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
         sids = self._host_ids(ids, n)
         state = core.export_streams(core.torch.from_numpy(sids).to(core.device))
-        return dict(state=state, stream_models=core.stream_models(sids),
+        snap = dict(state=state, stream_models=core.stream_models(sids),
                     stream_trigger=[core.stream_trigger(m, sids) for m in range(core.num_models)])
+        if core.pool_models:
+            snap['stream_pool'] = core.stream_pool(sids)
+        return snap
 
     def import_streams(self, snapshot, ids=None):
         """Continue the snapshot's streams (export_streams of a batch with the same front end and bank) as streams ids (host
-        int32 array; None: 0..n-1) of this batch.  Their masks, then each slot's trigger settings are set where they differ
-        from this batch's, so a batch never becomes routed or trigger-flagged for nothing; then the state is imported, which
-        overwrites the activations those two steps may have re-armed.  A snapshot that does not match raises ValueError
-        before anything changes.  History on / off is not carried: the streams keep this batch's setting, and one that has
-        history starts empty at the imported sample count."""
+        int32 array; None: 0..n-1) of this batch.  Their masks, then each slot's trigger settings, then their pool models are
+        set where they differ from this batch's, so a batch never becomes routed or trigger-flagged for nothing; then the state
+        is imported, which overwrites the activations those steps may have re-armed.  A snapshot that does not match (pool
+        models this batch does not hold included) raises ValueError before anything changes.  History on / off is not
+        carried: the streams keep this batch's setting, and one that has history starts empty at the imported sample count."""
         core = self.core
         torch = core.torch
         state = snapshot['state'].to(core.device)
@@ -130,6 +158,14 @@ class StreamBatch:
         # the record headers against this batch's own, so that the steps below never run for a snapshot import would refuse
         ref = core.export_streams(n=1)[0, :48]
         bad = (state[:, :48] != ref).any(1) | (state[:, 48:56].contiguous().view(torch.int64)[:, 0] < 0)
+        pool = None
+        if 'stream_pool' in snapshot:        # pool models this batch can take, before anything changes
+            pool = np.asarray(snapshot['stream_pool'], np.int32)
+            _check_np('stream_pool', pool, np.int32, (n,), optional=False)
+            on = pool[pool != -1]
+            if on.size and (on.min() < 0 or on.max() >= core.pool_models or not core.pool_loaded[on].all()):
+                raise ValueError('snapshot names pool models this batch does not hold (pool of %d slots); nothing was changed'
+                                 % core.pool_models)
         if n and bool(bad.any()):
             i = int(bad.nonzero()[0, 0])
             got, want = state[i, :48].cpu().numpy().view(np.int32), ref.cpu().numpy().view(np.int32)
@@ -145,6 +181,10 @@ class StreamBatch:
             differ = (cs.view(np.uint64) != sens.view(np.uint64)) | (cl != lvl) | (cc != chunk)
             if differ.any():
                 core.set_stream_trigger(slot, sens[differ], lvl[differ], chunk[differ], ids=sids[differ])
+        if pool is not None:
+            differ = core.stream_pool(sids) != pool
+            if differ.any():
+                core.set_stream_pool(pool[differ], sids[differ])
         core.import_streams(state, sids)
 
     def _bank_buffers(self, n):
@@ -187,6 +227,7 @@ class StreamBatch:
     def reset_count(self):
         self.count.zero_()
         self.counts.zero_()
+        self.pool_count.zero_()
 
     def clear(self, ids=None):
         self.core.clear(ids=ids) if ids is not None else self.core.clear()

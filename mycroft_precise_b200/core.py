@@ -73,6 +73,11 @@ SYMBOLS = {
     'pb_set_stream_history': (C.c_int, [_VP, _VP, _VP, _I64]),
     'pb_get_stream_history': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_read_history': (C.c_int, [_VP, _VP, _I64, _I64, _VP, _VP]),
+    'pb_set_pool': (C.c_int, [_VP, _I32]),
+    'pb_pool_load': (C.c_int, [_VP, _I32, C.POINTER(pb_config), _VP, _VP, _VP, _VP, C.c_float, _VP, _I64]),
+    'pb_set_stream_pool': (C.c_int, [_VP, _VP, _VP, _I64]),
+    'pb_get_stream_pool': (C.c_int, [_VP, _VP, _I64, _VP]),
+    'pb_update_pool': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
     'pb_corpus_windows': (_I64, [C.POINTER(pb_config), _I32, _I64, _I64]),
     'pb_score_corpus': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
@@ -86,6 +91,7 @@ SYMBOLS = {
     'pb_debug_force_generic': (C.c_int, [_VP, C.c_int]),
     'pb_debug_gru_mode': (C.c_int, [_VP, C.c_int]),
     'pb_debug_k1_mode': (C.c_int, [_VP, C.c_int]),
+    'pb_debug_pool_tiles': (C.c_int, [_VP, C.c_int]),
     'pb_debug_tc_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_mma_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_tc_mfcc_frame': (C.c_int, [_VP, _VP, _VP]),
@@ -245,6 +251,9 @@ class PreciseB200:
             check(self.lib.pb_set_cdf(h, cd.ctypes.data_as(C.c_void_p), len(cd)))
         self._count = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.history_samples = 0             # set_history's samples; 0 = no history pool
+        self.pool_models = 0                 # set_pool's max_models; 0 = no model pool
+        self.pool_loaded = np.zeros(0, bool)  # which pool slots hold a model
+        self._pool_cdfs = {}                 # numpy CDF tables of pool_load, by threshold_config
 
     def close(self):
         if getattr(self, '_h', None):
@@ -277,10 +286,8 @@ class PreciseB200:
         check(self.lib.pb_load_weights(self._h, vp(k), vp(u), vp(b), vp(w), float(np.asarray(dense_b).reshape(-1)[0])))
 
     # ---- model bank: more networks over the same MFCC front end (slot 0 is the network of load_weights)
-    def add_model(self, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False) -> int:
-        """Add a network to this handle's bank; returns its slot.  ``model`` is a GruModel or a .npz / .pb / .net path (its
-        .params file is read as the reference does).  ``params`` (else the model's .params, else this handle's params) gives
-        the model's decoder settings; its front end must equal this handle's."""
+    def _model_args(self, model, params, sensitivity, trigger_level, decode_legacy_f64, cdf):
+        """(cfg, weights, CDF table or None) of a network for this handle's front end, as add_model and pool_load take it."""
         from .runner import _resolve_model
         model, pr = _resolve_model(model)
         pr = params or pr or self.params
@@ -293,12 +300,105 @@ class PreciseB200:
         cfg = make_config(pr, model.hidden, self.max_streams, self.chunk_samples, self.device.index, sensitivity,
                           trigger_level, model.activation, model.recurrent_activation, decode_legacy_f64)
         k, u, b, w = self._weights(self.feature_size, model.hidden, model.kernel, model.recurrent, model.bias, model.dense_w)
-        cd, lo, hi = numpy_cdf(pr.threshold_config)
+        cd, lo, hi = cdf(pr.threshold_config)
+        return cfg, (k, u, b, w, float(model.dense_b)), (cd if hi > lo else None)
+
+    def add_model(self, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False) -> int:
+        """Add a network to this handle's bank; returns its slot.  ``model`` is a GruModel or a .npz / .pb / .net path (its
+        .params file is read as the reference does).  ``params`` (else the model's .params, else this handle's params) gives
+        the model's decoder settings; its front end must equal this handle's."""
+        cfg, (k, u, b, w, bd), cd = self._model_args(model, params, sensitivity, trigger_level, decode_legacy_f64, numpy_cdf)
         vp = lambda a: a.ctypes.data_as(C.c_void_p)
         slot = C.c_int32(-1)
-        check(self.lib.pb_add_model(self._h, C.byref(cfg), vp(k), vp(u), vp(b), vp(w), float(model.dense_b),
-                                    vp(cd) if hi > lo else None, len(cd) if hi > lo else 0, C.byref(slot)))
+        check(self.lib.pb_add_model(self._h, C.byref(cfg), vp(k), vp(u), vp(b), vp(w), bd, _np_ptr(cd),
+                                    0 if cd is None else len(cd), C.byref(slot)))
         return int(slot.value)
+
+    # ---- model pool: up to 2^24 networks of the fused family, at most one per stream (pb_set_pool in precise_b200.h)
+    def set_pool(self, max_models):
+        """A model pool of ``max_models`` empty slots, every stream on none.  Calling it again replaces the pool and
+        unassigns every stream; 0 frees it.  Synchronous."""
+        max_models = self._int('max_models', max_models)
+        if not -2 ** 31 <= max_models < 2 ** 31:
+            raise ValueError('max_models must fit in int32, got %d' % max_models)
+        rc = self.lib.pb_set_pool(self._h, max_models)
+        if rc != -1:                         # anything but a refused argument replaced the pool
+            self.pool_models = max_models if rc == 0 else 0
+            self.pool_loaded = np.zeros(self.pool_models, bool)
+        check(rc)
+
+    def _pool_cdf(self, threshold_config):
+        key = tuple(tuple(float(x) for x in p) for p in threshold_config)
+        if key not in self._pool_cdfs:
+            self._pool_cdfs[key] = numpy_cdf(threshold_config)
+        return self._pool_cdfs[key]
+
+    def pool_load(self, model_id, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3,
+                  decode_legacy_f64=False):
+        """Load a network (GruModel or weights path, as add_model takes it) into pool slot ``model_id``, replacing what the
+        slot held; streams on the slot get fresh detectors.  Networks outside the fused family (hidden <= 24, no deltas) raise
+        NotImplementedError.  Synchronous."""
+        model_id = self._slot(model_id)
+        cfg, (k, u, b, w, bd), cd = self._model_args(model, params, sensitivity, trigger_level, decode_legacy_f64, self._pool_cdf)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        check(self.lib.pb_pool_load(self._h, model_id, C.byref(cfg), vp(k), vp(u), vp(b), vp(w), bd, _np_ptr(cd),
+                                    0 if cd is None else len(cd)))
+        self.pool_loaded[model_id] = True
+
+    def set_stream_pool(self, model_ids, ids=None):
+        """Stream ids[i] (host int32 array; None: stream i) goes to pool slot model_ids[i] (host int32 array, -1 = none).  A
+        stream whose model changes gets a fresh detector.  Synchronous; bad input raises ValueError and changes nothing."""
+        model_ids = np.asarray(model_ids)
+        n = model_ids.shape[0] if model_ids.ndim == 1 else -1
+        _check_np('model_ids', model_ids, np.int32, (n,), optional=False)
+        _check_np('ids', ids, np.int32, (n,))
+        check(self.lib.pb_set_stream_pool(self._h, _np_ptr(ids), _np_ptr(model_ids), n))
+
+    def stream_pool(self, ids=None) -> np.ndarray:
+        """int32 pool model of streams ids (host int32 array), or of every stream; -1 = none."""
+        n = self.max_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
+        _check_np('ids', ids, np.int32, (n,))
+        out = np.zeros(n, np.int32)
+        check(self.lib.pb_get_stream_pool(self._h, _np_ptr(ids), n, _np_ptr(out)))
+        return out
+
+    def update_pool(self, pcm, ids=None, offsets=None, max_len=None, out=None, count=None):
+        """Pool tick: each item scored by its stream's pool model.  Without ``offsets``, pcm is int16 CUDA [n, chunk_samples]
+        (update's tick); with them, a 1-D int16 CUDA pcm and int64 CUDA offsets [n + 1] (update_ragged's tick).  Returns
+        dict(raw f32, conf f64, fired u8), each [n]; items whose stream has no pool model are NaN / NaN / 0.  ``count``
+        (int64 [1]) accumulates the tick's pool fires."""
+        torch = self.torch
+        if offsets is None:
+            n = self._check_pcm(pcm)
+            max_len = 0
+        else:
+            if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
+                    or pcm.device != self.device):
+                raise ValueError('pcm must be a contiguous 1-D int16 tensor on %s' % self.device)
+            if (not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1
+                    or not offsets.is_contiguous() or offsets.device != self.device):
+                raise ValueError('offsets must be a contiguous 1-D int64 [n + 1] tensor on %s' % self.device)
+            n = offsets.numel() - 1
+            if n > self.max_streams:
+                raise ValueError('n = %d exceeds max_streams = %d' % (n, self.max_streams))
+            if max_len is None:
+                max_len = max(1, int((offsets[1:] - offsets[:-1]).max())) if n else 1
+            max_len = int(max_len)
+            if max_len < 1:
+                raise ValueError('max_len must be >= 1, got %d' % max_len)
+        self._check_ids(ids, n)
+        if out is not None:
+            self._check_t("out['raw']", out.get('raw'), torch.float32, n)
+            self._check_t("out['conf']", out.get('conf'), torch.float64, n, optional=False)
+            self._check_t("out['fired']", out.get('fired'), torch.uint8, n)
+        self._check_t('count', count, torch.int64, 1)
+        if out is None:
+            out = dict(raw=torch.empty(n, dtype=torch.float32, device=self.device),
+                       conf=torch.empty(n, dtype=torch.float64, device=self.device),
+                       fired=torch.empty(n, dtype=torch.uint8, device=self.device))
+        check(self.lib.pb_update_pool(self._h, _ptr(pcm), _ptr(offsets), max_len, _ptr(ids), n, _ptr(out.get('raw')),
+                                      _ptr(out['conf']), _ptr(out.get('fired')), _ptr(count), self._stream()))
+        return out
 
     @property
     def num_models(self) -> int:

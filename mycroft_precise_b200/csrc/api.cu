@@ -15,6 +15,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <string>
 #include <utility>
 #include <vector>
 
@@ -32,6 +33,7 @@
 #include "stream_state.cuh"
 #include "history.cuh"
 #include "corpus.cuh"
+#include "pool.cuh"
 
 using namespace pb;
 
@@ -201,6 +203,25 @@ struct pb_handle {
     DevArray<long long> d_cw_frow;   // [n_rec] row of each recording's frame 0
     DevArray<CorpusRec> d_cw_recs;   // [n_rec + 1] recordings in pair-list order
     cudaEvent_t corpus_ev = nullptr; // recorded after each corpus call; the next one waits on it before reusing the workspace
+    // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
+    bool pool = false;               // a pool exists
+    int32_t pool_models = 0;         // max_models
+    DevArray<uint4> d_pool_slots;    // [max_models][POOL_SLOT_U4] each slot's weights as bank_scan stages them, then its record
+    DevArray<unsigned> d_pool_count; // [max_models] list lengths of the current tick (scratch)
+    DevArray<unsigned> d_pool_list0; // [max_models + 1] first list position of each model: exclusive prefix of pool_subs
+    DevArray<int> d_pool_id;         // [max_streams] model of each stream, -1 = none
+    DevArray<int> d_pool_trig;       // [max_streams] each stream's pool TriggerDetector.activation
+    DevArray<int2> d_pool_list;      // [max_streams] pool_route_kernel's (item, stream) lists (scratch)
+    DevArray<int2> d_pool_tiles[2][2];   // [block, warp][run-time activations, Keras's defaults] (model, first position)
+    int64_t pool_tiles[2][2] = {};   // ... and their lengths
+    std::vector<int> pool_id;        // host mirror of d_pool_id
+    std::vector<int64_t> pool_subs;  // [max_models] streams on each model
+    std::vector<uint8_t> pool_keras; // [max_models] 1: the slot's network has Keras's default activations
+    struct PoolCd { DevArray<double> d; int64_t refs = 0; };
+    std::map<std::string, PoolCd> pool_cd;                  // decoder tables, shared by content (the table's bytes)
+    std::vector<std::map<std::string, PoolCd>::iterator> pool_cd_of;  // [max_models] each slot's table; pool_cd.end() = empty slot
+    cudaEvent_t pool_ev = nullptr;   // recorded after each pool tick; the next one waits on it before reusing the scratch
+    bool pool_warp_only = false;     // pb_debug_pool_tiles: every position in warp tiles
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
     cudaEvent_t pipe_ev[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -228,6 +249,7 @@ struct pb_handle {
             for (auto e : p.ev) cudaEventDestroy(e);
         if (route_ev) cudaEventDestroy(route_ev);
         if (corpus_ev) cudaEventDestroy(corpus_ev);
+        if (pool_ev) cudaEventDestroy(pool_ev);
     }
 };
 
@@ -599,8 +621,14 @@ static bool bank_fused(const Network& net, int F) {
 // fp16 hi / lo weight fragments of the fused family (gru_bank_kernel).  Column (nt, g) -> gate nt / 3,
 // unit 8 (nt % 3) + g.  Recurrent weights: k-tile 0 = hidden units 0..15 as an m16n8k16 B fragment (b0: k = 2t, 2t + 1;
 // b1: k = 2t + 8, 2t + 9), k-tile 1 = units 16..23 as an m16n8k8 one (b0 only).  Input weights: features 0..15 as one k16
-// fragment.  Bias and dense weights padded to 24 units per gate.
-static int upload_frag16(NetWeights& w, int H, int F, const float* kernel, const float* recurrent, const float* bias, const float* dense_w) {
+// fragment.  Bias and dense weights padded to 24 units per gate.  Built on the host, then uploaded per bank model
+// (upload_frag16) or copied into a pool slot (pb_pool_load).
+struct Frag16 {
+    std::vector<uint4> bf16, xf16;   // [2][MMA_NT][32], [MMA_NT][32]
+    std::vector<float> mb, mw;       // [3][24], [24]
+};
+
+static void build_frag16(Frag16& fr, int H, int F, const float* kernel, const float* recurrent, const float* bias, const float* dense_w) {
     const int H3 = 3 * H;
     auto h2 = [](float lo16, float hi16) {
         const __half a = __float2half_rn(lo16), b = __float2half_rn(hi16);
@@ -608,7 +636,8 @@ static int upload_frag16(NetWeights& w, int H, int F, const float* kernel, const
         return (uint32_t)ua | ((uint32_t)ub << 16);
     };
     auto res = [](float v) { return v - __half2float(__float2half_rn(v)); };
-    std::vector<uint4> bf16((size_t)2 * MMA_NT * 32);
+    std::vector<uint4>& bf16 = fr.bf16;
+    bf16.assign((size_t)2 * MMA_NT * 32, uint4{});
     for (int kt = 0; kt < 2; ++kt)
         for (int nt = 0; nt < MMA_NT; ++nt)
             for (int lane = 0; lane < 32; ++lane) {
@@ -622,7 +651,8 @@ static int upload_frag16(NetWeights& w, int H, int F, const float* kernel, const
                 bf16[((size_t)kt * MMA_NT + nt) * 32 + lane] = make_uint4(h2(b[0][0], b[0][1]), h2(b[1][0], b[1][1]),
                                                                           h2(res(b[0][0]), res(b[0][1])), h2(res(b[1][0]), res(b[1][1])));
             }
-    std::vector<uint4> xf16((size_t)MMA_NT * 32);
+    std::vector<uint4>& xf16 = fr.xf16;
+    xf16.assign((size_t)MMA_NT * 32, uint4{});
     for (int nt = 0; nt < MMA_NT; ++nt)
         for (int lane = 0; lane < 32; ++lane) {
             const int g = lane >> 2, t = lane & 3, gate = nt / 3, unit = 8 * (nt % 3) + g;
@@ -635,14 +665,18 @@ static int upload_frag16(NetWeights& w, int H, int F, const float* kernel, const
             xf16[(size_t)nt * 32 + lane] = make_uint4(h2(b[0][0], b[0][1]), h2(b[1][0], b[1][1]),
                                                       h2(res(b[0][0]), res(b[0][1])), h2(res(b[1][0]), res(b[1][1])));
         }
-    std::vector<float> mb(72, 0.f), mw(24, 0.f);
+    fr.mb.assign(72, 0.f);
+    fr.mw.assign(24, 0.f);
     for (int gate = 0; gate < 3; ++gate)
-        for (int u = 0; u < H; ++u) mb[gate * 24 + u] = bias[gate * H + u];
-    for (int u = 0; u < H; ++u) mw[u] = dense_w[u];
-    CK(w.bfrag16.upload(bf16));
-    CK(w.xfrag16.upload(xf16));
-    CK(w.mma_bias.upload(mb));
-    CK(w.mma_wd.upload(mw));
+        for (int u = 0; u < H; ++u) fr.mb[gate * 24 + u] = bias[gate * H + u];
+    for (int u = 0; u < H; ++u) fr.mw[u] = dense_w[u];
+}
+
+static int upload_frag16(NetWeights& w, const Frag16& fr) {
+    CK(w.bfrag16.upload(fr.bf16));
+    CK(w.xfrag16.upload(fr.xf16));
+    CK(w.mma_bias.upload(fr.mb));
+    CK(w.mma_wd.upload(fr.mw));
     return PB_OK;
 }
 
@@ -719,7 +753,11 @@ static int load_weights(Network& net, int F, const float* kernel, const float* r
     w->wide_ok = !w->small_path && H <= WG_MAX_H && F <= WG_MAX_F;
     int rc = upload_tiled(*w, H, F, kernel, recurrent, bias, dense_w);
     if (rc == PB_OK && w->wide_ok) rc = upload_wide(*w, H, F, kernel, recurrent, bias);
-    if (rc == PB_OK && bank_fused(net, F)) rc = upload_frag16(*w, H, F, kernel, recurrent, bias, dense_w);
+    if (rc == PB_OK && bank_fused(net, F)) {
+        Frag16 fr;
+        build_frag16(fr, H, F, kernel, recurrent, bias, dense_w);
+        rc = upload_frag16(*w, fr);
+    }
     if (rc != PB_OK) return rc;
     if (w->wide_ok) {
         CK(ensure_dyn_smem(gru_wide_kernel<true>, wg_smem(w->wg_fp, w->wg_hp)));
@@ -1310,10 +1348,9 @@ PB_API int pb_update(pb_handle* h, const int16_t* d_pcm, const int32_t* d_ids, i
 
 // ------------------------------------------------------------------------------------------------
 // model bank
-PB_API int pb_add_model(pb_handle* h, const pb_config* cfg, const float* kernel, const float* recurrent, const float* bias,
-                        const float* dense_w, float dense_b, const double* cd, int64_t cd_len, int32_t* slot) {
-    if (!h || !cfg || !kernel || !recurrent || !bias || !dense_w) return fail(PB_ERR_INVALID, "null argument");
-    const pb_config& c = *cfg;
+
+// A model's cfg (pb_add_model, pb_pool_load): its front-end fields must equal the handle's.
+static int check_front_end(const pb_handle* h, const pb_config& c) {
     if (c.abi_version != PB_ABI_VERSION) return fail(PB_ERR_INVALID, "abi_version %d != %d", c.abi_version, PB_ABI_VERSION);
 #define PB_SAME_FRONT_END(f)                                                                                  \
     if (c.f != h->cfg.f)                                                                                      \
@@ -1323,8 +1360,17 @@ PB_API int pb_add_model(pb_handle* h, const pb_config* cfg, const float* kernel,
     PB_SAME_FRONT_END(n_filt); PB_SAME_FRONT_END(n_mfcc); PB_SAME_FRONT_END(n_features); PB_SAME_FRONT_END(use_delta);
     PB_SAME_FRONT_END(vectorizer); PB_SAME_FRONT_END(chunk_samples); PB_SAME_FRONT_END(device);
 #undef PB_SAME_FRONT_END
+    return PB_OK;
+}
+
+PB_API int pb_add_model(pb_handle* h, const pb_config* cfg, const float* kernel, const float* recurrent, const float* bias,
+                        const float* dense_w, float dense_b, const double* cd, int64_t cd_len, int32_t* slot) {
+    if (!h || !cfg || !kernel || !recurrent || !bias || !dense_w) return fail(PB_ERR_INVALID, "null argument");
+    const pb_config& c = *cfg;
+    int rc = check_front_end(h, c);
+    if (rc != PB_OK) return rc;
     if (h->models.size() >= PB_MAX_MODELS) return fail(PB_ERR_INVALID, "a bank holds at most %d models", PB_MAX_MODELS);
-    int rc = check_network(c);
+    rc = check_network(c);
     if (rc != PB_OK) return rc;
     CK(cudaSetDevice(c.device));
     // built aside and appended only when complete: a failure leaves the bank as it was
@@ -1768,6 +1814,10 @@ PB_API int pb_clear(pb_handle* h, const int32_t* d_ids, int64_t n, void* stream)
     for (size_t m = 0; m < h->models.size(); ++m) t.trig[m] = h->models[m].trig.get();
     clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->d_n_samples.get(), t, d_ids, n);
     CK(cudaGetLastError());
+    if (h->pool) {
+        pool_clear_kernel<<<(int)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(h->d_pool_trig.get(), d_ids, n);
+        CK(cudaGetLastError());
+    }
     return restart_history(h, d_ids, n, (cudaStream_t)stream);
 }
 
@@ -1983,6 +2033,11 @@ PB_API int pb_export_streams(pb_handle* h, const int32_t* d_ids, int64_t n, void
     export_state_kernel<<<(unsigned)((n + per - 1) / per), STATE_THREADS, 0, (cudaStream_t)stream>>>(
         state_layout(h), stream_state(h), d_ids, n, static_cast<uint4*>(d_out));
     CK(cudaGetLastError());
+    if (h->pool) {                                   // a handle without a pool leaves pool_activation 0
+        pool_state_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+            h->d_pool_trig.get(), d_ids, n, static_cast<int*>(d_out), state_layout(h).rec_vecs * 4);
+        CK(cudaGetLastError());
+    }
     return PB_OK;
 }
 
@@ -2028,6 +2083,11 @@ PB_API int pb_import_streams(pb_handle* h, const int32_t* h_ids, int64_t n, cons
     const int per = STATE_THREADS / 32;
     import_state_kernel<<<(unsigned)((n + per - 1) / per), STATE_THREADS>>>(L, stream_state(h), d_sids.get(), n, in);
     CK(cudaGetLastError());
+    if (h->pool) {                                   // the record's pool_activation; a handle without a pool ignores it
+        pool_state_kernel<false><<<(unsigned)((n + 255) / 256), 256>>>(h->d_pool_trig.get(), d_sids.get(), n,
+                                                                     static_cast<int*>(const_cast<void*>(d_in)), L.rec_vecs * 4);
+        CK(cudaGetLastError());
+    }
     rc = restart_history(h, d_sids.get(), n, 0);                   // history restarts at the record's n_samples
     if (rc != PB_OK) return rc;
     CK(cudaDeviceSynchronize());
@@ -2150,6 +2210,295 @@ PB_API int pb_read_history(pb_handle* h, const int32_t* d_ids, int64_t n, int64_
                                                               (int)samples, d_out);
     CK(cudaGetLastError());
     return PB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// model pool (pool.cuh)
+
+// Frees the pool, if any.  The device is the handle's and idle.
+static void drop_pool(pb_handle* h) {
+    h->pool = false;
+    h->pool_models = 0;
+    h->d_pool_slots = DevArray<uint4>();
+    h->d_pool_count = DevArray<unsigned>();
+    h->d_pool_list0 = DevArray<unsigned>();
+    h->d_pool_id = DevArray<int>();
+    h->d_pool_trig = DevArray<int>();
+    h->d_pool_list = DevArray<int2>();
+    for (int sh = 0; sh < 2; ++sh)
+        for (int ka = 0; ka < 2; ++ka) { h->d_pool_tiles[sh][ka] = DevArray<int2>(); h->pool_tiles[sh][ka] = 0; }
+    h->pool_id = std::vector<int>();
+    h->pool_subs = std::vector<int64_t>();
+    h->pool_keras = std::vector<uint8_t>();
+    h->pool_cd_of.clear();
+    h->pool_cd.clear();
+    h->pool_cd_of.shrink_to_fit();
+}
+
+PB_API int pb_set_pool(pb_handle* h, int32_t max_models) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (max_models < 0 || max_models > (1 << 24)) return fail(PB_ERR_INVALID, "max_models = %d outside [1, 2^24] (0 frees the pool)", max_models);
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued ticks finish with the old pool
+    drop_pool(h);                                    // the old pool goes first, so a failed allocation leaves none
+    if (max_models == 0) return PB_OK;
+    const size_t S = (size_t)h->cfg.max_streams, M = (size_t)max_models;
+    DevArray<uint4> slots;
+    DevArray<unsigned> count, list0;
+    DevArray<int> id, trig;
+    DevArray<int2> list;
+    CK(slots.alloc(M * POOL_SLOT_U4));
+    CK(count.alloc(M));
+    CK(list0.alloc(M + 1));
+    CK(id.alloc(S));
+    CK(trig.alloc(S));
+    CK(list.alloc(S));
+    CK(cudaMemset(list0.get(), 0, (M + 1) * sizeof(unsigned)));
+    CK(cudaMemset(id.get(), 0xFF, S * sizeof(int)));
+    CK(cudaMemset(trig.get(), 0, S * sizeof(int)));
+    CK(ensure_dyn_smem(pool_warp_kernel<true>, (size_t)(MMA_THREADS / 32) * BANK_MODEL_SMEM));
+    CK(ensure_dyn_smem(pool_warp_kernel<false>, (size_t)(MMA_THREADS / 32) * BANK_MODEL_SMEM));
+    // 4 CTAs of 56 832 B per SM need the largest shared-memory carveout
+    CK(cudaFuncSetAttribute(pool_warp_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    CK(cudaFuncSetAttribute(pool_warp_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    if (!h->pool_ev) CK(cudaEventCreateWithFlags(&h->pool_ev, cudaEventDisableTiming));
+    h->d_pool_slots = std::move(slots);
+    h->d_pool_count = std::move(count);
+    h->d_pool_list0 = std::move(list0);
+    h->d_pool_id = std::move(id);
+    h->d_pool_trig = std::move(trig);
+    h->d_pool_list = std::move(list);
+    h->pool_id.assign(S, -1);
+    h->pool_subs.assign(M, 0);
+    h->pool_keras.assign(M, 0);
+    h->pool_cd_of.assign(M, h->pool_cd.end());
+    h->pool_models = max_models;
+    h->pool = true;
+    return PB_OK;
+}
+
+// list0 and the four tile tables from the host's per-model stream counts: model m's list positions [0, subs[m]) as block
+// tiles of 64, the rest as warp tiles of 16.  Synchronous; the device is idle.
+static int pool_rebuild(pb_handle* h) {
+    const int M = h->pool_models;
+    std::vector<unsigned> list0((size_t)M + 1);
+    std::vector<int2> tiles[2][2];
+    unsigned at = 0;
+    for (int m = 0; m < M; ++m) {
+        list0[m] = at;
+        const int64_t s = h->pool_subs[m];
+        at += (unsigned)s;
+        const int ka = h->pool_keras[m];
+        const int64_t nb = h->pool_warp_only ? 0 : s / 64;
+        for (int64_t p = 0; p < nb * 64; p += 64) tiles[0][ka].push_back(make_int2(m, (int)p));
+        for (int64_t p = nb * 64; p < s; p += 16) tiles[1][ka].push_back(make_int2(m, (int)p));
+    }
+    list0[M] = at;
+    CK(cudaMemcpy(h->d_pool_list0.get(), list0.data(), list0.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
+    for (int sh = 0; sh < 2; ++sh)
+        for (int ka = 0; ka < 2; ++ka) {
+            CK(h->d_pool_tiles[sh][ka].upload(tiles[sh][ka]));
+            h->pool_tiles[sh][ka] = (int64_t)tiles[sh][ka].size();
+        }
+    return PB_OK;
+}
+
+PB_API int pb_pool_load(pb_handle* h, int32_t model_id, const pb_config* cfg, const float* kernel, const float* recurrent,
+                        const float* bias, const float* dense_w, float dense_b, const double* cd, int64_t cd_len) {
+    if (!h || !cfg || !kernel || !recurrent || !bias || !dense_w) return fail(PB_ERR_INVALID, "null argument");
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    if (model_id < 0 || model_id >= h->pool_models) return fail(PB_ERR_INVALID, "model_id %d outside [0, max_models = %d)", model_id, h->pool_models);
+    const pb_config& c = *cfg;
+    int rc = check_front_end(h, c);
+    if (rc != PB_OK) return rc;
+    rc = check_network(c);
+    if (rc != PB_OK) return rc;
+    Network net;                                     // the network's fields, decoder table and range
+    net.cfg = c;
+    net.cfg.max_streams = h->cfg.max_streams;
+    if (!bank_fused(net, h->feat))
+        return fail(PB_ERR_UNSUPPORTED, "the model pool holds networks of the fused family (hidden <= %d, feature size <= %d, no deltas); "
+                    "this one has hidden = %d, feature size = %d", BANK_MAX_H, BANK_MAX_F, c.hidden, h->feat);
+    build_cdf(net);
+    if (cd && cd_len != (int64_t)net.cd.size()) return fail(PB_ERR_INVALID, "cdf length %lld != %zu", (long long)cd_len, net.cd.size());
+    if (cd) memcpy(net.cd.data(), cd, cd_len * sizeof(double));
+    Frag16 fr;
+    build_frag16(fr, c.hidden, h->feat, kernel, recurrent, bias, dense_w);
+    std::vector<uint4> slot;
+    slot.reserve(POOL_SLOT_U4);
+    slot.insert(slot.end(), fr.bf16.begin(), fr.bf16.end());
+    slot.insert(slot.end(), fr.xf16.begin(), fr.xf16.end());
+    std::vector<float> tail(fr.mb);
+    tail.insert(tail.end(), fr.mw.begin(), fr.mw.end());
+    const size_t tail_u4 = tail.size() * sizeof(float) / 16;
+    slot.resize(slot.size() + tail_u4);
+    memcpy(slot.data() + slot.size() - tail_u4, tail.data(), tail.size() * sizeof(float));
+    if (slot.size() != (size_t)POOL_FRAG_U4) return fail(PB_ERR_INVALID, "pool slot layout");
+    slot.resize(POOL_SLOT_U4, uint4{});             // the record goes behind the weights
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued ticks finish with the old model
+    // the decoder table: an existing one with these bytes, else a new one (a failure here changes nothing)
+    std::string key(reinterpret_cast<const char*>(net.cd.data()), net.cd.size() * sizeof(double));
+    auto it = h->pool_cd.find(key);
+    if (it == h->pool_cd.end()) {
+        pb_handle::PoolCd fresh;
+        CK(fresh.d.upload(net.cd));
+        it = h->pool_cd.emplace(std::move(key), std::move(fresh)).first;
+    }
+    ++it->second.refs;
+    uint4* frag = h->d_pool_slots.get() + (size_t)model_id * POOL_SLOT_U4;
+    PoolModel rec{};
+    rec.w.bfrag = frag;
+    rec.w.xfrag = frag + 2 * MMA_NT * 32;
+    rec.w.bias = reinterpret_cast<const float*>(frag + BANK_FRAG_U4);
+    rec.w.wd = rec.w.bias + 72;
+    rec.w.bd = dense_b;
+    rec.w.act = c.activation;
+    rec.w.ract = c.recurrent_activation;
+    rec.dp = decode_params(net);
+    rec.dp.cd = it->second.d.get();
+    memcpy(slot.data() + POOL_FRAG_U4, &rec, sizeof(rec));
+    const cudaError_t e = cudaMemcpy(frag, slot.data(), slot.size() * sizeof(uint4), cudaMemcpyHostToDevice);   // weights and record at once
+    if (e != cudaSuccess) {
+        if (--it->second.refs == 0) h->pool_cd.erase(it);
+        return fail(PB_ERR_CUDA, "pool slot upload failed: %s", cudaGetErrorString(e));
+    }
+    auto& old = h->pool_cd_of[model_id];
+    if (old != h->pool_cd.end() && --old->second.refs == 0) h->pool_cd.erase(old);
+    old = it;
+    const uint8_t keras = keras_act(net);
+    const bool moved = keras != h->pool_keras[model_id];
+    h->pool_keras[model_id] = keras;
+    if (h->pool_subs[model_id] > 0) {                // a new runner for the streams on the slot: fresh detectors
+        const long long S = h->cfg.max_streams;
+        pool_rearm_model_kernel<<<(unsigned)((S + 255) / 256), 256>>>(h->d_pool_id.get(), h->d_pool_trig.get(), S, model_id);
+        CK(cudaGetLastError());
+        if (moved) {                                 // its tiles change activation class
+            rc = pool_rebuild(h);
+            if (rc != PB_OK) return rc;
+        }
+        CK(cudaDeviceSynchronize());
+    }
+    return PB_OK;
+}
+
+PB_API int pb_set_stream_pool(pb_handle* h, const int32_t* h_ids, const int32_t* h_models, int64_t n) {
+    int rc = check_route_ids(h, h_ids, n, true);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && !h_models) return fail(PB_ERR_INVALID, "null model ids");
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    for (int64_t i = 0; i < n; ++i) {
+        const int32_t m = h_models[i];
+        if (m < -1 || m >= h->pool_models)
+            return fail(PB_ERR_INVALID, "model id %d (entry %lld) outside [-1, max_models = %d); nothing changed", m, (long long)i, h->pool_models);
+        if (m >= 0 && h->pool_cd_of[m] == h->pool_cd.end())
+            return fail(PB_ERR_INVALID, "pool slot %d (entry %lld) holds no model: pb_pool_load it first; nothing changed", m, (long long)i);
+    }
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued ticks finish under the old assignments
+    std::vector<int> sids, models;
+    for (int64_t i = 0; i < n; ++i) {
+        const int sid = h_ids ? h_ids[i] : (int)i;
+        if (h->pool_id[sid] == h_models[i]) continue;    // unchanged: the detector keeps its state
+        sids.push_back(sid);
+        models.push_back(h_models[i]);
+    }
+    if (sids.empty()) return PB_OK;
+    DevArray<int> d_sids, d_models;
+    CK(d_sids.upload(sids));
+    CK(d_models.upload(models));
+    const long long k = (long long)sids.size();
+    pool_set_kernel<<<(unsigned)((k + 255) / 256), 256>>>(h->d_pool_id.get(), h->d_pool_trig.get(), d_sids.get(), d_models.get(), k);
+    CK(cudaGetLastError());
+    for (size_t j = 0; j < sids.size(); ++j) {
+        int& cur = h->pool_id[sids[j]];
+        if (cur >= 0) --h->pool_subs[cur];
+        if (models[j] >= 0) ++h->pool_subs[models[j]];
+        cur = models[j];
+    }
+    rc = pool_rebuild(h);
+    if (rc != PB_OK) return rc;
+    CK(cudaDeviceSynchronize());
+    return PB_OK;
+}
+
+PB_API int pb_get_stream_pool(const pb_handle* h, const int32_t* h_ids, int64_t n, int32_t* h_models) {
+    const int rc = check_route_ids(h, h_ids, n, false);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && !h_models) return fail(PB_ERR_INVALID, "null model ids");
+    for (int64_t i = 0; i < n; ++i) h_models[i] = h->pool ? h->pool_id[h_ids ? h_ids[i] : i] : -1;
+    return PB_OK;
+}
+
+PB_API int pb_debug_pool_tiles(pb_handle* h, int warp_only) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());
+    h->pool_warp_only = warp_only != 0;
+    const int rc = pool_rebuild(h);
+    if (rc != PB_OK) return rc;
+    CK(cudaDeviceSynchronize());
+    return PB_OK;
+}
+
+// The network half of a pool tick: the route, then the block and warp tiles of both activation classes.
+static int score_pool(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
+                      unsigned long long* d_count, cudaStream_t s) {
+    PoolTick t{};
+    t.pool_id = h->d_pool_id.get(); t.slots = h->d_pool_slots.get(); t.lists = h->d_pool_list.get();
+    t.count = h->d_pool_count.get(); t.list0 = h->d_pool_list0.get();
+    t.raw = d_raw; t.conf = d_conf; t.fired = d_fired; t.d_count = d_count; t.trig = h->d_pool_trig.get();
+    const K2In in = stream_k2in(h, d_ids);
+    ProfScope ps(h, 1, s);
+    // the lists and counts are the handle's: a pool tick on another stream may still be reading them
+    CK(cudaStreamWaitEvent(s, h->pool_ev, 0));
+    // the event is recorded after the tick's work even when a launch fails, so the next tick orders itself after it
+    auto launch = [&]() -> int {
+        CK(cudaMemsetAsync(t.count, 0, (size_t)h->pool_models * sizeof(unsigned), s));
+        pool_route_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_ids, n, t);
+        CK(cudaGetLastError());
+        constexpr int W = MMA_THREADS / 32;
+        for (int ka = 0; ka < 2; ++ka) {
+            const int64_t nb = h->pool_tiles[0][ka], nw = h->pool_tiles[1][ka];
+            const int2* tb = h->d_pool_tiles[0][ka].get();
+            const int2* tw = h->d_pool_tiles[1][ka].get();
+            if (nb && ka) pool_block_kernel<true><<<(unsigned)nb, MMA_THREADS, BANK_MODEL_SMEM + BANK_STAGE_SMEM, s>>>(tb, t, in);
+            else if (nb) pool_block_kernel<false><<<(unsigned)nb, MMA_THREADS, BANK_MODEL_SMEM + BANK_STAGE_SMEM, s>>>(tb, t, in);
+            CK(cudaGetLastError());
+            if (nw && ka) pool_warp_kernel<true><<<(unsigned)((nw + W - 1) / W), MMA_THREADS, W * BANK_MODEL_SMEM, s>>>(tw, nw, t, in);
+            else if (nw) pool_warp_kernel<false><<<(unsigned)((nw + W - 1) / W), MMA_THREADS, W * BANK_MODEL_SMEM, s>>>(tw, nw, t, in);
+            CK(cudaGetLastError());
+        }
+        return PB_OK;
+    };
+    const int rc = launch();
+    const cudaError_t er = cudaEventRecord(h->pool_ev, s);
+    if (rc != PB_OK) return rc;
+    if (er != cudaSuccess) return fail(PB_ERR_CUDA, "cudaEventRecord failed: %s", cudaGetErrorString(er));
+    return PB_OK;
+}
+
+PB_API int pb_update_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len, const int32_t* d_ids,
+                          int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_count, void* stream) {
+    int rc = check_tick(h, d_pcm, n);
+    if (rc != PB_OK) return rc;
+    if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
+    if (d_offsets && max_len < 1) return fail(PB_ERR_INVALID, "max_len = %lld must be >= 1", (long long)max_len);
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    if (d_offsets && h->k1_mode != 0) return fail(PB_ERR_STATE, "ragged ticks run only with k1 mode 0");
+    if (n == 0) return PB_OK;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (d_offsets) {                                 // pb_update_ragged's K1
+        h->ragged = true;
+        rc = append_history(h, d_pcm, d_offsets, max_len, d_ids, n, s);
+        if (rc == PB_OK) rc = launch_ragged_mfcc(h, d_pcm, d_offsets, max_len, d_ids, n, s);
+    } else {                                         // pb_update's
+        rc = tick_mfcc(h, d_pcm, d_ids, n, s);
+    }
+    if (rc != PB_OK) return rc;
+    return score_pool(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
 }
 
 // ------------------------------------------------------------------------------------------------

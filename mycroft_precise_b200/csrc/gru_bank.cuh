@@ -123,24 +123,31 @@ __device__ __forceinline__ void bank_stage(float* buf, const RingCursor& cur, bo
 // RING: rows from the stream ring (a tick), staged through shared memory up to NM = 2; otherwise from in.inputs,
 // [n][T][F_base] contiguous (pb_predict), loaded directly.  KERAS_ACT: every model uses Keras's GRU defaults (recurrent hard_sigmoid, activation
 // linear), compiled in; otherwise each model's pair is dispatched at run time.  Both compute the same expressions.
-template <int NM, bool RING, bool KERAS_ACT>
-__device__ __forceinline__ void bank_scan(const BankParams& P, int m0, const int2* list, long long tile, const K2In& in, long long n) {
+// PS: where P.w[k], P.dp[k] and P.o[k] come from (BankParams, or the model pool's per-model records, pool.cuh).
+// WARP: the scan of one warp instead (NM = 1, RING): its 16 entries tile * 16 .., its model loaded by its own lanes into its
+// own shared-memory slot (slot = warp), ring rows loaded directly.  The arithmetic is the same in every form.
+template <int NM, bool RING, bool KERAS_ACT, class PS = BankParams, bool WARP = false>
+__device__ __forceinline__ void bank_scan(const PS& P, int m0, const int2* list, long long tile, const K2In& in, long long n) {
     extern __shared__ __align__(16) unsigned char bank_smem[];
+    static_assert(!WARP || (NM == 1 && RING), "a warp scans one model over the stream ring");
+    const int ws = WARP ? (int)(threadIdx.x >> 5) : 0;                 // first shared-memory model slot of this scan
+    const int l0 = WARP ? (int)(threadIdx.x & 31) : (int)threadIdx.x, ls = WARP ? 32 : (int)blockDim.x;
 #pragma unroll 1
     for (int m = 0; m < NM; ++m) {
         const BankModelW& w = P.w[m0 + m];
-        uint4* sf = reinterpret_cast<uint4*>(bank_smem + m * BANK_MODEL_SMEM);
+        uint4* sf = reinterpret_cast<uint4*>(bank_smem + (ws + m) * BANK_MODEL_SMEM);
         float* sb = reinterpret_cast<float*>(sf + BANK_FRAG_U4);
-        for (int e = threadIdx.x; e < 2 * MMA_NT * 32; e += blockDim.x) sf[e] = __ldg(w.bfrag + e);
-        for (int e = threadIdx.x; e < MMA_NT * 32; e += blockDim.x) sf[2 * MMA_NT * 32 + e] = __ldg(w.xfrag + e);
-        for (int e = threadIdx.x; e < 72; e += blockDim.x) sb[e] = __ldg(w.bias + e);
-        for (int e = threadIdx.x; e < 24; e += blockDim.x) sb[72 + e] = __ldg(w.wd + e);
+        for (int e = l0; e < 2 * MMA_NT * 32; e += ls) sf[e] = __ldg(w.bfrag + e);
+        for (int e = l0; e < MMA_NT * 32; e += ls) sf[2 * MMA_NT * 32 + e] = __ldg(w.xfrag + e);
+        for (int e = l0; e < 72; e += ls) sb[e] = __ldg(w.bias + e);
+        for (int e = l0; e < 24; e += ls) sb[72 + e] = __ldg(w.wd + e);
     }
-    __syncthreads();
+    if (WARP) __syncwarp();
+    else __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
-    const long long base = (tile * (MMA_THREADS / 32) + warp) * 16;
+    const long long base = WARP ? tile * 16 : (tile * (MMA_THREADS / 32) + warp) * 16;
     if (base >= n) return;
-    constexpr bool STAGE = bank_stages(NM, RING);
+    constexpr bool STAGE = bank_stages(NM, RING) && !WARP;
     const int F = in.F_base;
     long long idx[2];
     int sid[2];
@@ -237,7 +244,7 @@ __device__ __forceinline__ void bank_scan(const BankParams& P, int m0, const int
         split_f16(xv[1][2], xv[1][3], xh[3], xl[3]);
 #pragma unroll
         for (int m = 0; m < NM; ++m) {
-            const uint4* sB = reinterpret_cast<const uint4*>(bank_smem + m * BANK_MODEL_SMEM);
+            const uint4* sB = reinterpret_cast<const uint4*>(bank_smem + (ws + m) * BANK_MODEL_SMEM);
             const uint4* sX = sB + 2 * MMA_NT * 32;
             const float* sBias = reinterpret_cast<const float*>(sB + BANK_FRAG_U4);
             const int ra = P.w[m0 + m].ract, ac = P.w[m0 + m].act;
@@ -296,7 +303,7 @@ __device__ __forceinline__ void bank_scan(const BankParams& P, int m0, const int
     // ---- per model: Dense(1) (per-thread partial over its 6 units per row, reduced over the quad) and the epilogue
 #pragma unroll
     for (int m = 0; m < NM; ++m) {
-        const float* sWd = reinterpret_cast<const float*>(bank_smem + m * BANK_MODEL_SMEM + BANK_FRAG_U4 * 16) + 72;
+        const float* sWd = reinterpret_cast<const float*>(bank_smem + (ws + m) * BANK_MODEL_SMEM + BANK_FRAG_U4 * 16) + 72;
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
             float part = 0.f;
