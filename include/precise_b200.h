@@ -354,15 +354,16 @@ int pb_read_history(pb_handle* h, const int32_t* d_stream_ids, int64_t n, int64_
 /* Model pool: a second, large set of networks on a handle, beside the bank, for a server whose devices each bring their own
  * wake word (custom models trained with precise-train, each used by one or a few devices).  Each stream points at at most one
  * pool model, or at none.  A pool tick runs K1 once, as every tick does, then scores every item whose stream has a pool model
- * with that model's network, ThresholdDecoder and TriggerDetector (the model's sensitivity and trigger_level; the refractory
- * count from the handle's chunk_samples).  One window scan per item, whatever the number of models: the scan of a model
+ * with that model's network, ThresholdDecoder and TriggerDetector (the model's sensitivity and trigger_level, and the
+ * refractory count from the handle's chunk_samples, unless pb_set_stream_pool_trigger gives the stream its own).  One window scan per item, whatever the number of models: the scan of a model
  * costs one 14 208 B weight load per tile of 64 (or of at most 16) of its streams.
  *   - Networks: the fused family only (hidden <= 24, feature size <= 16, no deltas), which every network precise-train builds
  *     at its defaults is in.  A pool stream's raw and conf are bit-identical to the same network's in a bank.
  *   - Memory: about 14.3 KB per slot, 51 200 B per distinct decoder table at the default thresholds (models whose tables
  *     are bit-identical share one copy), 16 B per stream.
  *   - The bank, its masks and trigger settings are independent of the pool; pb_update_models does not score pool models and
- *     pb_update_pool scores no bank model.  Not covered: pb_update_host, pb_score_corpus, per-stream trigger settings.
+ *     pb_update_pool scores no bank model.  pb_update_all scores both on one K1.  Not covered: pb_update_host,
+ *     pb_score_corpus, networks outside the fused family.
  *   - A handle that never calls pb_set_pool runs exactly as before.
  *
  * pb_set_pool: a pool of max_models slots (max_models in [1, 2^24]), every slot empty and every stream on none.  Synchronous.
@@ -399,6 +400,43 @@ int pb_get_stream_pool(const pb_handle* h, const int32_t* h_stream_ids, int64_t 
 int pb_update_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len,
                    const int32_t* d_stream_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
                    unsigned long long* d_count, void* stream);
+/* Combined tick: the bank and the pool on one chunk, for a stream that listens for shared bank words and for its own pool
+ * word.  d_offsets NULL: pb_update_models's uniform tick (d_pcm [n][chunk_samples], max_len ignored); otherwise
+ * pb_update_ragged's (and the handle becomes ragged).  The tick appends history once and runs K1 once, then the bank's network
+ * half exactly as pb_update_models / pb_update_ragged choose it (one model on a ragged tick: pb_update's path), then the pool's,
+ * all on `stream`.  Outputs are [(M + 1)][n] for M = pb_num_models: rows 0 .. M-1 are bit-identical to what
+ * pb_update_models / pb_update_ragged writes on a handle with the same bank, streams and audio (masks, NaN fill and per-stream
+ * trigger settings included); row M to what pb_update_pool writes on a handle with the same pool (NaN / NaN / 0 for a stream
+ * with no pool model).  d_raw and d_fired are optional.  d_counts [M] (optional) += each bank model's fires, d_pool_count [1]
+ * (optional) += the pool's.  Ordering across CUDA streams as for the two ticks it combines.  Every argument is checked before
+ * anything is enqueued, so a refused call changes no state.  PB_ERR_INVALID: as pb_update_ragged / pb_update_pool.
+ * PB_ERR_STATE: no pool, slot 0 without weights, offsets with a non-zero pb_debug_k1_mode. */
+int pb_update_all(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len, const int32_t* d_stream_ids,
+                  int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_counts,
+                  unsigned long long* d_pool_count, void* stream);
+/* Per-stream TriggerDetector settings of the streams' pool models, as pb_set_stream_trigger sets them for a bank slot: stream
+ * h_stream_ids[i] (HOST; NULL => 0..n-1) is scored by TriggerDetector(h_chunk_bytes[i], h_sensitivity[i],
+ * h_trigger_level[i]), whichever pool model it is on.  The settings belong to the stream, not to a model.
+ *   - Refractory count -(8*2048) // chunk_bytes (Python floor division).  chunk_bytes == 0 returns the stream to its model's
+ *     own values (cfg.sensitivity, cfg.trigger_level, and the refractory count from the handle's chunk_samples), the state of
+ *     a stream never set.  pb_get_stream_pool_trigger returns (NaN, 0, 0) for such a stream, otherwise exactly what was set
+ *     (the sensitivity bit for bit); (NaN, 0, 0) for every stream without a pool.
+ *   - A stream whose entry changes gets a fresh pool detector; an unchanged entry keeps it.  Settings survive
+ *     pb_set_stream_pool (a changed model still re-arms), pb_pool_load and pb_clear; pb_set_pool (replace or free) drops them.
+ *     pb_update_pool and pb_update_all honour them.
+ *   - Validates everything before it changes anything, then synchronises the device.  PB_ERR_INVALID: null handle, n outside
+ *     [0, max_streams], an id outside [0, max_streams), a duplicate id, a null array with n > 0, chunk_bytes < 0.
+ *     PB_ERR_STATE: no pool.
+ *   - Cost: the first call allocates a [max_streams] 16 B record array and a host mirror and flags the pool until it is
+ *     replaced: its ticks then scan without the trigger and run one pool_trigger_kernel afterwards.  A pool never set runs as
+ *     before. */
+int pb_set_stream_pool_trigger(pb_handle* h, const int32_t* h_stream_ids, const double* h_sensitivity,
+                               const int32_t* h_trigger_level, const int32_t* h_chunk_bytes, int64_t n);
+/* The pool trigger settings of the given streams (h_stream_ids NULL => 0..n-1) into h_sensitivity / h_trigger_level /
+ * h_chunk_bytes [n] (HOST).  PB_ERR_INVALID: null handle or output with n > 0, n outside [0, max_streams], an id outside
+ * [0, max_streams). */
+int pb_get_stream_pool_trigger(const pb_handle* h, const int32_t* h_stream_ids, int64_t n, double* h_sensitivity,
+                               int32_t* h_trigger_level, int32_t* h_chunk_bytes);
 
 /* Recorded corpora: whole recordings scored on the device in one call, the hot path of precise-simulate
  * (precise/scripts/simulate.py:92-129) and of false-activation mining (precise/scripts/train_incremental.py:113-137).

@@ -73,6 +73,22 @@ class StreamBatch:
         PreciseB200.update_pool."""
         return self.core.update_pool(pcm, ids, offsets, max_len, count=self.pool_count)
 
+    def update_all(self, pcm, ids=None, offsets=None, max_len=None):
+        """One combined tick, the bank and the pool on one K1 (uniform with pcm [n, chunk_samples], ragged with 1-D pcm and
+        ``offsets``) -> dict(raw, conf, fired), each [M + 1, n]: rows 0 .. M-1 as update_models / update_ragged, row M as
+        update_pool.  Accumulates ``self.counts`` and ``self.pool_count``.  See PreciseB200.update_all."""
+        return self.core.update_all(pcm, ids, offsets, max_len, counts=self.counts, pool_count=self.pool_count)
+
+    def set_stream_pool_trigger(self, sensitivity, trigger_level, chunk_size, ids=None):
+        """Each stream's TriggerDetector(chunk_size in bytes, sensitivity, trigger_level) on its pool model; chunk_size 0 =
+        the model's own settings; scalars broadcast.  See PreciseB200.set_stream_pool_trigger."""
+        self.core.set_stream_pool_trigger(sensitivity, trigger_level, chunk_size, ids)
+
+    def stream_pool_trigger(self, ids=None):
+        """(sensitivity, trigger_level, chunk_size) host arrays of the streams' pool settings; (NaN, 0, 0) = the model's own.
+        See PreciseB200.stream_pool_trigger."""
+        return self.core.stream_pool_trigger(ids)
+
     def set_history(self, samples=None, max_rows=None):
         """A device pool for the recent audio of up to ``max_rows`` streams, ``samples`` each (default buffer_samples, the
         reference's clip).  See PreciseB200.set_history."""
@@ -94,7 +110,8 @@ class StreamBatch:
         """The clip behind every activation of the tick just run, as listen.py saves it in on_activation: ``fired`` and ``ids``
         are that tick's output ([n] or [M, n]) and ids (int32 CUDA tensor; None: items are streams 0..n-1).  Returns dict(slot =
         bank slot, stream = stream id, audio = int16 [k, samples] ending with that tick's chunk) for every fired (model, item)
-        pair whose stream has history, in torch.nonzero order (model-major).  Call it before the next tick on those streams."""
+        pair whose stream has history, in torch.nonzero order (model-major).  On update_all's [M + 1, n] output, slot == M
+        means the stream's pool model.  Call it before the next tick on those streams."""
         core = self.core
         torch = core.torch
         f = fired if fired.dim() == 2 else fired.reshape(1, -1)
@@ -104,13 +121,17 @@ class StreamBatch:
         core._check_t('ids', ids, torch.int32, n, optional=False)
         pairs = torch.nonzero(f)
         streams = ids[pairs[:, 1]]
-        keep = torch.from_numpy(core.stream_history(streams.cpu().numpy().astype(np.int32))).to(core.device)
+        # a stream that fired on several rows appears once per row: look it up and read its clip once
+        uniq, inv = torch.unique(streams, return_inverse=True)
+        has = torch.from_numpy(core.stream_history(uniq.cpu().numpy().astype(np.int32))).to(core.device)
+        keep = has[inv]
         pairs, streams = pairs[keep], streams[keep].contiguous()
         if streams.numel() == 0:
             s = core.history_samples if samples is None else int(samples)
             audio = torch.empty((0, s), dtype=torch.int16, device=core.device)
         else:
-            audio = core.read_history(streams, samples)
+            uniq, inv = torch.unique(streams, return_inverse=True)
+            audio = core.read_history(uniq.contiguous(), samples)[inv]
         return dict(slot=pairs[:, 0], stream=streams, audio=audio)
 
     def _host_ids(self, ids, n):
@@ -124,7 +145,8 @@ class StreamBatch:
     def export_streams(self, ids=None):
         """A snapshot of streams ids (host int32 array; None: every stream): dict(state = their state records, a uint8 CUDA
         tensor [n, stream_state_bytes]; stream_models = their masks; stream_trigger = each bank slot's (sensitivity,
-        trigger_level, chunk_size); with a model pool, stream_pool = their pool models).  The tensor may go through .cpu() or
+        trigger_level, chunk_size); with a model pool, stream_pool = their pool models and stream_pool_trigger = their pool
+        (sensitivity, trigger_level, chunk_size)).  The tensor may go through .cpu() or
         .to(another device) and come back.  Whether a stream has audio history, and that audio, are not part of a snapshot.
         See PreciseB200.export_streams."""
         core = self.core
@@ -135,14 +157,16 @@ class StreamBatch:
                     stream_trigger=[core.stream_trigger(m, sids) for m in range(core.num_models)])
         if core.pool_models:
             snap['stream_pool'] = core.stream_pool(sids)
+            snap['stream_pool_trigger'] = core.stream_pool_trigger(sids)
         return snap
 
     def import_streams(self, snapshot, ids=None):
         """Continue the snapshot's streams (export_streams of a batch with the same front end and bank) as streams ids (host
-        int32 array; None: 0..n-1) of this batch.  Their masks, then each slot's trigger settings, then their pool models are
-        set where they differ from this batch's, so a batch never becomes routed or trigger-flagged for nothing; then the state
-        is imported, which overwrites the activations those steps may have re-armed.  A snapshot that does not match (pool
-        models this batch does not hold included) raises ValueError before anything changes.  History on / off is not
+        int32 array; None: 0..n-1) of this batch.  Their masks, then each slot's trigger settings, then their pool models,
+        then their pool trigger settings are set where they differ from this batch's, so a batch never becomes routed or
+        trigger-flagged for nothing; then the state is imported, which overwrites the activations those steps may have
+        re-armed.  A snapshot that does not match (pool models this batch does not hold, or pool trigger settings it cannot
+        take, included) raises ValueError before anything changes.  History on / off is not
         carried: the streams keep this batch's setting, and one that has history starts empty at the imported sample count."""
         core = self.core
         torch = core.torch
@@ -166,6 +190,24 @@ class StreamBatch:
             if on.size and (on.min() < 0 or on.max() >= core.pool_models or not core.pool_loaded[on].all()):
                 raise ValueError('snapshot names pool models this batch does not hold (pool of %d slots); nothing was changed'
                                  % core.pool_models)
+        ptrig = None
+        if 'stream_pool_trigger' in snapshot:    # pool trigger settings this batch can take, before anything changes
+            ptrig = snapshot['stream_pool_trigger']
+            if not isinstance(ptrig, (tuple, list)) or len(ptrig) != 3:
+                raise ValueError('stream_pool_trigger must be (sensitivity, trigger_level, chunk_size); nothing was changed')
+            ptrig = [np.asarray(v) for v in ptrig]
+            for name, v, kinds in zip(('sensitivity', 'trigger_level', 'chunk_size'), ptrig, ('biuf', 'iu', 'iu')):
+                if v.shape != (n,) or v.dtype.kind not in kinds:
+                    raise ValueError('stream_pool_trigger %s must be a [%d] array of %s, got %s %s; nothing was changed'
+                                     % (name, n, 'real numbers' if kinds == 'biuf' else 'integers', v.dtype, v.shape))
+                if kinds == 'iu' and v.size and (int(v.min()) < -2 ** 31 or int(v.max()) >= 2 ** 31):
+                    raise ValueError('stream_pool_trigger %s must fit in int32; nothing was changed' % name)
+            ptrig = [np.ascontiguousarray(ptrig[0], np.float64), np.ascontiguousarray(ptrig[1], np.int32),
+                     np.ascontiguousarray(ptrig[2], np.int32)]
+            if n and int(ptrig[2].min()) < 0:
+                raise ValueError('stream_pool_trigger chunk_size must be >= 0; nothing was changed')
+            if not core.pool_models and ptrig[2].any():
+                raise ValueError('snapshot sets pool trigger settings and this batch has no model pool; nothing was changed')
         if n and bool(bad.any()):
             i = int(bad.nonzero()[0, 0])
             got, want = state[i, :48].cpu().numpy().view(np.int32), ref.cpu().numpy().view(np.int32)
@@ -185,6 +227,13 @@ class StreamBatch:
             differ = core.stream_pool(sids) != pool
             if differ.any():
                 core.set_stream_pool(pool[differ], sids[differ])
+        if ptrig is not None and core.pool_models:
+            sens, lvl, chunk = ptrig
+            cs, cl, cc = core.stream_pool_trigger(sids)
+            # (NaN, 0, 0) entries follow the model: they differ only from a stream that has its own settings
+            differ = (cc != chunk) | ((chunk != 0) & ((cs.view(np.uint64) != sens.view(np.uint64)) | (cl != lvl)))
+            if differ.any():
+                core.set_stream_pool_trigger(sens[differ], lvl[differ], chunk[differ], ids=sids[differ])
         core.import_streams(state, sids)
 
     def _bank_buffers(self, n):

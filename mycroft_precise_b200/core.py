@@ -78,6 +78,9 @@ SYMBOLS = {
     'pb_set_stream_pool': (C.c_int, [_VP, _VP, _VP, _I64]),
     'pb_get_stream_pool': (C.c_int, [_VP, _VP, _I64, _VP]),
     'pb_update_pool': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _VP, _VP, _VP]),
+    'pb_update_all': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _VP, _VP, _VP, _VP]),
+    'pb_set_stream_pool_trigger': (C.c_int, [_VP, _VP, _VP, _VP, _VP, _I64]),
+    'pb_get_stream_pool_trigger': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP]),
     'pb_corpus_windows': (_I64, [C.POINTER(pb_config), _I32, _I64, _I64]),
     'pb_score_corpus': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
@@ -367,38 +370,80 @@ class PreciseB200:
         (update's tick); with them, a 1-D int16 CUDA pcm and int64 CUDA offsets [n + 1] (update_ragged's tick).  Returns
         dict(raw f32, conf f64, fired u8), each [n]; items whose stream has no pool model are NaN / NaN / 0.  ``count``
         (int64 [1]) accumulates the tick's pool fires."""
-        torch = self.torch
-        if offsets is None:
-            n = self._check_pcm(pcm)
-            max_len = 0
-        else:
-            if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
-                    or pcm.device != self.device):
-                raise ValueError('pcm must be a contiguous 1-D int16 tensor on %s' % self.device)
-            if (not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1
-                    or not offsets.is_contiguous() or offsets.device != self.device):
-                raise ValueError('offsets must be a contiguous 1-D int64 [n + 1] tensor on %s' % self.device)
-            n = offsets.numel() - 1
-            if n > self.max_streams:
-                raise ValueError('n = %d exceeds max_streams = %d' % (n, self.max_streams))
-            if max_len is None:
-                max_len = max(1, int((offsets[1:] - offsets[:-1]).max())) if n else 1
-            max_len = int(max_len)
-            if max_len < 1:
-                raise ValueError('max_len must be >= 1, got %d' % max_len)
+        n, max_len = self._tick_shape(pcm, offsets, max_len)
         self._check_ids(ids, n)
-        if out is not None:
-            self._check_t("out['raw']", out.get('raw'), torch.float32, n)
-            self._check_t("out['conf']", out.get('conf'), torch.float64, n, optional=False)
-            self._check_t("out['fired']", out.get('fired'), torch.uint8, n)
-        self._check_t('count', count, torch.int64, 1)
-        if out is None:
-            out = dict(raw=torch.empty(n, dtype=torch.float32, device=self.device),
-                       conf=torch.empty(n, dtype=torch.float64, device=self.device),
-                       fired=torch.empty(n, dtype=torch.uint8, device=self.device))
+        out = self._tick_out(out, 1, n, (n,))
+        self._check_t('count', count, self.torch.int64, 1)
         check(self.lib.pb_update_pool(self._h, _ptr(pcm), _ptr(offsets), max_len, _ptr(ids), n, _ptr(out.get('raw')),
                                       _ptr(out['conf']), _ptr(out.get('fired')), _ptr(count), self._stream()))
         return out
+
+    def update_all(self, pcm, ids=None, offsets=None, max_len=None, out=None, counts=None, pool_count=None):
+        """Combined tick: the bank and the pool on one chunk, with one history append and one K1.  pcm and ``offsets`` as
+        update_pool takes them (uniform without offsets, ragged with them).  Returns dict(raw f32, conf f64, fired u8), each
+        [M + 1, n]: rows 0 .. M-1 are update_models's (update_ragged's with offsets), row M is update_pool's.  ``counts``
+        (int64 [M]) accumulates each bank model's fires and ``pool_count`` (int64 [1]) the pool's."""
+        n, max_len = self._tick_shape(pcm, offsets, max_len)
+        self._check_ids(ids, n)
+        M = self.num_models
+        out = self._tick_out(out, M + 1, n, (M + 1, n))
+        self._check_t('counts', counts, self.torch.int64, M)
+        self._check_t('pool_count', pool_count, self.torch.int64, 1)
+        check(self.lib.pb_update_all(self._h, _ptr(pcm), _ptr(offsets), max_len, _ptr(ids), n, _ptr(out.get('raw')),
+                                     _ptr(out['conf']), _ptr(out.get('fired')), _ptr(counts), _ptr(pool_count),
+                                     self._stream()))
+        return out
+
+    def _tick_shape(self, pcm, offsets, max_len):
+        """(n, max_len) of a tick that is uniform without ``offsets`` and ragged with them, as update_pool takes it."""
+        torch = self.torch
+        if offsets is None:
+            return self._check_pcm(pcm), 0
+        if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
+                or pcm.device != self.device):
+            raise ValueError('pcm must be a contiguous 1-D int16 tensor on %s' % self.device)
+        if (not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1
+                or not offsets.is_contiguous() or offsets.device != self.device):
+            raise ValueError('offsets must be a contiguous 1-D int64 [n + 1] tensor on %s' % self.device)
+        n = offsets.numel() - 1
+        if n > self.max_streams:
+            raise ValueError('n = %d exceeds max_streams = %d' % (n, self.max_streams))
+        if max_len is None:
+            max_len = max(1, int((offsets[1:] - offsets[:-1]).max())) if n else 1
+        max_len = int(max_len)
+        if max_len < 1:
+            raise ValueError('max_len must be >= 1, got %d' % max_len)
+        return n, max_len
+
+    def _tick_out(self, out, rows, n, shape):
+        """``out`` checked for ``rows`` x n outputs, or new buffers of ``shape``."""
+        torch = self.torch
+        if out is not None:
+            self._check_t("out['raw']", out.get('raw'), torch.float32, rows * n)
+            self._check_t("out['conf']", out.get('conf'), torch.float64, rows * n, optional=False)
+            self._check_t("out['fired']", out.get('fired'), torch.uint8, rows * n)
+            return out
+        return dict(raw=torch.empty(shape, dtype=torch.float32, device=self.device),
+                    conf=torch.empty(shape, dtype=torch.float64, device=self.device),
+                    fired=torch.empty(shape, dtype=torch.uint8, device=self.device))
+
+    def set_stream_pool_trigger(self, sensitivity, trigger_level, chunk_size, ids=None):
+        """Stream ids[i] is scored by TriggerDetector(chunk_size[i], sensitivity[i], trigger_level[i]) on whichever pool model
+        it is on.  ``chunk_size`` is in BYTES; 0 returns the stream to its model's own settings.  Scalars broadcast as in
+        set_stream_trigger.  A stream whose entry changes gets a fresh pool detector; an unchanged entry keeps it.  The
+        settings survive set_stream_pool, pool_load and clear; set_pool drops them.  Synchronous; bad input raises ValueError
+        and changes nothing."""
+        ids, sens, level, chunk, n = self._trigger_args(sensitivity, trigger_level, chunk_size, ids, 0)
+        check(self.lib.pb_set_stream_pool_trigger(self._h, _np_ptr(ids), _np_ptr(sens), _np_ptr(level), _np_ptr(chunk), n))
+
+    def stream_pool_trigger(self, ids=None):
+        """(sensitivity f64[n], trigger_level i32[n], chunk_size i32[n], in bytes) of the pool settings of streams ids (host
+        int32 array), or of every stream.  A stream that follows its model reports (NaN, 0, 0)."""
+        n = self.max_streams if ids is None else (ids.shape[0] if isinstance(ids, np.ndarray) and ids.ndim == 1 else -1)
+        _check_np('ids', ids, np.int32, (n,))
+        sens, level, chunk = np.zeros(n, np.float64), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        check(self.lib.pb_get_stream_pool_trigger(self._h, _np_ptr(ids), n, _np_ptr(sens), _np_ptr(level), _np_ptr(chunk)))
+        return sens, level, chunk
 
     @property
     def num_models(self) -> int:
@@ -611,6 +656,12 @@ class PreciseB200:
         are scalars.  A stream whose values change gets a fresh detector; unchanged values keep its state.  Synchronous; bad
         input raises ValueError and changes nothing."""
         slot = self._slot(slot)
+        ids, sens, level, chunk, n = self._trigger_args(sensitivity, trigger_level, chunk_size, ids, 1)
+        check(self.lib.pb_set_stream_trigger(self._h, slot, _np_ptr(ids), _np_ptr(sens), _np_ptr(level), _np_ptr(chunk), n))
+
+    def _trigger_args(self, sensitivity, trigger_level, chunk_size, ids, min_chunk):
+        """(ids, sensitivity f64[n], trigger_level i32[n], chunk_size i32[n], n) of a trigger setter, scalars broadcast;
+        ValueError for anything the C ABI would misread or refuse, chunk sizes below ``min_chunk`` included."""
         vals = [np.asarray(sensitivity), np.asarray(trigger_level), np.asarray(chunk_size)]
         if any(v.ndim > 1 for v in vals):
             raise ValueError('sensitivity, trigger_level and chunk_size must be scalars or 1-D arrays')
@@ -635,12 +686,14 @@ class PreciseB200:
                 raise ValueError('%s must be integers, got %s' % (name, v.dtype))
             if v.size and (int(v.min()) < -2 ** 31 or int(v.max()) >= 2 ** 31):
                 raise ValueError('%s must fit in int32' % name)
-        if chunk.size and int(chunk.min()) < 1:
-            raise ValueError('chunk_size must be >= 1 byte (TriggerDetector divides by it), got %d' % int(chunk.min()))
+        if chunk.size and int(chunk.min()) < min_chunk:
+            if min_chunk == 1:
+                raise ValueError('chunk_size must be >= 1 byte (TriggerDetector divides by it), got %d' % int(chunk.min()))
+            raise ValueError('chunk_size must be >= 0 bytes (0: the model\'s own settings), got %d' % int(chunk.min()))
         sens = np.ascontiguousarray(np.broadcast_to(sens, (n,)), dtype=np.float64)
         level = np.ascontiguousarray(np.broadcast_to(level, (n,)), dtype=np.int32)
         chunk = np.ascontiguousarray(np.broadcast_to(chunk, (n,)), dtype=np.int32)
-        check(self.lib.pb_set_stream_trigger(self._h, slot, _np_ptr(ids), _np_ptr(sens), _np_ptr(level), _np_ptr(chunk), n))
+        return ids, sens, level, chunk, n
 
     def stream_trigger(self, slot, ids=None):
         """(sensitivity f64[n], trigger_level i32[n], chunk_size i32[n], in bytes) of bank slot ``slot`` for streams ids

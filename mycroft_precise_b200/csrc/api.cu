@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <map>
 #include <cuda_fp16.h>
+#include <limits>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -222,6 +223,11 @@ struct pb_handle {
     std::vector<std::map<std::string, PoolCd>::iterator> pool_cd_of;  // [max_models] each slot's table; pool_cd.end() = empty slot
     cudaEvent_t pool_ev = nullptr;   // recorded after each pool tick; the next one waits on it before reusing the scratch
     bool pool_warp_only = false;     // pb_debug_pool_tiles: every position in warp tiles
+    // per-stream pool TriggerDetector settings (pb_set_stream_pool_trigger); a pool that never gets them keeps pool_trig_set =
+    // false and its scans update the trigger in epilogue
+    bool pool_trig_set = false;      // sticky until the pool is replaced or freed
+    std::vector<StreamTrig> pool_trig_host;  // [max_streams] the settings as set; (NaN, 0, 0) = the stream's model's own
+    DevArray<TrigRec> d_pool_trig_rec;       // [max_streams] their records (trigger_reset 0 = the model's own), read by pool_trigger_kernel
     // host pipeline
     cudaStream_t pipe[HOST_PIPE] = {nullptr, nullptr, nullptr};
     cudaEvent_t pipe_ev[HOST_PIPE] = {nullptr, nullptr, nullptr};
@@ -2233,6 +2239,9 @@ static void drop_pool(pb_handle* h) {
     h->pool_cd_of.clear();
     h->pool_cd.clear();
     h->pool_cd_of.shrink_to_fit();
+    h->pool_trig_set = false;
+    h->pool_trig_host = std::vector<StreamTrig>();
+    h->d_pool_trig_rec = DevArray<TrigRec>();
 }
 
 PB_API int pb_set_pool(pb_handle* h, int32_t max_models) {
@@ -2442,13 +2451,20 @@ PB_API int pb_debug_pool_tiles(pb_handle* h, int warp_only) {
     return PB_OK;
 }
 
-// The network half of a pool tick: the route, then the block and warp tiles of both activation classes.
+// The network half of a pool tick: the route, then the block and warp tiles of both activation classes; with per-stream
+// trigger settings, the scans write raw and conf only and pool_trigger_kernel follows them.
 static int score_pool(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired,
                       unsigned long long* d_count, cudaStream_t s) {
     PoolTick t{};
     t.pool_id = h->d_pool_id.get(); t.slots = h->d_pool_slots.get(); t.lists = h->d_pool_list.get();
     t.count = h->d_pool_count.get(); t.list0 = h->d_pool_list0.get();
     t.raw = d_raw; t.conf = d_conf; t.fired = d_fired; t.d_count = d_count; t.trig = h->d_pool_trig.get();
+    PoolTrig pt{};
+    if (h->pool_trig_set) {
+        pt.ids = d_ids; pt.n = n; pt.pool_id = t.pool_id; pt.slots = t.slots;
+        pt.conf = d_conf; pt.fired = d_fired; pt.d_count = d_count; pt.trig = t.trig; pt.rec = h->d_pool_trig_rec.get();
+        t.fired = nullptr; t.d_count = nullptr; t.trig = nullptr;
+    }
     const K2In in = stream_k2in(h, d_ids);
     ProfScope ps(h, 1, s);
     // the lists and counts are the handle's: a pool tick on another stream may still be reading them
@@ -2468,6 +2484,10 @@ static int score_pool(pb_handle* h, const int32_t* d_ids, int64_t n, float* d_ra
             CK(cudaGetLastError());
             if (nw && ka) pool_warp_kernel<true><<<(unsigned)((nw + W - 1) / W), MMA_THREADS, W * BANK_MODEL_SMEM, s>>>(tw, nw, t, in);
             else if (nw) pool_warp_kernel<false><<<(unsigned)((nw + W - 1) / W), MMA_THREADS, W * BANK_MODEL_SMEM, s>>>(tw, nw, t, in);
+            CK(cudaGetLastError());
+        }
+        if (h->pool_trig_set) {
+            pool_trigger_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(pt);
             CK(cudaGetLastError());
         }
         return PB_OK;
@@ -2499,6 +2519,104 @@ PB_API int pb_update_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* d_o
     }
     if (rc != PB_OK) return rc;
     return score_pool(h, d_ids, n, d_raw, d_conf, d_fired, d_count, s);
+}
+
+PB_API int pb_update_all(pb_handle* h, const int16_t* d_pcm, const int64_t* d_offsets, int64_t max_len, const int32_t* d_ids,
+                         int64_t n, float* d_raw, double* d_conf, uint8_t* d_fired, unsigned long long* d_counts,
+                         unsigned long long* d_pool_count, void* stream) {
+    int rc = check_tick(h, d_pcm, n);
+    if (rc != PB_OK) return rc;
+    if (!d_conf) return fail(PB_ERR_INVALID, "null d_conf");
+    if (d_offsets && max_len < 1) return fail(PB_ERR_INVALID, "max_len = %lld must be >= 1", (long long)max_len);
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (d_offsets && h->k1_mode != 0) return fail(PB_ERR_STATE, "ragged ticks run only with k1 mode 0");
+    if (n == 0) return PB_OK;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int64_t M = (int64_t)h->models.size();
+    // K1 and the bank exactly as pb_update_ragged (offsets) or pb_update_models (none) run them, then the pool into row M
+    if (d_offsets) {
+        h->ragged = true;
+        rc = append_history(h, d_pcm, d_offsets, max_len, d_ids, n, s);
+        if (rc == PB_OK) rc = launch_ragged_mfcc(h, d_pcm, d_offsets, max_len, d_ids, n, s);
+        if (rc == PB_OK)
+            rc = M == 1 ? score_model0(h, d_ids, n, d_raw, d_conf, d_fired, d_counts, s)
+                        : score_bank(h, d_ids, n, d_raw, d_conf, d_fired, d_counts, s);
+    } else {
+        rc = tick_mfcc(h, d_pcm, d_ids, n, s);
+        if (rc == PB_OK) rc = score_bank(h, d_ids, n, d_raw, d_conf, d_fired, d_counts, s);
+    }
+    if (rc != PB_OK) return rc;
+    return score_pool(h, d_ids, n, d_raw ? d_raw + M * n : nullptr, d_conf + M * n, d_fired ? d_fired + M * n : nullptr,
+                      d_pool_count, s);
+}
+
+// ------------------------------------------------------------------------------------------------
+// per-stream pool TriggerDetector settings
+
+// A stream that follows its model: (NaN, 0, 0) on the host, trigger_reset 0 on the device.
+static StreamTrig pool_follow_trig() {
+    return StreamTrig{std::numeric_limits<double>::quiet_NaN(), 0, 0};
+}
+
+PB_API int pb_set_stream_pool_trigger(pb_handle* h, const int32_t* h_ids, const double* h_sensitivity,
+                                      const int32_t* h_trigger_level, const int32_t* h_chunk_bytes, int64_t n) {
+    int rc = check_route_ids(h, h_ids, n, true);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && (!h_sensitivity || !h_trigger_level || !h_chunk_bytes)) return fail(PB_ERR_INVALID, "null settings");
+    for (int64_t i = 0; i < n; ++i)
+        if (h_chunk_bytes[i] < 0)
+            return fail(PB_ERR_INVALID, "chunk_bytes = %d (entry %lld) must be >= 0 (0: the model's own settings)", h_chunk_bytes[i], (long long)i);
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    CK(cudaSetDevice(h->cfg.device));
+    CK(cudaDeviceSynchronize());                     // queued work finishes under the old settings
+    if (!h->pool_trig_set) {                         // the first call: every stream follows its model
+        const size_t S = (size_t)h->cfg.max_streams;
+        DevArray<TrigRec> rec;
+        CK(rec.upload(std::vector<TrigRec>(S, TrigRec{0.0, 0, 0})));
+        h->d_pool_trig_rec = std::move(rec);
+        h->pool_trig_host.assign(S, pool_follow_trig());
+        h->pool_trig_set = true;
+    }
+    std::vector<int> sids;
+    std::vector<StreamTrig> vals;
+    std::vector<TrigRec> recs;
+    for (int64_t i = 0; i < n; ++i) {
+        const int sid = h_ids ? h_ids[i] : (int)i;
+        const bool follow = h_chunk_bytes[i] == 0;
+        const StreamTrig v = follow ? pool_follow_trig() : StreamTrig{h_sensitivity[i], h_trigger_level[i], h_chunk_bytes[i]};
+        if (same_trig(v, h->pool_trig_host[sid])) continue;  // unchanged: the detector keeps its state
+        sids.push_back(sid);
+        vals.push_back(v);
+        recs.push_back(follow ? TrigRec{0.0, 0, 0} : trig_record(v));
+    }
+    if (sids.empty()) return PB_OK;
+    DevArray<int> d_sids;
+    DevArray<TrigRec> d_recs;
+    CK(d_sids.upload(sids));
+    CK(d_recs.upload(recs));
+    const long long k = (long long)sids.size();
+    set_trigger_kernel<<<(int)((k + 255) / 256), 256>>>(h->d_pool_trig_rec.get(), h->d_pool_trig.get(), d_sids.get(), d_recs.get(), k);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    for (size_t j = 0; j < sids.size(); ++j) h->pool_trig_host[sids[j]] = vals[j];
+    return PB_OK;
+}
+
+PB_API int pb_get_stream_pool_trigger(const pb_handle* h, const int32_t* h_ids, int64_t n, double* h_sensitivity,
+                                      int32_t* h_trigger_level, int32_t* h_chunk_bytes) {
+    const int rc = check_route_ids(h, h_ids, n, false);
+    if (rc != PB_OK) return rc;
+    if (n > 0 && (!h_sensitivity || !h_trigger_level || !h_chunk_bytes)) return fail(PB_ERR_INVALID, "null output");
+    const StreamTrig d = pool_follow_trig();
+    for (int64_t i = 0; i < n; ++i) {
+        const StreamTrig& v = h->pool_trig_set ? h->pool_trig_host[h_ids ? h_ids[i] : i] : d;
+        h_sensitivity[i] = v.sensitivity;
+        h_trigger_level[i] = v.trigger_level;
+        h_chunk_bytes[i] = v.chunk_bytes;
+    }
+    return PB_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

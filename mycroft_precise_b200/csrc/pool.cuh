@@ -9,6 +9,8 @@
 //                       gru_bank_routed_kernel scans a model).
 //   pool_warp_kernel    one warp per warp tile: the at most 63 positions past a model's last block tile, as tiles of 16.  The
 //                       4 warps of a CTA may score 4 different models, each from its own shared-memory slot.
+//   pool_trigger_kernel only once pb_set_stream_pool_trigger has been called: the scans then write raw and conf only, and
+//                       this kernel runs each stream's TriggerDetector with its own settings or its model's.
 // The tile tables (model, first position) are built on the host whenever assignments or models change, one per tile shape and
 // activation class, so a tick reads nothing back.  A tile whose first position is at or past its model's count this tick (a
 // tick over a subset of the streams) exits before it loads weights.  Every scan is bank_scan's, with the bank's per-model
@@ -18,6 +20,7 @@
 #include <stdint.h>
 
 #include "gru_bank.cuh"
+#include "trigger.cuh"
 
 namespace pb {
 
@@ -103,6 +106,53 @@ __device__ __forceinline__ PoolScanP pool_scan_params(const PoolTick& t, int m) 
     P.o.o = K2Out{};
     P.o.o.raw = t.raw; P.o.o.conf = t.conf; P.o.o.fired = t.fired; P.o.o.count = t.d_count; P.o.o.trig = t.trig;
     return P;
+}
+
+// A pool with per-stream trigger settings (pb_set_stream_pool_trigger): its scans run with trig = fired = d_count = null, so
+// epilogue writes raw and conf only, and pool_trigger_kernel updates the detectors afterwards.
+struct PoolTrig {
+    const int* ids;                  // item -> stream id (null = identity)
+    long long n;
+    const int* pool_id;              // [max_streams] model of each stream, -1 = none
+    const uint4* slots;              // the pool's slots: a stream that follows its model reads the model's DecodeParams
+    const double* conf;              // [n] the tick's pool conf
+    uint8_t* fired;                  // [n] or null
+    unsigned long long* d_count;     // or null
+    int* trig;                       // [max_streams] each stream's pool TriggerDetector.activation
+    const TrigRec* rec;              // [max_streams] each stream's settings; trigger_reset == 0: the model's own
+};
+
+// TriggerDetector.update (runner.py:127-142), one thread per item.  An item whose stream has no pool model gets fired 0 and
+// its detector does not move.  Fires are counted with one atomicAdd per warp, as in epilogue.
+__global__ void __launch_bounds__(256) pool_trigger_kernel(const __grid_constant__ PoolTrig t) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool ok = i < t.n;
+    const int sid = ok ? (t.ids ? t.ids[i] : (int)i) : 0;
+    const int m = ok ? t.pool_id[sid] : -1;
+    bool fired = false;
+    if (m >= 0) {
+        const double conf = t.conf[i];
+        TrigRec r = t.rec[sid];
+        if (r.trigger_reset == 0) {
+            const DecodeParams& d = pool_rec(t.slots, m)->dp;
+            r.hot_threshold = d.hot_threshold; r.trigger_level = d.trigger_level; r.trigger_reset = d.trigger_reset;
+        }
+        int a = t.trig[sid];
+        const bool hot = conf > r.hot_threshold;
+        if (hot || a < 0) {
+            a += 1;
+            fired = a > r.trigger_level;
+            if (fired || (hot && a < 0)) a = r.trigger_reset;
+        } else if (a > 0) {
+            a -= 1;
+        }
+        t.trig[sid] = a;
+    }
+    if (ok && t.fired) t.fired[i] = fired ? 1 : 0;
+    if (t.d_count) {
+        const unsigned b = __ballot_sync(0xffffffffu, fired);
+        if (b && (threadIdx.x & 31) == 0) atomicAdd(t.d_count, (unsigned long long)__popc(b));
+    }
 }
 
 // tiles[blockIdx.x] = (model, first list position, a multiple of 64).
