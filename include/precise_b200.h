@@ -362,8 +362,9 @@ int pb_read_history(pb_handle* h, const int32_t* d_stream_ids, int64_t n, int64_
  *   - Memory: about 14.3 KB per slot, 51 200 B per distinct decoder table at the default thresholds (models whose tables
  *     are bit-identical share one copy), 16 B per stream.
  *   - The bank, its masks and trigger settings are independent of the pool; pb_update_models does not score pool models and
- *     pb_update_pool scores no bank model.  pb_update_all scores both on one K1.  Not covered: pb_update_host,
- *     pb_score_corpus, networks outside the fused family.
+ *     pb_update_pool scores no bank model.  pb_update_all scores both on one K1.  pb_score_corpus scores the bank only;
+ *     pb_score_corpus_pool scores chosen pool models over a recorded corpus.  Not covered: pb_update_host, networks outside
+ *     the fused family.
  *   - A handle that never calls pb_set_pool runs exactly as before.
  *
  * pb_set_pool: a pool of max_models slots (max_models in [1, 2^24]), every slot empty and every stream on none.  Synchronous.
@@ -487,6 +488,30 @@ int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets
                     int32_t divisor, int32_t schedule, int64_t chunk, double threshold,
                     float* d_raw, double* d_conf, uint8_t* d_fired,
                     int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream);
+/* Pool models over recorded corpora: "how often does each custom wake word fire on this corpus" for many pool models in one
+ * call.  Pool models h_model_ids[0 .. k) (HOST; repeats allowed, each gives its own identical row) score every window of the
+ * n_rec recordings: a cross product.  Recordings, divisor, schedules, chunk and threshold mean exactly what they mean for
+ * pb_score_corpus.  K1 and the window table run once per call, whatever k.
+ *   - Outputs are model-major in the order of h_model_ids: d_raw, d_conf, d_fired [k][W_total]; d_activations, d_above,
+ *     d_sum [k][n_rec].  Every output is optional, d_raw included, but not all of them at once.  Row i is bit-identical to
+ *     the row pb_score_corpus writes for the same network in a bank of two or more models.
+ *   - Listener schedule: each model's own decoder, cfg.sensitivity and cfg.trigger_level, refractory count from
+ *     TriggerDetector(2c bytes), as pb_score_corpus.  Per-stream pool trigger settings do not apply (no stream is involved).
+ *   - Reads and writes no stream state, pool assignments or pool detectors; needs no slot-0 weights; the bank is not scored.
+ *   - Memory: the workspace of pb_score_corpus, shared with it, plus about 12 B per requested model.  Without d_raw, when a trigger pass is wanted, raw of a batch of max(1, 256 MB / (4 W_total)) rows is
+ *     kept in the workspace (at most 256 MB, or one row's 4 W_total bytes): rows are scanned batch after batch, each followed by
+ *     its trigger pass.
+ *   - Asynchronous on `stream`, ordered against other corpus calls as pb_score_corpus.  pb_pool_load and pb_set_pool wait for
+ *     queued calls, so a load after a call does not change what it scores.  Profile slot 0 counts K1, slot 1 the scans and
+ *     trigger passes.  Every argument is checked before anything is enqueued, so a refused call changes no state.
+ * PB_ERR_INVALID: pb_score_corpus's argument errors (but a null d_raw), every output null, k < 0, a null h_model_ids with
+ * k > 0, an id outside [0, max_models) or a slot that holds no model.  PB_ERR_STATE: no pool.  PB_ERR_CUDA: the workspace
+ * cannot be allocated (the handle is then unchanged). */
+int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                         const int32_t* h_model_ids, int64_t k,
+                         int32_t divisor, int32_t schedule, int64_t chunk, double threshold,
+                         float* d_raw, double* d_conf, uint8_t* d_fired,
+                         int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream);
 
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
@@ -527,6 +552,13 @@ int pb_debug_k1_mode(pb_handle* h, int mode);
 /* Test / A-B hook for the model pool's tiles: 0 = block tiles of 64 for each model's full groups, warp tiles of 16 for the
  * rest; 1 = warp tiles of 16 for every position.  Both score bit-identical outputs.  PB_ERR_STATE without a pool. */
 int pb_debug_pool_tiles(pb_handle* h, int warp_only);
+/* Test hook for pb_score_corpus_pool without d_raw: at most `rows` model rows per batch (rows >= 1), so that small corpora
+ * reach the multi-batch path; 0 restores the default (the 256 MB raw cap).  PB_ERR_INVALID: null handle, rows < 0. */
+int pb_debug_corpus_pool_rows(pb_handle* h, int64_t rows);
+/* A/B hook for pb_score_corpus_pool's scan: nm models per CTA (1, 2, 4 or 8; 0 = the default), and grid order groups_fast
+ * (1: consecutive CTAs take every model group of one window tile; 0: every tile of one group; -1 = the default).  Every
+ * choice scores bit-identical outputs.  PB_ERR_INVALID: null handle, a value out of range. */
+int pb_debug_corpus_pool_scan(pb_handle* h, int32_t nm, int32_t groups_fast);
 /* CPU model of a tensor-core formulation of the DFT (csrc/mfcc_tc.cuh: radix-16 butterflies, second stage as an fp16 hi / lo
  * matrix product) for one frame of 512 int16 samples -> |X[k]|^2, k = 0..256.  No device needed.  Test hook. */
 int pb_debug_tc_dft_power(const int16_t* x512, double* power257);

@@ -83,6 +83,8 @@ SYMBOLS = {
     'pb_get_stream_pool_trigger': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP]),
     'pb_corpus_windows': (_I64, [C.POINTER(pb_config), _I32, _I64, _I64]),
     'pb_score_corpus': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    'pb_score_corpus_pool': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP,
+                                       _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -95,6 +97,8 @@ SYMBOLS = {
     'pb_debug_gru_mode': (C.c_int, [_VP, C.c_int]),
     'pb_debug_k1_mode': (C.c_int, [_VP, C.c_int]),
     'pb_debug_pool_tiles': (C.c_int, [_VP, C.c_int]),
+    'pb_debug_corpus_pool_rows': (C.c_int, [_VP, _I64]),
+    'pb_debug_corpus_pool_scan': (C.c_int, [_VP, _I32, _I32]),
     'pb_debug_tc_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_mma_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_tc_mfcc_frame': (C.c_int, [_VP, _VP, _VP]),
@@ -819,11 +823,8 @@ class PreciseB200:
             check(n)
         return n
 
-    def score_corpus(self, pcm, offsets, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
-        """Every bank model over recordings pcm[offsets[r]:offsets[r + 1]] (pcm a 1-D int16 CUDA tensor, offsets a host int64
-        array [n_rec + 1]).  Returns dict(raw f32 [M, W], conf f64 [M, W], fired u8 [M, W], activations i64 [M, n_rec], and
-        for the simulate schedule above i64 [M, n_rec] and sum f64 [M, n_rec]; None otherwise), W the total window count.
-        Asynchronous on the current stream.  Schedules and outputs: pb_score_corpus in include/precise_b200.h."""
+    def _corpus_args(self, pcm, offsets, schedule, chunk):
+        """(schedule code, int64 offsets, n_rec, W) of a corpus call, checked."""
         torch = self.torch
         sched = _schedule(schedule)
         if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
@@ -840,6 +841,15 @@ class PreciseB200:
         if lens.size and lens.min() < 0:
             raise ValueError('offsets must be non-decreasing')
         W = sum(self.corpus_windows(int(L), schedule, chunk) for L in lens)
+        return sched, offsets, n_rec, W
+
+    def score_corpus(self, pcm, offsets, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
+        """Every bank model over recordings pcm[offsets[r]:offsets[r + 1]] (pcm a 1-D int16 CUDA tensor, offsets a host int64
+        array [n_rec + 1]).  Returns dict(raw f32 [M, W], conf f64 [M, W], fired u8 [M, W], activations i64 [M, n_rec], and
+        for the simulate schedule above i64 [M, n_rec] and sum f64 [M, n_rec]; None otherwise), W the total window count.
+        Asynchronous on the current stream.  Schedules and outputs: pb_score_corpus in include/precise_b200.h."""
+        torch = self.torch
+        sched, offsets, n_rec, W = self._corpus_args(pcm, offsets, schedule, chunk)
         M = self.num_models
         f = lambda shape, dt: torch.empty(shape, dtype=dt, device=self.device)
         out = dict(raw=f((M, W), torch.float32), conf=f((M, W), torch.float64), fired=f((M, W), torch.uint8),
@@ -851,6 +861,39 @@ class PreciseB200:
                                        float(threshold), _ptr(out['raw']), _ptr(out['conf']), _ptr(out['fired']),
                                        _ptr(out['activations']), _ptr(out['above']), _ptr(out['sum']), self._stream()))
         return out
+
+    def score_corpus_pool(self, pcm, offsets, model_ids, schedule='listener', chunk=1024, threshold=0.5, divisor=32768,
+                          per_window=True):
+        """Pool models ``model_ids`` (host int32 array [k], repeats allowed) over recordings pcm[offsets[r]:offsets[r + 1]], as
+        score_corpus takes them: every model scores every recording, K1 runs once.  Returns score_corpus's dict with k rows in
+        the order of model_ids.  per_window=False: raw, conf and fired are None and only the reductions (activations, and
+        for the simulate schedule above and sum) are computed, without a [k, W] buffer.  Asynchronous on the current stream.
+        pb_score_corpus_pool in include/precise_b200.h."""
+        torch = self.torch
+        sched, offsets, n_rec, W = self._corpus_args(pcm, offsets, schedule, chunk)
+        model_ids = np.asarray(model_ids)
+        k = model_ids.shape[0] if model_ids.ndim == 1 else -1
+        _check_np('model_ids', model_ids, np.int32, (k,), optional=False)
+        f = lambda shape, dt: torch.empty(shape, dtype=dt, device=self.device)
+        out = dict(raw=None, conf=None, fired=None, activations=f((k, n_rec), torch.int64), above=None, sum=None)
+        if per_window:
+            out.update(raw=f((k, W), torch.float32), conf=f((k, W), torch.float64), fired=f((k, W), torch.uint8))
+        if sched == 1:
+            out['above'] = f((k, n_rec), torch.int64)
+            out['sum'] = f((k, n_rec), torch.float64)
+        check(self.lib.pb_score_corpus_pool(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, _np_ptr(model_ids), k, int(divisor),
+                                            sched, int(chunk), float(threshold), _ptr(out['raw']), _ptr(out['conf']),
+                                            _ptr(out['fired']), _ptr(out['activations']), _ptr(out['above']),
+                                            _ptr(out['sum']), self._stream()))
+        return out
+
+    def corpus_pool_rows(self, rows):
+        """Test hook: score_corpus_pool with per_window=False scans at most ``rows`` models per batch (0 = the default)."""
+        check(self.lib.pb_debug_corpus_pool_rows(self._h, int(rows)))
+
+    def corpus_pool_scan(self, nm=0, groups_fast=-1):
+        """A/B hook: score_corpus_pool's models per CTA (1, 2, 4, 8; 0 = default) and grid order (-1 = default)."""
+        check(self.lib.pb_debug_corpus_pool_scan(self._h, int(nm), int(groups_fast)))
 
     def update_host(self, pcm_np, conf_np, raw_np=None, fired_np=None, ids_np=None) -> int:
         """Host-buffer tick (numpy arrays, ideally backed by pinned memory).  Returns this tick's count."""

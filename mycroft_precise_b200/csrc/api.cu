@@ -34,6 +34,7 @@
 #include "stream_state.cuh"
 #include "history.cuh"
 #include "corpus.cuh"
+#include "corpus_pool.cuh"
 #include "pool.cuh"
 
 using namespace pb;
@@ -204,6 +205,12 @@ struct pb_handle {
     DevArray<long long> d_cw_frow;   // [n_rec] row of each recording's frame 0
     DevArray<CorpusRec> d_cw_recs;   // [n_rec + 1] recordings in pair-list order
     cudaEvent_t corpus_ev = nullptr; // recorded after each corpus call; the next one waits on it before reusing the workspace
+    DevArray<int2> d_cp_groups;      // pb_score_corpus_pool: the scan's model groups, (pool slot, output row) entries
+    DevArray<int> d_cp_ids;          // ... the requested pool slots, one per output row
+    DevArray<float> d_cp_raw;        // ... raw of one batch of rows when the caller passes no d_raw (at most CORPUS_POOL_RAW_CAP bytes)
+    int64_t corpus_pool_rows = 0;    // pb_debug_corpus_pool_rows: at most this many rows per batch (0 = the cap's)
+    int corpus_pool_nm = 0;          // pb_debug_corpus_pool_scan: models per group (0 = CORPUS_POOL_NM)
+    int corpus_pool_order = -1;      // ... grid order (-1 = CORPUS_POOL_GROUPS_FAST)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
     int32_t pool_models = 0;         // max_models
@@ -1601,159 +1608,377 @@ static cudaError_t corpus_grow(const DevArray<T>& a, size_t n, DevArray<T>& fres
     return fresh.alloc(n + n / 4);
 }
 
-PB_API int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
-                           int32_t schedule, int64_t chunk, double threshold, float* d_raw, double* d_conf, uint8_t* d_fired,
-                           int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream) {
-    if (!h) return fail(PB_ERR_INVALID, "null handle");
+// The checks every corpus call shares (pb_score_corpus, pb_score_corpus_pool); raw_required: d_raw may not be null.
+static int check_corpus(const pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
+                        int32_t schedule, int64_t chunk, const float* d_raw, bool raw_required, const int64_t* d_above,
+                        const double* d_sum) {
     const pb_config& c = h->cfg;
     if (n_rec < 0 || n_rec > INT32_MAX) return fail(PB_ERR_INVALID, "n_rec = %lld outside [0, 2^31)", (long long)n_rec);
     if (!h_offsets) return fail(PB_ERR_INVALID, "null h_offsets");
-    if (!d_raw) return fail(PB_ERR_INVALID, "null d_raw");
+    if (raw_required && !d_raw) return fail(PB_ERR_INVALID, "null d_raw");
     if (divisor != 32768 && divisor != 32767) return fail(PB_ERR_INVALID, "divisor %d: 32768 (buffer_to_audio) or 32767 (load_audio)", divisor);
-    int rc = check_corpus_schedule(c, schedule, chunk);
+    const int rc = check_corpus_schedule(c, schedule, chunk);
     if (rc != PB_OK) return rc;
     if (schedule == PB_CORPUS_LISTENER && (d_above || d_sum)) return fail(PB_ERR_INVALID, "d_above and d_sum belong to the simulate schedule");
     if (h_offsets[0] < 0) return fail(PB_ERR_INVALID, "offset 0 = %lld is negative", (long long)h_offsets[0]);
     for (int64_t r = 0; r < n_rec; ++r)
         if (h_offsets[r + 1] < h_offsets[r]) return fail(PB_ERR_INVALID, "offsets decrease at recording %lld", (long long)r);
     if (h_offsets[n_rec] > h_offsets[0] && !d_pcm) return fail(PB_ERR_INVALID, "null d_pcm");
-    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
-    if (n_rec == 0) return PB_OK;
-    CK(cudaSetDevice(c.device));
-    cudaStream_t s = (cudaStream_t)stream;
-    const int M = (int)h->models.size(), T = c.n_features;
-    // host plan: window prefix, frame rows, and the recordings in pair-list order (aligned geometry first)
-    const bool fast = h->fast_ok && !h->force_generic && (uintptr_t)d_pcm % 16 == 0;
-    std::vector<long long> win0((size_t)n_rec + 1), frow((size_t)n_rec);
+    return PB_OK;
+}
+
+// K1's host plan of a corpus call: window prefix, frame rows, and the recordings in pair-list order (aligned geometry first).
+struct CorpusPlan {
+    std::vector<long long> win0, frow;
     std::vector<CorpusRec> recs;
-    recs.reserve((size_t)n_rec + 1);
-    long long rows = 1, n_fast_pairs = 0, n_pairs = 0;
-    win0[0] = 0;
+    long long rows = 1, n_fast_pairs = 0, n_pairs = 0, W = 0;
+};
+
+static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t schedule,
+                              int64_t chunk) {
+    const pb_config& c = h->cfg;
+    const int T = c.n_features;
+    const bool fast = h->fast_ok && !h->force_generic && (uintptr_t)d_pcm % 16 == 0;
+    CorpusPlan p;
+    p.win0.resize((size_t)n_rec + 1);
+    p.frow.resize((size_t)n_rec);
+    p.recs.reserve((size_t)n_rec + 1);
+    p.win0[0] = 0;
     for (int pass = 0; pass < 2; ++pass)
         for (int64_t r = 0; r < n_rec; ++r) {
             const int64_t L = h_offsets[r + 1] - h_offsets[r], nf = corpus_frames(c, L);
             const bool fr = fast && h_offsets[r] % 8 == 0;
             if (pass == 0) {
-                win0[r + 1] = win0[r] + corpus_windows(c, schedule, chunk, L);
-                frow[r] = rows + T - 1;
-                rows += T - 1 + nf;
+                p.win0[r + 1] = p.win0[r] + corpus_windows(c, schedule, chunk, L);
+                p.frow[r] = p.rows + T - 1;
+                p.rows += T - 1 + nf;
             }
             if (fr != (pass == 0)) continue;
-            recs.push_back(CorpusRec{h_offsets[r], frow[r], nf, n_pairs});
-            n_pairs += (nf + 1) / 2;
-            if (fr) n_fast_pairs = n_pairs;
+            p.recs.push_back(CorpusRec{h_offsets[r], p.frow[r], nf, p.n_pairs});
+            p.n_pairs += (nf + 1) / 2;
+            if (fr) p.n_fast_pairs = p.n_pairs;
         }
-    recs.push_back(CorpusRec{0, 0, 0, n_pairs});
-    const long long W = win0[n_rec];
-    // the workspace: grown all at once, so that a failed allocation leaves the handle as it was
+    p.recs.push_back(CorpusRec{0, 0, 0, p.n_pairs});
+    p.W = p.win0[n_rec];
+    return p;
+}
+
+// Sizes of pb_score_corpus_pool's own workspace arrays (0 for pb_score_corpus).
+struct CorpusPoolSizes {
+    size_t groups = 0, ids = 0, raw = 0;
+};
+
+// Grows the workspace for plan p, all at once, so that a failed allocation leaves the handle as it was; then orders s after
+// the previous corpus call.
+static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, const CorpusPoolSizes& ps, cudaStream_t s) {
     if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
-    {
-        DevArray<float> f_rows; DevArray<CorpusPair> f_pairs; DevArray<long long> f_starts, f_win0, f_frow; DevArray<CorpusRec> f_recs;
-        cudaError_t e = corpus_grow(h->d_cw_rows, (size_t)rows * h->row_stride, f_rows);
-        if (e == cudaSuccess) e = corpus_grow(h->d_cw_pairs, (size_t)n_pairs, f_pairs);
-        if (e == cudaSuccess) e = corpus_grow(h->d_cw_starts, (size_t)W, f_starts);
-        if (e == cudaSuccess) e = corpus_grow(h->d_cw_win0, (size_t)n_rec + 1, f_win0);
-        if (e == cudaSuccess) e = corpus_grow(h->d_cw_frow, (size_t)n_rec, f_frow);
-        if (e == cudaSuccess) e = corpus_grow(h->d_cw_recs, recs.size(), f_recs);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(PB_ERR_CUDA, "corpus workspace allocation failed (%lld frame rows, %lld windows): %s", rows, W, cudaGetErrorString(e));
-        }
-        const bool grows = f_rows.get() || f_pairs.get() || f_starts.get() || f_win0.get() || f_frow.get() || f_recs.get();
-        if (grows) CK(cudaEventSynchronize(h->corpus_ev));            // the previous call may still read what is replaced
-        if (f_rows.get()) h->d_cw_rows = std::move(f_rows);
-        if (f_pairs.get()) h->d_cw_pairs = std::move(f_pairs);
-        if (f_starts.get()) h->d_cw_starts = std::move(f_starts);
-        if (f_win0.get()) h->d_cw_win0 = std::move(f_win0);
-        if (f_frow.get()) h->d_cw_frow = std::move(f_frow);
-        if (f_recs.get()) h->d_cw_recs = std::move(f_recs);
+    DevArray<float> f_rows, f_raw; DevArray<CorpusPair> f_pairs; DevArray<long long> f_starts, f_win0, f_frow; DevArray<CorpusRec> f_recs;
+    DevArray<int2> f_groups; DevArray<int> f_ids;
+    cudaError_t e = corpus_grow(h->d_cw_rows, (size_t)p.rows * h->row_stride, f_rows);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cw_pairs, (size_t)p.n_pairs, f_pairs);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cw_starts, (size_t)p.W, f_starts);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cw_win0, (size_t)n_rec + 1, f_win0);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cw_frow, (size_t)n_rec, f_frow);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cw_recs, p.recs.size(), f_recs);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cp_groups, ps.groups, f_groups);
+    if (e == cudaSuccess) e = corpus_grow(h->d_cp_ids, ps.ids, f_ids);
+    if (e == cudaSuccess && h->d_cp_raw.size() < ps.raw) e = f_raw.alloc(ps.raw);     // capped: no headroom
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(PB_ERR_CUDA, "corpus workspace allocation failed (%lld frame rows, %lld windows): %s", p.rows, p.W, cudaGetErrorString(e));
     }
+    const bool grows = f_rows.get() || f_pairs.get() || f_starts.get() || f_win0.get() || f_frow.get() || f_recs.get() ||
+                       f_groups.get() || f_ids.get() || f_raw.get();
+    if (grows) CK(cudaEventSynchronize(h->corpus_ev));            // the previous call may still read what is replaced
+    if (f_rows.get()) h->d_cw_rows = std::move(f_rows);
+    if (f_pairs.get()) h->d_cw_pairs = std::move(f_pairs);
+    if (f_starts.get()) h->d_cw_starts = std::move(f_starts);
+    if (f_win0.get()) h->d_cw_win0 = std::move(f_win0);
+    if (f_frow.get()) h->d_cw_frow = std::move(f_frow);
+    if (f_recs.get()) h->d_cw_recs = std::move(f_recs);
+    if (f_groups.get()) h->d_cp_groups = std::move(f_groups);
+    if (f_ids.get()) h->d_cp_ids = std::move(f_ids);
+    if (f_raw.get()) h->d_cp_raw = std::move(f_raw);
     CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));                      // a corpus call on another stream may still use it
-    // the call's work on s; the event is recorded after it even when a launch fails, so the next call orders itself after
-    // whatever this one queued
+    return PB_OK;
+}
+
+// K1 of a corpus call: the plan's device copies, the frame buffer and the window table (profile slot 0).
+static int corpus_k1(pb_handle* h, const CorpusPlan& p, const int16_t* d_pcm, int64_t n_rec, int32_t divisor, int32_t schedule,
+                     int64_t chunk, cudaStream_t s) {
+    const pb_config& c = h->cfg;
+    CK(cudaMemcpyAsync(h->d_cw_win0.get(), p.win0.data(), p.win0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->d_cw_frow.get(), p.frow.data(), p.frow.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->d_cw_recs.get(), p.recs.data(), p.recs.size() * sizeof(CorpusRec), cudaMemcpyHostToDevice, s));
+    if (p.n_pairs == 0 && p.W == 0) return PB_OK;
+    float* frames = h->d_cw_rows.get();
+    ProfScope ps(h, 0, s);
+    CK(cudaMemsetAsync(frames, 0, (size_t)p.rows * h->row_stride * sizeof(float), s));
+    const float inv = 1.0f / (float)divisor, scale = inv * inv / (float)c.n_fft;
+    if (p.n_pairs > 0) {
+        corpus_pairs_kernel<<<(unsigned)((p.n_pairs + 255) / 256), 256, 0, s>>>(h->d_cw_recs.get(), (int)p.recs.size() - 1, p.n_pairs,
+                                                                              c.hop_samples, h->d_cw_pairs.get());
+        CK(cudaGetLastError());
+    }
+    if (p.n_fast_pairs > 0) {
+        const int grid = (int)std::min<int64_t>((p.n_fast_pairs + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
+        mfcc_fast_corpus_kernel<<<grid, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, h->d_cw_pairs.get(), p.n_fast_pairs, c.hop_samples, scale,
+                                                                          mel_tables(h), fast_tables(h), frames, h->row_stride);
+        CK(cudaGetLastError());
+    }
+    if (p.n_pairs > p.n_fast_pairs) {
+        const int64_t tiles = (p.n_pairs - p.n_fast_pairs + K1_TILE / 2 - 1) / (K1_TILE / 2);
+        const int grid = (int)std::min<int64_t>(tiles, (int64_t)h->sm_count * 4);
+        mfcc_corpus_kernel<<<grid, K1_THREADS, h->k1_batch_smem, s>>>(d_pcm, h->d_cw_pairs.get() + p.n_fast_pairs, p.n_pairs - p.n_fast_pairs,
+                                                                     c.hop_samples, h->used, scale, mel_tables(h), frames, h->row_stride);
+        CK(cudaGetLastError());
+    }
+    if (p.W > 0) {
+        corpus_windows_kernel<<<(unsigned)((p.W + 255) / 256), 256, 0, s>>>(h->d_cw_win0.get(), h->d_cw_frow.get(), (int)n_rec, p.W, schedule, chunk,
+                                                                          h->rel_window, c.hop_samples, c.n_features, h->d_cw_starts.get());
+        CK(cudaGetLastError());
+    }
+    return PB_OK;
+}
+
+// Predict-mode input of a corpus call's scans: the windows in place in the frame buffer.
+static K2In corpus_k2in(const pb_handle* h) {
+    K2In in{};
+    in.inputs = h->d_cw_rows.get(); in.starts = h->d_cw_starts.get(); in.row_stride = h->row_stride;
+    in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
+    return in;
+}
+
+// The trigger pass's fields shared by every row.
+static CorpusTrig corpus_trig(const pb_handle* h, int64_t n_rec, int64_t W, int32_t schedule, int64_t chunk, double threshold) {
+    CorpusTrig t{};
+    t.win0 = h->d_cw_win0.get(); t.W = W; t.n_rec = (int)n_rec; t.schedule = schedule;
+    t.hot_f = (float)(1.0 - threshold); t.above_f = (float)threshold;
+    t.sim_reset = trigger_reset(chunk);
+    return t;
+}
+
+// Records corpus_ev after the call's work, even when a launch failed, so the next call orders itself after whatever this
+// one queued.
+static int corpus_done(pb_handle* h, cudaStream_t s, int rc) {
+    const cudaError_t er = cudaEventRecord(h->corpus_ev, s);
+    if (rc != PB_OK) return rc;
+    if (er != cudaSuccess) return fail(PB_ERR_CUDA, "cudaEventRecord failed: %s", cudaGetErrorString(er));
+    return PB_OK;
+}
+
+PB_API int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
+                           int32_t schedule, int64_t chunk, double threshold, float* d_raw, double* d_conf, uint8_t* d_fired,
+                           int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, schedule, chunk, d_raw, true, d_above, d_sum);
+    if (rc != PB_OK) return rc;
+    if (!h->models[0].w) return fail(PB_ERR_STATE, "pb_load_weights has not been called");
+    if (n_rec == 0) return PB_OK;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int M = (int)h->models.size();
+    const CorpusPlan p = corpus_plan(h, d_pcm, h_offsets, n_rec, schedule, chunk);
+    const long long W = p.W;
+    rc = corpus_reserve(h, p, n_rec, CorpusPoolSizes{}, s);
+    if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        CK(cudaMemcpyAsync(h->d_cw_win0.get(), win0.data(), win0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_cw_frow.get(), frow.data(), frow.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_cw_recs.get(), recs.data(), recs.size() * sizeof(CorpusRec), cudaMemcpyHostToDevice, s));
-        float* frames = h->d_cw_rows.get();
-        if (n_pairs > 0 || W > 0) {
-            ProfScope ps(h, 0, s);
-            CK(cudaMemsetAsync(frames, 0, (size_t)rows * h->row_stride * sizeof(float), s));
-            const float inv = 1.0f / (float)divisor, scale = inv * inv / (float)c.n_fft;
-            if (n_pairs > 0) {
-                corpus_pairs_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, s>>>(h->d_cw_recs.get(), (int)recs.size() - 1, n_pairs,
-                                                                                    c.hop_samples, h->d_cw_pairs.get());
-                CK(cudaGetLastError());
-            }
-            if (n_fast_pairs > 0) {
-                const int grid = (int)std::min<int64_t>((n_fast_pairs + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
-                mfcc_fast_corpus_kernel<<<grid, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, h->d_cw_pairs.get(), n_fast_pairs, c.hop_samples, scale,
-                                                                                  mel_tables(h), fast_tables(h), frames, h->row_stride);
-                CK(cudaGetLastError());
-            }
-            if (n_pairs > n_fast_pairs) {
-                const int64_t tiles = (n_pairs - n_fast_pairs + K1_TILE / 2 - 1) / (K1_TILE / 2);
-                const int grid = (int)std::min<int64_t>(tiles, (int64_t)h->sm_count * 4);
-                mfcc_corpus_kernel<<<grid, K1_THREADS, h->k1_batch_smem, s>>>(d_pcm, h->d_cw_pairs.get() + n_fast_pairs, n_pairs - n_fast_pairs,
-                                                                             c.hop_samples, h->used, scale, mel_tables(h), frames, h->row_stride);
-                CK(cudaGetLastError());
-            }
-            if (W > 0) {
-                corpus_windows_kernel<<<(unsigned)((W + 255) / 256), 256, 0, s>>>(h->d_cw_win0.get(), h->d_cw_frow.get(), (int)n_rec, W, schedule, chunk,
-                                                                                h->rel_window, c.hop_samples, T, h->d_cw_starts.get());
-                CK(cudaGetLastError());
-            }
-        }
-        {
-            ProfScope ps(h, 1, s);
-            if (W > 0) {
-                // every model scans the windows in place.  One model runs pb_predict's dispatch (the warp-per-window kernel up to
-                // 8 192 windows for the default network); a bank runs its fused family in one predict-mode bank launch, the others
-                // one launch each
-                K2In in{};
-                in.inputs = frames; in.starts = h->d_cw_starts.get(); in.row_stride = h->row_stride;
-                in.T = T; in.F_base = h->n_out; in.use_delta = c.use_delta;
-                BankParams P{};
-                int nm = 0;
-                for (int m = 0; m < M; ++m) {
-                    const Network& net = h->models[m];
-                    K2Out o{};
-                    o.raw = d_raw + (int64_t)m * W;
-                    o.conf = d_conf ? d_conf + (int64_t)m * W : nullptr;
-                    if (M > 1 && bank_fused(net, h->feat)) {
-                        set_bank_slot(P, nm++, net, o);
-                    } else {
-                        rc = launch_gru_kernels(net, h->feat, in, false, W, o, s);
-                        if (rc != PB_OK) return rc;
-                    }
-                }
-                if (nm) {
-                    rc = launch_bank<false>(P, nm, in, W, s);
+        rc = corpus_k1(h, p, d_pcm, n_rec, divisor, schedule, chunk, s);
+        if (rc != PB_OK) return rc;
+        ProfScope ps(h, 1, s);
+        if (W > 0) {
+            // every model scans the windows in place.  One model runs pb_predict's dispatch (the warp-per-window kernel up to
+            // 8 192 windows for the default network); a bank runs its fused family in one predict-mode bank launch, the others
+            // one launch each
+            const K2In in = corpus_k2in(h);
+            BankParams P{};
+            int nm = 0;
+            for (int m = 0; m < M; ++m) {
+                const Network& net = h->models[m];
+                K2Out o{};
+                o.raw = d_raw + (int64_t)m * W;
+                o.conf = d_conf ? d_conf + (int64_t)m * W : nullptr;
+                if (M > 1 && bank_fused(net, h->feat)) {
+                    set_bank_slot(P, nm++, net, o);
+                } else {
+                    rc = launch_gru_kernels(net, h->feat, in, false, W, o, s);
                     if (rc != PB_OK) return rc;
                 }
             }
-            if (d_fired || d_activations || d_above || d_sum) {
-                CorpusTrig t{};
-                t.raw = d_raw; t.conf = d_conf; t.fired = d_fired; t.activations = d_activations; t.above = d_above; t.sum = d_sum;
-                t.win0 = h->d_cw_win0.get(); t.W = W; t.n_rec = (int)n_rec; t.schedule = schedule;
-                t.hot_f = (float)(1.0 - threshold); t.above_f = (float)threshold;
-                t.sim_reset = trigger_reset(chunk);
-                for (int m = 0; m < M; ++m) {
-                    t.dp[m] = decode_params(h->models[m]);
-                    t.dp[m].trigger_reset = trigger_reset(2 * chunk);            // TriggerDetector(2c bytes, ...) of a chunk-c listener
+            if (nm) {
+                rc = launch_bank<false>(P, nm, in, W, s);
+                if (rc != PB_OK) return rc;
+            }
+        }
+        if (d_fired || d_activations || d_above || d_sum) {
+            CorpusTrig t = corpus_trig(h, n_rec, W, schedule, chunk, threshold);
+            t.raw = d_raw; t.conf = d_conf; t.fired = d_fired; t.activations = d_activations; t.above = d_above; t.sum = d_sum;
+            CorpusBankDP dp{};
+            for (int m = 0; m < M; ++m) {
+                dp.dp[m] = decode_params(h->models[m]);
+                dp.dp[m].trigger_reset = trigger_reset(2 * chunk);            // TriggerDetector(2c bytes, ...) of a chunk-c listener
+            }
+            const unsigned per = CORPUS_TRIG_THREADS / 32;
+            corpus_trigger_kernel<<<dim3((unsigned)((n_rec + per - 1) / per), (unsigned)M), CORPUS_TRIG_THREADS, 0, s>>>(t, dp);
+            CK(cudaGetLastError());
+        }
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+// ------------------------------------------------------------------------------------------------
+// pool models over a recorded corpus (corpus_pool.cuh)
+
+// Bytes of raw a pb_score_corpus_pool call without d_raw keeps on the device for its trigger pass: rows are scanned in
+// batches of max(1, cap / (4 W)) models.
+constexpr int64_t CORPUS_POOL_RAW_CAP = 256ll << 20;
+// Models per group and grid order of the scan (DESIGN §6, "Pool models over a recorded corpus"); pb_debug_corpus_pool_scan
+// picks others for A/B timing.
+constexpr int CORPUS_POOL_NM = 1;
+constexpr int CORPUS_POOL_GROUPS_FAST = 1;
+
+template <int NM, bool KERAS_ACT>
+static int launch_pool_corpus(PoolCorpus c, const K2In& in, cudaStream_t s) {
+    constexpr size_t smem = (size_t)NM * BANK_MODEL_SMEM;
+    if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(pool_corpus_kernel<NM, KERAS_ACT>, smem));
+    const int64_t total = c.n_groups * c.n_tiles;
+    if (total == 0) return PB_OK;
+    const int64_t gx = std::min<int64_t>(total, 1ll << 30), gy = (total + gx - 1) / gx;
+    pool_corpus_kernel<NM, KERAS_ACT><<<dim3((unsigned)gx, (unsigned)gy), MMA_THREADS, smem, s>>>(c, in);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+static int launch_pool_corpus_nm(int nm, bool keras, const PoolCorpus& c, const K2In& in, cudaStream_t s) {
+    switch (nm) {
+        case 1: return keras ? launch_pool_corpus<1, true>(c, in, s) : launch_pool_corpus<1, false>(c, in, s);
+        case 2: return keras ? launch_pool_corpus<2, true>(c, in, s) : launch_pool_corpus<2, false>(c, in, s);
+        case 4: return launch_pool_corpus<4, false>(c, in, s);
+        case 8: return launch_pool_corpus<8, false>(c, in, s);
+    }
+    return fail(PB_ERR_INVALID, "%d models per group", nm);
+}
+
+PB_API int pb_debug_corpus_pool_rows(pb_handle* h, int64_t rows) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (rows < 0) return fail(PB_ERR_INVALID, "rows = %lld is negative", (long long)rows);
+    h->corpus_pool_rows = rows;
+    return PB_OK;
+}
+
+PB_API int pb_debug_corpus_pool_scan(pb_handle* h, int32_t nm, int32_t groups_fast) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (nm != 0 && nm != 1 && nm != 2 && nm != 4 && nm != 8) return fail(PB_ERR_INVALID, "nm = %d: 0 (default), 1, 2, 4 or 8", nm);
+    if (groups_fast < -1 || groups_fast > 1) return fail(PB_ERR_INVALID, "groups_fast = %d: -1 (default), 0 or 1", groups_fast);
+    h->corpus_pool_nm = nm;
+    h->corpus_pool_order = groups_fast;
+    return PB_OK;
+}
+
+PB_API int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                                const int32_t* h_model_ids, int64_t k, int32_t divisor, int32_t schedule, int64_t chunk,
+                                double threshold, float* d_raw, double* d_conf, uint8_t* d_fired, int64_t* d_activations,
+                                int64_t* d_above, double* d_sum, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, schedule, chunk, d_raw, false, d_above, d_sum);
+    if (rc != PB_OK) return rc;
+    const bool reduce = d_fired || d_activations || d_above || d_sum;
+    if (!d_raw && !d_conf && !reduce) return fail(PB_ERR_INVALID, "every output is null");
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    if (k < 0) return fail(PB_ERR_INVALID, "k = %lld is negative", (long long)k);
+    if (k > 0 && !h_model_ids) return fail(PB_ERR_INVALID, "null h_model_ids");
+    for (int64_t i = 0; i < k; ++i) {
+        const int32_t m = h_model_ids[i];
+        if (m < 0 || m >= h->pool_models)
+            return fail(PB_ERR_INVALID, "model id %d (entry %lld) outside [0, max_models = %d)", m, (long long)i, h->pool_models);
+        if (h->pool_cd_of[m] == h->pool_cd.end())
+            return fail(PB_ERR_INVALID, "pool slot %d (entry %lld) holds no model: pb_pool_load it first", m, (long long)i);
+    }
+    if (n_rec == 0 || k == 0) return PB_OK;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const CorpusPlan p = corpus_plan(h, d_pcm, h_offsets, n_rec, schedule, chunk);
+    const long long W = p.W;
+    // rows per batch: all of them when the caller's d_raw holds raw (or no trigger pass needs it), else as many as the cap holds
+    const bool own_raw = !d_raw && reduce && W > 0;
+    int64_t rows = k;
+    if (own_raw) {
+        rows = std::max<int64_t>(1, CORPUS_POOL_RAW_CAP / (4 * W));
+        if (h->corpus_pool_rows > 0) rows = std::min<int64_t>(rows, h->corpus_pool_rows);
+        rows = std::min<int64_t>(rows, k);
+    }
+    // the scan's groups, batch after batch: within a batch, per activation class (Keras's defaults first where they are
+    // compiled in), NM requested rows each in request order, a partial last group padded with row -1
+    const int NM = h->corpus_pool_nm ? h->corpus_pool_nm : CORPUS_POOL_NM;
+    const bool split = pool_corpus_keras(NM);
+    const int64_t n_batches = (k + rows - 1) / rows;
+    std::vector<int2> groups;
+    std::vector<int64_t> g0((size_t)n_batches * 2 + 1);                // batch b, class ka: groups [g0[2b + ka], g0[2b + ka + 1])
+    for (int64_t b = 0; b < n_batches; ++b) {
+        const int64_t b0 = b * rows, b1 = std::min<int64_t>(k, b0 + rows);
+        for (int ka = 0; ka < 2; ++ka) {
+            g0[2 * b + ka] = (int64_t)groups.size() / NM;
+            int at = 0;
+            for (int64_t i = b0; i < b1; ++i) {
+                if ((split ? h->pool_keras[h_model_ids[i]] : 1) != ka) continue;
+                groups.push_back(make_int2(h_model_ids[i], (int)(i - b0)));
+                at = (at + 1) % NM;
+            }
+            for (const int2 first = at ? groups[groups.size() - at] : int2{}; at && at < NM; ++at)
+                groups.push_back(make_int2(first.x, -1));
+        }
+    }
+    g0[2 * n_batches] = (int64_t)groups.size() / NM;
+    CorpusPoolSizes ps;
+    ps.groups = groups.size();
+    ps.ids = (size_t)k;
+    ps.raw = own_raw ? (size_t)(rows * W) : 0;
+    rc = corpus_reserve(h, p, n_rec, ps, s);
+    if (rc != PB_OK) return rc;
+    const int order = h->corpus_pool_order >= 0 ? h->corpus_pool_order : CORPUS_POOL_GROUPS_FAST;
+    auto launch = [&]() -> int {
+        rc = corpus_k1(h, p, d_pcm, n_rec, divisor, schedule, chunk, s);
+        if (rc != PB_OK) return rc;
+        if (W == 0 && !reduce) return PB_OK;
+        CK(cudaMemcpyAsync(h->d_cp_groups.get(), groups.data(), groups.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_cp_ids.get(), h_model_ids, (size_t)k * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        ProfScope ps(h, 1, s);
+        const K2In in = corpus_k2in(h);
+        for (int64_t b = 0; b < n_batches; ++b) {
+            const int64_t b0 = b * rows, nb = std::min<int64_t>(k, b0 + rows) - b0;
+            float* raw = own_raw ? h->d_cp_raw.get() : d_raw ? d_raw + b0 * W : nullptr;
+            if (W > 0) {
+                PoolCorpus c{};
+                c.slots = h->d_pool_slots.get(); c.n_tiles = (W + 63) / 64; c.raw = raw;
+                c.conf = d_conf ? d_conf + b0 * W : nullptr; c.W = W; c.groups_fast = order;
+                for (int ka = 0; ka < 2; ++ka) {
+                    c.groups = h->d_cp_groups.get() + g0[2 * b + ka] * NM;
+                    c.n_groups = g0[2 * b + ka + 1] - g0[2 * b + ka];
+                    rc = launch_pool_corpus_nm(NM, split && ka == 1, c, in, s);
+                    if (rc != PB_OK) return rc;
                 }
+            }
+            if (!reduce) continue;
+            // rows b0 .. b0 + nb - 1, at most 65 535 per launch (gridDim.y)
+            for (int64_t y0 = 0; y0 < nb; y0 += 65535) {
+                const int64_t r0 = b0 + y0, ny = std::min<int64_t>(65535, nb - y0);
+                CorpusTrig t = corpus_trig(h, n_rec, W, schedule, chunk, threshold);
+                t.raw = raw ? raw + y0 * W : nullptr;
+                t.conf = d_conf ? d_conf + r0 * W : nullptr;
+                t.fired = d_fired ? d_fired + r0 * W : nullptr;
+                t.activations = d_activations ? d_activations + r0 * n_rec : nullptr;
+                t.above = d_above ? d_above + r0 * n_rec : nullptr;
+                t.sum = d_sum ? d_sum + r0 * n_rec : nullptr;
+                CorpusPoolDP dp{h->d_pool_slots.get(), h->d_cp_ids.get() + r0, trigger_reset(2 * chunk)};
                 const unsigned per = CORPUS_TRIG_THREADS / 32;
-                corpus_trigger_kernel<<<dim3((unsigned)((n_rec + per - 1) / per), (unsigned)M), CORPUS_TRIG_THREADS, 0, s>>>(t);
+                corpus_trigger_kernel<<<dim3((unsigned)((n_rec + per - 1) / per), (unsigned)ny), CORPUS_TRIG_THREADS, 0, s>>>(t, dp);
                 CK(cudaGetLastError());
             }
         }
         return PB_OK;
     };
-    rc = launch();
-    const cudaError_t er = cudaEventRecord(h->corpus_ev, s);
-    if (rc != PB_OK) return rc;
-    if (er != cudaSuccess) return fail(PB_ERR_CUDA, "cudaEventRecord failed: %s", cudaGetErrorString(er));
-    return PB_OK;
+    return corpus_done(h, s, launch());
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {

@@ -224,19 +224,27 @@ struct CorpusTrig {
     int schedule;
     float hot_f, above_f;            // simulate: (float)(1 - threshold), (float)threshold
     int sim_reset;                   // simulate: -(8 * 2048) // chunk
-    DecodeParams dp[PB_MAX_MODELS];  // listener: the model's decoder and detector (hot_threshold, trigger_level, trigger_reset)
+};
+
+// Listener: row m's decoder and detector (hot_threshold, trigger_level, trigger_reset), here a bank model's.  The model pool's
+// rows read theirs from their slot records (corpus_pool.cuh, CorpusPoolDP).
+struct CorpusBankDP {
+    DecodeParams dp[PB_MAX_MODELS];
+    __device__ __forceinline__ const DecodeParams& operator()(int m) const { return dp[m]; }
 };
 
 constexpr int CORPUS_TRIG_THREADS = 256;
 
-// A warp per (model = blockIdx.y, recording).  Lanes load 32 consecutive windows at once (the next 32 are in flight while
+// A warp per (row = blockIdx.y, recording).  Lanes load 32 consecutive windows at once (the next 32 are in flight while
 // these are used) and decide hot in parallel; the detector's serial recurrence then runs over the warp's ballot of hot
 // flags, identically in every lane, and lane j keeps fired of its window.
-__global__ void __launch_bounds__(CORPUS_TRIG_THREADS) corpus_trigger_kernel(const __grid_constant__ CorpusTrig P) {
+template <class DP>
+__global__ void __launch_bounds__(CORPUS_TRIG_THREADS) corpus_trigger_kernel(const __grid_constant__ CorpusTrig P,
+                                                                             const __grid_constant__ DP dps) {
     const int m = blockIdx.y, lane = threadIdx.x & 31;
     const long long r = (long long)blockIdx.x * (CORPUS_TRIG_THREADS / 32) + (threadIdx.x >> 5);
     if (r >= P.n_rec) return;                                     // whole warp
-    const DecodeParams& d = P.dp[m];
+    const DecodeParams& d = dps(m);
     const bool sim = P.schedule == CORPUS_SIMULATE;
     const int level = sim ? 0 : d.trigger_level, reset = sim ? P.sim_reset : d.trigger_reset;
     const long long w0 = __ldg(P.win0 + r), w1 = __ldg(P.win0 + r + 1), off = (long long)m * P.W;

@@ -11,7 +11,9 @@ the network run in the CUDA library.
 
 Recorded corpora (many recordings per device call, no window materialised: pb_score_corpus):
   score_corpus      every bank model over a list of recordings, listener or simulate schedule
+  score_corpus_pool chosen pool models over a list of recordings (pb_score_corpus_pool)
   Metric, simulate  ~ precise/scripts/simulate.py:45-80, :106-129 (SimulateScript.run's per-file metrics and total)
+  simulate_pool     simulate for many pool models in one device call per batch of recordings
   false_activations ~ precise/scripts/train_incremental.py:113-137 (train_on_audio's selection of clips, fixed weights)
 """
 from dataclasses import dataclass
@@ -134,12 +136,10 @@ def _check_recording(core: PreciseB200, r):
     return r if isinstance(r, np.ndarray) else r.contiguous()
 
 
-def score_corpus(core: PreciseB200, recordings, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
-    """Every bank model of ``core`` over ``recordings`` (a list of 1-D int16 numpy arrays or CUDA tensors of any lengths).
-    Returns dict(raw f32 [M, W], conf f64 [M, W], fired u8 [M, W], window_offsets (host int64 [n + 1]: recording r's windows
-    are columns window_offsets[r] .. window_offsets[r + 1] - 1), activations i64 [M, n], and for the simulate schedule
-    above i64 [M, n] and sum f64 [M, n], else None).  Schedules: include/precise_b200.h, pb_score_corpus.  divisor: 32768 for
-    audio as the stream path reads it (buffer_to_audio), 32767 for audio as load_audio reads wav files."""
+def _score_groups(core: PreciseB200, recordings, schedule, chunk, call):
+    """Packs ``recordings`` into library calls of at most CORPUS_CALL_SAMPLES samples, runs call(pcm, offsets) on each and
+    joins the results along the recording axis (window columns for raw / conf / fired, recording columns for the rest).
+    Output names score_corpus returns; None outputs stay None."""
     torch = core.torch
     recs = [_check_recording(core, r) for r in recordings]
     groups, cur, size = [], [], 0
@@ -154,7 +154,7 @@ def score_corpus(core: PreciseB200, recordings, schedule='listener', chunk=1024,
     parts = []
     for g in groups:
         pcm, offsets, entry = _pack(core, g)
-        res = core.score_corpus(pcm, offsets, schedule, chunk, threshold, divisor)
+        res = call(pcm, offsets)
         if len(entry) < len(offsets) - 1:                     # drop the padding entries
             counts = np.array([core.corpus_windows(int(L), schedule, chunk) for L in np.diff(offsets)], np.int64)
             w0 = np.concatenate([[0], np.cumsum(counts)])
@@ -168,6 +168,26 @@ def score_corpus(core: PreciseB200, recordings, schedule='listener', chunk=1024,
     counts = [core.corpus_windows(int(r.shape[0]), schedule, chunk) for r in recs]
     out['window_offsets'] = np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)
     return out
+
+
+def score_corpus(core: PreciseB200, recordings, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
+    """Every bank model of ``core`` over ``recordings`` (a list of 1-D int16 numpy arrays or CUDA tensors of any lengths).
+    Returns dict(raw f32 [M, W], conf f64 [M, W], fired u8 [M, W], window_offsets (host int64 [n + 1]: recording r's windows
+    are columns window_offsets[r] .. window_offsets[r + 1] - 1), activations i64 [M, n], and for the simulate schedule
+    above i64 [M, n] and sum f64 [M, n], else None).  Schedules: include/precise_b200.h, pb_score_corpus.  divisor: 32768 for
+    audio as the stream path reads it (buffer_to_audio), 32767 for audio as load_audio reads wav files."""
+    return _score_groups(core, recordings, schedule, chunk,
+                         lambda pcm, offsets: core.score_corpus(pcm, offsets, schedule, chunk, threshold, divisor))
+
+
+def score_corpus_pool(core: PreciseB200, recordings, model_ids, schedule='listener', chunk=1024, threshold=0.5, divisor=32768,
+                      per_window=True):
+    """score_corpus for pool models ``model_ids`` (int32 [k], repeats allowed): the same dict with k rows in the order of
+    model_ids.  per_window=False: raw, conf and fired are None, only the reductions are computed (pb_score_corpus_pool)."""
+    ids = np.ascontiguousarray(model_ids, dtype=np.int32)
+    return _score_groups(core, recordings, schedule, chunk,
+                         lambda pcm, offsets: core.score_corpus_pool(pcm, offsets, ids, schedule, chunk, threshold, divisor,
+                                                                     per_window))
 
 
 @dataclass
@@ -209,9 +229,12 @@ def simulate(core: PreciseB200, recordings, chunk_size=4096, threshold=0.5):
     A recording too short for one window (fewer than n_features + 1 frames) counts its seconds with no windows, where the
     reference's Runner.predict fails on an empty input."""
     res = score_corpus(core, recordings, 'simulate', chunk_size, threshold, divisor=32767)
-    above = res['above'][0].cpu().numpy()
-    acts = res['activations'][0].cpu().numpy()
-    sums = res['sum'][0].cpu().numpy()
+    return _metrics(core, recordings, chunk_size, res['above'][0].cpu().numpy(), res['activations'][0].cpu().numpy(),
+                    res['sum'][0].cpu().numpy())
+
+
+def _metrics(core: PreciseB200, recordings, chunk_size, above, acts, sums):
+    """Per-recording Metrics of one model (None for an empty recording) and their total."""
     sr = core.params.sample_rate
     total = Metric(chunk_size, sample_rate=sr)
     metrics = []
@@ -224,6 +247,21 @@ def simulate(core: PreciseB200, recordings, chunk_size=4096, threshold=0.5):
         total.add(m)
         metrics.append(m)
     return metrics, total
+
+
+def simulate_pool(core: PreciseB200, recordings, model_ids, chunk_size=4096, threshold=0.5):
+    """simulate for many pool models on one K1: returns (metrics, totals), metrics[i][r] model_ids[i]'s Metric for recording
+    r (None for an empty recording) and totals[i] its total.  Only the per-recording reductions leave the device."""
+    res = score_corpus_pool(core, recordings, model_ids, 'simulate', chunk_size, threshold, divisor=32767, per_window=False)
+    above = res['above'].cpu().numpy()
+    acts = res['activations'].cpu().numpy()
+    sums = res['sum'].cpu().numpy()
+    metrics, totals = [], []
+    for i in range(above.shape[0]):
+        m, t = _metrics(core, recordings, chunk_size, above[i], acts[i], sums[i])
+        metrics.append(m)
+        totals.append(t)
+    return metrics, totals
 
 
 def false_activations(core: PreciseB200, recordings, chunk_size=2048, threshold=0.5):

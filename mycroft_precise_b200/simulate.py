@@ -1,7 +1,7 @@
 """``precise-simulate`` on the GPU (reference: precise/scripts/simulate.py): false-activation metrics of a model over a
 folder of long recordings.
 
-    python -m mycroft_precise_b200.simulate MODEL FOLDER [-c CHUNK_SIZE] [-t THRESHOLD]
+    python -m mycroft_precise_b200.simulate MODEL [MODEL ...] FOLDER [-c CHUNK_SIZE] [-t THRESHOLD]
 
 Every ``*.wav`` of FOLDER (glob order, as the reference) is read as load_audio reads it (precise/util.py:55-72): 16-bit
 PCM at the model's sample rate, samples / 32767; a file the wave module cannot parse counts as empty and is skipped; any
@@ -9,6 +9,11 @@ other sample width or rate raises.  All files are scored in one batch on the dev
 metric block and the Total block are printed in the reference's format.  The reference's progress lines (MFCCs... /
 Splitting... / Predicting...) are not printed.  A file too short for one window counts its hours with no windows; the
 reference fails on it.
+
+With two or more models, every model must share the first one's front end and be of the fused family (hidden <= 24,
+feature size <= 16, no deltas).  They are loaded into a model pool and scored together over one MFCC pass
+(offline.simulate_pool); for each model, in the order given, a ``=== <model file> ===`` heading is printed, then that
+model's per-file blocks and its Total block.
 """
 import argparse
 import wave
@@ -42,7 +47,7 @@ def read_wav(path: str, sample_rate: int = 16000) -> np.ndarray:
 def main(argv=None):
     ap = argparse.ArgumentParser(prog='precise-simulate', description=__doc__,
                                  formatter_class=argparse.RawDescriptionHelpFormatter)
-    ap.add_argument('model', help='weights file (.npz, .net or .pb) with its .params next to it')
+    ap.add_argument('model', nargs='+', help='weights file(s) (.npz, .net or .pb) with their .params next to them')
     ap.add_argument('folder', help='folder with a set of long wav files to test against')
     ap.add_argument('-c', '--chunk_size', type=int, default=4096, help='number of samples between tests')
     ap.add_argument('-t', '--threshold', type=float, default=0.5, help='network output required to be considered an activation')
@@ -50,17 +55,51 @@ def main(argv=None):
     args = ap.parse_args(argv)
 
     from .core import PreciseB200
-    from .offline import simulate
     from .params import ListenerParams
     from .runner import _resolve_model
-    model, pr = _resolve_model(args.model)
-    pr = pr or ListenerParams()
+    models = [_resolve_model(m) for m in args.model]
+    models = [(model, pr or ListenerParams()) for model, pr in models]
+    if len(models) > 1:
+        check_pool_models(args.model, models)
+    model, pr = models[0]
     core = PreciseB200(pr, hidden=model.hidden, device=args.device, activation=model.activation,
                        recurrent_activation=model.recurrent_activation)
-    core.load_weights(model.kernel, model.recurrent, model.bias, model.dense_w, model.dense_b)
     files = glob(join(args.folder, '*.wav'))
     audio = [read_wav(f, pr.sample_rate) for f in files]
-    metrics, total = simulate(core, audio, args.chunk_size, args.threshold)
+    if len(models) == 1:
+        from .offline import simulate
+        core.load_weights(model.kernel, model.recurrent, model.bias, model.dense_w, model.dense_b)
+        metrics, total = simulate(core, audio, args.chunk_size, args.threshold)
+        print_metrics(files, metrics, total)
+    else:
+        from .offline import simulate_pool
+        core.set_pool(len(models))
+        for i, (m, p) in enumerate(models):
+            core.pool_load(i, m, p)
+        metrics, totals = simulate_pool(core, audio, np.arange(len(models), dtype=np.int32), args.chunk_size, args.threshold)
+        for name, ms, total in zip(args.model, metrics, totals):
+            print()
+            print('=== %s ===' % name)
+            print_metrics(files, ms, total)
+    core.close()
+
+
+def check_pool_models(names, models):
+    """Two or more models are scored as one pool: each must share the first one's front end and be of the fused family."""
+    from .core import FRONT_END_FIELDS
+    pr0 = models[0][1]
+    for name, (model, pr) in zip(names, models):
+        diff = [f for f in FRONT_END_FIELDS if getattr(pr, f) != getattr(pr0, f)]
+        if diff:
+            raise ValueError('%s: front end differs from %s in %s; models scored together share one MFCC front end'
+                             % (name, names[0], ', '.join(diff)))
+        if model.hidden > 24 or model.feature_size > 16 or pr.use_delta:
+            raise ValueError('%s: only networks of the fused family (hidden <= 24, feature size <= 16, no deltas) can be '
+                             'scored together; this one has hidden = %d, feature size = %d%s'
+                             % (name, model.hidden, model.feature_size, ', deltas' if pr.use_delta else ''))
+
+
+def print_metrics(files, metrics, total):
     for f, m in zip(files, metrics):
         if m is None:
             continue
@@ -69,7 +108,6 @@ def main(argv=None):
     print()
     print()
     print(total.info_string('Total'))
-    core.close()
 
 
 if __name__ == '__main__':
