@@ -363,7 +363,8 @@ int pb_read_history(pb_handle* h, const int32_t* d_stream_ids, int64_t n, int64_
  *     are bit-identical share one copy), 16 B per stream.
  *   - The bank, its masks and trigger settings are independent of the pool; pb_update_models does not score pool models and
  *     pb_update_pool scores no bank model.  pb_update_all scores both on one K1.  pb_score_corpus scores the bank only;
- *     pb_score_corpus_pool scores chosen pool models over a recorded corpus.  Not covered: pb_update_host, networks outside
+ *     pb_score_corpus_pool scores chosen pool models over a recorded corpus, pb_score_corpus_pairs chosen (pool model,
+ *     recording) pairs.  Not covered: pb_update_host, networks outside
  *     the fused family.
  *   - A handle that never calls pb_set_pool runs exactly as before.
  *
@@ -512,6 +513,39 @@ int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_t* h_of
                          int32_t divisor, int32_t schedule, int64_t chunk, double threshold,
                          float* d_raw, double* d_conf, uint8_t* d_fired,
                          int64_t* d_activations, int64_t* d_above, double* d_sum, void* stream);
+/* Pool models over chosen recordings: each custom wake word over its owner's own audio (recorded samples, clips saved behind
+ * past activations), and false-activation mining for pool models, without the cross product.  Pair p is pool slot
+ * h_pair_models[p] over recording h_pair_recs[p] (both HOST, n_pairs entries; pairs may repeat and come in any order).
+ * Recordings, divisor, schedules, chunk and threshold mean exactly what they mean for pb_score_corpus_pool, each model's own
+ * decoder, sensitivity and trigger level included.  K1 runs over every recording, also one that no pair names.
+ *   - Outputs are pair-major in request order.  d_raw, d_conf, d_fired [Wp]: pair p's windows are entries P[p] .. P[p+1] - 1,
+ *     P the exclusive prefix over pairs of pb_corpus_windows of the pair's recording.  d_activations, d_above, d_sum
+ *     [n_pairs].  Every output is optional (d_n_hits counts as one), but not all of them at once.  Pair p's outputs are
+ *     bit-identical to the slice of recording h_pair_recs[p] in the row pb_score_corpus_pool writes for h_pair_models[p].
+ *   - Hits (listener schedule only): with d_n_hits, *d_n_hits receives the number of pair-windows q in [0, Wp) whose decoded
+ *     conf > hit_threshold (train_incremental.py:125's selection), and the first min(total, hit_capacity) of them go to
+ *     d_hits [hit_capacity] (int64), in no particular order; the set is exact.  Hits need neither d_conf nor d_raw.
+ *   - Pairs are scanned in batches of consecutive pairs of at most 2^25 pair-windows (a larger pair alone), each followed by
+ *     its trigger and hit passes.  Scan tiles hold up to 64 consecutive pair-windows of one model, across the pairs of a run
+ *     of consecutive pairs on that model: list a model's pairs together to fill them.
+ *   - Memory: the workspace of pb_score_corpus, shared with it, plus 8 B per pair-window of the largest batch (its window
+ *     table, at most 256 MB, or one pair's), 4 B more for raw when d_raw is NULL and a trigger or hit pass is wanted, and
+ *     about 32 B per pair.
+ *   - Reads and writes no stream state, pool assignments or pool detectors; needs no slot-0 weights.  Asynchronous on
+ *     `stream`, ordered against other corpus calls as pb_score_corpus; pb_pool_load and pb_set_pool wait for queued calls.
+ *     Profile slot 0 counts K1, slot 1 the scans, trigger and hit passes.  Every argument is checked before anything is
+ *     enqueued, so a refused call changes no state.
+ * PB_ERR_INVALID: pb_score_corpus_pool's argument errors, n_pairs outside [0, 2^31), a null pair array with n_pairs > 0, a
+ * model id outside [0, max_models) or a slot that holds no model, a recording id outside [0, n_rec), hit_capacity < 0, a null
+ * d_hits with hit_capacity > 0, d_hits without d_n_hits, hits with the simulate schedule.  PB_ERR_STATE: no pool.
+ * PB_ERR_CUDA: the workspace cannot be allocated (the handle is then unchanged). */
+int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                          const int32_t* h_pair_models, const int32_t* h_pair_recs, int64_t n_pairs,
+                          int32_t divisor, int32_t schedule, int64_t chunk, double threshold,
+                          float* d_raw, double* d_conf, uint8_t* d_fired,
+                          int64_t* d_activations, int64_t* d_above, double* d_sum,
+                          double hit_threshold, int64_t* d_hits, int64_t hit_capacity,
+                          unsigned long long* d_n_hits, void* stream);
 
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
@@ -559,6 +593,9 @@ int pb_debug_corpus_pool_rows(pb_handle* h, int64_t rows);
  * (1: consecutive CTAs take every model group of one window tile; 0: every tile of one group; -1 = the default).  Every
  * choice scores bit-identical outputs.  PB_ERR_INVALID: null handle, a value out of range. */
 int pb_debug_corpus_pool_scan(pb_handle* h, int32_t nm, int32_t groups_fast);
+/* Test hook for pb_score_corpus_pairs: at most `windows` pair-windows per batch (a larger pair still forms one batch), so that
+ * small corpora reach the multi-batch path; 0 restores the default (2^25).  PB_ERR_INVALID: null handle, windows < 0. */
+int pb_debug_corpus_pairs_batch(pb_handle* h, int64_t windows);
 /* CPU model of a tensor-core formulation of the DFT (csrc/mfcc_tc.cuh: radix-16 butterflies, second stage as an fp16 hi / lo
  * matrix product) for one frame of 512 int16 samples -> |X[k]|^2, k = 0..256.  No device needed.  Test hook. */
 int pb_debug_tc_dft_power(const int16_t* x512, double* power257);

@@ -85,6 +85,8 @@ SYMBOLS = {
     'pb_score_corpus': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     'pb_score_corpus_pool': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP, _VP,
                                        _VP, _VP]),
+    'pb_score_corpus_pairs': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP,
+                                        _VP, _VP, C.c_double, _VP, _I64, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -99,6 +101,7 @@ SYMBOLS = {
     'pb_debug_pool_tiles': (C.c_int, [_VP, C.c_int]),
     'pb_debug_corpus_pool_rows': (C.c_int, [_VP, _I64]),
     'pb_debug_corpus_pool_scan': (C.c_int, [_VP, _I32, _I32]),
+    'pb_debug_corpus_pairs_batch': (C.c_int, [_VP, _I64]),
     'pb_debug_tc_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_mma_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_tc_mfcc_frame': (C.c_int, [_VP, _VP, _VP]),
@@ -886,6 +889,60 @@ class PreciseB200:
                                             _ptr(out['fired']), _ptr(out['activations']), _ptr(out['above']),
                                             _ptr(out['sum']), self._stream()))
         return out
+
+    def score_corpus_pairs(self, pcm, offsets, model_ids, rec_ids, schedule='listener', chunk=1024, threshold=0.5,
+                           divisor=32768, per_window=True, hit_threshold=None, hit_capacity=None):
+        """Pool model model_ids[p] over recording rec_ids[p] for each pair p (host int32 arrays [n_pairs], repeats and any
+        order allowed), recordings as score_corpus takes them.  Returns score_corpus_pool's keys with 1-D pair-major outputs:
+        raw, conf, fired [Wp] (pair p's windows at pair_offsets[p] .. pair_offsets[p + 1] - 1; None with per_window=False),
+        activations [n_pairs], above and sum [n_pairs] for the simulate schedule, and pair_offsets (host int64 [n_pairs + 1]).
+        With a hit_threshold (listener schedule), also hits: the sorted int64 pair-window indices whose conf is above it,
+        computed on the device; when more than hit_capacity are found the call runs once more with room for all of them, and
+        this (and only this) waits for the device.  pb_score_corpus_pairs in include/precise_b200.h."""
+        torch = self.torch
+        sched, offsets, n_rec, _ = self._corpus_args(pcm, offsets, schedule, chunk)
+        model_ids, rec_ids = np.asarray(model_ids), np.asarray(rec_ids)
+        n = model_ids.shape[0] if model_ids.ndim == 1 else -1
+        _check_np('model_ids', model_ids, np.int32, (n,), optional=False)
+        _check_np('rec_ids', rec_ids, np.int32, (n,), optional=False)
+        if n and (rec_ids.min() < 0 or rec_ids.max() >= n_rec):
+            raise ValueError('recording ids must lie in [0, %d)' % n_rec)
+        counts = np.asarray([self.corpus_windows(int(L), schedule, chunk) for L in np.diff(offsets)], np.int64)
+        pw = np.concatenate([[0], np.cumsum(counts[rec_ids], dtype=np.int64)]).astype(np.int64)
+        Wp = int(pw[-1])
+        f = lambda shape, dt: torch.empty(shape, dtype=dt, device=self.device)
+        out = dict(raw=None, conf=None, fired=None, activations=f((n,), torch.int64), above=None, sum=None, pair_offsets=pw)
+        if per_window:
+            out.update(raw=f((Wp,), torch.float32), conf=f((Wp,), torch.float64), fired=f((Wp,), torch.uint8))
+        if sched == 1:
+            out['above'] = f((n,), torch.int64)
+            out['sum'] = f((n,), torch.float64)
+        hits = hit_threshold is not None
+        n_hits = f((1,), torch.int64) if hits else None
+        cap = self._int('hit_capacity', 1 << 16 if hit_capacity is None else hit_capacity) if hits else 0
+
+        def run(cap):
+            d_hits = f((max(cap, 1),), torch.int64) if hits else None
+            check(self.lib.pb_score_corpus_pairs(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, _np_ptr(model_ids),
+                                                 _np_ptr(rec_ids), n, int(divisor), sched, int(chunk), float(threshold),
+                                                 _ptr(out['raw']), _ptr(out['conf']), _ptr(out['fired']),
+                                                 _ptr(out['activations']), _ptr(out['above']), _ptr(out['sum']),
+                                                 float(hit_threshold) if hits else 0.0, _ptr(d_hits) if cap else None, cap,
+                                                 _ptr(n_hits), self._stream()))
+            return d_hits
+
+        d_hits = run(cap)
+        if hits:
+            total = int(n_hits.item())
+            if total > cap:
+                cap = total
+                d_hits = run(cap)
+            out['hits'] = torch.sort(d_hits[:total])[0]
+        return out
+
+    def corpus_pairs_batch(self, windows):
+        """Test hook: score_corpus_pairs scans at most ``windows`` pair-windows per batch (0 = the default)."""
+        check(self.lib.pb_debug_corpus_pairs_batch(self._h, int(windows)))
 
     def corpus_pool_rows(self, rows):
         """Test hook: score_corpus_pool with per_window=False scans at most ``rows`` models per batch (0 = the default)."""

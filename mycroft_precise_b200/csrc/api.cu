@@ -35,6 +35,7 @@
 #include "history.cuh"
 #include "corpus.cuh"
 #include "corpus_pool.cuh"
+#include "corpus_pairs.cuh"
 #include "pool.cuh"
 
 using namespace pb;
@@ -211,6 +212,11 @@ struct pb_handle {
     int64_t corpus_pool_rows = 0;    // pb_debug_corpus_pool_rows: at most this many rows per batch (0 = the cap's)
     int corpus_pool_nm = 0;          // pb_debug_corpus_pool_scan: models per group (0 = CORPUS_POOL_NM)
     int corpus_pool_order = -1;      // ... grid order (-1 = CORPUS_POOL_GROUPS_FAST)
+    DevArray<int2> d_pp_pairs;       // pb_score_corpus_pairs: [n_pairs] (pool slot, recording); raw of a batch goes to d_cp_raw
+    DevArray<long long> d_pp_pw0;    // ... each batch's pair-window prefix, batch b's at [p0 + b, p1 + b]
+    DevArray<long long> d_pp_starts; // ... [batch pair-windows] the batch's window table
+    DevArray<PairTile> d_pp_tiles;   // ... the batch's scan tiles, one activation class after the other
+    int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
     int32_t pool_models = 0;         // max_models
@@ -1663,9 +1669,10 @@ static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const in
     return p;
 }
 
-// Sizes of pb_score_corpus_pool's own workspace arrays (0 for pb_score_corpus).
+// Sizes of pb_score_corpus_pool's and pb_score_corpus_pairs's own workspace arrays (0 for pb_score_corpus).
 struct CorpusPoolSizes {
     size_t groups = 0, ids = 0, raw = 0;
+    size_t pairs = 0, pw0 = 0, starts = 0, tiles = 0;
 };
 
 // Grows the workspace for plan p, all at once, so that a failed allocation leaves the handle as it was; then orders s after
@@ -1674,6 +1681,7 @@ static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, cons
     if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
     DevArray<float> f_rows, f_raw; DevArray<CorpusPair> f_pairs; DevArray<long long> f_starts, f_win0, f_frow; DevArray<CorpusRec> f_recs;
     DevArray<int2> f_groups; DevArray<int> f_ids;
+    DevArray<int2> f_ppairs; DevArray<long long> f_pw0, f_pstarts; DevArray<PairTile> f_tiles;
     cudaError_t e = corpus_grow(h->d_cw_rows, (size_t)p.rows * h->row_stride, f_rows);
     if (e == cudaSuccess) e = corpus_grow(h->d_cw_pairs, (size_t)p.n_pairs, f_pairs);
     if (e == cudaSuccess) e = corpus_grow(h->d_cw_starts, (size_t)p.W, f_starts);
@@ -1683,12 +1691,17 @@ static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, cons
     if (e == cudaSuccess) e = corpus_grow(h->d_cp_groups, ps.groups, f_groups);
     if (e == cudaSuccess) e = corpus_grow(h->d_cp_ids, ps.ids, f_ids);
     if (e == cudaSuccess && h->d_cp_raw.size() < ps.raw) e = f_raw.alloc(ps.raw);     // capped: no headroom
+    if (e == cudaSuccess) e = corpus_grow(h->d_pp_pairs, ps.pairs, f_ppairs);
+    if (e == cudaSuccess) e = corpus_grow(h->d_pp_pw0, ps.pw0, f_pw0);
+    if (e == cudaSuccess && h->d_pp_starts.size() < ps.starts) e = f_pstarts.alloc(ps.starts);   // capped: no headroom
+    if (e == cudaSuccess) e = corpus_grow(h->d_pp_tiles, ps.tiles, f_tiles);
     if (e != cudaSuccess) {
         cudaGetLastError();
         return fail(PB_ERR_CUDA, "corpus workspace allocation failed (%lld frame rows, %lld windows): %s", p.rows, p.W, cudaGetErrorString(e));
     }
     const bool grows = f_rows.get() || f_pairs.get() || f_starts.get() || f_win0.get() || f_frow.get() || f_recs.get() ||
-                       f_groups.get() || f_ids.get() || f_raw.get();
+                       f_groups.get() || f_ids.get() || f_raw.get() || f_ppairs.get() || f_pw0.get() || f_pstarts.get() ||
+                       f_tiles.get();
     if (grows) CK(cudaEventSynchronize(h->corpus_ev));            // the previous call may still read what is replaced
     if (f_rows.get()) h->d_cw_rows = std::move(f_rows);
     if (f_pairs.get()) h->d_cw_pairs = std::move(f_pairs);
@@ -1699,6 +1712,10 @@ static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, cons
     if (f_groups.get()) h->d_cp_groups = std::move(f_groups);
     if (f_ids.get()) h->d_cp_ids = std::move(f_ids);
     if (f_raw.get()) h->d_cp_raw = std::move(f_raw);
+    if (f_ppairs.get()) h->d_pp_pairs = std::move(f_ppairs);
+    if (f_pw0.get()) h->d_pp_pw0 = std::move(f_pw0);
+    if (f_pstarts.get()) h->d_pp_starts = std::move(f_pstarts);
+    if (f_tiles.get()) h->d_pp_tiles = std::move(f_tiles);
     CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));                      // a corpus call on another stream may still use it
     return PB_OK;
 }
@@ -1973,6 +1990,179 @@ PB_API int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_
                 CorpusPoolDP dp{h->d_pool_slots.get(), h->d_cp_ids.get() + r0, trigger_reset(2 * chunk)};
                 const unsigned per = CORPUS_TRIG_THREADS / 32;
                 corpus_trigger_kernel<<<dim3((unsigned)((n_rec + per - 1) / per), (unsigned)ny), CORPUS_TRIG_THREADS, 0, s>>>(t, dp);
+                CK(cudaGetLastError());
+            }
+        }
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+// ------------------------------------------------------------------------------------------------
+// pool models over chosen recordings (corpus_pairs.cuh)
+
+// Pair-windows per batch: the batch's window table takes 8 B per pair-window (256 MB), its raw without d_raw 4 B.
+constexpr int64_t CORPUS_PAIRS_BATCH = 1ll << 25;
+
+template <bool KERAS_ACT>
+static int launch_pairs_corpus(const PairsCorpus& c, const K2In& in, cudaStream_t s) {
+    if (c.n_tiles == 0) return PB_OK;
+    const int64_t gx = std::min<int64_t>(c.n_tiles, 1ll << 30), gy = (c.n_tiles + gx - 1) / gx;
+    pairs_corpus_kernel<KERAS_ACT><<<dim3((unsigned)gx, (unsigned)gy), MMA_THREADS, BANK_MODEL_SMEM, s>>>(c, in);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
+PB_API int pb_debug_corpus_pairs_batch(pb_handle* h, int64_t windows) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (windows < 0) return fail(PB_ERR_INVALID, "windows = %lld is negative", (long long)windows);
+    h->corpus_pairs_batch = windows;
+    return PB_OK;
+}
+
+PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                                 const int32_t* h_pair_models, const int32_t* h_pair_recs, int64_t n_pairs,
+                                 int32_t divisor, int32_t schedule, int64_t chunk, double threshold,
+                                 float* d_raw, double* d_conf, uint8_t* d_fired,
+                                 int64_t* d_activations, int64_t* d_above, double* d_sum,
+                                 double hit_threshold, int64_t* d_hits, int64_t hit_capacity,
+                                 unsigned long long* d_n_hits, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, schedule, chunk, d_raw, false, d_above, d_sum);
+    if (rc != PB_OK) return rc;
+    const bool reduce = d_fired || d_activations || d_above || d_sum, hits = d_n_hits != nullptr;
+    if (!d_raw && !d_conf && !reduce && !hits) return fail(PB_ERR_INVALID, "every output is null");
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    if (n_pairs < 0 || n_pairs > INT32_MAX) return fail(PB_ERR_INVALID, "n_pairs = %lld outside [0, 2^31)", (long long)n_pairs);
+    if (n_pairs > 0 && (!h_pair_models || !h_pair_recs)) return fail(PB_ERR_INVALID, "null h_pair_models or h_pair_recs");
+    for (int64_t i = 0; i < n_pairs; ++i) {
+        const int32_t m = h_pair_models[i], r = h_pair_recs[i];
+        if (m < 0 || m >= h->pool_models)
+            return fail(PB_ERR_INVALID, "model id %d (pair %lld) outside [0, max_models = %d)", m, (long long)i, h->pool_models);
+        if (h->pool_cd_of[m] == h->pool_cd.end())
+            return fail(PB_ERR_INVALID, "pool slot %d (pair %lld) holds no model: pb_pool_load it first", m, (long long)i);
+        if (r < 0 || r >= n_rec)
+            return fail(PB_ERR_INVALID, "recording id %d (pair %lld) outside [0, n_rec = %lld)", r, (long long)i, (long long)n_rec);
+    }
+    if (hit_capacity < 0) return fail(PB_ERR_INVALID, "hit_capacity = %lld is negative", (long long)hit_capacity);
+    if (hit_capacity > 0 && !d_hits) return fail(PB_ERR_INVALID, "null d_hits with hit_capacity = %lld", (long long)hit_capacity);
+    if (d_hits && !hits) return fail(PB_ERR_INVALID, "d_hits without d_n_hits");
+    if (hits && schedule == PB_CORPUS_SIMULATE) return fail(PB_ERR_INVALID, "hits belong to the listener schedule");
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n_pairs == 0) {
+        if (hits) CK(cudaMemsetAsync(d_n_hits, 0, sizeof(unsigned long long), s));
+        return PB_OK;
+    }
+    const CorpusPlan plan = corpus_plan(h, d_pcm, h_offsets, n_rec, schedule, chunk);
+    // pair p's windows are P[p] .. P[p + 1] - 1 of every per-window output
+    std::vector<long long> P((size_t)n_pairs + 1);
+    std::vector<int2> pairs((size_t)n_pairs);
+    P[0] = 0;
+    for (int64_t i = 0; i < n_pairs; ++i) {
+        const int r = h_pair_recs[i];
+        P[i + 1] = P[i] + (plan.win0[r + 1] - plan.win0[r]);
+        pairs[i] = make_int2(h_pair_models[i], r);
+    }
+    // batches of consecutive pairs, bp[b] .. bp[b + 1] - 1, of at most `cap` pair-windows (or one larger pair), each with its
+    // own prefix in pw0 at [bp[b] + b, bp[b + 1] + b]; and the scan tiles of the largest one
+    const int64_t cap = h->corpus_pairs_batch > 0 ? h->corpus_pairs_batch : CORPUS_PAIRS_BATCH;
+    std::vector<int64_t> bp{0};
+    std::vector<long long> pw0;
+    pw0.reserve((size_t)n_pairs + 1);
+    int64_t max_bw = 0, max_tiles = 0;
+    for (int64_t i = 0; i < n_pairs;) {
+        int64_t j = i + 1;
+        while (j < n_pairs && P[j + 1] - P[i] <= cap) ++j;
+        for (int64_t q = i; q <= j; ++q) pw0.push_back(P[q] - P[i]);
+        int64_t tiles = 0;
+        for (int64_t a = i; a < j;) {                                 // runs of one model
+            int64_t e = a + 1;
+            while (e < j && pairs[e].x == pairs[a].x) ++e;
+            tiles += (P[e] - P[a] + 63) / 64;
+            a = e;
+        }
+        max_bw = std::max<int64_t>(max_bw, P[j] - P[i]);
+        max_tiles = std::max(max_tiles, tiles);
+        bp.push_back(j);
+        i = j;
+    }
+    const int64_t n_batches = (int64_t)bp.size() - 1;
+    const long long Wp = P[n_pairs];
+    const bool own_raw = !d_raw && (reduce || hits) && Wp > 0;
+    CorpusPoolSizes ps;
+    ps.raw = own_raw ? (size_t)max_bw : 0;
+    ps.pairs = (size_t)n_pairs;
+    ps.pw0 = pw0.size();
+    ps.starts = (size_t)max_bw;
+    ps.tiles = (size_t)max_tiles;
+    rc = corpus_reserve(h, plan, n_rec, ps, s);
+    if (rc != PB_OK) return rc;
+    auto launch = [&]() -> int {
+        rc = corpus_k1(h, plan, d_pcm, n_rec, divisor, schedule, chunk, s);
+        if (rc != PB_OK) return rc;
+        if (hits) CK(cudaMemsetAsync(d_n_hits, 0, sizeof(unsigned long long), s));
+        CK(cudaMemcpyAsync(h->d_pp_pairs.get(), pairs.data(), pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_pp_pw0.get(), pw0.data(), pw0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        ProfScope prof(h, 1, s);
+        const K2In in = corpus_k2in(h);
+        const uint4* slots = h->d_pool_slots.get();
+        std::vector<PairTile> tiles;
+        for (int64_t b = 0; b < n_batches; ++b) {
+            const int64_t p0 = bp[b], p1 = bp[b + 1], nb = p1 - p0;
+            const long long q0 = P[p0], nw = P[p1] - q0;
+            const long long* bpw0 = h->d_pp_pw0.get() + p0 + b;
+            const int2* bpairs = h->d_pp_pairs.get() + p0;
+            float* raw = own_raw ? h->d_cp_raw.get() : d_raw ? d_raw + q0 : nullptr;
+            double* conf = d_conf ? d_conf + q0 : nullptr;
+            if (nw > 0) {
+                pairs_windows_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(bpw0, bpairs, (int)nb, nw, h->d_cw_win0.get(),
+                                                                                 h->d_cw_starts.get(), h->d_pp_starts.get());
+                CK(cudaGetLastError());
+                // tiles of 64 pair-windows within each run of one model, the Keras-activation class first
+                tiles.clear();
+                int64_t n_keras = 0;
+                for (int ka = 1; ka >= 0; --ka) {
+                    for (int64_t a = p0; a < p1;) {
+                        int64_t e = a + 1;
+                        while (e < p1 && pairs[e].x == pairs[a].x) ++e;
+                        if (h->pool_keras[pairs[a].x] == ka)
+                            for (long long q = P[a]; q < P[e]; q += 64)
+                                tiles.push_back(PairTile{q - q0, pairs[a].x, (int)std::min<long long>(64, P[e] - q)});
+                        a = e;
+                    }
+                    if (ka == 1) n_keras = (int64_t)tiles.size();
+                }
+                CK(cudaMemcpyAsync(h->d_pp_tiles.get(), tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
+                PairsCorpus c{};
+                c.slots = slots; c.starts = h->d_pp_starts.get(); c.raw = raw; c.conf = conf;
+                c.tiles = h->d_pp_tiles.get(); c.n_tiles = n_keras;
+                rc = launch_pairs_corpus<true>(c, in, s);
+                if (rc != PB_OK) return rc;
+                c.tiles += n_keras; c.n_tiles = (int64_t)tiles.size() - n_keras;
+                rc = launch_pairs_corpus<false>(c, in, s);
+                if (rc != PB_OK) return rc;
+            }
+            if (reduce) {
+                // one "recording" per pair of the batch, one row
+                CorpusTrig t = corpus_trig(h, nb, nw, schedule, chunk, threshold);
+                t.win0 = bpw0;
+                t.raw = raw; t.conf = conf;
+                t.fired = d_fired ? d_fired + q0 : nullptr;
+                t.activations = d_activations ? d_activations + p0 : nullptr;
+                t.above = d_above ? d_above + p0 : nullptr;
+                t.sum = d_sum ? d_sum + p0 : nullptr;
+                CorpusPairsDP dp{slots, bpairs, trigger_reset(2 * chunk)};
+                const unsigned per = CORPUS_TRIG_THREADS / 32;
+                corpus_trigger_kernel<<<dim3((unsigned)((nb + per - 1) / per), 1), CORPUS_TRIG_THREADS, 0, s>>>(t, dp);
+                CK(cudaGetLastError());
+            }
+            if (hits && nw > 0) {
+                PairsHits H{};
+                H.raw = raw; H.pw0 = bpw0; H.slots = slots; H.pairs = bpairs;
+                H.n = nw; H.q_base = q0; H.capacity = hit_capacity; H.n_pairs = (int)nb;
+                H.threshold = hit_threshold; H.hits = d_hits; H.n_hits = d_n_hits;
+                pairs_hits_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(H);
                 CK(cudaGetLastError());
             }
         }

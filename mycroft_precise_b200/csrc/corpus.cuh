@@ -226,11 +226,12 @@ struct CorpusTrig {
     int sim_reset;                   // simulate: -(8 * 2048) // chunk
 };
 
-// Listener: row m's decoder and detector (hot_threshold, trigger_level, trigger_reset), here a bank model's.  The model pool's
-// rows read theirs from their slot records (corpus_pool.cuh, CorpusPoolDP).
+// Listener: the decoder and detector (hot_threshold, trigger_level, trigger_reset) of row m over recording r, here row m's
+// bank model.  The model pool's rows read theirs from their slot records (corpus_pool.cuh, CorpusPoolDP), and pairs, whose
+// one row holds a model per "recording", from the slot record of recording r's model (corpus_pairs.cuh, CorpusPairsDP).
 struct CorpusBankDP {
     DecodeParams dp[PB_MAX_MODELS];
-    __device__ __forceinline__ const DecodeParams& operator()(int m) const { return dp[m]; }
+    __device__ __forceinline__ const DecodeParams& operator()(int m, long long) const { return dp[m]; }
 };
 
 constexpr int CORPUS_TRIG_THREADS = 256;
@@ -244,7 +245,7 @@ __global__ void __launch_bounds__(CORPUS_TRIG_THREADS) corpus_trigger_kernel(con
     const int m = blockIdx.y, lane = threadIdx.x & 31;
     const long long r = (long long)blockIdx.x * (CORPUS_TRIG_THREADS / 32) + (threadIdx.x >> 5);
     if (r >= P.n_rec) return;                                     // whole warp
-    const DecodeParams& d = dps(m);
+    const DecodeParams& d = dps(m, r);
     const bool sim = P.schedule == CORPUS_SIMULATE;
     const int level = sim ? 0 : d.trigger_level, reset = sim ? P.sim_reset : d.trigger_reset;
     const long long w0 = __ldg(P.win0 + r), w1 = __ldg(P.win0 + r + 1), off = (long long)m * P.W;

@@ -79,7 +79,7 @@ struct CorpusPoolDP {
     const uint4* slots;
     const int* ids;
     int reset;                       // TriggerDetector(2c bytes)
-    __device__ __forceinline__ DecodeParams operator()(int m) const {
+    __device__ __forceinline__ DecodeParams operator()(int m, long long) const {
         DecodeParams d = pool_rec(slots, __ldg(ids + m))->dp;
         d.trigger_reset = reset;
         return d;

@@ -12,9 +12,12 @@ the network run in the CUDA library.
 Recorded corpora (many recordings per device call, no window materialised: pb_score_corpus):
   score_corpus      every bank model over a list of recordings, listener or simulate schedule
   score_corpus_pool chosen pool models over a list of recordings (pb_score_corpus_pool)
+  score_corpus_pairs chosen (pool model, recording) pairs (pb_score_corpus_pairs)
   Metric, simulate  ~ precise/scripts/simulate.py:45-80, :106-129 (SimulateScript.run's per-file metrics and total)
   simulate_pool     simulate for many pool models in one device call per batch of recordings
+  simulate_pairs    simulate for each pool model over its own recordings
   false_activations ~ precise/scripts/train_incremental.py:113-137 (train_on_audio's selection of clips, fixed weights)
+  false_activations_pool  the same selection for pool models, the chunks above the threshold found on the device
 """
 from dataclasses import dataclass
 
@@ -136,12 +139,8 @@ def _check_recording(core: PreciseB200, r):
     return r if isinstance(r, np.ndarray) else r.contiguous()
 
 
-def _score_groups(core: PreciseB200, recordings, schedule, chunk, call):
-    """Packs ``recordings`` into library calls of at most CORPUS_CALL_SAMPLES samples, runs call(pcm, offsets) on each and
-    joins the results along the recording axis (window columns for raw / conf / fired, recording columns for the rest).
-    Output names score_corpus returns; None outputs stay None."""
-    torch = core.torch
-    recs = [_check_recording(core, r) for r in recordings]
+def _call_groups(recs):
+    """Consecutive runs of ``recs`` of at most CORPUS_CALL_SAMPLES samples each (a single longer recording alone)."""
     groups, cur, size = [], [], 0
     for r in recs:
         L = int(r.shape[0])
@@ -151,6 +150,16 @@ def _score_groups(core: PreciseB200, recordings, schedule, chunk, call):
         cur.append(r)
         size += L + 8
     groups.append(cur)
+    return groups
+
+
+def _score_groups(core: PreciseB200, recordings, schedule, chunk, call):
+    """Packs ``recordings`` into library calls of at most CORPUS_CALL_SAMPLES samples, runs call(pcm, offsets) on each and
+    joins the results along the recording axis (window columns for raw / conf / fired, recording columns for the rest).
+    Output names score_corpus returns; None outputs stay None."""
+    torch = core.torch
+    recs = [_check_recording(core, r) for r in recordings]
+    groups = _call_groups(recs)
     parts = []
     for g in groups:
         pcm, offsets, entry = _pack(core, g)
@@ -188,6 +197,64 @@ def score_corpus_pool(core: PreciseB200, recordings, model_ids, schedule='listen
     return _score_groups(core, recordings, schedule, chunk,
                          lambda pcm, offsets: core.score_corpus_pool(pcm, offsets, ids, schedule, chunk, threshold, divisor,
                                                                      per_window))
+
+
+def score_corpus_pairs(core: PreciseB200, recordings, model_ids, rec_ids, schedule='listener', chunk=1024, threshold=0.5,
+                       divisor=32768, per_window=True, hit_threshold=None, hit_capacity=None):
+    """Pool model model_ids[p] over recordings[rec_ids[p]] for each pair p (pb_score_corpus_pairs), recordings packed and
+    split into library calls as score_corpus splits them; each call scores the pairs whose recordings it holds.  Returns
+    PreciseB200.score_corpus_pairs's dict over all pairs, in pair order: raw / conf / fired [Wp] (None with
+    per_window=False), activations (and for simulate above, sum) [n_pairs], pair_offsets, and hits with a hit_threshold."""
+    torch = core.torch
+    recs = [_check_recording(core, r) for r in recordings]
+    model_ids = np.ascontiguousarray(model_ids, dtype=np.int32)
+    rec_ids = np.ascontiguousarray(rec_ids, dtype=np.int64)
+    n = model_ids.shape[0]
+    if rec_ids.shape != (n,):
+        raise ValueError('model_ids and rec_ids must be 1-D arrays of one length')
+    if n and (rec_ids.min() < 0 or rec_ids.max() >= len(recs)):
+        raise ValueError('recording ids must lie in [0, %d)' % len(recs))
+    counts = np.asarray([core.corpus_windows(int(r.shape[0]), schedule, chunk) for r in recs], np.int64)
+    P = np.concatenate([[0], np.cumsum(counts[rec_ids], dtype=np.int64)]).astype(np.int64)
+    Wp = int(P[-1])
+    parts, first = [], 0
+    for g in _call_groups(recs):
+        sel = np.nonzero((rec_ids >= first) & (rec_ids < first + len(g)))[0]
+        if sel.size:
+            pcm, offsets, entry = _pack(core, g)
+            res = core.score_corpus_pairs(pcm, offsets, model_ids[sel], entry[rec_ids[sel] - first].astype(np.int32),
+                                          schedule, chunk, threshold, divisor, per_window, hit_threshold, hit_capacity)
+            parts.append((sel, res))
+        first += len(g)
+    if len(parts) == 1 and parts[0][0].size == n:                # one call over every pair, in order
+        res = parts[0][1]
+        res['pair_offsets'] = P
+        return res
+    f = lambda size, dt: torch.zeros(size, dtype=dt, device=core.device)
+    out = dict(raw=None, conf=None, fired=None, activations=f(n, torch.int64), above=None, sum=None, pair_offsets=P)
+    if per_window:
+        out.update(raw=f(Wp, torch.float32), conf=f(Wp, torch.float64), fired=f(Wp, torch.uint8))
+    if schedule == 'simulate':
+        out.update(above=f(n, torch.int64), sum=f(n, torch.float64))
+    hits = []
+    for sel, res in parts:
+        rows = torch.from_numpy(sel).to(core.device)
+        for k in ('activations', 'above', 'sum'):
+            if out[k] is not None:
+                out[k].index_copy_(0, rows, res[k])
+        local = res['pair_offsets']
+        if per_window:                                           # this call's pair-windows, placed at their pairs' columns
+            cols = np.concatenate([np.arange(P[p], P[p + 1]) for p in sel] + [np.zeros(0, np.int64)])
+            cols = torch.from_numpy(cols).to(core.device)
+            for k in ('raw', 'conf', 'fired'):
+                out[k].index_copy_(0, cols, res[k])
+        if hit_threshold is not None:
+            q = res['hits'].cpu().numpy()
+            j = np.searchsorted(local, q, side='right') - 1
+            hits.append(P[sel[j]] + (q - local[j]))
+    if hit_threshold is not None:
+        out['hits'] = torch.from_numpy(np.sort(np.concatenate(hits + [np.zeros(0, np.int64)]))).to(core.device)
+    return out
 
 
 @dataclass
@@ -264,6 +331,29 @@ def simulate_pool(core: PreciseB200, recordings, model_ids, chunk_size=4096, thr
     return metrics, totals
 
 
+def simulate_pairs(core: PreciseB200, recordings, model_ids, rec_ids, chunk_size=4096, threshold=0.5):
+    """simulate for chosen (pool model, recording) pairs, each custom wake word over its own recordings: returns (metrics,
+    totals), metrics[p] pair p's Metric (None for an empty recording) and totals {model id: the total over its pairs, in
+    pair order}.  Only the per-pair reductions leave the device."""
+    res = score_corpus_pairs(core, recordings, model_ids, rec_ids, 'simulate', chunk_size, threshold, divisor=32767,
+                             per_window=False)
+    above = res['above'].cpu().numpy()
+    acts = res['activations'].cpu().numpy()
+    sums = res['sum'].cpu().numpy()
+    sr = core.params.sample_rate
+    metrics, totals = [], {}
+    for p, (mid, r) in enumerate(zip(np.asarray(model_ids).tolist(), np.asarray(rec_ids).tolist())):
+        t = totals.setdefault(mid, Metric(chunk_size, sample_rate=sr))
+        L = int(recordings[r].shape[0])
+        if L == 0:
+            metrics.append(None)
+            continue
+        m = Metric(chunk_size, L / sr, int(above[p]), int(acts[p]), float(sums[p]), sr)
+        t.add(m)
+        metrics.append(m)
+    return metrics, totals
+
+
 def false_activations(core: PreciseB200, recordings, chunk_size=2048, threshold=0.5):
     """train_on_audio's selection (train_incremental.py:113-137) with fixed weights, bank slot 0, recordings read as
     load_audio reads them (samples / 32767).  Each recording is cut as chunk_audio cuts it (util.py:30-32: chunks end at
@@ -273,7 +363,7 @@ def false_activations(core: PreciseB200, recordings, chunk_size=2048, threshold=
     Deliberate differences: the reference's audio_buffer carries the previous file's tail into the next file (glob order),
     here every recording starts from zeros; and it retrains between chunks, which is out of scope here."""
     c = int(chunk_size)
-    recs = [r[:((int(r.shape[0]) - 1) // c) * c] if int(r.shape[0]) else r for r in recordings]
+    recs = _chunk_cut(recordings, c)
     res = score_corpus(core, recs, 'listener', c, divisor=32767)
     conf = res['conf'][0].cpu().numpy()
     wo = res['window_offsets']
@@ -285,9 +375,48 @@ def false_activations(core: PreciseB200, recordings, chunk_size=2048, threshold=
             continue
         a = r if isinstance(r, np.ndarray) else r.cpu().numpy()
         for k in hits:
-            end = (int(k) + 1) * c
-            clip = np.zeros(bs, np.float32)
-            seg = a[max(0, end - bs):end].astype(np.float32) / np.float32(32767)
-            clip[bs - seg.shape[0]:] = seg
-            out.append((i, int(k), clip))
+            out.append((i, int(k), _clip(a, (int(k) + 1) * c, bs)))
+    return out
+
+
+def _chunk_cut(recordings, c):
+    """Each recording cut as chunk_audio cuts it (util.py:30-32): floor((L - 1) / c) chunks of c."""
+    return [r[:((int(r.shape[0]) - 1) // c) * c] if int(r.shape[0]) else r for r in recordings]
+
+
+def _clip(a, end, bs):
+    """The float32 audio (load_audio's scale) of the last bs samples of ``a`` up to ``end``, zeros before its start."""
+    clip = np.zeros(bs, np.float32)
+    seg = a[max(0, end - bs):end].astype(np.float32) / np.float32(32767)
+    clip[bs - seg.shape[0]:] = seg
+    return clip
+
+
+def false_activations_pool(core: PreciseB200, recordings, model_ids, rec_ids=None, chunk_size=2048, threshold=0.5):
+    """false_activations for pool models: pool model model_ids[p] over recordings[rec_ids[p]] for each pair p (rec_ids None:
+    every model over every recording, model-major, pair p = i * len(recordings) + r).  Recordings are cut and clips built as
+    false_activations does; the chunks above ``threshold`` are found on the device, and only they leave it.  Returns a list
+    of (pair index, recording index, chunk index, clip), in pair order and chunk order within a pair."""
+    c = int(chunk_size)
+    recs = _chunk_cut(recordings, c)
+    model_ids = np.ascontiguousarray(model_ids, dtype=np.int32)
+    if rec_ids is None:
+        n_rec = len(recs)
+        rec_ids = np.tile(np.arange(n_rec, dtype=np.int32), model_ids.shape[0])
+        model_ids = np.repeat(model_ids, n_rec)
+    rec_ids = np.ascontiguousarray(rec_ids, dtype=np.int32)
+    res = score_corpus_pairs(core, recs, model_ids, rec_ids, 'listener', c, divisor=32767, per_window=False,
+                             hit_threshold=threshold)
+    P = res['pair_offsets']
+    q = res['hits'].cpu().numpy()
+    pair = np.searchsorted(P, q, side='right') - 1
+    bs = core.params.buffer_samples
+    host = {}
+    out = []
+    for p, k in zip(pair.tolist(), (q - P[pair]).tolist()):
+        r = int(rec_ids[p])
+        if r not in host:
+            a = recs[r]
+            host[r] = a if isinstance(a, np.ndarray) else a.cpu().numpy()
+        out.append((p, r, k, _clip(host[r], (k + 1) * c, bs)))
     return out
