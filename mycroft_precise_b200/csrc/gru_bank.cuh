@@ -29,13 +29,19 @@ __device__ __forceinline__ void mma_f16_k8(float (&d)[4], uint32_t a0, uint32_t 
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                  : "r"(a0), "r"(a1), "r"(b0));
 }
-// (x, y) -> fp16 hi pair and the pair of residuals
+// (x, y) -> half2 (x in the low half, as __floats2half2_rn), rounded to nearest and saturated to +-65504 instead of
+// overflowing to +-inf.  PTX puts the first source operand in the upper half.  One F2FP.SATFINITE.F16.F32.PACK_AB.
+__device__ __forceinline__ uint32_t pack_f16x2_sat(float x, float y) {
+    uint32_t r;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(y), "f"(x));
+    return r;
+}
+// (x, y) -> fp16 hi pair and the pair of residuals.  Exact fp16 x 3 operands for |v| < 65504; beyond that both pieces
+// saturate, so the products see a finite operand of the same sign (|hi + lo| <= 131008) instead of inf - inf = NaN.
 __device__ __forceinline__ void split_f16(float x, float y, uint32_t& hi, uint32_t& lo) {
-    const __half2 h = __floats2half2_rn(x, y);
-    const float2 f = __half22float2(h);
-    const __half2 l = __floats2half2_rn(x - f.x, y - f.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
+    hi = pack_f16x2_sat(x, y);
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+    lo = pack_f16x2_sat(x - f.x, y - f.y);
 }
 // A fragments of a 24-unit vector held in accumulator layout v[tile][e]: k-tile 0 (units 0..15) as a k16 fragment, units 16..23 as a k8 one
 __device__ __forceinline__ void frag_f16(const float (&v)[3][4], uint32_t (&ah)[4], uint32_t (&al)[4], uint32_t (&bh)[2], uint32_t (&bl)[2]) {

@@ -100,6 +100,79 @@ def gru_forward(w: GruWeights, x: np.ndarray, dtype=np.float32, return_hidden=Fa
     return prob, logit
 
 
+F16_MAX = 65504.0
+
+
+def _f16(v, saturate):
+    """float32 v rounded to the nearest fp16 (as float32); ``saturate``: +-65504 instead of +-inf for |v| >= 65520."""
+    with np.errstate(over='ignore'):
+        h = np.asarray(v, np.float32).astype(np.float16).astype(np.float32)
+    if saturate:
+        h = np.where(np.isinf(h) & np.isfinite(v), np.copysign(np.float32(F16_MAX), v), h).astype(np.float32)
+    return h
+
+
+def split_f16(v, saturate=True):
+    """float32 v -> (hi, lo), float64 values of fp16 numbers: hi = fp16(v), lo = fp16(v - hi) with v - hi in float32.
+    ``saturate``: the kernel's operand split (cvt.rn.satfinite); otherwise the host's weight split (build_frag16)."""
+    v = np.asarray(v, np.float32)
+    hi = _f16(v, saturate)
+    with np.errstate(invalid='ignore'):
+        lo = _f16(v - hi, saturate)
+    return hi.astype(np.float64), lo.astype(np.float64)
+
+
+def _mm3(a, b):
+    """a . b as the fused family's fp16 x 3 products: a_lo b_hi + a_hi b_lo + a_hi b_hi (lo . lo dropped), summed in
+    float64.  a: (hi, lo) of a split operand, b: (hi, lo) of a split weight matrix."""
+    with np.errstate(invalid='ignore'):
+        return a[1] @ b[0] + a[0] @ b[1] + a[0] @ b[0]
+
+
+def _f32(v):
+    return np.asarray(v, np.float64).astype(np.float32)
+
+
+_ACT32 = {
+    'linear': lambda x: x,
+    'tanh': lambda x: np.tanh(x.astype(np.float32)),
+    'hard_sigmoid': lambda x: np.clip(_f32(np.float64(np.float32(0.2)) * x.astype(np.float64) + 0.5), 0, 1),
+    'sigmoid': lambda x: sigmoid(x.astype(np.float32)),
+}
+
+
+def gru_forward_f16x3(w: GruWeights, x: np.ndarray):
+    """x[N, T, F] -> (prob[N], logit[N]) float32, as the fused family's tensor-core scan (gru_bank.cuh: bank_scan) computes
+    them: every product x . W, h . U and (r * h) . U in fp16 x 3 with operands split by ``split_f16`` (saturating, as the
+    kernel splits x, h and r * h) and weights by the host's non-saturating split.  Each product is summed exactly and added
+    to the float32 accumulator in the kernel's order: bias, then the x part, then the h part.  Activations are float32
+    (hard_sigmoid as fma(0.2, x, 0.5)), r * h is rounded to float32 before its split, h = fma(z, h, (1 - z) a) is rounded to
+    float32 and the Dense layer is summed exactly and rounded once.  A reference for tests: what the scan should return,
+    not a model of the tensor cores' internal rounding."""
+    x = np.asarray(x, np.float32)
+    if x.ndim == 2:
+        x = x[None]
+    N, T, F = x.shape
+    assert F == w.F, (F, w.F)
+    H = w.H
+    K = split_f16(w.kernel, saturate=False)
+    Uzr = split_f16(w.recurrent[:, :2 * H], saturate=False)
+    Uh = split_f16(w.recurrent[:, 2 * H:], saturate=False)
+    b = w.bias.astype(np.float64)
+    act, ract = _ACT32[w.activation], _ACT32[w.recurrent_activation]
+    h = np.zeros((N, H), np.float32)
+    for t in range(T):
+        ax = _f32(b + _mm3(split_f16(x[:, t, :]), K))                 # bias, then the x part
+        zr = ract(_f32(ax[:, :2 * H].astype(np.float64) + _mm3(split_f16(h), Uzr)))
+        z, r = zr[:, :H].astype(np.float32), zr[:, H:].astype(np.float32)
+        rh = _f32(r.astype(np.float64) * h)
+        a = act(_f32(ax[:, 2 * H:].astype(np.float64) + _mm3(split_f16(rh), Uh))).astype(np.float32)
+        p = _f32((np.float32(1) - z).astype(np.float64) * a)
+        h = _f32(z.astype(np.float64) * h + p)
+    logit = _f32(h.astype(np.float64) @ w.dense_w.astype(np.float64) + w.dense_b)
+    return sigmoid(logit), logit
+
+
 def predict(w: GruWeights, inputs: np.ndarray) -> np.ndarray:
     """``Runner.predict`` contract (network_runner.py:35-37): [N,T,F] -> float32 [N,1]."""
     return gru_forward(w, inputs, np.float32)[0].astype(np.float32)[:, None]
