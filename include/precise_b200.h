@@ -546,6 +546,56 @@ int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64_t* h_o
                           int64_t* d_activations, int64_t* d_above, double* d_sum,
                           double hit_threshold, int64_t* d_hits, int64_t hit_capacity,
                           unsigned long long* d_n_hits, void* stream);
+/* Pool models over labelled clips: one network input per recording, and per-model statistics over the outputs, for many
+ * custom wake words in one call.  It is the device side of the reference's tools that work on Runner.predict(vectorize(clip)):
+ * precise-test / precise-eval (precise/scripts/test.py, eval.py, precise/stats.py: true / false positives and negatives at a
+ * threshold, the misclassified files), precise-graph (scripts/graph.py:147-152: the rates over ~100 thresholds) and
+ * precise-calc-threshold (scripts/calc_threshold.py:66-83: mean and std of -log(1 / out - 1) over the positive clips).
+ *   - Input per clip (vectorize, precise/vectorization.py:62-84): recording r, as pb_score_corpus takes recordings, cropped
+ *     to its LAST max_samples samples (ListenerParams.max_samples) and framed from the cropped clip's first sample:
+ *     nf = pb_mfcc_frames(min(L, max_samples)) frames, of which the network sees the last n_features, zero rows before them
+ *     when there are fewer.  A clip too short for one frame scores the all-zero input.  No deltas (the pool's networks have
+ *     none).  An empty recording is refused (the reference raises InvalidAudio).
+ *   - Entries.  Cross product (h_pair_rows = h_pair_recs = NULL, n_pairs = 0): every model of h_model_ids [k] (HOST; pool
+ *     slots, repeats allowed) over every recording; entry (i, r) at d_raw[i * n_rec + r].  Pairs (n_pairs > 0): entry p is
+ *     model h_model_ids[h_pair_rows[p]] over recording h_pair_recs[p] (both HOST), at d_raw[p]: each word over its owner's
+ *     own clips.  Scan tiles hold 64 consecutive pairs of one model: list a model's pairs together.  Raw outputs are
+ *     bit-identical to pb_score_corpus_pool's / pb_score_corpus_pairs's for the same input rows.
+ *   - Statistics, row i for h_model_ids[i] in both forms, all int64: exact, independent of the order of evaluation, and
+ *     summed over calls by adding the arrays.  The label of an entry is h_targets[r] != 0 (HOST [n_rec]).  The call zeroes
+ *     them first.
+ *       d_count [k][2]               entries per label.
+ *       d_hist  [k][2][2 n_thr + 1]  h_thresholds [n_thr] (HOST, 1 <= n_thr <= 1024) are rounded to float32 (numpy compares a
+ *                                    float32 array with a Python float in float32) and must then be strictly ascending.  Bin
+ *                                    2j + 1 counts raw == t_j, bin 2j counts t_(j-1) < raw < t_j (t_(-1) = -inf, t_n = +inf);
+ *                                    NaN goes to bin 0.  Suffix sums give #(raw > t_j) (Stats.calc_metric, stats.py:102-107)
+ *                                    and #(raw >= t_j) (Stats.num_correct, stats.py:54-56).
+ *       d_fit   [k][2][3]            over entries with raw != 0 and raw != 1 (calc_threshold.py:66) and a finite
+ *                                    v = -log((double)(1.0f / raw - 1.0f)) (the 1 / x - 1 in float32, as conf's decode; not
+ *                                    finite for NaN and for float32 denormals): their number, the sum of llrint(v 2^32) and
+ *                                    the sum of llrint(v^2 2^24).  |v| < 104, so no sum overflows while a (row, label) has at
+ *                                    most 2^24 entries; a call with d_fit in which one would have more is refused.
+ *     Misclassified entries (what precise-test lists): with d_n_miss, *d_n_miss receives the number of entries with
+ *     (raw > (float)miss_threshold) != label, and the first min(total, miss_capacity) of them go to d_miss [miss_capacity] as
+ *     i * n_rec + r (cross product) or p (pairs), in no particular order; the set is exact.
+ *   - Every output is optional, d_raw included, but not all of them at once.  Without d_raw, raw of a batch (rows of at most
+ *     256 MB, or 2^25 pairs) is kept in the corpus workspace, each batch followed by its statistics pass.
+ *   - Reads and writes no stream state, pool assignment or detector; needs no slot-0 weights.  Asynchronous on `stream`,
+ *     ordered against the corpus calls as pb_score_corpus (it shares their workspace).  Profile slot 0 counts K1, slot 1 the
+ *     scans and statistics.  Every argument is checked before anything is enqueued, so a refused call changes no state.
+ * PB_ERR_INVALID: pb_score_corpus's argument errors (but a null d_raw), every output null, max_samples < 1, a null h_targets,
+ * an empty recording, k outside [0, 2^30), a null h_model_ids with k > 0, an id outside [0, max_models) or a slot that holds no
+ * model, n_pairs outside [0, 2^31), one null pair array with n_pairs > 0, a row outside [0, k), a recording id outside
+ * [0, n_rec), n_thr outside [0, 1024] or 0 with d_hist, null, NaN or not strictly ascending thresholds, miss_capacity < 0, a
+ * null d_miss with miss_capacity > 0, d_miss without d_n_miss, more than 2^24 entries of one (row, label) with d_fit.
+ * PB_ERR_STATE: no pool.  PB_ERR_CUDA: the workspace cannot be allocated (the handle is then unchanged). */
+int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                     const uint8_t* h_targets, const int32_t* h_model_ids, int64_t k,
+                     const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs,
+                     int32_t divisor, int64_t max_samples, const double* h_thresholds, int32_t n_thr,
+                     float* d_raw, int64_t* d_count, int64_t* d_hist, int64_t* d_fit,
+                     double miss_threshold, int64_t* d_miss, int64_t miss_capacity, unsigned long long* d_n_miss,
+                     void* stream);
 
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);

@@ -26,6 +26,7 @@ class StreamBatch:
         self.pool_count = torch.zeros(1, dtype=torch.int64, device=self.core.device)   # pool fires, update_pool
         self._out = None
         self._bank_out = None
+        self._pool_specs = {}                # pool slot -> pool_load's arguments, for pool_calibrate
 
     def add_model(self, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False) -> int:
         """Score another network (GruModel or weights path) on the same streams' MFCC frames; returns its bank slot.
@@ -54,10 +55,31 @@ class StreamBatch:
         """A model pool of ``max_models`` slots beside the bank; each stream is scored by at most one pool model.  See
         PreciseB200.set_pool."""
         self.core.set_pool(max_models)
+        self._pool_specs = {}
 
     def pool_load(self, model_id, model, params: ListenerParams = None, sensitivity=0.5, trigger_level=3, decode_legacy_f64=False):
         """Load a network (GruModel or weights path) into pool slot ``model_id``.  See PreciseB200.pool_load."""
         self.core.pool_load(model_id, model, params, sensitivity, trigger_level, decode_legacy_f64)
+        self._pool_specs[int(model_id)] = (model, params, sensitivity, trigger_level, decode_legacy_f64)
+
+    def pool_calibrate(self, model_ids, clips, rows=None, recs=None, smoothing=1.2):
+        """precise-calc-threshold for pool slots ``model_ids`` (int32 [k], loaded through this batch's pool_load) from
+        wake-word clips: entry p is model_ids[rows[p]] over clips[recs[p]], each word over its owner's recordings (rows /
+        recs None: every model over every clip).  Each slot whose clips give a fit is loaded again with
+        threshold_config ((mu, std),) through pool_load, which re-arms its streams as a newly loaded model does; a slot
+        without data keeps its table.  Returns the list of k fits, (mu, std) or None.  See offline.calc_threshold."""
+        from .offline import calc_threshold, test_pool
+        from .runner import _resolve_model
+        specs = [self._pool_specs[int(m)] for m in model_ids]
+        stats = test_pool(self.core, clips, np.ones(len(clips), np.uint8), model_ids, rows, recs)
+        fits = [calc_threshold(st, smoothing) for st in stats]
+        for mid, fit, (model, params, sens, lvl, legacy) in zip(model_ids, fits, specs):
+            if fit is None:
+                continue
+            base = params or _resolve_model(model)[1] or self.pr
+            pr = ListenerParams(**dict(base.to_dict(), threshold_config=(fit,)))
+            self.pool_load(int(mid), model, pr, sens, lvl, legacy)
+        return fits
 
     def set_stream_pool(self, model_ids, ids=None):
         """Each stream's pool model (host int32, -1 = none).  See PreciseB200.set_stream_pool."""

@@ -87,6 +87,8 @@ SYMBOLS = {
                                        _VP, _VP]),
     'pb_score_corpus_pairs': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _I32, _I32, _I64, C.c_double, _VP, _VP, _VP, _VP,
                                         _VP, _VP, C.c_double, _VP, _I64, _VP, _VP]),
+    'pb_score_dataset': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, _I32, _I64, _VP, _I32, _VP, _VP, _VP, _VP,
+                                   C.c_double, _VP, _I64, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -198,6 +200,20 @@ def numpy_cdf(threshold_config, resolution=200, min_z=-4, max_z=4):
 
     pd = np.sum([pdf(points, mu, std) for mu, std in mu_stds], axis=0) / (resolution * len(mu_stds))
     return np.ascontiguousarray(np.cumsum(pd), dtype=np.float64), min_out, max_out
+
+
+def threshold_encode(threshold_config, center, thresholds):
+    """ThresholdDecoder.encode (threshold_decoder.py:59-66) of each decoded threshold: the network output it stands for,
+    from the same table numpy_cdf builds for the decoder."""
+    from math import exp
+    cd, min_out, max_out = numpy_cdf(threshold_config)
+    out = []
+    for t in thresholds:
+        t = 0.5 * float(t) / center
+        cp = t * center * 2 if t < 0.5 else (t - 0.5) * 2 * (1 - center) + center
+        ratio = np.searchsorted(cd, cp) / len(cd)
+        out.append(1 / (1 + exp(-(min_out + (max_out - min_out) * ratio))))
+    return np.asarray(out, np.float64)
 
 
 def _schedule(schedule) -> int:
@@ -828,8 +844,14 @@ class PreciseB200:
 
     def _corpus_args(self, pcm, offsets, schedule, chunk):
         """(schedule code, int64 offsets, n_rec, W) of a corpus call, checked."""
-        torch = self.torch
         sched = _schedule(schedule)
+        offsets, n_rec = self._corpus_recordings(pcm, offsets)
+        W = sum(self.corpus_windows(int(L), schedule, chunk) for L in np.diff(offsets))
+        return sched, offsets, n_rec, W
+
+    def _corpus_recordings(self, pcm, offsets):
+        """(int64 offsets, n_rec) of the recordings of a corpus call, checked."""
+        torch = self.torch
         if (not isinstance(pcm, torch.Tensor) or pcm.dtype != torch.int16 or pcm.dim() != 1 or not pcm.is_contiguous()
                 or pcm.device != self.device):
             raise ValueError('pcm must be a contiguous 1-D int16 tensor on %s' % self.device)
@@ -843,8 +865,7 @@ class PreciseB200:
         lens = np.diff(offsets)
         if lens.size and lens.min() < 0:
             raise ValueError('offsets must be non-decreasing')
-        W = sum(self.corpus_windows(int(L), schedule, chunk) for L in lens)
-        return sched, offsets, n_rec, W
+        return offsets, n_rec
 
     def score_corpus(self, pcm, offsets, schedule='listener', chunk=1024, threshold=0.5, divisor=32768):
         """Every bank model over recordings pcm[offsets[r]:offsets[r + 1]] (pcm a 1-D int16 CUDA tensor, offsets a host int64
@@ -938,6 +959,70 @@ class PreciseB200:
                 cap = total
                 d_hits = run(cap)
             out['hits'] = torch.sort(d_hits[:total])[0]
+        return out
+
+    def score_dataset(self, pcm, offsets, targets, model_ids, rows=None, recs=None, thresholds=(0.5,), divisor=32767,
+                      per_entry=True, miss_threshold=None, miss_capacity=None):
+        """Pool models over labelled clips pcm[offsets[r]:offsets[r + 1]] (as score_corpus takes recordings; none empty), each
+        cropped to its last params.max_samples samples and scored once, as the reference's vectorize + Runner.predict score
+        a clip.  targets: host uint8 [n_rec], non-zero = wake word.  model_ids: host int32 [k] pool slots; statistics row i
+        belongs to model_ids[i].  rows / recs None: every model over every clip, raw [k, n_rec].  Otherwise host int32
+        arrays [n_pairs]: entry p is model_ids[rows[p]] over clip recs[p], raw [n_pairs].  Returns dict(raw (None with
+        per_entry=False), count i64 [k, 2], hist i64 [k, 2, 2 n_thr + 1], fit i64 [k, 2, 3], thresholds (the float32 values
+        the histogram used)), and with a miss_threshold also misses: the sorted int64 indices (i * n_rec + r, or p) of the
+        entries with (raw > miss_threshold) != label; when more than miss_capacity are found the call runs once more with
+        room for all of them, and this (and only this) waits for the device.  divisor 32767: clips read as load_audio reads
+        wav files.  Asynchronous on the current stream.  pb_score_dataset in include/precise_b200.h."""
+        torch = self.torch
+        offsets, n_rec = self._corpus_recordings(pcm, offsets)
+        targets, model_ids = np.asarray(targets), np.asarray(model_ids)
+        _check_np('targets', targets, np.uint8, (n_rec,), optional=False)
+        k = model_ids.shape[0] if model_ids.ndim == 1 else -1
+        _check_np('model_ids', model_ids, np.int32, (k,), optional=False)
+        if (rows is None) != (recs is None):
+            raise ValueError('rows and recs come together')
+        n = 0
+        if rows is not None:
+            rows, recs = np.asarray(rows), np.asarray(recs)
+            n = rows.shape[0] if rows.ndim == 1 else -1
+            _check_np('rows', rows, np.int32, (n,), optional=False)
+            _check_np('recs', recs, np.int32, (n,), optional=False)
+        thr = np.ascontiguousarray(thresholds, dtype=np.float64)
+        if thr.ndim != 1:
+            raise ValueError('thresholds must be a 1-D list')
+        n_thr = thr.shape[0]
+        f = lambda shape, dt: torch.empty(shape, dtype=dt, device=self.device)
+        out = dict(raw=None, count=f((k, 2), torch.int64), hist=f((k, 2, 2 * n_thr + 1), torch.int64),
+                   fit=f((k, 2, 3), torch.int64), thresholds=thr.astype(np.float32))
+        if per_entry:
+            out['raw'] = f((n,), torch.float32) if rows is not None else f((k, n_rec), torch.float32)
+        misses = miss_threshold is not None
+        n_miss = f((1,), torch.int64) if misses else None
+        cap = self._int('miss_capacity', 1 << 16 if miss_capacity is None else miss_capacity) if misses else 0
+
+        def run(cap):
+            d_miss = f((max(cap, 1),), torch.int64) if misses else None
+            check(self.lib.pb_score_dataset(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, _np_ptr(targets), _np_ptr(model_ids), k,
+                                            _np_ptr(rows) if n else None, _np_ptr(recs) if n else None, n, int(divisor),
+                                            int(self.params.max_samples), _np_ptr(thr), n_thr, _ptr(out['raw']),
+                                            _ptr(out['count']), _ptr(out['hist']), _ptr(out['fit']),
+                                            float(miss_threshold) if misses else 0.0, _ptr(d_miss) if cap else None, cap,
+                                            _ptr(n_miss), self._stream()))
+            return d_miss
+
+        if k == 0 or (rows is not None and n == 0):           # no entry (the library reads an empty pair list as "every pair")
+            for key in ('count', 'hist', 'fit'):
+                out[key].zero_()
+            if misses:
+                out['misses'] = f((0,), torch.int64)
+            return out
+        d_miss = run(cap)
+        if misses:
+            total = int(n_miss.item())
+            if total > cap:
+                cap = total
+                d_miss = run(cap)
+            out['misses'] = torch.sort(d_miss[:total])[0]
         return out
 
     def corpus_pairs_batch(self, windows):

@@ -36,6 +36,7 @@
 #include "corpus.cuh"
 #include "corpus_pool.cuh"
 #include "corpus_pairs.cuh"
+#include "dataset.cuh"
 #include "pool.cuh"
 
 using namespace pb;
@@ -216,6 +217,8 @@ struct pb_handle {
     DevArray<long long> d_pp_pw0;    // ... each batch's pair-window prefix, batch b's at [p0 + b, p1 + b]
     DevArray<long long> d_pp_starts; // ... [batch pair-windows] the batch's window table
     DevArray<PairTile> d_pp_tiles;   // ... the batch's scan tiles, one activation class after the other
+    DevArray<float> d_ds_thr;        // pb_score_dataset: the histogram's float32 thresholds
+    DevArray<uint8_t> d_ds_targets;  // ... [n_rec] the recordings' labels
     int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
@@ -1636,12 +1639,15 @@ static int check_corpus(const pb_handle* h, const int16_t* d_pcm, const int64_t*
 // K1's host plan of a corpus call: window prefix, frame rows, and the recordings in pair-list order (aligned geometry first).
 struct CorpusPlan {
     std::vector<long long> win0, frow;
+    std::vector<long long> starts;   // labelled clips: the window table itself, one window per recording
     std::vector<CorpusRec> recs;
     long long rows = 1, n_fast_pairs = 0, n_pairs = 0, W = 0;
 };
 
+// crop > 0 (labelled clips, vectorization.py:73-82): each recording is its last `crop` samples, framed from the first of
+// them, and has one window, the n_features rows ending at its last frame (row 0's zeros when it has no frame).
 static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t schedule,
-                              int64_t chunk) {
+                              int64_t chunk, int64_t crop = 0) {
     const pb_config& c = h->cfg;
     const int T = c.n_features;
     const bool fast = h->fast_ok && !h->force_generic && (uintptr_t)d_pcm % 16 == 0;
@@ -1650,17 +1656,20 @@ static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const in
     p.frow.resize((size_t)n_rec);
     p.recs.reserve((size_t)n_rec + 1);
     p.win0[0] = 0;
+    if (crop > 0) p.starts.resize((size_t)n_rec);
     for (int pass = 0; pass < 2; ++pass)
         for (int64_t r = 0; r < n_rec; ++r) {
-            const int64_t L = h_offsets[r + 1] - h_offsets[r], nf = corpus_frames(c, L);
-            const bool fr = fast && h_offsets[r] % 8 == 0;
+            const int64_t len = h_offsets[r + 1] - h_offsets[r], L = crop > 0 ? std::min(len, crop) : len;
+            const int64_t src = h_offsets[r] + len - L, nf = corpus_frames(c, L);
+            const bool fr = fast && src % 8 == 0;
             if (pass == 0) {
-                p.win0[r + 1] = p.win0[r] + corpus_windows(c, schedule, chunk, L);
+                p.win0[r + 1] = p.win0[r] + (crop > 0 ? 1 : corpus_windows(c, schedule, chunk, L));
                 p.frow[r] = p.rows + T - 1;
                 p.rows += T - 1 + nf;
+                if (crop > 0) p.starts[r] = nf ? p.frow[r] + nf - T : 0;
             }
             if (fr != (pass == 0)) continue;
-            p.recs.push_back(CorpusRec{h_offsets[r], p.frow[r], nf, p.n_pairs});
+            p.recs.push_back(CorpusRec{src, p.frow[r], nf, p.n_pairs});
             p.n_pairs += (nf + 1) / 2;
             if (fr) p.n_fast_pairs = p.n_pairs;
         }
@@ -1673,6 +1682,7 @@ static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const in
 struct CorpusPoolSizes {
     size_t groups = 0, ids = 0, raw = 0;
     size_t pairs = 0, pw0 = 0, starts = 0, tiles = 0;
+    size_t thr = 0, targets = 0;     // pb_score_dataset
 };
 
 // Grows the workspace for plan p, all at once, so that a failed allocation leaves the handle as it was; then orders s after
@@ -1682,6 +1692,7 @@ static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, cons
     DevArray<float> f_rows, f_raw; DevArray<CorpusPair> f_pairs; DevArray<long long> f_starts, f_win0, f_frow; DevArray<CorpusRec> f_recs;
     DevArray<int2> f_groups; DevArray<int> f_ids;
     DevArray<int2> f_ppairs; DevArray<long long> f_pw0, f_pstarts; DevArray<PairTile> f_tiles;
+    DevArray<float> f_thr; DevArray<uint8_t> f_targets;
     cudaError_t e = corpus_grow(h->d_cw_rows, (size_t)p.rows * h->row_stride, f_rows);
     if (e == cudaSuccess) e = corpus_grow(h->d_cw_pairs, (size_t)p.n_pairs, f_pairs);
     if (e == cudaSuccess) e = corpus_grow(h->d_cw_starts, (size_t)p.W, f_starts);
@@ -1695,13 +1706,15 @@ static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, cons
     if (e == cudaSuccess) e = corpus_grow(h->d_pp_pw0, ps.pw0, f_pw0);
     if (e == cudaSuccess && h->d_pp_starts.size() < ps.starts) e = f_pstarts.alloc(ps.starts);   // capped: no headroom
     if (e == cudaSuccess) e = corpus_grow(h->d_pp_tiles, ps.tiles, f_tiles);
+    if (e == cudaSuccess) e = corpus_grow(h->d_ds_thr, ps.thr, f_thr);
+    if (e == cudaSuccess) e = corpus_grow(h->d_ds_targets, ps.targets, f_targets);
     if (e != cudaSuccess) {
         cudaGetLastError();
         return fail(PB_ERR_CUDA, "corpus workspace allocation failed (%lld frame rows, %lld windows): %s", p.rows, p.W, cudaGetErrorString(e));
     }
     const bool grows = f_rows.get() || f_pairs.get() || f_starts.get() || f_win0.get() || f_frow.get() || f_recs.get() ||
                        f_groups.get() || f_ids.get() || f_raw.get() || f_ppairs.get() || f_pw0.get() || f_pstarts.get() ||
-                       f_tiles.get();
+                       f_tiles.get() || f_thr.get() || f_targets.get();
     if (grows) CK(cudaEventSynchronize(h->corpus_ev));            // the previous call may still read what is replaced
     if (f_rows.get()) h->d_cw_rows = std::move(f_rows);
     if (f_pairs.get()) h->d_cw_pairs = std::move(f_pairs);
@@ -1716,6 +1729,8 @@ static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, cons
     if (f_pw0.get()) h->d_pp_pw0 = std::move(f_pw0);
     if (f_pstarts.get()) h->d_pp_starts = std::move(f_pstarts);
     if (f_tiles.get()) h->d_pp_tiles = std::move(f_tiles);
+    if (f_thr.get()) h->d_ds_thr = std::move(f_thr);
+    if (f_targets.get()) h->d_ds_targets = std::move(f_targets);
     CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));                      // a corpus call on another stream may still use it
     return PB_OK;
 }
@@ -1750,7 +1765,9 @@ static int corpus_k1(pb_handle* h, const CorpusPlan& p, const int16_t* d_pcm, in
                                                                      c.hop_samples, h->used, scale, mel_tables(h), frames, h->row_stride);
         CK(cudaGetLastError());
     }
-    if (p.W > 0) {
+    if (!p.starts.empty()) {
+        CK(cudaMemcpyAsync(h->d_cw_starts.get(), p.starts.data(), p.starts.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    } else if (p.W > 0) {
         corpus_windows_kernel<<<(unsigned)((p.W + 255) / 256), 256, 0, s>>>(h->d_cw_win0.get(), h->d_cw_frow.get(), (int)n_rec, p.W, schedule, chunk,
                                                                           h->rel_window, c.hop_samples, c.n_features, h->d_cw_starts.get());
         CK(cudaGetLastError());
@@ -1877,6 +1894,31 @@ static int launch_pool_corpus_nm(int nm, bool keras, const PoolCorpus& c, const 
     return fail(PB_ERR_INVALID, "%d models per group", nm);
 }
 
+// The scan's groups of k requested models in batches of `rows`: within a batch, per activation class (Keras's defaults first
+// where they are compiled in), NM requested rows each in request order, a partial last group padded with row -1.  Batch b,
+// class ka: groups [g0[2b + ka], g0[2b + ka + 1]).
+static void pool_corpus_groups(const pb_handle* h, const int32_t* h_model_ids, int64_t k, int64_t rows, int NM,
+                               std::vector<int2>& groups, std::vector<int64_t>& g0) {
+    const bool split = pool_corpus_keras(NM);
+    const int64_t n_batches = (k + rows - 1) / rows;
+    g0.assign((size_t)n_batches * 2 + 1, 0);
+    for (int64_t b = 0; b < n_batches; ++b) {
+        const int64_t b0 = b * rows, b1 = std::min<int64_t>(k, b0 + rows);
+        for (int ka = 0; ka < 2; ++ka) {
+            g0[2 * b + ka] = (int64_t)groups.size() / NM;
+            int at = 0;
+            for (int64_t i = b0; i < b1; ++i) {
+                if ((split ? h->pool_keras[h_model_ids[i]] : 1) != ka) continue;
+                groups.push_back(make_int2(h_model_ids[i], (int)(i - b0)));
+                at = (at + 1) % NM;
+            }
+            for (const int2 first = at ? groups[groups.size() - at] : int2{}; at && at < NM; ++at)
+                groups.push_back(make_int2(first.x, -1));
+        }
+    }
+    g0[2 * n_batches] = (int64_t)groups.size() / NM;
+}
+
 PB_API int pb_debug_corpus_pool_rows(pb_handle* h, int64_t rows) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (rows < 0) return fail(PB_ERR_INVALID, "rows = %lld is negative", (long long)rows);
@@ -1925,28 +1967,12 @@ PB_API int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_
         if (h->corpus_pool_rows > 0) rows = std::min<int64_t>(rows, h->corpus_pool_rows);
         rows = std::min<int64_t>(rows, k);
     }
-    // the scan's groups, batch after batch: within a batch, per activation class (Keras's defaults first where they are
-    // compiled in), NM requested rows each in request order, a partial last group padded with row -1
     const int NM = h->corpus_pool_nm ? h->corpus_pool_nm : CORPUS_POOL_NM;
     const bool split = pool_corpus_keras(NM);
     const int64_t n_batches = (k + rows - 1) / rows;
     std::vector<int2> groups;
-    std::vector<int64_t> g0((size_t)n_batches * 2 + 1);                // batch b, class ka: groups [g0[2b + ka], g0[2b + ka + 1])
-    for (int64_t b = 0; b < n_batches; ++b) {
-        const int64_t b0 = b * rows, b1 = std::min<int64_t>(k, b0 + rows);
-        for (int ka = 0; ka < 2; ++ka) {
-            g0[2 * b + ka] = (int64_t)groups.size() / NM;
-            int at = 0;
-            for (int64_t i = b0; i < b1; ++i) {
-                if ((split ? h->pool_keras[h_model_ids[i]] : 1) != ka) continue;
-                groups.push_back(make_int2(h_model_ids[i], (int)(i - b0)));
-                at = (at + 1) % NM;
-            }
-            for (const int2 first = at ? groups[groups.size() - at] : int2{}; at && at < NM; ++at)
-                groups.push_back(make_int2(first.x, -1));
-        }
-    }
-    g0[2 * n_batches] = (int64_t)groups.size() / NM;
+    std::vector<int64_t> g0;
+    pool_corpus_groups(h, h_model_ids, k, rows, NM, groups, g0);
     CorpusPoolSizes ps;
     ps.groups = groups.size();
     ps.ids = (size_t)k;
@@ -2011,6 +2037,26 @@ static int launch_pairs_corpus(const PairsCorpus& c, const K2In& in, cudaStream_
     pairs_corpus_kernel<KERAS_ACT><<<dim3((unsigned)gx, (unsigned)gy), MMA_THREADS, BANK_MODEL_SMEM, s>>>(c, in);
     CK(cudaGetLastError());
     return PB_OK;
+}
+
+// Scan tiles of pairs p0 .. p1 - 1 (pool slot, recording), pair p's windows at P[p] .. P[p + 1] - 1: tiles of 64 pair-windows
+// within each run of one model, batch-local, the Keras-activation class first.  Returns that class's tile count.
+static int64_t pair_tiles(const pb_handle* h, const std::vector<int2>& pairs, const std::vector<long long>& P, int64_t p0,
+                          int64_t p1, std::vector<PairTile>& tiles) {
+    tiles.clear();
+    int64_t n_keras = 0;
+    for (int ka = 1; ka >= 0; --ka) {
+        for (int64_t a = p0; a < p1;) {
+            int64_t e = a + 1;
+            while (e < p1 && pairs[e].x == pairs[a].x) ++e;
+            if (h->pool_keras[pairs[a].x] == ka)
+                for (long long q = P[a]; q < P[e]; q += 64)
+                    tiles.push_back(PairTile{q - P[p0], pairs[a].x, (int)std::min<long long>(64, P[e] - q)});
+            a = e;
+        }
+        if (ka == 1) n_keras = (int64_t)tiles.size();
+    }
+    return n_keras;
 }
 
 PB_API int pb_debug_corpus_pairs_batch(pb_handle* h, int64_t windows) {
@@ -2119,20 +2165,7 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
                 pairs_windows_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(bpw0, bpairs, (int)nb, nw, h->d_cw_win0.get(),
                                                                                  h->d_cw_starts.get(), h->d_pp_starts.get());
                 CK(cudaGetLastError());
-                // tiles of 64 pair-windows within each run of one model, the Keras-activation class first
-                tiles.clear();
-                int64_t n_keras = 0;
-                for (int ka = 1; ka >= 0; --ka) {
-                    for (int64_t a = p0; a < p1;) {
-                        int64_t e = a + 1;
-                        while (e < p1 && pairs[e].x == pairs[a].x) ++e;
-                        if (h->pool_keras[pairs[a].x] == ka)
-                            for (long long q = P[a]; q < P[e]; q += 64)
-                                tiles.push_back(PairTile{q - q0, pairs[a].x, (int)std::min<long long>(64, P[e] - q)});
-                        a = e;
-                    }
-                    if (ka == 1) n_keras = (int64_t)tiles.size();
-                }
+                const int64_t n_keras = pair_tiles(h, pairs, P, p0, p1, tiles);
                 CK(cudaMemcpyAsync(h->d_pp_tiles.get(), tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
                 PairsCorpus c{};
                 c.slots = slots; c.starts = h->d_pp_starts.get(); c.raw = raw; c.conf = conf;
@@ -2165,6 +2198,198 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
                 pairs_hits_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(H);
                 CK(cudaGetLastError());
             }
+        }
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+// ------------------------------------------------------------------------------------------------
+// pool models over labelled clips (dataset.cuh)
+
+PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                            const uint8_t* h_targets, const int32_t* h_model_ids, int64_t k,
+                            const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs,
+                            int32_t divisor, int64_t max_samples, const double* h_thresholds, int32_t n_thr,
+                            float* d_raw, int64_t* d_count, int64_t* d_hist, int64_t* d_fit,
+                            double miss_threshold, int64_t* d_miss, int64_t miss_capacity, unsigned long long* d_n_miss,
+                            void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, PB_CORPUS_LISTENER, 1, d_raw, false, nullptr, nullptr);
+    if (rc != PB_OK) return rc;
+    const bool misses = d_n_miss != nullptr, stats = d_count || d_hist || d_fit || misses;
+    if (!d_raw && !stats) return fail(PB_ERR_INVALID, "every output is null");
+    if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
+    if (max_samples < 1) return fail(PB_ERR_INVALID, "max_samples = %lld must be >= 1", (long long)max_samples);
+    if (n_rec > 0 && !h_targets) return fail(PB_ERR_INVALID, "null h_targets");
+    for (int64_t r = 0; r < n_rec; ++r)
+        if (h_offsets[r + 1] == h_offsets[r]) return fail(PB_ERR_INVALID, "recording %lld is empty: cannot vectorize empty audio", (long long)r);
+    if (k < 0 || k > INT32_MAX / 2) return fail(PB_ERR_INVALID, "k = %lld outside [0, 2^30)", (long long)k);
+    if (k > 0 && !h_model_ids) return fail(PB_ERR_INVALID, "null h_model_ids");
+    for (int64_t i = 0; i < k; ++i) {
+        const int32_t m = h_model_ids[i];
+        if (m < 0 || m >= h->pool_models)
+            return fail(PB_ERR_INVALID, "model id %d (entry %lld) outside [0, max_models = %d)", m, (long long)i, h->pool_models);
+        if (h->pool_cd_of[m] == h->pool_cd.end())
+            return fail(PB_ERR_INVALID, "pool slot %d (entry %lld) holds no model: pb_pool_load it first", m, (long long)i);
+    }
+    if (n_pairs < 0 || n_pairs > INT32_MAX) return fail(PB_ERR_INVALID, "n_pairs = %lld outside [0, 2^31)", (long long)n_pairs);
+    const bool by_pairs = n_pairs > 0;
+    if (by_pairs && (!h_pair_rows || !h_pair_recs)) return fail(PB_ERR_INVALID, "null h_pair_rows or h_pair_recs");
+    for (int64_t i = 0; i < n_pairs; ++i) {
+        const int32_t row = h_pair_rows[i], r = h_pair_recs[i];
+        if (row < 0 || row >= k) return fail(PB_ERR_INVALID, "row %d (pair %lld) outside [0, k = %lld)", row, (long long)i, (long long)k);
+        if (r < 0 || r >= n_rec)
+            return fail(PB_ERR_INVALID, "recording id %d (pair %lld) outside [0, n_rec = %lld)", r, (long long)i, (long long)n_rec);
+    }
+    if (n_thr < 0 || n_thr > DS_MAX_THR) return fail(PB_ERR_INVALID, "n_thr = %d outside [0, %d]", n_thr, DS_MAX_THR);
+    if (d_hist && n_thr < 1) return fail(PB_ERR_INVALID, "d_hist needs at least one threshold");
+    if (n_thr > 0 && !h_thresholds) return fail(PB_ERR_INVALID, "null h_thresholds");
+    std::vector<float> thr((size_t)n_thr);
+    for (int i = 0; i < n_thr; ++i) {
+        thr[i] = (float)h_thresholds[i];
+        if (!(i == 0 ? thr[i] == thr[i] : thr[i] > thr[i - 1]))
+            return fail(PB_ERR_INVALID, "threshold %d = %g: rounded to float32, thresholds must be strictly ascending", i, h_thresholds[i]);
+    }
+    if (miss_capacity < 0) return fail(PB_ERR_INVALID, "miss_capacity = %lld is negative", (long long)miss_capacity);
+    if (miss_capacity > 0 && !d_miss) return fail(PB_ERR_INVALID, "null d_miss with miss_capacity = %lld", (long long)miss_capacity);
+    if (d_miss && !misses) return fail(PB_ERR_INVALID, "d_miss without d_n_miss");
+    if (d_fit) {
+        // the fit's int64 sums hold 2^24 entries of one (row, label)
+        const int64_t limit = 1ll << 24;
+        if (by_pairs) {
+            std::vector<int64_t> per((size_t)k * 2, 0);
+            for (int64_t i = 0; i < n_pairs; ++i)
+                if (++per[(size_t)h_pair_rows[i] * 2 + (h_targets[h_pair_recs[i]] != 0)] > limit)
+                    return fail(PB_ERR_INVALID, "row %d has more than 2^24 entries of one label: split the call", h_pair_rows[i]);
+        } else {
+            int64_t pos = 0;
+            for (int64_t r = 0; r < n_rec; ++r) pos += h_targets[r] != 0;
+            if (k > 0 && std::max(pos, n_rec - pos) > limit)
+                return fail(PB_ERR_INVALID, "%lld recordings of one label, more than 2^24: split the call", (long long)std::max(pos, n_rec - pos));
+        }
+    }
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int bins = 2 * n_thr + 1;
+    auto zero = [&]() -> int {
+        if (d_count) CK(cudaMemsetAsync(d_count, 0, (size_t)k * 2 * sizeof(int64_t), s));
+        if (d_hist) CK(cudaMemsetAsync(d_hist, 0, (size_t)k * 2 * bins * sizeof(int64_t), s));
+        if (d_fit) CK(cudaMemsetAsync(d_fit, 0, (size_t)k * 6 * sizeof(int64_t), s));
+        if (misses) CK(cudaMemsetAsync(d_n_miss, 0, sizeof(unsigned long long), s));
+        return PB_OK;
+    };
+    if (n_rec == 0 || k == 0) return zero();
+    const CorpusPlan plan = corpus_plan(h, d_pcm, h_offsets, n_rec, PB_CORPUS_LISTENER, 1, max_samples);
+    // entries per batch: all of them into the caller's d_raw, else as many as the capped raw buffer holds; the cross product
+    // in whole rows, pairs in runs of consecutive pairs
+    const int NM = h->corpus_pool_nm ? h->corpus_pool_nm : CORPUS_POOL_NM;
+    int64_t rows = k, cap = 0;
+    std::vector<int2> groups, slot_pairs, row_pairs;
+    std::vector<int64_t> g0;
+    std::vector<long long> P;
+    CorpusPoolSizes ps;
+    ps.thr = d_hist ? (size_t)n_thr : 0;
+    ps.targets = stats ? (size_t)n_rec : 0;
+    if (by_pairs) {
+        cap = std::min<int64_t>(n_pairs, h->corpus_pairs_batch > 0 ? h->corpus_pairs_batch : CORPUS_PAIRS_BATCH);
+        slot_pairs.resize((size_t)n_pairs);
+        row_pairs.resize((size_t)n_pairs);
+        P.resize((size_t)n_pairs + 1);
+        for (int64_t i = 0; i < n_pairs; ++i) {
+            slot_pairs[i] = make_int2(h_model_ids[h_pair_rows[i]], h_pair_recs[i]);
+            row_pairs[i] = make_int2(h_pair_rows[i], h_pair_recs[i]);
+            P[i] = i;
+        }
+        P[n_pairs] = n_pairs;
+        ps.raw = !d_raw ? (size_t)cap : 0;
+        ps.pairs = (size_t)n_pairs;
+        ps.pw0 = (size_t)cap + 1;
+        ps.starts = (size_t)cap;
+        for (int64_t p0 = 0; p0 < n_pairs; p0 += cap) {               // the scan tiles of the largest batch
+            const int64_t p1 = std::min(n_pairs, p0 + cap);
+            size_t tiles = 0;
+            for (int64_t a = p0, e; a < p1; a = e) {
+                for (e = a + 1; e < p1 && slot_pairs[e].x == slot_pairs[a].x;) ++e;
+                tiles += (size_t)((e - a + 63) / 64);
+            }
+            ps.tiles = std::max(ps.tiles, tiles);
+        }
+    } else {
+        if (!d_raw) {
+            rows = std::max<int64_t>(1, CORPUS_POOL_RAW_CAP / (4 * n_rec));
+            if (h->corpus_pool_rows > 0) rows = std::min<int64_t>(rows, h->corpus_pool_rows);
+            rows = std::min<int64_t>(rows, k);
+        }
+        pool_corpus_groups(h, h_model_ids, k, rows, NM, groups, g0);
+        ps.groups = groups.size();
+        ps.raw = !d_raw ? (size_t)(rows * n_rec) : 0;
+    }
+    rc = corpus_reserve(h, plan, n_rec, ps, s);
+    if (rc != PB_OK) return rc;
+    auto launch = [&]() -> int {
+        rc = corpus_k1(h, plan, d_pcm, n_rec, divisor, PB_CORPUS_LISTENER, 1, s);
+        if (rc != PB_OK) return rc;
+        rc = zero();
+        if (rc != PB_OK) return rc;
+        if (d_hist) CK(cudaMemcpyAsync(h->d_ds_thr.get(), thr.data(), thr.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (stats) CK(cudaMemcpyAsync(h->d_ds_targets.get(), h_targets, (size_t)n_rec, cudaMemcpyHostToDevice, s));
+        ProfScope prof(h, 1, s);
+        const K2In in = corpus_k2in(h);
+        DatasetStats D{};
+        D.targets = h->d_ds_targets.get(); D.thr = d_hist ? h->d_ds_thr.get() : nullptr; D.n_thr = n_thr;
+        D.count = d_count; D.hist = d_hist; D.fit = d_fit;
+        D.miss_thr = (float)miss_threshold; D.miss = d_miss; D.capacity = miss_capacity; D.n_miss = d_n_miss;
+        if (!by_pairs) {
+            CK(cudaMemcpyAsync(h->d_cp_groups.get(), groups.data(), groups.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+            const bool split = pool_corpus_keras(NM);
+            const int order = h->corpus_pool_order >= 0 ? h->corpus_pool_order : CORPUS_POOL_GROUPS_FAST;
+            for (int64_t b0 = 0, b = 0; b0 < k; b0 += rows, ++b) {
+                const int64_t nb = std::min<int64_t>(k, b0 + rows) - b0;
+                float* raw = d_raw ? d_raw + b0 * n_rec : h->d_cp_raw.get();
+                PoolCorpus c{};
+                c.slots = h->d_pool_slots.get(); c.n_tiles = (n_rec + 63) / 64; c.raw = raw; c.W = n_rec; c.groups_fast = order;
+                for (int ka = 0; ka < 2; ++ka) {
+                    c.groups = h->d_cp_groups.get() + g0[2 * b + ka] * NM;
+                    c.n_groups = g0[2 * b + ka + 1] - g0[2 * b + ka];
+                    rc = launch_pool_corpus_nm(NM, split && ka == 1, c, in, s);
+                    if (rc != PB_OK) return rc;
+                }
+                if (!stats) continue;
+                const unsigned gx = (unsigned)((n_rec + DS_THREADS * DS_ITERS - 1) / (DS_THREADS * DS_ITERS));
+                for (int64_t y0 = 0; y0 < nb; y0 += 65535) {          // gridDim.y
+                    D.raw = raw + y0 * n_rec; D.row0 = (int)(b0 + y0); D.n = n_rec;
+                    dataset_stats_kernel<false><<<dim3(gx, (unsigned)std::min<int64_t>(65535, nb - y0)), DS_THREADS, 0, s>>>(D);
+                    CK(cudaGetLastError());
+                }
+            }
+            return PB_OK;
+        }
+        CK(cudaMemcpyAsync(h->d_pp_pairs.get(), row_pairs.data(), row_pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_pp_pw0.get(), P.data(), (size_t)(cap + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+        std::vector<PairTile> tiles;
+        for (int64_t p0 = 0; p0 < n_pairs; p0 += cap) {
+            const int64_t p1 = std::min(n_pairs, p0 + cap), nb = p1 - p0;
+            const int2* bpairs = h->d_pp_pairs.get() + p0;
+            float* raw = d_raw ? d_raw + p0 : h->d_cp_raw.get();
+            // one pair-window per pair: the batch's prefix is 0 .. nb
+            pairs_windows_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, s>>>(h->d_pp_pw0.get(), bpairs, (int)nb, nb, h->d_cw_win0.get(),
+                                                                             h->d_cw_starts.get(), h->d_pp_starts.get());
+            CK(cudaGetLastError());
+            const int64_t n_keras = pair_tiles(h, slot_pairs, P, p0, p1, tiles);
+            CK(cudaMemcpyAsync(h->d_pp_tiles.get(), tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
+            PairsCorpus c{};
+            c.slots = h->d_pool_slots.get(); c.starts = h->d_pp_starts.get(); c.raw = raw;
+            c.tiles = h->d_pp_tiles.get(); c.n_tiles = n_keras;
+            rc = launch_pairs_corpus<true>(c, in, s);
+            if (rc != PB_OK) return rc;
+            c.tiles += n_keras; c.n_tiles = (int64_t)tiles.size() - n_keras;
+            rc = launch_pairs_corpus<false>(c, in, s);
+            if (rc != PB_OK) return rc;
+            if (!stats) continue;
+            D.raw = raw; D.pairs = bpairs; D.n = nb; D.base = p0;
+            dataset_stats_kernel<true><<<(unsigned)((nb + DS_THREADS - 1) / DS_THREADS), DS_THREADS, 0, s>>>(D);
+            CK(cudaGetLastError());
         }
         return PB_OK;
     };

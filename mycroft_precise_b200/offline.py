@@ -18,12 +18,18 @@ Recorded corpora (many recordings per device call, no window materialised: pb_sc
   simulate_pairs    simulate for each pool model over its own recordings
   false_activations ~ precise/scripts/train_incremental.py:113-137 (train_on_audio's selection of clips, fixed weights)
   false_activations_pool  the same selection for pool models, the chunks above the threshold found on the device
+
+Labelled clips (one network input per clip, vectorize's; statistics per pool model on the device: pb_score_dataset):
+  DatasetStats      ~ precise/stats.py (Stats' counts, rates and format strings, from the device's histograms)
+  test_pool         ~ precise/scripts/test.py, eval.py for many pool models in one device call per batch of clips
+  graph_thresholds, roc ~ precise/scripts/graph.py:147-152 (the thresholds and the curve precise-graph plots)
+  calc_threshold    ~ precise/scripts/calc_threshold.py:66-83 (a model's threshold_config from its positive clips)
 """
 from dataclasses import dataclass
 
 import numpy as np
 
-from .core import PreciseB200
+from .core import PreciseB200, threshold_encode
 
 
 def _as_device_audio(core: PreciseB200, audio):
@@ -420,3 +426,192 @@ def false_activations_pool(core: PreciseB200, recordings, model_ids, rec_ids=Non
             host[r] = a if isinstance(a, np.ndarray) else a.cpu().numpy()
         out.append((p, r, k, _clip(host[r], (k + 1) * c, bs)))
     return out
+
+
+COUNTS_STR = """=== Counts ===
+False Positives: {false_pos}
+True Negatives: {true_neg}
+False Negatives: {false_neg}
+True Positives: {true_pos}"""
+
+SUMMARY_STR = """
+=== Summary ===
+{num_correct} out of {total}
+{accuracy_ratio:.2%}
+
+{false_pos_ratio:.2%} false positives
+{false_neg_ratio:.2%} false negatives
+"""
+
+
+class DatasetStats:
+    """One model's statistics over labelled clips, as pb_score_dataset returns them: count [2] (clips per label, 1 = wake
+    word), hist [2, 2 n + 1] (the outputs binned at and between the n float32 thresholds) and fit [2, 3] (calc_threshold's
+    sums), all int64.  It answers what precise/stats.py's Stats answers from the outputs themselves, at the thresholds the
+    call was given: any other threshold raises KeyError.  Two DatasetStats over the same thresholds add."""
+
+    def __init__(self, thresholds, count, hist, fit):
+        self.thresholds = np.asarray(thresholds, np.float32)
+        self.count = np.asarray(count, np.int64)
+        self.hist = np.asarray(hist, np.int64)
+        self.fit = np.asarray(fit, np.int64)
+        if self.count.shape != (2,) or self.hist.shape != (2, 2 * self.thresholds.shape[0] + 1) or self.fit.shape != (2, 3):
+            raise ValueError('count [2], hist [2, 2 n_thr + 1] and fit [2, 3] expected')
+
+    def __add__(self, other):
+        if not np.array_equal(self.thresholds, other.thresholds):
+            raise ValueError('statistics over different thresholds do not add')
+        return DatasetStats(self.thresholds, self.count + other.count, self.hist + other.hist, self.fit + other.fit)
+
+    def __len__(self):
+        return int(self.count.sum())
+
+    def _above(self, label, threshold, equal):
+        """#(output > threshold) of one label, or with ``equal`` #(output >= threshold); float32 comparisons, as numpy's."""
+        t = np.float32(threshold)
+        j = int(np.searchsorted(self.thresholds, t))
+        if j == self.thresholds.shape[0] or self.thresholds[j] != t:
+            raise KeyError('threshold %r is not one of this call\'s' % (threshold,))
+        return int(self.hist[label, 2 * j + (1 if equal else 2):].sum())
+
+    def true_pos(self, threshold=0.5):
+        return self._above(1, threshold, False)
+
+    def false_pos(self, threshold=0.5):
+        return self._above(0, threshold, False)
+
+    def true_neg(self, threshold=0.5):
+        return int(self.count[0]) - self.false_pos(threshold)
+
+    def false_neg(self, threshold=0.5):
+        return int(self.count[1]) - self.true_pos(threshold)
+
+    def false_positives(self, threshold=0.5):
+        return self.false_pos(threshold) / max(1, int(self.count[0]))
+
+    def false_negatives(self, threshold=0.5):
+        return self.false_neg(threshold) / max(1, int(self.count[1]))
+
+    def num_correct(self, threshold=0.5):
+        """Stats.num_correct (stats.py:54-56) compares with >=, where the counts above compare with >."""
+        return self._above(1, threshold, True) + int(self.count[0]) - self._above(0, threshold, True)
+
+    def num_incorrect(self, threshold=0.5):
+        return len(self) - self.num_correct(threshold)
+
+    def accuracy(self, threshold=0.5):
+        return self.num_correct(threshold) / max(1, len(self))
+
+    def counts_str(self, threshold=0.5):
+        return COUNTS_STR.format(false_pos=self.false_pos(threshold), true_neg=self.true_neg(threshold),
+                                 false_neg=self.false_neg(threshold), true_pos=self.true_pos(threshold))
+
+    def summary_str(self, threshold=0.5):
+        return SUMMARY_STR.format(num_correct=self.num_correct(threshold), total=len(self),
+                                  accuracy_ratio=self.accuracy(threshold), false_pos_ratio=self.false_positives(threshold),
+                                  false_neg_ratio=self.false_negatives(threshold))
+
+
+def _pack_clips(core: PreciseB200, clips):
+    """Clips -> (1-D int16 device tensor, host int64 offsets [n + 1], clip index of each entry), each clip cropped to the
+    last max_samples samples the network sees and packed back to back: pb_score_dataset's cross product scores every entry,
+    so there are no padding entries.  Clips whose length is a multiple of 8 samples go first, so that all of them start
+    aligned and take the fast MFCC kernel at the default geometry."""
+    torch = core.torch
+    ms = core.params.max_samples
+    clips = [c[-ms:] if int(c.shape[0]) > ms else c for c in clips]
+    order = sorted(range(len(clips)), key=lambda i: int(clips[i].shape[0]) % 8 != 0)
+    offsets = np.concatenate([[0], np.cumsum([int(clips[i].shape[0]) for i in order], dtype=np.int64)]).astype(np.int64)
+    pcm = torch.zeros(max(int(offsets[-1]), 1), dtype=torch.int16, device=core.device)
+    for e, i in enumerate(order):
+        c = clips[i]
+        pcm[offsets[e]:offsets[e + 1]].copy_(torch.from_numpy(np.ascontiguousarray(c)) if isinstance(c, np.ndarray) else c)
+    return pcm, offsets, np.asarray(order, np.int64)
+
+
+def test_pool(core: PreciseB200, clips, targets, model_ids, rows=None, recs=None, thresholds=(0.5,), misses=False,
+              miss_threshold=0.5):
+    """precise-test's statistics for pool models ``model_ids`` (int32 [k]) over labelled ``clips`` (1-D int16 numpy arrays or
+    CUDA tensors read as load_audio reads them, none empty; targets[c] non-zero = wake word).  rows / recs None: every model
+    over every clip.  Otherwise entry p is model_ids[rows[p]] over clips[recs[p]]: each word over its owner's clips.  Clips
+    are split into library calls as score_corpus splits recordings, and the calls' statistics are added.  Returns a list of
+    k DatasetStats; with misses=True also a list of k sorted arrays, the clip indices model i misclassifies at
+    ``miss_threshold`` ((output > miss_threshold) != label, Stats.calc_filenames' rule).  Only statistics and misclassified
+    indices leave the device."""
+    clips = [_check_recording(core, c) for c in clips]
+    targets = np.ascontiguousarray(np.asarray(targets) != 0, dtype=np.uint8)
+    model_ids = np.ascontiguousarray(model_ids, dtype=np.int32)
+    if targets.shape != (len(clips),):
+        raise ValueError('one target per clip')
+    k = model_ids.shape[0]
+    if (rows is None) != (recs is None):
+        raise ValueError('rows and recs come together')
+    if rows is not None:
+        rows, recs = np.ascontiguousarray(rows, dtype=np.int32), np.ascontiguousarray(recs, dtype=np.int64)
+        if rows.ndim != 1 or rows.shape != recs.shape:
+            raise ValueError('rows and recs must be 1-D arrays of one length')
+        if rows.size and (recs.min() < 0 or recs.max() >= len(clips) or rows.min() < 0 or rows.max() >= k):
+            raise ValueError('rows must lie in [0, %d) and recs in [0, %d)' % (k, len(clips)))
+    thr = np.unique(np.asarray(thresholds, np.float32))
+    n_thr = thr.shape[0]
+    count, hist, fit = np.zeros((k, 2), np.int64), np.zeros((k, 2, 2 * n_thr + 1), np.int64), np.zeros((k, 2, 3), np.int64)
+    missed = [[] for _ in range(k)]
+    first = 0
+    for g in _call_groups(clips):
+        pcm, offsets, order = _pack_clips(core, g)
+        entry = np.empty(len(g), np.int64)                    # clip (within the group) -> entry of the call
+        entry[order] = np.arange(len(g))
+        tg = np.ascontiguousarray(targets[first + order])
+        kw = dict(thresholds=thr.astype(np.float64), per_entry=False, miss_threshold=miss_threshold if misses else None)
+        if rows is None:
+            res = core.score_dataset(pcm, offsets, tg, model_ids, **kw)
+        else:
+            sel = np.nonzero((recs >= first) & (recs < first + len(g)))[0]
+            res = core.score_dataset(pcm, offsets, tg, model_ids, rows[sel], entry[recs[sel] - first].astype(np.int32), **kw)
+        count += res['count'].cpu().numpy()
+        hist += res['hist'].cpu().numpy()
+        fit += res['fit'].cpu().numpy()
+        if misses:
+            q = res['misses'].cpu().numpy()
+            if rows is None:
+                for i, e in zip((q // len(g)).tolist(), (q % len(g)).tolist()):
+                    missed[i].append(first + int(order[e]))
+            else:
+                for p in sel[q].tolist():
+                    missed[int(rows[p])].append(int(recs[p]))
+        first += len(g)
+    stats = [DatasetStats(thr, count[i], hist[i], fit[i]) for i in range(k)]
+    if misses:
+        return stats, [np.asarray(sorted(m), np.int64) for m in missed]
+    return stats
+
+
+test_pool.__test__ = False        # not a pytest test, whatever module imports it
+
+
+def graph_thresholds(params, resolution=100):
+    """The network outputs precise-graph evaluates (graph.py:147-148): ThresholdDecoder.encode of
+    linspace(0, 1, resolution)[1:-1] under the model's threshold_config and center, sorted and de-duplicated in float32 (the
+    precision the outputs are compared in)."""
+    enc = threshold_encode(params.threshold_config, params.threshold_center, np.linspace(0.0, 1.0, resolution)[1:-1])
+    return np.unique(enc.astype(np.float32))
+
+
+def roc(stats: DatasetStats):
+    """(false-positive rates, false-negative rates) over the statistics' thresholds, ascending: precise-graph's x and y."""
+    t = stats.thresholds
+    return (np.asarray([stats.false_positives(v) for v in t]), np.asarray([stats.false_negatives(v) for v in t]))
+
+
+def calc_threshold(stats: DatasetStats, smoothing=1.2):
+    """precise-calc-threshold's (mu, std) (calc_threshold.py:66-76) from the wake-word clips' fit sums: the mean of
+    v = -log(1 / output - 1) over outputs other than 0 and 1, and sqrt(mean(v^2) - mu^2) * smoothing; the model's
+    threshold_config is ((mu, std),).  None when no wake-word clip's output lies strictly between 0 and 1 (the reference
+    prints "No data").  The reference computes v and both means in float32; here v is a double (of the float32
+    1 / output - 1) summed in fixed point, exact to 2^-32 in mu."""
+    n, s1, s2 = (int(v) for v in stats.fit[1])
+    if n == 0:
+        return None
+    mu = s1 / 2.0 ** 32 / n
+    var = s2 / 2.0 ** 24 / n - mu * mu
+    return mu, float(np.sqrt(max(var, 0.0))) * smoothing
