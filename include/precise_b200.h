@@ -597,6 +597,81 @@ int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offset
                      double miss_threshold, int64_t* d_miss, int64_t miss_capacity, unsigned long long* d_n_miss,
                      void* stream);
 
+/* ---- training (csrc/train.cuh): precise-train and precise-train-incremental's Keras fit (precise/model.py:57-91,
+ * scripts/train.py:159-166, scripts/train_incremental.py:96-111) for many fused-family networks at once ---- */
+
+/* The network input of each labelled clip, vectorize(clip) (precise/vectorization.py:62-84), as pb_score_dataset builds it:
+ * recording r cropped to its last max_samples samples, the last n_features MFCC rows, zero rows in front when there are
+ * fewer.  d_inputs [n_rec][n_features][feature_size] (DEVICE) receives rows bit-identical to the windows pb_score_dataset's
+ * scans read.  Needs no pool.  Ordered against the corpus calls as pb_score_corpus (it shares their workspace).
+ * PB_ERR_INVALID: pb_score_dataset's refusals of the clips (null or decreasing offsets, an empty recording, divisor,
+ * max_samples < 1) and a null d_inputs.  PB_ERR_UNSUPPORTED: a front end outside the fused family (deltas, or feature size
+ * > 16).  PB_ERR_CUDA: the workspace cannot be allocated. */
+int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
+                       int64_t max_samples, float* d_inputs, void* stream);
+
+/* Floats per network of pb_train's weight and accumulator arrays.  A row holds Keras's order, flat: kernel[F][3H],
+ * recurrent[H][3H], bias[3H], dense_w[H], dense_b; the tail after 3H(F + H + 1) + H + 1 floats (2 977 at H = 24, F = 16) is
+ * zero and stays zero. */
+#define PB_TRAIN_STRIDE 2980
+
+/* One trained network: hidden size (1 .. 24), PB_ACT_* and PB_RACT_* codes, and the seed of its shuffles and dropout masks. */
+typedef struct pb_train_row {
+    int32_t hidden;
+    int32_t activation;
+    int32_t recurrent_activation;
+    uint32_t seed;
+} pb_train_row;
+
+/* Training settings (pb_train_opts_default: scripts/train.py's -e 10, -b 5000, -s 0.2 -> loss_bias 0.8 (train.py:86),
+ * model.py:80's dropout 0.2, Keras RMSprop's lr 0.001, rho 0.9, epsilon 1e-7). */
+typedef struct pb_train_opts {
+    int32_t epochs;            /* >= 1                                                            */
+    int32_t epoch0;            /* epoch number of the first epoch (>= 0): the shuffles and masks of a resumed fit */
+    int32_t batch_size;        /* >= 1                                                            */
+    float lr, rho, epsilon;    /* RMSprop: a = rho a + (1 - rho) g^2; w -= lr g / (sqrt(a) + epsilon) */
+    float loss_bias;           /* [0, 1]: 1 - sensitivity                                          */
+    float dropout;             /* [0, 1): input dropout rate                                      */
+} pb_train_opts;
+
+int pb_train_opts_default(pb_train_opts* opts);
+
+/* Trains k networks on the handle's front end (feature size F, n_features steps T) over network inputs d_inputs
+ * [n_rec][T][F] (DEVICE, pb_vectorize_clips') with labels h_targets [n_rec] (HOST, non-zero = wake word).
+ *   - Entries as in pb_score_dataset: without pairs (n_pairs = 0) every row trains on every clip; with pairs, entry p belongs to
+ *     row h_pair_rows[p] and uses clip h_pair_recs[p] (both HOST).  j, an entry's index within its row, counts in request order.
+ *   - Per row and epoch e (epoch0 .. epoch0 + epochs - 1): the entries are sorted by (key(s, e, j, 0), j), cut into consecutive
+ *     batches of batch_size (the last may be short) and each batch makes one RMSprop update of the mean loss over it:
+ *     loss_bias mean(-(1-y) log(1-p+1e-7)) + (1-loss_bias) mean(-y log(p+1e-7)) (precise/functions.py:39-50), p the network's
+ *     output with the entry's input dropout: feature f reaches gate g (z, r, h) scaled by 1.0f / (1.0f - dropout) iff
+ *     float32((key(s, e, j, 1 + 3f + g) >> 40) 2^-24) >= dropout, else 0.  key(s, e, j, c) = mix(mix(mix(mix(s) + e) + j) + c) on
+ *     uint64, mix the splitmix64 finalizer, s the row's seed.  Arithmetic is float32.
+ *   - d_weights and d_rms [k][PB_TRAIN_STRIDE] (DEVICE) are read and updated in place: the optimizer's accumulators survive
+ *     between calls, as the repeated fit of train_incremental keeps them.  d_loss [k][epochs] (DEVICE, optional) receives each
+ *     epoch's loss, the batch-size-weighted mean of its batch losses (what Keras prints), as double.  A row with no entries is
+ *     left untouched and its losses are NaN.
+ *   - Results are bit-identical run to run, for a row alone or among any other rows in any order, and for E epochs in one call
+ *     or in E calls with epoch0 advancing.
+ *   - Asynchronous on `stream`, ordered against the corpus calls as pb_score_corpus.  Rows are trained in groups whose
+ *     workspace stays under 256 MB.  Every argument is checked before anything is enqueued, so a refused call changes no buffer.
+ * PB_ERR_INVALID: a null handle, opts, h_rows (k > 0), d_weights or d_rms (k > 0), d_inputs or h_targets (with entries), k
+ * outside [0, 2^30), n_rec outside [0, 2^31), hidden outside [1, 24], an unknown activation code, n_pairs outside [0, 2^31), one
+ * null pair array, a row outside [0, k), a clip outside [0, n_rec), epochs < 1, epoch0 < 0, batch_size < 1, a non-finite or
+ * negative lr or epsilon, rho outside [0, 1), loss_bias outside [0, 1], dropout outside [0, 1).  PB_ERR_UNSUPPORTED: a front end
+ * outside the fused family (deltas, or feature size > 16) or n_features > 112.  PB_ERR_CUDA: the workspace cannot be allocated. */
+int pb_train(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows, int64_t k,
+             const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
+             float* d_weights, float* d_rms, double* d_loss, void* stream);
+
+/* Each row's loss over all its entries as one batch, in request order, with the dropout masks of `epoch` (dropout 0: Keras's
+ * evaluate, the val_loss train.py monitors), from d_weights (DEVICE, read only).  d_loss [k] (DEVICE) receives it (NaN for a
+ * row with no entries); d_grad [k][PB_TRAIN_STRIDE] (DEVICE, optional) its gradient in the row layout (a row with no entries is
+ * left untouched).  pb_train computes its updates with the same kernels.  Refusals as pb_train's, plus epoch < 0 and d_loss
+ * and d_grad both null. */
+int pb_train_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                  int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
+                  float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream);
+
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);

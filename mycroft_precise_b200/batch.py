@@ -81,6 +81,27 @@ class StreamBatch:
             self.pool_load(int(mid), model, pr, sens, lvl, legacy)
         return fits
 
+    def pool_train(self, model_ids, models, clips, targets, rows=None, recs=None, seeds=None, **opts):
+        """precise-train for pool slots ``model_ids`` (int32 [k]) starting from ``models`` (k GruModels, e.g. the slots'
+        current networks or GruModel.init), on labelled ``clips`` (1-D int16, read as load_audio reads them; targets non-zero =
+        wake word): rows / recs as offline.train takes them, ``opts`` its keyword arguments, seeds [k] (default 0 .. k-1).
+        Each trained network is loaded into its slot through pool_load with the slot's earlier settings (those of this batch's
+        pool_load, or the defaults), which re-arms its streams as a newly loaded model does.  Returns the k trained GruModels."""
+        from .offline import TrainState, train, vectorize_clips
+        from .runner import _resolve_model
+        inputs = vectorize_clips(self.core, clips)
+        state = TrainState.from_models(self.core, models, range(len(models)) if seeds is None else seeds)
+        train(self.core, state, inputs, targets, rows, recs, **opts)
+        out = state.models()
+        for mid, m in zip(model_ids, out):
+            spec = self._pool_specs.get(int(mid))
+            if spec is None:
+                self.pool_load(int(mid), m)
+                continue
+            model, params, sens, lvl, legacy = spec
+            self.pool_load(int(mid), m, params or _resolve_model(model)[1] or self.pr, sens, lvl, legacy)
+        return out
+
     def set_stream_pool(self, model_ids, ids=None):
         """Each stream's pool model (host int32, -1 = none).  See PreciseB200.set_stream_pool."""
         self.core.set_stream_pool(model_ids, ids)

@@ -39,6 +39,18 @@ class pb_config(C.Structure):
     ]
 
 
+PB_TRAIN_STRIDE = 2980             # floats per network of pb_train's weight and accumulator rows
+
+
+class pb_train_row(C.Structure):
+    _fields_ = [('hidden', C.c_int32), ('activation', C.c_int32), ('recurrent_activation', C.c_int32), ('seed', C.c_uint32)]
+
+
+class pb_train_opts(C.Structure):
+    _fields_ = [('epochs', C.c_int32), ('epoch0', C.c_int32), ('batch_size', C.c_int32), ('lr', C.c_float), ('rho', C.c_float),
+                ('epsilon', C.c_float), ('loss_bias', C.c_float), ('dropout', C.c_float)]
+
+
 # name -> (restype, argtypes); must list every symbol include/precise_b200.h declares
 _VP, _I64, _I32 = C.c_void_p, C.c_int64, C.c_int32
 SYMBOLS = {
@@ -89,6 +101,10 @@ SYMBOLS = {
                                         _VP, _VP, C.c_double, _VP, _I64, _VP, _VP]),
     'pb_score_dataset': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, _I32, _I64, _VP, _I32, _VP, _VP, _VP, _VP,
                                    C.c_double, _VP, _I64, _VP, _VP]),
+    'pb_vectorize_clips': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I64, _VP, _VP]),
+    'pb_train_opts_default': (C.c_int, [C.POINTER(pb_train_opts)]),
+    'pb_train': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.POINTER(pb_train_opts), _VP, _VP, _VP, _VP]),
+    'pb_train_loss': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.c_float, C.c_float, _I32, _VP, _VP, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -1024,6 +1040,88 @@ class PreciseB200:
                 d_miss = run(cap)
             out['misses'] = torch.sort(d_miss[:total])[0]
         return out
+
+    # ---- training (pb_vectorize_clips, pb_train, pb_train_loss)
+    def vectorize_clips(self, pcm, offsets, divisor=32767):
+        """The network input of each clip pcm[offsets[r]:offsets[r + 1]] (as score_dataset takes them; none empty): float32
+        [n_rec, n_features, feature_size] on the device, vectorize(clip) of the last params.max_samples samples, bit for bit
+        the window score_dataset scores.  Asynchronous on the current stream.  pb_vectorize_clips in include/precise_b200.h."""
+        offsets, n_rec = self._corpus_recordings(pcm, offsets)
+        out = self.torch.empty((n_rec, self.n_features, self.feature_size), dtype=self.torch.float32, device=self.device)
+        check(self.lib.pb_vectorize_clips(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, int(divisor), int(self.params.max_samples),
+                                          _ptr(out), self._stream()))
+        return out
+
+    def _train_args(self, inputs, targets, k, rows_of, recs, weights):
+        """(n_rec, targets, pair rows, pair recs, n_pairs) of a training call, checked."""
+        torch = self.torch
+        if (not isinstance(inputs, torch.Tensor) or inputs.dtype != torch.float32 or not inputs.is_contiguous()
+                or inputs.device != self.device or inputs.dim() != 3 or tuple(inputs.shape[1:]) != (self.n_features, self.feature_size)):
+            raise ValueError('inputs must be a contiguous float32 tensor [n, %d, %d] on %s' % (self.n_features, self.feature_size,
+                                                                                              self.device))
+        n_rec = inputs.shape[0]
+        targets = np.ascontiguousarray(np.asarray(targets) != 0, dtype=np.uint8)
+        if targets.shape != (n_rec,):
+            raise ValueError('one target per input')
+        self._check_t('weights', weights, torch.float32, k * PB_TRAIN_STRIDE, optional=False)
+        if (rows_of is None) != (recs is None):
+            raise ValueError('rows_of and recs come together')
+        if rows_of is None:
+            return n_rec, targets, None, None, 0
+        pr, pc = np.ascontiguousarray(rows_of, dtype=np.int32), np.ascontiguousarray(recs, dtype=np.int32)
+        if pr.ndim != 1 or pr.shape != pc.shape:
+            raise ValueError('rows_of and recs must be 1-D arrays of one length')
+        return n_rec, targets, pr, pc, pr.shape[0]
+
+    @staticmethod
+    def train_rows(hidden, activation, recurrent_activation, seed):
+        """ctypes array of pb_train_row from per-row lists (activation names as GruModel holds them)."""
+        acts = {'linear': 0, 'tanh': 1}
+        racts = {'hard_sigmoid': 0, 'sigmoid': 1}
+        k = len(hidden)
+        arr = (pb_train_row * max(k, 1))()
+        for i in range(k):
+            arr[i] = pb_train_row(int(hidden[i]), acts[activation[i]], racts[recurrent_activation[i]], int(seed[i]) & 0xFFFFFFFF)
+        return arr, k
+
+    def train(self, inputs, targets, rows, weights, rms, rows_of=None, recs=None, epochs=10, epoch0=0, batch_size=5000, lr=0.001,
+              rho=0.9, epsilon=1e-7, loss_bias=0.8, dropout=0.2):
+        """pb_train: trains the k networks of ``rows`` (train_rows' array) in place in ``weights`` and ``rms`` (float32 CUDA
+        tensors [k, PB_TRAIN_STRIDE]) over ``inputs`` (vectorize_clips' tensor) with labels ``targets`` (host, non-zero = wake
+        word).  rows_of / recs None: every network on every input; otherwise entry p is input recs[p] of network rows_of[p].
+        Returns the float64 epoch losses [k, epochs] (NaN for a network without entries) on the device.  Asynchronous on the
+        current stream.  pb_train in include/precise_b200.h."""
+        arr, k = rows
+        n_rec, targets, pr, pc, n = self._train_args(inputs, targets, k, rows_of, recs, weights)
+        self._check_t('rms', rms, self.torch.float32, k * PB_TRAIN_STRIDE, optional=False)
+        o = pb_train_opts()
+        check(self.lib.pb_train_opts_default(C.byref(o)))
+        o.epochs, o.epoch0, o.batch_size = int(epochs), int(epoch0), int(batch_size)
+        o.lr, o.rho, o.epsilon, o.loss_bias, o.dropout = lr, rho, epsilon, loss_bias, dropout
+        loss = self.torch.empty((k, max(int(epochs), 0)), dtype=self.torch.float64, device=self.device)
+        if rows_of is not None and n == 0:                     # no entry (the library reads an empty pair list as "every pair")
+            loss.fill_(float('nan'))
+            return loss
+        check(self.lib.pb_train(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n, C.byref(o),
+                                _ptr(weights), _ptr(rms), _ptr(loss), self._stream()))
+        return loss
+
+    def train_loss(self, inputs, targets, rows, weights, rows_of=None, recs=None, loss_bias=0.8, dropout=0.0, epoch=0, grad=False):
+        """pb_train_loss: each network's loss over all its entries as one batch (dropout 0: Keras's evaluate) -> float64
+        [k] on the device, and with grad=True also its gradient, float32 [k, PB_TRAIN_STRIDE].  Arguments as train's.
+        pb_train_loss in include/precise_b200.h."""
+        arr, k = rows
+        n_rec, targets, pr, pc, n = self._train_args(inputs, targets, k, rows_of, recs, weights)
+        torch = self.torch
+        loss = torch.empty(k, dtype=torch.float64, device=self.device)
+        g = torch.zeros((k, PB_TRAIN_STRIDE), dtype=torch.float32, device=self.device) if grad else None
+        if rows_of is not None and n == 0:
+            loss.fill_(float('nan'))
+            return (loss, g) if grad else loss
+        check(self.lib.pb_train_loss(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n,
+                                     float(loss_bias), float(dropout), int(epoch), _ptr(weights), _ptr(loss), _ptr(g),
+                                     self._stream()))
+        return (loss, g) if grad else loss
 
     def corpus_pairs_batch(self, windows):
         """Test hook: score_corpus_pairs scans at most ``windows`` pair-windows per batch (0 = the default)."""

@@ -38,6 +38,9 @@
 #include "corpus_pairs.cuh"
 #include "dataset.cuh"
 #include "pool.cuh"
+#include "train.cuh"
+
+#include <cub/device/device_segmented_sort.cuh>
 
 using namespace pb;
 
@@ -219,6 +222,7 @@ struct pb_handle {
     DevArray<PairTile> d_pp_tiles;   // ... the batch's scan tiles, one activation class after the other
     DevArray<float> d_ds_thr;        // pb_score_dataset: the histogram's float32 thresholds
     DevArray<uint8_t> d_ds_targets;  // ... [n_rec] the recordings' labels
+    DevArray<uint8_t> d_tr_ws;       // pb_train / pb_train_loss: one arena, carved per call (at most TRAIN_WS_CAP bytes per group)
     int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
@@ -2394,6 +2398,354 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
         return PB_OK;
     };
     return corpus_done(h, s, launch());
+}
+
+// ------------------------------------------------------------------------------------------------
+// training (train.cuh)
+
+constexpr size_t TRAIN_WS_CAP = size_t(256) << 20;     // workspace of one group of rows
+constexpr size_t TRAIN_ALIGN = 256;
+
+// The fused family's front end, which pb_vectorize_clips and the training kernels cover.
+static int check_train_front_end(const pb_handle* h) {
+    if (h->cfg.use_delta || h->feat > TR_MAX_F)
+        return fail(PB_ERR_UNSUPPORTED, "training covers the fused family's front end (feature size <= %d, no deltas); this handle "
+                    "has feature size %d%s", TR_MAX_F, h->feat, h->cfg.use_delta ? " with deltas" : "");
+    if (train_smem(h->cfg.n_features) > 227 * 1024)
+        return fail(PB_ERR_UNSUPPORTED, "n_features = %d: the training kernel keeps at most 112 steps in shared memory", h->cfg.n_features);
+    return PB_OK;
+}
+
+PB_API int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
+                              int64_t max_samples, float* d_inputs, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = check_train_front_end(h);
+    if (rc != PB_OK) return rc;
+    rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, PB_CORPUS_LISTENER, 1, d_inputs, true, nullptr, nullptr);
+    if (rc != PB_OK) return rc;
+    if (max_samples < 1) return fail(PB_ERR_INVALID, "max_samples = %lld must be >= 1", (long long)max_samples);
+    for (int64_t r = 0; r < n_rec; ++r)
+        if (h_offsets[r + 1] == h_offsets[r]) return fail(PB_ERR_INVALID, "recording %lld is empty: cannot vectorize empty audio", (long long)r);
+    if (n_rec == 0) return PB_OK;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const CorpusPlan plan = corpus_plan(h, d_pcm, h_offsets, n_rec, PB_CORPUS_LISTENER, 1, max_samples);
+    rc = corpus_reserve(h, plan, n_rec, CorpusPoolSizes{}, s);
+    if (rc != PB_OK) return rc;
+    auto launch = [&]() -> int {
+        rc = corpus_k1(h, plan, d_pcm, n_rec, divisor, PB_CORPUS_LISTENER, 1, s);
+        if (rc != PB_OK) return rc;
+        const int T = h->cfg.n_features, F = h->feat;
+        const long long total = (long long)n_rec * T * F;
+        vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->row_stride,
+                                                                               T, F, n_rec, d_inputs);
+        CK(cudaGetLastError());
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+PB_API int pb_train_opts_default(pb_train_opts* o) {
+    if (!o) return fail(PB_ERR_INVALID, "opts is null");
+    o->epochs = 10; o->epoch0 = 0; o->batch_size = 5000;
+    o->lr = 0.001f; o->rho = 0.9f; o->epsilon = 1e-7f;
+    o->loss_bias = 0.8f; o->dropout = 0.2f;
+    return PB_OK;
+}
+
+// The entries of a training call: row r's entry j uses clip ent[off[r] + j].
+struct TrainEntries {
+    std::vector<int64_t> off;        // [k + 1]
+    std::vector<int> ent;
+};
+
+// A group of consecutive rows with entries, trained together, and its tile tables: batch b's gradient tiles are
+// tiles[tile0[b] .. tile0[b + 1]), its row updates steps[step0[b] .. step0[b + 1]).
+struct TrainGroup {
+    std::vector<int> rows;
+    int64_t e0 = 0, n = 0;           // entries [e0, e0 + n) of TrainEntries::ent
+    std::vector<int> seg;            // [rows + 1] group-local entry offsets
+    std::vector<TrainTile> tiles;
+    std::vector<TrainStep> steps;
+    std::vector<int64_t> tile0, step0;
+    int64_t max_tiles = 0;
+    size_t sort_bytes = 0;
+};
+
+// Checks the arguments both training calls share and lists the entries.
+static int check_train(const pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                       int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, TrainEntries& te) {
+    int rc = check_train_front_end(h);
+    if (rc != PB_OK) return rc;
+    if (k < 0 || k > INT32_MAX / 2) return fail(PB_ERR_INVALID, "k = %lld outside [0, 2^30)", (long long)k);
+    if (k > 0 && !h_rows) return fail(PB_ERR_INVALID, "null h_rows");
+    for (int64_t i = 0; i < k; ++i) {
+        const pb_train_row& r = h_rows[i];
+        if (r.hidden < 1 || r.hidden > TR_MAX_H) return fail(PB_ERR_INVALID, "row %lld: hidden = %d outside [1, %d]", (long long)i, r.hidden, TR_MAX_H);
+        if ((r.activation != PB_ACT_LINEAR && r.activation != PB_ACT_TANH) ||
+            (r.recurrent_activation != PB_RACT_HARD_SIGMOID && r.recurrent_activation != PB_RACT_SIGMOID))
+            return fail(PB_ERR_INVALID, "row %lld: unknown activation codes (%d, %d)", (long long)i, r.activation, r.recurrent_activation);
+    }
+    if (n_rec < 0 || n_rec > INT32_MAX) return fail(PB_ERR_INVALID, "n_rec = %lld outside [0, 2^31)", (long long)n_rec);
+    if (n_pairs < 0 || n_pairs > INT32_MAX) return fail(PB_ERR_INVALID, "n_pairs = %lld outside [0, 2^31)", (long long)n_pairs);
+    const bool by_pairs = n_pairs > 0;
+    if (by_pairs && (!h_pair_rows || !h_pair_recs)) return fail(PB_ERR_INVALID, "null h_pair_rows or h_pair_recs");
+    for (int64_t i = 0; i < n_pairs; ++i) {
+        const int32_t row = h_pair_rows[i], r = h_pair_recs[i];
+        if (row < 0 || row >= k) return fail(PB_ERR_INVALID, "row %d (pair %lld) outside [0, k = %lld)", row, (long long)i, (long long)k);
+        if (r < 0 || r >= n_rec)
+            return fail(PB_ERR_INVALID, "clip %d (pair %lld) outside [0, n_rec = %lld)", r, (long long)i, (long long)n_rec);
+    }
+    const int64_t total = by_pairs ? n_pairs : k * n_rec;
+    if (total > 0 && (!d_inputs || !h_targets)) return fail(PB_ERR_INVALID, "null d_inputs or h_targets");
+    // one row's entries must fit one group's workspace
+    const int64_t per_row_max = (int64_t)(TRAIN_WS_CAP / 64);
+    te.off.assign((size_t)k + 1, 0);
+    if (by_pairs) {
+        for (int64_t i = 0; i < n_pairs; ++i) ++te.off[(size_t)h_pair_rows[i] + 1];
+    } else {
+        for (int64_t i = 0; i < k; ++i) te.off[(size_t)i + 1] = n_rec;
+    }
+    for (int64_t i = 0; i < k; ++i) {
+        if (te.off[(size_t)i + 1] > per_row_max)
+            return fail(PB_ERR_INVALID, "row %lld has %lld entries, more than %lld: split the call", (long long)i,
+                        (long long)te.off[(size_t)i + 1], (long long)per_row_max);
+        te.off[(size_t)i + 1] += te.off[(size_t)i];
+    }
+    te.ent.resize((size_t)total);
+    if (by_pairs) {
+        std::vector<int64_t> at(te.off.begin(), te.off.end() - 1);
+        for (int64_t i = 0; i < n_pairs; ++i) te.ent[(size_t)at[(size_t)h_pair_rows[i]]++] = h_pair_recs[i];
+    } else {
+        for (int64_t i = 0; i < k; ++i)
+            for (int64_t r = 0; r < n_rec; ++r) te.ent[(size_t)(i * n_rec + r)] = (int)r;
+    }
+    return PB_OK;
+}
+
+// Entries per batch of row with n entries at batch size bs: tiles of TR_TILE entries.
+static int64_t train_tiles(int64_t n, int64_t bs) {
+    int64_t t = 0;
+    for (int64_t b0 = 0; b0 < n; b0 += bs) t += (std::min(bs, n - b0) + TR_TILE - 1) / TR_TILE;
+    return t;
+}
+
+// Groups of consecutive rows with entries whose workspace stays under TRAIN_WS_CAP, with their tile tables.
+static std::vector<TrainGroup> train_groups(const TrainEntries& te, int64_t k, int64_t bs) {
+    std::vector<TrainGroup> out;
+    size_t bytes = 0;
+    for (int64_t r = 0; r < k; ++r) {
+        const int64_t n = te.off[(size_t)r + 1] - te.off[(size_t)r];
+        if (n == 0) continue;
+        const int64_t b = std::min(bs, n), nb = (n + bs - 1) / bs;
+        const size_t cost = (size_t)n * 40 + (size_t)((b + TR_TILE - 1) / TR_TILE) * (TR_STRIDE * 4 + 8) +
+                            (size_t)train_tiles(n, bs) * sizeof(TrainTile) + (size_t)nb * sizeof(TrainStep) + 64;
+        if (out.empty() || bytes + cost > TRAIN_WS_CAP || out.back().rows.size() >= 65535) {
+            out.emplace_back();
+            out.back().e0 = te.off[(size_t)r];
+            out.back().seg.push_back(0);
+            bytes = 0;
+        }
+        TrainGroup& g = out.back();
+        g.rows.push_back((int)r);
+        g.n += n;
+        g.seg.push_back((int)g.n);
+        bytes += cost;
+    }
+    for (TrainGroup& g : out) {
+        int64_t nb_max = 0;
+        for (size_t i = 0; i < g.rows.size(); ++i) nb_max = std::max<int64_t>(nb_max, (g.seg[i + 1] - g.seg[i] + bs - 1) / bs);
+        for (int64_t b = 0; b < nb_max; ++b) {
+            g.tile0.push_back((int64_t)g.tiles.size());
+            g.step0.push_back((int64_t)g.steps.size());
+            int t_launch = 0;
+            for (size_t i = 0; i < g.rows.size(); ++i) {
+                const int64_t n = g.seg[i + 1] - g.seg[i], b0 = b * bs;
+                if (b0 >= n) continue;
+                const int B = (int)std::min(bs, n - b0);
+                const int t0 = t_launch;
+                for (int q = 0; q < B; q += TR_TILE)
+                    g.tiles.push_back(TrainTile{g.rows[i], g.seg[i], (int)b0 + q, std::min(TR_TILE, B - q), B}), ++t_launch;
+                g.steps.push_back(TrainStep{g.rows[i], t0, t_launch, b0 + bs >= n ? TR_LAST : 0, (int)n});
+            }
+            g.max_tiles = std::max<int64_t>(g.max_tiles, t_launch);
+        }
+        g.tile0.push_back((int64_t)g.tiles.size());
+        g.step0.push_back((int64_t)g.steps.size());
+    }
+    return out;
+}
+
+// Carves typed arrays out of the training arena (a null base only measures).
+struct TrainCarve {
+    uint8_t* base;
+    size_t at = 0;
+    template <typename T> T* take(size_t n) {
+        at = (at + TRAIN_ALIGN - 1) / TRAIN_ALIGN * TRAIN_ALIGN;
+        T* p = base ? reinterpret_cast<T*>(base + at) : nullptr;
+        at += std::max<size_t>(n, 1) * sizeof(T);
+        return p;
+    }
+};
+
+struct TrainWs {
+    TrainRowDev* rows; uint8_t* targets; double* loss_acc;
+    int* ent; int* order; int* vals; uint64_t* keys; uint64_t* keys2; int* seg; int* seg_row;
+    TrainTile* tiles; TrainStep* steps; float* part; double* part_loss; void* sort_tmp;
+};
+
+static TrainWs train_layout(uint8_t* base, int64_t k, int64_t n_rec, int64_t n, int64_t rows, int64_t tiles, int64_t steps,
+                            int64_t max_tiles, size_t sort_bytes, size_t* bytes) {
+    TrainCarve c{base};
+    TrainWs w{};
+    w.rows = c.take<TrainRowDev>((size_t)k); w.targets = c.take<uint8_t>((size_t)n_rec); w.loss_acc = c.take<double>((size_t)k);
+    w.ent = c.take<int>((size_t)n); w.order = c.take<int>((size_t)n); w.vals = c.take<int>((size_t)n);
+    w.keys = c.take<uint64_t>((size_t)n); w.keys2 = c.take<uint64_t>((size_t)n);
+    w.seg = c.take<int>((size_t)rows + 1); w.seg_row = c.take<int>((size_t)rows);
+    w.tiles = c.take<TrainTile>((size_t)tiles); w.steps = c.take<TrainStep>((size_t)steps);
+    w.part = c.take<float>((size_t)max_tiles * TR_STRIDE); w.part_loss = c.take<double>((size_t)max_tiles);
+    w.sort_tmp = c.take<uint8_t>(sort_bytes);
+    if (bytes) *bytes = c.at;
+    return w;
+}
+
+// Shared body of pb_train (train = true: shuffle, batches, RMSprop) and pb_train_loss (one batch per row in request order,
+// the gradient to d_grad).
+static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                     int64_t k, const TrainEntries& te, bool train, int epochs, int epoch0, int64_t bs, float lr, float rho,
+                     float eps, float loss_bias, float dropout, const float* d_weights_in, float* d_weights, float* d_rms,
+                     double* d_loss, float* d_grad, cudaStream_t s) {
+    CK(cudaSetDevice(h->cfg.device));
+    std::vector<TrainGroup> groups = train_groups(te, k, train ? bs : std::numeric_limits<int64_t>::max() / 2);
+    int64_t rows_max = 0, n_max = 0, tiles_max = 0, steps_max = 0, ptiles_max = 0;
+    size_t sort_max = 0;
+    for (TrainGroup& g : groups) {
+        if (train) {
+            size_t sb = 0;
+            CK(cub::DeviceSegmentedSort::StableSortPairs(nullptr, sb, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int*)nullptr,
+                                                         (int*)nullptr, (int)g.n, (int)g.rows.size(), (const int*)nullptr,
+                                                         (const int*)nullptr, s));
+            g.sort_bytes = sb;
+        }
+        rows_max = std::max<int64_t>(rows_max, (int64_t)g.rows.size());
+        n_max = std::max(n_max, g.n);
+        tiles_max = std::max<int64_t>(tiles_max, (int64_t)g.tiles.size());
+        steps_max = std::max<int64_t>(steps_max, (int64_t)g.steps.size());
+        ptiles_max = std::max(ptiles_max, g.max_tiles);
+        sort_max = std::max(sort_max, g.sort_bytes);
+    }
+    size_t bytes = 0;
+    train_layout(nullptr, k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, &bytes);
+    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
+    if (h->d_tr_ws.size() < bytes) {
+        DevArray<uint8_t> fresh;
+        const cudaError_t e = fresh.alloc(bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(PB_ERR_CUDA, "training workspace allocation failed (%zu bytes): %s", bytes, cudaGetErrorString(e));
+        }
+        CK(cudaEventSynchronize(h->corpus_ev));                     // the previous call may still use the arena
+        h->d_tr_ws = std::move(fresh);
+    }
+    CK(ensure_dyn_smem(train_grad_kernel, train_smem(h->cfg.n_features)));
+    CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
+    const TrainWs w = train_layout(h->d_tr_ws.get(), k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, nullptr);
+    auto launch = [&]() -> int {
+        const int n_loss = train ? epochs : 1;
+        if (d_loss) {
+            const std::vector<double> nan((size_t)k * n_loss, std::numeric_limits<double>::quiet_NaN());
+            CK(cudaMemcpyAsync(d_loss, nan.data(), nan.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+        }
+        if (groups.empty()) return PB_OK;
+        std::vector<TrainRowDev> rd((size_t)k);
+        for (int64_t i = 0; i < k; ++i)
+            rd[i] = TrainRowDev{h_rows[i].hidden, h_rows[i].activation, h_rows[i].recurrent_activation, h_rows[i].seed};
+        CK(cudaMemcpyAsync(w.rows, rd.data(), rd.size() * sizeof(TrainRowDev), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(w.targets, h_targets, (size_t)n_rec, cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(w.loss_acc, 0, (size_t)k * sizeof(double), s));
+        ProfScope prof(h, 1, s);
+        const float scale = 1.0f / (1.0f - dropout);
+        for (const TrainGroup& g : groups) {
+            CK(cudaMemcpyAsync(w.ent, te.ent.data() + g.e0, (size_t)g.n * sizeof(int), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(w.seg, g.seg.data(), g.seg.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(w.seg_row, g.rows.data(), g.rows.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(w.tiles, g.tiles.data(), g.tiles.size() * sizeof(TrainTile), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(w.steps, g.steps.data(), g.steps.size() * sizeof(TrainStep), cudaMemcpyHostToDevice, s));
+            int64_t seg_max = 0;
+            for (size_t i = 0; i < g.rows.size(); ++i) seg_max = std::max<int64_t>(seg_max, g.seg[i + 1] - g.seg[i]);
+            for (int ep = 0; ep < (train ? epochs : 1); ++ep) {
+                const long long epoch = (long long)epoch0 + ep;
+                if (train) {
+                    const dim3 grid((unsigned)std::min<int64_t>((seg_max + 255) / 256, 64), (unsigned)g.rows.size());
+                    train_keys_kernel<<<grid, 256, 0, s>>>(w.rows, w.seg, w.seg_row, (int)g.rows.size(), epoch, w.keys, w.vals);
+                    CK(cudaGetLastError());
+                    size_t sb = g.sort_bytes;
+                    CK(cub::DeviceSegmentedSort::StableSortPairs(w.sort_tmp, sb, w.keys, w.keys2, w.vals, w.order, (int)g.n,
+                                                                 (int)g.rows.size(), w.seg, w.seg + 1, s));
+                }
+                for (size_t b = 0; b + 1 < g.tile0.size(); ++b) {
+                    TrainGrad G{};
+                    G.weights = train ? d_weights : d_weights_in; G.rows = w.rows; G.inputs = d_inputs; G.targets = w.targets;
+                    G.ent = w.ent; G.order = train ? w.order : nullptr; G.tiles = w.tiles + g.tile0[b];
+                    G.part = w.part; G.part_loss = w.part_loss;
+                    G.T = h->cfg.n_features; G.F = h->feat; G.epoch = epoch;
+                    G.rate = dropout; G.scale = scale; G.loss_bias = loss_bias;
+                    const unsigned nt = (unsigned)(g.tile0[b + 1] - g.tile0[b]);
+                    train_grad_kernel<<<nt, TR_THREADS, train_smem(G.T), s>>>(G);
+                    CK(cudaGetLastError());
+                    TrainUpdate P{};
+                    P.steps = w.steps + g.step0[b]; P.rows = w.rows; P.part = w.part; P.part_loss = w.part_loss;
+                    P.weights = train ? d_weights : nullptr; P.rms = d_rms; P.grad = train ? nullptr : d_grad;
+                    P.loss_acc = w.loss_acc; P.loss = d_loss; P.n_loss = n_loss; P.loss_col = ep; P.F = h->feat;
+                    P.lr = lr; P.rho = rho; P.eps = eps;
+                    train_update_kernel<<<(unsigned)(g.step0[b + 1] - g.step0[b]), TR_UPDATE_THREADS, 0, s>>>(P);
+                    CK(cudaGetLastError());
+                }
+            }
+        }
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+PB_API int pb_train(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows, int64_t k,
+                    const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
+                    float* d_weights, float* d_rms, double* d_loss, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (!opts) return fail(PB_ERR_INVALID, "null opts");
+    const pb_train_opts o = *opts;
+    if (o.epochs < 1) return fail(PB_ERR_INVALID, "epochs = %d must be >= 1", o.epochs);
+    if (o.epoch0 < 0) return fail(PB_ERR_INVALID, "epoch0 = %d is negative", o.epoch0);
+    if (o.batch_size < 1) return fail(PB_ERR_INVALID, "batch_size = %d must be >= 1", o.batch_size);
+    if (!(std::isfinite(o.lr) && o.lr >= 0.f)) return fail(PB_ERR_INVALID, "lr = %g must be finite and >= 0", o.lr);
+    if (!(o.rho >= 0.f && o.rho < 1.f)) return fail(PB_ERR_INVALID, "rho = %g outside [0, 1)", o.rho);
+    if (!(std::isfinite(o.epsilon) && o.epsilon >= 0.f)) return fail(PB_ERR_INVALID, "epsilon = %g must be finite and >= 0", o.epsilon);
+    if (!(o.loss_bias >= 0.f && o.loss_bias <= 1.f)) return fail(PB_ERR_INVALID, "loss_bias = %g outside [0, 1]", o.loss_bias);
+    if (!(o.dropout >= 0.f && o.dropout < 1.f)) return fail(PB_ERR_INVALID, "dropout = %g outside [0, 1)", o.dropout);
+    TrainEntries te;
+    const int rc = check_train(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, te);
+    if (rc != PB_OK) return rc;
+    if (k > 0 && (!d_weights || !d_rms)) return fail(PB_ERR_INVALID, "null d_weights or d_rms");
+    if (k == 0) return PB_OK;
+    return train_run(h, d_inputs, n_rec, h_targets, h_rows, k, te, true, o.epochs, o.epoch0, o.batch_size, o.lr, o.rho, o.epsilon,
+                     o.loss_bias, o.dropout, nullptr, d_weights, d_rms, d_loss, nullptr, (cudaStream_t)stream);
+}
+
+PB_API int pb_train_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                         int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
+                         float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (!(loss_bias >= 0.f && loss_bias <= 1.f)) return fail(PB_ERR_INVALID, "loss_bias = %g outside [0, 1]", loss_bias);
+    if (!(dropout >= 0.f && dropout < 1.f)) return fail(PB_ERR_INVALID, "dropout = %g outside [0, 1)", dropout);
+    if (epoch < 0) return fail(PB_ERR_INVALID, "epoch = %d is negative", epoch);
+    TrainEntries te;
+    const int rc = check_train(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, te);
+    if (rc != PB_OK) return rc;
+    if (k > 0 && !d_weights) return fail(PB_ERR_INVALID, "null d_weights");
+    if (!d_loss && !d_grad) return fail(PB_ERR_INVALID, "d_loss and d_grad are both null");
+    if (k == 0) return PB_OK;
+    return train_run(h, d_inputs, n_rec, h_targets, h_rows, k, te, false, 1, epoch, 0, 0.f, 0.f, 0.f, loss_bias, dropout, d_weights,
+                     nullptr, nullptr, d_loss, d_grad, (cudaStream_t)stream);
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {

@@ -33,6 +33,22 @@ class GruModel:
         return GruModel(rs.randn(feature_size, 3 * hidden) * scale, rs.randn(hidden, 3 * hidden) * scale,
                         rs.randn(3 * hidden) * scale, rs.randn(hidden) * scale, rs.randn(1) * scale)
 
+    @staticmethod
+    def init(feature_size=13, hidden=20, seed=0, activation='linear', recurrent_activation='hard_sigmoid'):
+        """A new network as Keras initialises GRU and Dense layers, from numpy's RandomState(seed): glorot_uniform kernel
+        and dense weights (uniform in +-sqrt(6 / (fan_in + fan_out))), an orthogonal recurrent kernel [H, 3H] (the Q factor
+        of a standard normal matrix, as keras.initializers.Orthogonal builds it) and zero biases."""
+        rs = np.random.RandomState(seed)
+        F, H = feature_size, hidden
+        lim = np.sqrt(6.0 / (F + 3 * H))
+        kernel = rs.uniform(-lim, lim, (F, 3 * H))
+        a = rs.normal(0.0, 1.0, (H, 3 * H))
+        u, _, v = np.linalg.svd(a, full_matrices=False)
+        recurrent = u if u.shape == (H, 3 * H) else v
+        lim_d = np.sqrt(6.0 / (H + 1))
+        dense_w = rs.uniform(-lim_d, lim_d, H)
+        return GruModel(kernel, recurrent, np.zeros(3 * H), dense_w, 0.0, activation, recurrent_activation)
+
 
 def save_weights(path: str, m: GruModel):
     np.savez(path, kernel=m.kernel, recurrent=m.recurrent, bias=m.bias, dense_w=m.dense_w,

@@ -24,12 +24,17 @@ Labelled clips (one network input per clip, vectorize's; statistics per pool mod
   test_pool         ~ precise/scripts/test.py, eval.py for many pool models in one device call per batch of clips
   graph_thresholds, roc ~ precise/scripts/graph.py:147-152 (the thresholds and the curve precise-graph plots)
   calc_threshold    ~ precise/scripts/calc_threshold.py:66-83 (a model's threshold_config from its positive clips)
+
+Training (fused-family networks, many per call: pb_vectorize_clips, pb_train, pb_train_loss):
+  vectorize_clips   vectorize(clip) of every clip, on the device
+  TrainState, train ~ precise/model.py:57-91, scripts/train.py:159-166 (Keras fit: loss, dropout, RMSprop; val_loss)
 """
 from dataclasses import dataclass
 
 import numpy as np
 
-from .core import PreciseB200, threshold_encode
+from .core import PB_TRAIN_STRIDE, PreciseB200, threshold_encode
+from .model_io import GruModel
 
 
 def _as_device_audio(core: PreciseB200, audio):
@@ -615,3 +620,91 @@ def calc_threshold(stats: DatasetStats, smoothing=1.2):
     mu = s1 / 2.0 ** 32 / n
     var = s2 / 2.0 ** 24 / n - mu * mu
     return mu, float(np.sqrt(max(var, 0.0))) * smoothing
+
+
+# ---- training ---------------------------------------------------------------------------------------------------------------
+
+def vectorize_clips(core: PreciseB200, clips, divisor=32767):
+    """vectorize(clip) of every clip (1-D int16 numpy arrays or CUDA tensors, none empty; divisor 32767: read as load_audio
+    reads wav files) -> float32 CUDA tensor [n, n_features, feature_size], bit for bit the input score_dataset scores.  Clips
+    are split into library calls as test_pool splits them."""
+    clips = [_check_recording(core, c) for c in clips]
+    parts = []
+    for g in _call_groups(clips):
+        pcm, offsets, order = _pack_clips(core, g)
+        res = core.vectorize_clips(pcm, offsets, divisor)
+        out = core.torch.empty_like(res)
+        out[core.torch.from_numpy(order).to(core.device)] = res
+        parts.append(out)
+    if not parts:
+        return core.torch.empty((0, core.n_features, core.feature_size), dtype=core.torch.float32, device=core.device)
+    return core.torch.cat(parts) if len(parts) > 1 else parts[0]
+
+
+class TrainState:
+    """Networks being trained on one handle's front end: their weights and RMSprop accumulators as device rows
+    [k, PB_TRAIN_STRIDE] (Keras's order: kernel, recurrent, bias, dense_w, dense_b), each row's hidden size, activations and
+    seed, and the next epoch's number (the shuffles and dropout masks of a resumed fit continue from it)."""
+
+    def __init__(self, core: PreciseB200, weights, rms, hidden, activation, recurrent_activation, seeds, epoch=0):
+        self.core = core
+        self.weights, self.rms = weights, rms
+        self.hidden, self.activation, self.recurrent_activation = list(hidden), list(activation), list(recurrent_activation)
+        self.seeds = [int(s) for s in seeds]
+        self.epoch = int(epoch)
+        self.rows = core.train_rows(self.hidden, self.activation, self.recurrent_activation, self.seeds)
+
+    @staticmethod
+    def from_models(core: PreciseB200, models, seeds):
+        """One row per GruModel (feature size core.feature_size, hidden <= 24), accumulators at zero."""
+        torch = core.torch
+        w = np.zeros((len(models), PB_TRAIN_STRIDE), np.float32)
+        for i, m in enumerate(models):
+            if m.feature_size != core.feature_size:
+                raise ValueError('model %d has feature size %d, the handle %d' % (i, m.feature_size, core.feature_size))
+            flat = np.concatenate([m.kernel.ravel(), m.recurrent.ravel(), m.bias, m.dense_w, [np.float32(m.dense_b)]])
+            w[i, :flat.size] = flat
+        weights = torch.from_numpy(w).to(core.device)
+        return TrainState(core, weights, torch.zeros_like(weights), [m.hidden for m in models], [m.activation for m in models],
+                          [m.recurrent_activation for m in models], seeds)
+
+    def models(self):
+        """The current weights as GruModels."""
+        w = self.weights.cpu().numpy()
+        F = self.core.feature_size
+        out = []
+        for i, H in enumerate(self.hidden):
+            a = 0
+            parts = []
+            for n in (3 * H * F, 3 * H * H, 3 * H, H, 1):
+                parts.append(w[i, a:a + n])
+                a += n
+            out.append(GruModel(parts[0].reshape(F, 3 * H), parts[1].reshape(H, 3 * H), parts[2], parts[3], parts[4],
+                                self.activation[i], self.recurrent_activation[i]))
+        return out
+
+
+def train(core: PreciseB200, state: TrainState, inputs, targets, rows=None, recs=None, epochs=10, batch_size=5000,
+          sensitivity=0.2, dropout=0.2, lr=0.001, validation=None):
+    """precise-train's fit for every network of ``state`` at once (pb_train): ``epochs`` epochs over ``inputs``
+    (vectorize_clips' tensor) with labels ``targets`` (non-zero = wake word), loss_bias = 1 - sensitivity (train.py:86).
+    rows / recs None: every network on every input; otherwise entry p is inputs[recs[p]] for network rows[p] (each word
+    on its owner's clips plus shared negatives).  state.epoch advances by ``epochs``.  Returns the epoch losses, float64
+    [k, epochs]; with validation=(inputs, targets) or (inputs, targets, rows, recs) also val_loss [k, epochs], each
+    network's loss over its validation entries without dropout after each epoch (pb_train_loss, Keras's evaluate)."""
+    kw = dict(rows_of=rows, recs=recs, batch_size=batch_size, lr=lr, loss_bias=1.0 - sensitivity, dropout=dropout)
+    if validation is None:
+        loss = core.train(inputs, targets, state.rows, state.weights, state.rms, epochs=epochs, epoch0=state.epoch, **kw)
+        state.epoch += epochs
+        return loss.cpu().numpy()
+    v_in, v_tg = validation[0], validation[1]
+    v_rows, v_recs = (validation[2], validation[3]) if len(validation) > 2 else (None, None)
+    losses, vals = [], []
+    for _ in range(epochs):
+        losses.append(core.train(inputs, targets, state.rows, state.weights, state.rms, epochs=1, epoch0=state.epoch, **kw))
+        state.epoch += 1
+        vals.append(core.train_loss(v_in, v_tg, state.rows, state.weights, v_rows, v_recs, loss_bias=1.0 - sensitivity))
+    k = len(state.hidden)
+    loss = core.torch.cat(losses, 1).cpu().numpy() if losses else np.zeros((k, 0))
+    val = core.torch.stack(vals, 1).cpu().numpy() if vals else np.zeros((k, 0))
+    return loss, val
