@@ -86,13 +86,16 @@ __device__ __forceinline__ float tr_act(int code, float x) {        // PB_ACT_LI
 __device__ __forceinline__ float tr_act_grad(int code, float y) {   // from the output
     return code == 0 ? 1.f : 1.f - y * y;
 }
+// hard_sigmoid's argument of clip_by_value, rounded as Keras computes it: 0.2 x in float32, then + 0.5.  Not fused: at
+// x = -2.5 fmaf(0.2f, x, 0.5f) is -2^-27 instead of 0, which would move the gradient's lower bound.
+__device__ __forceinline__ float tr_hard_sigmoid_arg(float x) { return __fadd_rn(__fmul_rn(0.2f, x), 0.5f); }
 __device__ __forceinline__ float tr_ract(int code, float x) {       // PB_RACT_HARD_SIGMOID / PB_RACT_SIGMOID
-    return code == 0 ? fminf(fmaxf(fmaf(0.2f, x, 0.5f), 0.f), 1.f) : 1.f / (1.f + expf(-x));
+    return code == 0 ? fminf(fmaxf(tr_hard_sigmoid_arg(x), 0.f), 1.f) : 1.f / (1.f + expf(-x));
 }
 // hard_sigmoid passes 0.2 where 0 <= 0.2 x + 0.5 <= 1, bounds included (the gradient of clip_by_value); sigmoid y (1 - y)
 __device__ __forceinline__ float tr_ract_grad(int code, float x, float y) {
     if (code == 0) {
-        const float s = fmaf(0.2f, x, 0.5f);
+        const float s = tr_hard_sigmoid_arg(x);
         return s >= 0.f && s <= 1.f ? 0.2f : 0.f;
     }
     return y * (1.f - y);

@@ -84,7 +84,9 @@ def unpack(row, F, H):
     return out
 
 
-def _act(name, x, dt):
+def _act(name, x, dt, kink=0.0):
+    """(value, derivative) of an activation; ``kink`` widens (> 0) or narrows (< 0) the band of s = 0.2 x + 0.5 where
+    hard_sigmoid's derivative is 0.2, for bounding a float32 computation whose pre-activation falls on the other side."""
     if name == 'linear':
         return x, np.ones_like(x)
     if name == 'tanh':
@@ -95,14 +97,15 @@ def _act(name, x, dt):
         return y, y * (dt(1) - y)
     if name == 'hard_sigmoid':
         s = dt(0.2) * x + dt(0.5)
-        return np.clip(s, 0, 1), np.where((s >= 0) & (s <= 1), dt(0.2), dt(0))
+        return np.clip(s, 0, 1), np.where((s >= -dt(kink)) & (s <= 1 + dt(kink)), dt(0.2), dt(0))
     raise ValueError(name)
 
 
-def loss_grad(row, F, H, x, y, mask, loss_bias, activation='linear', recurrent_activation='hard_sigmoid', dtype=np.float64):
+def loss_grad(row, F, H, x, y, mask, loss_bias, activation='linear', recurrent_activation='hard_sigmoid', dtype=np.float64,
+              kink=0.0):
     """One batch: x [B, T, F], y [B] (0 / 1), mask [B, 3, F] (masks()).  Returns (loss, gradient row [STRIDE], sum of the
     per-entry losses): loss = bias mean(-(1-y) log(1-p+1e-7)) + (1-bias) mean(-y log(p+1e-7)) and its gradient by
-    hand-written BPTT, everything in ``dtype``."""
+    hand-written BPTT, everything in ``dtype``.  ``kink``: see _act (0: Keras's bounds)."""
     dt = np.dtype(dtype).type
     w = unpack(np.asarray(row, dtype), F, H)
     K, U, b, dw, db = w['kernel'], w['recurrent'], w['bias'], w['dense_w'], w['dense_b']
@@ -115,8 +118,8 @@ def loss_grad(row, F, H, x, y, mask, loss_bias, activation='linear', recurrent_a
     for t in range(T):
         az = xm[:, 0, t] @ K[:, :H] + b[:H] + h @ U[:, :H]
         ar = xm[:, 1, t] @ K[:, H:2 * H] + b[H:2 * H] + h @ U[:, H:2 * H]
-        z, dz_da = _act(recurrent_activation, az, dt)
-        r, dr_da = _act(recurrent_activation, ar, dt)
+        z, dz_da = _act(recurrent_activation, az, dt, kink)
+        r, dr_da = _act(recurrent_activation, ar, dt, kink)
         ah = xm[:, 2, t] @ K[:, 2 * H:] + b[2 * H:] + (r * h) @ U[:, 2 * H:]
         hh, dhh_da = _act(activation, ah, dt)
         saved.append((h, z, r, hh, dz_da, dr_da, dhh_da))

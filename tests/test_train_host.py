@@ -151,3 +151,59 @@ def test_oracle_training_learns_the_synthetic_task():
     after = accuracy(row)
     assert before < 0.7 and after >= train_task.MIN_ACCURACY, (before, after)
     assert losses[-1] < losses[0]
+
+
+def _fma32(a, x, b):
+    """float32 fmaf(a, x, b): the product of two float32 values and the sum with b are exact in float64 here (|a x| < 1,
+    b = 0.5), so one rounding to float32 is the fused result."""
+    return np.float32(np.float64(np.float32(a)) * np.float64(np.float32(x)) + np.float64(np.float32(b)))
+
+
+def test_hard_sigmoid_gradient_bounds_and_why_the_kernel_does_not_fuse():
+    """hard_sigmoid's gradient is 0.2 where 0 <= 0.2 x + 0.5 <= 1, bounds included, with 0.2 x rounded before + 0.5 (Keras's
+    float32 order).  At x = -2.5 that is 0 exactly in float64 and float32, so both include it; fmaf rounds once and gives
+    -2^-27, which would exclude it.  Just past +2.5 float32 rounds 1 + 2^-24 to 1 (a tie to even) and includes the point
+    where float64 does not: an inherent float32 difference that the restatement shares with the kernel."""
+    f32 = np.float32
+    lo, hi = f32(-2.5), f32(2.5)
+    below, above = np.nextafter(lo, f32(-np.inf)), np.nextafter(hi, f32(np.inf))
+    inside = [np.nextafter(lo, f32(0)), lo, f32(0), hi, np.nextafter(hi, f32(0))]
+    for dt in (np.float64, np.float32):
+        for x in inside:
+            y, g = ot._act('hard_sigmoid', np.asarray([x], dt), dt)
+            assert g[0] == dt(0.2) and 0 <= y[0] <= 1, (dt, x)
+        assert ot._act('hard_sigmoid', np.asarray([below], dt), dt)[1][0] == 0
+        y, _ = ot._act('hard_sigmoid', np.asarray([lo, hi], dt), dt)
+        assert y[0] == 0 and y[1] == 1
+    # float64 excludes the float just past 2.5; float32's mul-then-add includes it
+    assert ot._act('hard_sigmoid', np.asarray([above], np.float64), np.float64)[1][0] == 0
+    assert ot._act('hard_sigmoid', np.asarray([above], np.float32), np.float32)[1][0] == f32(0.2)
+    # the fused form moves the lower bound: -2.5 falls out, and nothing else of these points changes side
+    s = _fma32(0.2, lo, 0.5)
+    assert s == -f32(2.0 ** -27) and s < 0
+    assert f32(0.2) * lo + f32(0.5) == 0
+    for x in [below, above] + inside:
+        if x != lo:
+            assert (0 <= _fma32(0.2, x, 0.5) <= 1) == (0 <= f32(0.2) * x + f32(0.5) <= 1), x
+    assert _fma32(0.2, hi, 0.5) == 1
+
+
+@pytest.mark.parametrize('seed,epoch', [(0, 0), (1, 5), (2 ** 31, 2 ** 31 - 1), (2 ** 32 - 1, 5), (2 ** 32 - 1, 2 ** 31 - 1)])
+def test_mask_counter_layout_up_to_47(seed, epoch):
+    """keep's [g, f] is counter 1 + c of the key with c = 3 f + g, c up to 47 at F = 16: the device reads c < 32 from one
+    ballot over counters 1 + lane and c >= 32 from a second over 33 + lane.  A smaller F keeps F = 16's first F columns."""
+    rate = np.float32(0.5)
+    for j in (0, 1, 70):
+        base = ot.mix(ot.mix(ot.mix(seed) + epoch) + j)
+        assert all(ot.key(seed, epoch, j, c) == ot.mix(base + c) for c in (0, 1, 33, 48))
+        u = lambda c: np.float32(float(ot.mix(base + c) >> 40) * 2.0 ** -24)
+        m0 = sum(1 << lane for lane in range(32) if u(1 + lane) >= rate)
+        m1 = sum(1 << lane for lane in range(32) if u(33 + lane) >= rate)
+        mask = m0 | (m1 << 32)
+        k = ot.keep(seed, epoch, j, 16, rate)
+        for f in range(16):
+            for g in range(3):
+                assert bool((mask >> (3 * f + g)) & 1) == k[g, f], (j, f, g)
+        assert 8 < np.count_nonzero(~k) < 40            # rate 0.5: a fair share of the 48 columns dropped
+        for F in (1, 5, 13):
+            assert np.array_equal(ot.keep(seed, epoch, j, F, rate), k[:, :F])
