@@ -173,6 +173,74 @@ def gru_forward_f16x3(w: GruWeights, x: np.ndarray):
     return sigmoid(logit), logit
 
 
+_TF32_MASK = np.uint32(0xffffe000)
+
+
+def _tf32_trunc(v):
+    """float32 v with its 13 low mantissa bits cleared (float32)."""
+    return (np.asarray(v, np.float32).view(np.uint32) & _TF32_MASK).view(np.float32)
+
+
+def _tf32_round(v):
+    """float32 v rounded to TF32 as the host's weight split does: (bits + 0x1000) & 0xffffe000 (float32)."""
+    u = np.asarray(v, np.float32).view(np.uint32)
+    return ((u + np.uint32(0x1000)) & _TF32_MASK).view(np.float32)
+
+
+def split_tf32_weights(v):
+    """float32 weights v -> (hi, lo) as upload_wide splits them: hi = v rounded to TF32, lo = (v - hi) rounded to TF32, with
+    v - hi in float32.  float64 values."""
+    v = np.asarray(v, np.float32)
+    hi = _tf32_round(v)
+    lo = _tf32_round(v - hi)
+    return hi.astype(np.float64), lo.astype(np.float64)
+
+
+def split_tf32(v):
+    """float32 operands v -> (hi, lo) as gru_wide_kernel splits x, h and r * h (split_tf32 in gru_kernels.cuh): hi = v with
+    the 13 low mantissa bits cleared, lo = v - hi in float32 (exact).  The tensor core then reads only lo's top 19 bits;
+    that truncation is an assumption about the hardware (the PTX ISA leaves a .tf32 operand's unused bits unspecified), and
+    lo is returned truncated so.  float64 values; |hi + lo - v| < 2^-21 |v|."""
+    v = np.asarray(v, np.float32)
+    hi = _tf32_trunc(v)
+    lo = _tf32_trunc(v - hi)
+    return hi.astype(np.float64), lo.astype(np.float64)
+
+
+def gru_forward_tf32x3(w: GruWeights, x: np.ndarray):
+    """x[N, T, F] -> (prob[N], logit[N]) float32, as the wide networks' tensor-core scan (gru_wide.cuh: gru_wide_kernel, 3 x
+    TF32) computes them: each gate's pre-activation is the bias plus the products lo . hi + hi . lo + hi . hi (lo . lo
+    dropped) of operands split by ``split_tf32`` and weights split by ``split_tf32_weights``, summed exactly and rounded to
+    float32 once.  z and r come from one product over [x | h], the candidate from one over [x | r * h].  Activations are
+    float32 (hard_sigmoid as fma(0.2, x, 0.5)), r * h is rounded to float32 before its split, h = fma(z, h, (1 - z) a) is
+    rounded to float32 and the Dense layer is an fmaf chain from the bias over the units in order.  A reference for tests:
+    what the scan should return, not a model of the tensor cores' internal rounding."""
+    x = np.asarray(x, np.float32)
+    if x.ndim == 2:
+        x = x[None]
+    N, T, F = x.shape
+    assert F == w.F, (F, w.F)
+    H = w.H
+    Kzr, Kh = split_tf32_weights(w.kernel[:, :2 * H]), split_tf32_weights(w.kernel[:, 2 * H:])
+    Uzr, Uh = split_tf32_weights(w.recurrent[:, :2 * H]), split_tf32_weights(w.recurrent[:, 2 * H:])
+    b = w.bias.astype(np.float64)
+    act, ract = _ACT32[w.activation], _ACT32[w.recurrent_activation]
+    h = np.zeros((N, H), np.float32)
+    with np.errstate(over='ignore', invalid='ignore'):
+        for t in range(T):
+            xs = split_tf32(x[:, t, :])
+            zr = ract(_f32(b[:2 * H] + _mm3(xs, Kzr) + _mm3(split_tf32(h), Uzr)))
+            z, r = zr[:, :H].astype(np.float32), zr[:, H:].astype(np.float32)
+            rh = _f32(r.astype(np.float64) * h)
+            a = act(_f32(b[2 * H:] + _mm3(xs, Kh) + _mm3(split_tf32(rh), Uh))).astype(np.float32)
+            p = _f32((np.float32(1) - z).astype(np.float64) * a)
+            h = _f32(z.astype(np.float64) * h + p)
+        logit = np.full(N, np.float32(w.dense_b), np.float32)
+        for j in range(H):
+            logit = _f32(h[:, j].astype(np.float64) * np.float64(w.dense_w[j]) + logit)
+        return sigmoid(logit), logit
+
+
 def predict(w: GruWeights, inputs: np.ndarray) -> np.ndarray:
     """``Runner.predict`` contract (network_runner.py:35-37): [N,T,F] -> float32 [N,1]."""
     return gru_forward(w, inputs, np.float32)[0].astype(np.float32)[:, None]

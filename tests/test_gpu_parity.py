@@ -6,7 +6,10 @@ Tolerances
   * GRU output on identical inputs: abs 1e-5 (BASELINE.json north_star), vs the fp32 AND fp64 oracle.  The fused
     family's fp16 x 3 scan (H <= 24, feature_size <= 16, no deltas: pools, banks, corpus calls and the default network above
     8 192 streams) is anchored to float64 over its shapes, front ends, weight magnitudes and operand range in
-    test_gpu_fused_scan.py, with oracle.gru.gru_forward_f16x3 bounding what larger weights may cost.
+    test_gpu_fused_scan.py, with oracle.gru.gru_forward_f16x3 bounding what larger weights may cost.  The other networks'
+    scans (gru_wide_kernel's 3 x TF32, gru_tiled_kernel) and the default network's CUDA-core scans (gru_warp_kernel,
+    gru_small_kernel) are anchored the same way in test_gpu_wide_scan.py, with oracle.gru.gru_forward_tf32x3 as the wide
+    kernel's reference.
   * decode: bit-identical conf for the same raw, except that the LUT index may move by one bin
     when CUDA's log() and libm's differ in the last ulp (rate reported, must be < 0.2 %).
   * trigger / count: exact.
