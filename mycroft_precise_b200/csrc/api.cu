@@ -174,6 +174,8 @@ struct pb_handle {
     DevArray<float4> d_ptab;
     DevArray<unsigned char> d_ctab;
     DevArray<float> d_dct_t;
+    bool pipe_fixed = false;         // the mel shape is the one mfcc_pipe_stream_kernel compiles in (K1P_FIX_*): d_pm_* hold its tables
+    DevArray<int4> d_pm_off; DevArray<float4> d_pm_w; DevArray<uint4> d_pm_crow; DevArray<float4> d_pm_dct;
     std::vector<double> fb;          // [n_filt][n_bins] (pb_get_filterbank)
     // device tables
     DevArray<float> d_wrise, d_wfall, d_dct;
@@ -531,7 +533,10 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     const size_t k1_fast_tables = (size_t)h->npl * 128 * sizeof(float4) + (size_t)c.n_filt * 16 * h->nol * sizeof(float) +
                                   (((size_t)c.n_filt * h->maxc + 15) & ~(size_t)15);
     h->k1_fast_smem = K1F_WARPS * sizeof(K1FWarp) + k1_fast_tables;
-    h->k1_pipe_smem = K1F_WARPS * sizeof(K1PWarp) + 256 * sizeof(float2) + k1_fast_tables;
+    h->pipe_fixed = c.vectorizer != PB_VEC_MELS && h->npl == K1P_FIX_NPL && h->maxc == K1P_FIX_MAXC && c.n_filt == K1P_FIX_NF &&
+                    h->n_out == K1P_FIX_NOUT;
+    h->k1_pipe_smem = K1F_WARPS * sizeof(K1PWarp) + 256 * sizeof(float2) +
+                      (h->pipe_fixed ? PipeMelShape<K1P_FIX_NPL, K1P_FIX_NF>::BYTES : k1_fast_tables);
     h->k1_ragged_smem = K1F_WARPS * sizeof(K1RWarp) + k1_fast_tables;
     // DCT-II, norm='ortho' (scipy.fftpack.dct as sonopy.mfcc_spec calls it), first n_out rows
     std::vector<float> dct((size_t)h->n_out * c.n_filt);
@@ -572,6 +577,39 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     }
     CK(h->d_ptab.upload(ptab));
     CK(h->d_ctab.upload(ctab));
+    if (h->pipe_fixed) {             // mel16_fixed's tables: the same entries and coefficients, regrouped (mfcc_fast.cuh)
+        constexpr int NPL = K1P_FIX_NPL, NF = K1P_FIX_NF, ROWS = PipeMelShape<K1P_FIX_NPL, K1P_FIX_NF>::ROWS;
+        std::vector<int4> poff((size_t)NPL * 2 * 32);
+        std::vector<float4> pw((size_t)NPL * 4 * 32);
+        for (int q = 0; q < NPL; ++q)
+            for (int lane = 0; lane < 32; ++lane) {
+                const int l16 = lane & 15, rot = ((l16 >> 2) + ((lane >> 4) << 2)) & 7;
+                int off[8];
+                float w[16];
+                for (int i = 0; i < 8; ++i) {
+                    const float4 e = ptab[((size_t)q * 8 + ((i + rot) & 7)) * 16 + l16];
+                    memcpy(&off[i], &e.x, 4);
+                    w[2 * i] = e.y; w[2 * i + 1] = e.z;
+                }
+                poff[(size_t)(2 * q) * 32 + lane] = make_int4(off[0], off[1], off[2], off[3]);
+                poff[(size_t)(2 * q + 1) * 32 + lane] = make_int4(off[4], off[5], off[6], off[7]);
+                for (int k = 0; k < 4; ++k) pw[(size_t)(4 * q + k) * 32 + lane] = make_float4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]);
+            }
+        std::vector<uint4> crow(ROWS);
+        for (int j = 0; j < ROWS; ++j) {
+            unsigned char b[16];
+            memset(b, 128, sizeof(b));
+            if (j < NF) memcpy(b, &ctab[(size_t)j * h->maxc], h->maxc);
+            memcpy(&crow[j], b, 16);
+        }
+        std::vector<float4> pd((size_t)16 * NF / 4, make_float4(0.f, 0.f, 0.f, 0.f));
+        for (int k = 0; k < h->n_out; ++k)
+            for (int n = 0; n < NF; ++n) reinterpret_cast<float*>(pd.data())[(size_t)k * NF + n] = dct[(size_t)k * NF + n];
+        CK(h->d_pm_off.upload(poff));
+        CK(h->d_pm_w.upload(pw));
+        CK(h->d_pm_crow.upload(crow));
+        CK(h->d_pm_dct.upload(pd));
+    }
     const size_t S = (size_t)c.max_streams;
     CK(h->d_n_samples.alloc(S));
     CK(h->d_tail.alloc(S * h->tail_cap));
@@ -588,9 +626,12 @@ PB_API int pb_create(const pb_config* cfg, pb_handle** out) {
     CK(ensure_dyn_smem(mfcc_fast_batch_kernel, (size_t)(h->k1_fast_smem)));
     CK(ensure_dyn_smem(mfcc_fast_stream_kernel<false>, (size_t)(h->k1_fast_smem)));
     CK(ensure_dyn_smem(mfcc_fast_stream_kernel<true>, (size_t)(h->k1_fast_smem)));
-    CK(ensure_dyn_smem(mfcc_pipe_stream_kernel, (size_t)(h->k1_pipe_smem)));
-    // K1P_CTAS_PER_SM CTAs of k1_pipe_smem each need the largest shared-memory carveout
-    CK(cudaFuncSetAttribute(mfcc_pipe_stream_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    {
+        auto kp = h->pipe_fixed ? mfcc_pipe_stream_kernel<K1P_FIX_NPL, K1P_FIX_MAXC, K1P_FIX_NF, K1P_FIX_NOUT> : mfcc_pipe_stream_kernel<0, 0, 0, 0>;
+        CK(ensure_dyn_smem(kp, (size_t)(h->k1_pipe_smem)));
+        // K1P_CTAS_PER_SM CTAs of k1_pipe_smem each need the largest shared-memory carveout
+        CK(cudaFuncSetAttribute(kp, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    }
     CK(ensure_dyn_smem(mfcc_stream_kernel<true>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<false>, (size_t)(h->k1_stream_smem)));
     CK(ensure_dyn_smem(mfcc_stream_kernel<false, true>, (size_t)(h->k1_stream_smem)));
@@ -1261,8 +1302,11 @@ static int launch_stream_mfcc(pb_handle* h, const int16_t* d_pcm, const int32_t*
         const int gridf = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
         if (h->k1_mode == 0) {                   // default: the pipelined kernel (bit-identical rows, tails and counts to mode 2)
             const int gridp = (int)std::min<int64_t>((tilesf + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * K1P_CTAS_PER_SM);
-            mfcc_pipe_stream_kernel<<<gridp, K1F_THREADS, h->k1_pipe_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
-                                                                              mel_tables(h), fast_tables(h), st);
+            PipeMelTables pm;
+            pm.poff = h->d_pm_off.get(); pm.pw = h->d_pm_w.get(); pm.crow = h->d_pm_crow.get(); pm.dct = h->d_pm_dct.get();
+            auto kp = h->pipe_fixed ? mfcc_pipe_stream_kernel<K1P_FIX_NPL, K1P_FIX_MAXC, K1P_FIX_NF, K1P_FIX_NOUT> : mfcc_pipe_stream_kernel<0, 0, 0, 0>;
+            kp<<<gridp, K1F_THREADS, h->k1_pipe_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
+                                                           mel_tables(h), fast_tables(h), pm, st);
         } else if (h->k1_mode != 3)              // the kernel mode 0 replaced: 32-bit per-pass set-up; 3 = its 64-bit original
             mfcc_fast_stream_kernel<true><<<gridf, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, d_ids, (int)n, h->cfg.chunk_samples, h->cfg.hop_samples, spw, scale,
                                                                                       mel_tables(h), fast_tables(h), st);

@@ -423,6 +423,89 @@ constexpr int K1P_IN_WORDS = 256 + 16;         // 1 KB frame +64 B: the two half
 static_assert(K1F_PART + K1_MAX_FILT <= K1P_IN_WORDS, "mel16's part | mel must fit in an input stage");
 static_assert(K1F_ZERO_BIN < XCH_ELEMS, "the zero bin must lie in the exchange scratch");
 
+// The mel shape the pipe kernel compiles in (mel16_fixed): the reference's default front end (16 kHz, n_fft 512, 20 filters,
+// 13 MFCCs) cuts the spectrum into 41 pieces, three piece blocks of 16 lanes, and sums at most 9 partials into one filter.
+// Every other shape runs mel16 with the shape read from the tables.
+constexpr int K1P_FIX_NPL = 3, K1P_FIX_MAXC = 9, K1P_FIX_NF = 20, K1P_FIX_NOUT = 13;
+
+struct PipeMelTables {         // mel16_fixed's tables (built by api.cu from ptab / ctab / dct_t); shared-memory copies in the kernel
+    const int4* poff;          // [npl][2][32]  lane L's 8 piece entries in L's walk order (see mel16): byte offsets of the bins in P
+    const float4* pw;          // [npl][4][32]  the same entries' (w_rise, w_fall), two entries per vector
+    const uint4* crow;         // [16 * (n_filt / 16 + 1)]  ctab row j as 16 bytes, padded with the zero slot 128; rows >= n_filt: all 128
+    const float4* dct;         // [16][n_filt / 4]  DCT row c (dct_t transposed back), zero for c >= n_out
+};
+
+template <int NPL, int NF>
+struct PipeMelShape {
+    static constexpr int ROWS = 16 * (NF / 16 + 1);                   // filter rows j = l16 + 16 it, slot NF included
+    static constexpr size_t BYTES = (size_t)NPL * 6 * 32 * sizeof(int4) + ROWS * sizeof(uint4) + 16 * NF * sizeof(float);
+};
+
+// mel16 for a compile-time shape, on the tables above: the same float operations in the same order (the rotated entry walk,
+// the r / f / tot chains, the m0 / m1 slot chains, the a0 / a1 DCT chains), with every loop unrolled, the piece entries read
+// as 6 vectors per block instead of 8, a filter's slot list as one vector, and the DCT and log-mels 4 filters per load.
+// The filter pass has idle lanes when n_filt is not a multiple of 16: lane n_filt - 16 (it) takes log(max(tot, eps)) there,
+// which mel16 computes in the DCT for row 0.
+template <int NPL, int MAXC, int NF, int NOUT>
+__device__ __forceinline__ void mel16_fixed(const float* P, const PipeMelTables& tb, float* part, float* mel, int lane, int l16,
+                                            bool active, float* __restrict__ out) {
+    static_assert(16 * NPL <= 64 && MAXC <= 16 && NF % 4 == 0 && PipeMelShape<NPL, NF>::ROWS <= K1_MAX_FILT && NOUT <= 16, "shape");
+    const char* Pb = reinterpret_cast<const char*>(P);
+    float tot = 0.f;
+#pragma unroll
+    for (int q = 0; q < NPL; ++q) {
+        const int4 o0 = tb.poff[(2 * q) * 32 + lane], o1 = tb.poff[(2 * q + 1) * 32 + lane];
+        const int off[8] = {o0.x, o0.y, o0.z, o0.w, o1.x, o1.y, o1.z, o1.w};
+        float w[16];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float4 v = tb.pw[(4 * q + k) * 32 + lane];
+            w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+        }
+        float r = 0.f, f = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const float pw = *reinterpret_cast<const float*>(Pb + off[i]);
+            tot += pw;
+            r = fmaf(w[2 * i], pw, r);
+            f = fmaf(w[2 * i + 1], pw, f);
+        }
+        part[q * 16 + l16] = r;
+        part[64 + q * 16 + l16] = f;
+    }
+#pragma unroll
+    for (int d = 8; d >= 1; d >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, d);   // every lane of the half ends with the same sum
+    __syncwarp();
+#pragma unroll
+    for (int it = 0; it <= NF / 16; ++it) {
+        const int j = l16 + 16 * it;
+        const uint4 row = tb.crow[j];
+        const unsigned cw[4] = {row.x, row.y, row.z, row.w};
+        float m0 = 0.f, m1 = 0.f;
+#pragma unroll
+        for (int c = 0; c + 1 < MAXC; c += 2) {
+            m0 += part[(cw[c >> 2] >> (8 * (c & 3))) & 255u];
+            m1 += part[(cw[(c + 1) >> 2] >> (8 * ((c + 1) & 3))) & 255u];
+        }
+        if (MAXC & 1) m0 += part[(cw[(MAXC - 1) >> 2] >> (8 * ((MAXC - 1) & 3))) & 255u];
+        const float v = (it == NF / 16 && j == NF) ? tot : m0 + m1;
+        mel[j] = logf(fmaxf(v, K1_EPS));
+    }
+    __syncwarp();
+    const float4* d = tb.dct + l16 * (NF / 4);
+    const float4* m4 = reinterpret_cast<const float4*>(mel);
+    float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+    for (int k = 0; k < NF / 4; ++k) {
+        const float4 dv = d[k], mv = m4[k];
+        a0 = fmaf(dv.x, mv.x, a0); a1 = fmaf(dv.y, mv.y, a1);
+        a0 = fmaf(dv.z, mv.z, a0); a1 = fmaf(dv.w, mv.w, a1);
+    }
+    const float v = l16 == 0 ? mel[NF] : a0 + a1;
+    if (active && l16 < NOUT) out[l16] = v;
+    __syncwarp();
+}
+
 struct K1PWarp {               // per warp
     int in[2][2][K1P_IN_WORDS];                // [stage][half]: 1 KB input frame (int16 pairs); once read: mel16's part | mel
     float xch[2][XCH_ELEMS];                   // [half]: FFT exchange scratch -> power bins (272 words apart: disjoint bank halves)
@@ -434,11 +517,13 @@ struct K1PWarp {               // per warp
 };
 static_assert(sizeof(K1PWarp) % 16 == 0, "every warp's input stages start 16-byte aligned (bulk copy destinations)");
 
-// fast_pass for K1PWarp: the same conversion, FFT and mel16, with the scratch and mel16's arrays placed as above.  mel16's entry
-// offsets are rebuilt from `rot` per pass (the same values) rather than held in 8 registers across the tile.
+// fast_pass for K1PWarp: the same conversion, FFT and mel stage, with the scratch and the mel stage's arrays placed as above.
+// NPL = 0: mel16 on the shape in the tables; its entry offsets are rebuilt from `rot` per pass (the same values) rather than held
+// in 8 registers across the tile.  NPL > 0: mel16_fixed.
+template <int NPL, int MAXC, int NF, int NOUT>
 __device__ __forceinline__ void pipe_pass(K1PWarp& ws, int stage, uint32_t parity, const FftSmemConst& lc, const K1FTab& tb,
-                                          const FastTables& ft, const MelTables& t, float scale, int rot,
-                                          int l16, int half, bool active, float* __restrict__ out) {
+                                          const PipeMelTables& pt, const FastTables& ft, const MelTables& t, float scale, int rot,
+                                          int lane, int l16, int half, bool active, float* __restrict__ out) {
     mbar_wait(&ws.bar[stage], parity);
     const int* in = ws.in[stage][half];
     cpx z[16];
@@ -453,22 +538,43 @@ __device__ __forceinline__ void pipe_pass(K1PWarp& ws, int stage, uint32_t parit
     fft512_power(z, lc, P, P, scale, l16, active); // P aliases the scratch: written after the last scratch read
     float* part = reinterpret_cast<float*>(ws.in[stage][half]);
     if (l16 == 0) { P[K1F_ZERO_BIN] = 0.f; part[128] = 0.f; }
-    int eoff[8];
+    if constexpr (NPL == 0) {
+        int eoff[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) eoff[i] = ((i + rot) & 7) * 16 + l16;
-    __syncwarp();
-    mel16<K1P_MEL_UQ, K1P_MEL_UC>(P, tb, ft, t, part, part + K1F_PART, eoff, l16, active, out);
+        for (int i = 0; i < 8; ++i) eoff[i] = ((i + rot) & 7) * 16 + l16;
+        __syncwarp();
+        mel16<K1P_MEL_UQ, K1P_MEL_UC>(P, tb, ft, t, part, part + K1F_PART, eoff, l16, active, out);
+    } else {
+        __syncwarp();
+        mel16_fixed<NPL, MAXC, NF, NOUT>(P, pt, part, part + K1F_PART, lane, l16, active, out);
+    }
 }
 
+template <int NPL, int MAXC, int NF, int NOUT>
 __global__ void __launch_bounds__(K1F_THREADS, K1P_CTAS_PER_SM)
 mfcc_pipe_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__ ids, int n, int chunk, int hop, int spw,
-                        float scale, MelTables tab, FastTables ft, StreamState st) {
+                        float scale, MelTables tab, FastTables ft, PipeMelTables pmt, StreamState st) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     K1PWarp* wsm = reinterpret_cast<K1PWarp*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, l16 = lane & 15, half = lane >> 4;
     K1PWarp& ws = wsm[warp];
     float2* tws = reinterpret_cast<float2*>(smem_raw + K1F_WARPS * sizeof(K1PWarp));
-    const K1FTab tb = load_fast_tables(reinterpret_cast<unsigned char*>(tws + 256), tab, ft);
+    K1FTab tb{};
+    PipeMelTables pt{};
+    if constexpr (NPL == 0) {
+        tb = load_fast_tables(reinterpret_cast<unsigned char*>(tws + 256), tab, ft);
+    } else {                                          // [poff | pw | crow | dct]
+        constexpr int NO = NPL * 2 * 32, NW = NPL * 4 * 32, NC = PipeMelShape<NPL, NF>::ROWS, ND = 16 * NF / 4;
+        int4* po = reinterpret_cast<int4*>(tws + 256);
+        float4* pw = reinterpret_cast<float4*>(po + NO);
+        uint4* pc = reinterpret_cast<uint4*>(pw + NW);
+        float4* pd = reinterpret_cast<float4*>(pc + NC);
+        for (int k = threadIdx.x; k < NO; k += blockDim.x) po[k] = __ldg(pmt.poff + k);
+        for (int k = threadIdx.x; k < NW; k += blockDim.x) pw[k] = __ldg(pmt.pw + k);
+        for (int k = threadIdx.x; k < NC; k += blockDim.x) pc[k] = __ldg(pmt.crow + k);
+        for (int k = threadIdx.x; k < ND; k += blockDim.x) pd[k] = __ldg(pmt.dct + k);
+        pt.poff = po; pt.pw = pw; pt.crow = pc; pt.dct = pd;
+    }
     for (int k = threadIdx.x; k < 256; k += blockDim.x) tws[k] = tab.tw_stage[(k & 15) * 16 + (k >> 4)];   // [n2][k1] -> [k1][n2]
     if (lane == 0) { mbar_init(&ws.bar[0], 1); mbar_init(&ws.bar[1], 1); fence_mbar_init(); }
     const int rot = ((l16 >> 2) + (half << 2)) & 7;   // rotated walk through a piece: see mel16
@@ -544,7 +650,7 @@ mfcc_pipe_stream_kernel(const int16_t* __restrict__ pcm, const int* __restrict__
                 row = st.ring + ((long long)ws.st_id[t] * st.ring_rows + slot) * st.row_stride;
             }
             const uint32_t parity = (stage == 0 ? uses0 : uses1) & 1;
-            pipe_pass(ws, stage, parity, lc, tb, ft, tab, scale, rot, l16, half, active, row);
+            pipe_pass<NPL, MAXC, NF, NOUT>(ws, stage, parity, lc, tb, pt, ft, tab, scale, rot, lane, l16, half, active, row);
             if (stage == 0) ++uses0; else ++uses1;
         }
         // the next tile's sample counts: its ids have landed during the passes, the loads overlap the tail update below
