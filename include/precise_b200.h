@@ -610,6 +610,31 @@ int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offset
 int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
                        int64_t max_samples, float* d_inputs, void* stream);
 
+/* precise-add-noise (precise/scripts/add_noise.py:56-90): background noise mixed into clips.  Item i is recording
+ * h_items[i] (HOST int32 [n_items], repeats allowed) of d_pcm / h_offsets (as pb_vectorize_clips takes them) with ratio
+ * h_ratios[i] (HOST double [n_items]).  The noise corpus d_noise [n_noise] (DEVICE int16) is read cyclically: item i's span
+ * starts at (noise_pos + the lengths of items 0 .. i-1) mod n_noise and wraps as often as it needs; the caller carries the
+ * position on to its next call.  With x the clip and n its span, Sa = sum x^2 and Sn = sum n^2 (exact int64 sums of the
+ * raw int16 samples):
+ *     g = Sn > 0 ? r sqrt(Sa) / sqrt(Sn) : 0,  y = (1 - r) x + g n  (IEEE double, each operation rounded),
+ *     out = int16(clamp(trunc(y), -32768, 32767)).
+ * The reference gives NaN for a silent span and casts out-of-range values without saturation; its sums are float32.
+ *   - d_out (DEVICE int16, optional) receives the mixed clips back to back, item i at the sum of the lengths before it.
+ *   - d_inputs [n_items][n_features][feature_size] (DEVICE, optional) receives vectorize(mixed clip), bit-identical to
+ *     pb_vectorize_clips' rows of the mixed clips when each clip's last max_samples samples start at a multiple of 8 samples
+ *     (the fast K1 at the default geometry, or the generic one under pb_debug_force_generic).
+ * Asynchronous on `stream`; shares and orders itself against the corpus workspace as pb_vectorize_clips.  Every argument is
+ * checked before anything is enqueued, so a refused call changes no buffer.
+ * PB_ERR_INVALID: pb_vectorize_clips' refusals of the clips (null or decreasing offsets, divisor, max_samples < 1), a null
+ * d_noise, n_noise < 1, noise_pos outside [0, n_noise), n_items outside [0, 2^31), null item or ratio arrays with
+ * n_items > 0, an item outside [0, n_rec), a ratio that is NaN or outside [0, 1], both outputs null, an empty item with
+ * d_inputs (empty items are fine with d_out alone: their clips are empty).  PB_ERR_UNSUPPORTED: d_inputs on a front end
+ * outside the fused family.  PB_ERR_CUDA: the workspace cannot be allocated. */
+int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
+                 const int16_t* d_noise, int64_t n_noise, const int32_t* h_items, const double* h_ratios,
+                 int64_t n_items, int64_t noise_pos, int32_t divisor, int64_t max_samples,
+                 int16_t* d_out, float* d_inputs, void* stream);
+
 /* Floats per network of pb_train's weight and accumulator arrays.  A row holds Keras's order, flat: kernel[F][3H],
  * recurrent[H][3H], bias[3H], dense_w[H], dense_b; the tail after 3H(F + H + 1) + H + 1 floats (2 977 at H = 24, F = 16) is
  * zero and stays zero. */

@@ -102,6 +102,7 @@ SYMBOLS = {
     'pb_score_dataset': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, _I32, _I64, _VP, _I32, _VP, _VP, _VP, _VP,
                                    C.c_double, _VP, _I64, _VP, _VP]),
     'pb_vectorize_clips': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I64, _VP, _VP]),
+    'pb_add_noise': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _I64, _I64, _I32, _I64, _VP, _VP, _VP]),
     'pb_train_opts_default': (C.c_int, [C.POINTER(pb_train_opts)]),
     'pb_train': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.POINTER(pb_train_opts), _VP, _VP, _VP, _VP]),
     'pb_train_loss': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.c_float, C.c_float, _I32, _VP, _VP, _VP, _VP]),
@@ -1051,6 +1052,30 @@ class PreciseB200:
         check(self.lib.pb_vectorize_clips(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, int(divisor), int(self.params.max_samples),
                                           _ptr(out), self._stream()))
         return out
+
+    def add_noise(self, pcm, offsets, noise, items, ratios, noise_pos=0, divisor=32767, out=True, inputs=False):
+        """Noise from the int16 corpus tensor ``noise`` mixed into clips pcm[offsets[r]:offsets[r + 1]]: item i is clip
+        items[i] (int32) with ratio ratios[i] (float64), its noise span read on cyclically from ``noise_pos``.  Returns
+        (mixed clips back to back as an int16 tensor, or None with out=False; vectorize of each mixed clip, float32
+        [n_items, n_features, feature_size], or None with inputs=False).  Asynchronous on the current stream.  pb_add_noise in
+        include/precise_b200.h."""
+        torch = self.torch
+        offsets, n_rec = self._corpus_recordings(pcm, offsets)
+        if (not isinstance(noise, torch.Tensor) or noise.dtype != torch.int16 or noise.dim() != 1 or not noise.is_contiguous()
+                or noise.device != self.device):
+            raise ValueError('noise must be a contiguous 1-D int16 tensor on %s' % self.device)
+        items = np.ascontiguousarray(items, dtype=np.int32)
+        ratios = np.ascontiguousarray(ratios, dtype=np.float64)
+        n = items.shape[0]
+        _check_np('items', items, np.int32, (n,), optional=False)
+        _check_np('ratios', ratios, np.float64, (n,), optional=False)
+        total = int(np.diff(offsets)[items].sum()) if n and items.min() >= 0 and items.max() < n_rec else 0
+        d_out = torch.empty(max(total, 1), dtype=torch.int16, device=self.device) if out else None    # non-null when empty
+        d_in = torch.empty((n, self.n_features, self.feature_size), dtype=torch.float32, device=self.device) if inputs else None
+        check(self.lib.pb_add_noise(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, _ptr(noise), noise.numel(), _np_ptr(items),
+                                    _np_ptr(ratios), n, int(noise_pos), int(divisor), int(self.params.max_samples), _ptr(d_out),
+                                    _ptr(d_in), self._stream()))
+        return (None if d_out is None else d_out[:total]), d_in
 
     def _train_args(self, inputs, targets, k, rows_of, recs, weights):
         """(n_rec, targets, pair rows, pair recs, n_pairs) of a training call, checked."""

@@ -39,6 +39,7 @@
 #include "dataset.cuh"
 #include "pool.cuh"
 #include "train.cuh"
+#include "noise.cuh"
 
 #include <cub/device/device_segmented_sort.cuh>
 
@@ -225,6 +226,10 @@ struct pb_handle {
     DevArray<float> d_ds_thr;        // pb_score_dataset: the histogram's float32 thresholds
     DevArray<uint8_t> d_ds_targets;  // ... [n_rec] the recordings' labels
     DevArray<uint8_t> d_tr_ws;       // pb_train / pb_train_loss: one arena, carved per call (at most TRAIN_WS_CAP bytes per group)
+    DevArray<NoiseItem> d_nz_items;  // pb_add_noise: [n_items] the items
+    DevArray<long long> d_nz_seg0;   // ... [n_items + 1] each item's first segment
+    DevArray<unsigned long long> d_nz_sums;  // ... [n_items][2] (sum x^2, sum n^2)
+    DevArray<int16_t> d_nz_pcm;      // ... the mixed clips' cropped tails, each at a multiple of 8 samples (K1's recordings)
     int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
@@ -1694,8 +1699,10 @@ struct CorpusPlan {
 
 // crop > 0 (labelled clips, vectorization.py:73-82): each recording is its last `crop` samples, framed from the first of
 // them, and has one window, the n_features rows ending at its last frame (row 0's zeros when it has no frame).
+// h_lens (pb_add_noise's workspace, where recordings have gaps between them): recording r is h_lens[r] samples from
+// h_offsets[r]; without it, recording r ends where r + 1 starts.
 static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t schedule,
-                              int64_t chunk, int64_t crop = 0) {
+                              int64_t chunk, int64_t crop = 0, const int64_t* h_lens = nullptr) {
     const pb_config& c = h->cfg;
     const int T = c.n_features;
     const bool fast = h->fast_ok && !h->force_generic && (uintptr_t)d_pcm % 16 == 0;
@@ -1707,7 +1714,7 @@ static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const in
     if (crop > 0) p.starts.resize((size_t)n_rec);
     for (int pass = 0; pass < 2; ++pass)
         for (int64_t r = 0; r < n_rec; ++r) {
-            const int64_t len = h_offsets[r + 1] - h_offsets[r], L = crop > 0 ? std::min(len, crop) : len;
+            const int64_t len = h_lens ? h_lens[r] : h_offsets[r + 1] - h_offsets[r], L = crop > 0 ? std::min(len, crop) : len;
             const int64_t src = h_offsets[r] + len - L, nf = corpus_frames(c, L);
             const bool fr = fast && src % 8 == 0;
             if (pass == 0) {
@@ -2483,6 +2490,106 @@ PB_API int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t*
         const long long total = (long long)n_rec * T * F;
         vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->row_stride,
                                                                                T, F, n_rec, d_inputs);
+        CK(cudaGetLastError());
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+// ------------------------------------------------------------------------------------------------
+// noise augmentation (noise.cuh)
+
+PB_API int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, const int16_t* d_noise,
+                        int64_t n_noise, const int32_t* h_items, const double* h_ratios, int64_t n_items, int64_t noise_pos,
+                        int32_t divisor, int64_t max_samples, int16_t* d_out, float* d_inputs, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = d_inputs ? check_train_front_end(h) : PB_OK;
+    if (rc != PB_OK) return rc;
+    if (!d_out && !d_inputs) return fail(PB_ERR_INVALID, "d_out and d_inputs are both null");
+    rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, PB_CORPUS_LISTENER, 1, nullptr, false, nullptr, nullptr);
+    if (rc != PB_OK) return rc;
+    if (max_samples < 1) return fail(PB_ERR_INVALID, "max_samples = %lld must be >= 1", (long long)max_samples);
+    if (n_noise < 1) return fail(PB_ERR_INVALID, "n_noise = %lld: the noise corpus is empty", (long long)n_noise);
+    if (!d_noise) return fail(PB_ERR_INVALID, "null d_noise");
+    if (noise_pos < 0 || noise_pos >= n_noise)
+        return fail(PB_ERR_INVALID, "noise_pos = %lld outside [0, %lld)", (long long)noise_pos, (long long)n_noise);
+    if (n_items < 0 || n_items > INT32_MAX) return fail(PB_ERR_INVALID, "n_items = %lld outside [0, 2^31)", (long long)n_items);
+    if (n_items > 0 && (!h_items || !h_ratios)) return fail(PB_ERR_INVALID, "null h_items or h_ratios");
+    for (int64_t i = 0; i < n_items; ++i) {
+        const int32_t r = h_items[i];
+        if (r < 0 || r >= n_rec) return fail(PB_ERR_INVALID, "item %lld: recording %d outside [0, %lld)", (long long)i, r, (long long)n_rec);
+        if (!(h_ratios[i] >= 0.0 && h_ratios[i] <= 1.0)) return fail(PB_ERR_INVALID, "item %lld: ratio %g outside [0, 1]", (long long)i, h_ratios[i]);
+        if (d_inputs && h_offsets[r + 1] == h_offsets[r])
+            return fail(PB_ERR_INVALID, "item %lld: recording %d is empty: cannot vectorize empty audio", (long long)i, r);
+    }
+    if (n_items == 0) return PB_OK;
+
+    // The items' table: clip, noise position (the corpus read on from noise_pos, item after item), place in d_out, and with
+    // d_inputs the place of its last max_samples samples in the workspace, each at a multiple of 8 samples.
+    std::vector<NoiseItem> items((size_t)n_items);
+    std::vector<long long> seg0((size_t)n_items + 1, 0);
+    std::vector<int64_t> ws_off, ws_len;
+    long long pos = noise_pos, out = 0, ws = 0;
+    for (int64_t i = 0; i < n_items; ++i) {
+        const int32_t r = h_items[i];
+        const long long len = h_offsets[r + 1] - h_offsets[r], crop = d_inputs ? std::min<long long>(len, max_samples) : 0;
+        items[i] = NoiseItem{h_offsets[r], len, pos, out, ws, crop, h_ratios[i]};
+        seg0[i + 1] = seg0[i] + (len + NZ_SEG - 1) / NZ_SEG;
+        out += len;
+        pos = (pos + len % n_noise) % n_noise;
+        if (d_inputs) {
+            ws_off.push_back(ws);
+            ws_len.push_back(crop);
+            ws += (crop + 7) / 8 * 8;
+        }
+    }
+    ws_off.push_back(ws);
+    const long long n_seg = seg0[n_items];
+    if (n_seg == 0) return PB_OK;                      // only empty items, d_out only: nothing to write
+
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
+    DevArray<NoiseItem> f_items; DevArray<long long> f_seg0; DevArray<unsigned long long> f_sums; DevArray<int16_t> f_pcm;
+    cudaError_t e = corpus_grow(h->d_nz_items, (size_t)n_items, f_items);
+    if (e == cudaSuccess) e = corpus_grow(h->d_nz_seg0, (size_t)n_items + 1, f_seg0);
+    if (e == cudaSuccess) e = corpus_grow(h->d_nz_sums, 2 * (size_t)n_items, f_sums);
+    if (e == cudaSuccess) e = corpus_grow(h->d_nz_pcm, (size_t)ws, f_pcm);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(PB_ERR_CUDA, "noise workspace allocation failed (%lld items): %s", (long long)n_items, cudaGetErrorString(e));
+    }
+    if (f_items.get() || f_seg0.get() || f_sums.get() || f_pcm.get()) CK(cudaEventSynchronize(h->corpus_ev));
+    if (f_items.get()) h->d_nz_items = std::move(f_items);
+    if (f_seg0.get()) h->d_nz_seg0 = std::move(f_seg0);
+    if (f_sums.get()) h->d_nz_sums = std::move(f_sums);
+    if (f_pcm.get()) h->d_nz_pcm = std::move(f_pcm);
+    CorpusPlan plan;
+    if (d_inputs) {
+        plan = corpus_plan(h, h->d_nz_pcm.get(), ws_off.data(), n_items, PB_CORPUS_LISTENER, 1, max_samples, ws_len.data());
+        rc = corpus_reserve(h, plan, n_items, CorpusPoolSizes{}, s);
+        if (rc != PB_OK) return rc;
+    } else {
+        CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
+    }
+    auto launch = [&]() -> int {
+        CK(cudaMemcpyAsync(h->d_nz_items.get(), items.data(), items.size() * sizeof(NoiseItem), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_nz_seg0.get(), seg0.data(), seg0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(h->d_nz_sums.get(), 0, 2 * (size_t)n_items * sizeof(unsigned long long), s));
+        noise_sums_kernel<<<(unsigned)n_seg, NZ_THREADS, 0, s>>>(d_pcm, d_noise, n_noise, h->d_nz_items.get(), h->d_nz_seg0.get(),
+                                                                 (int)n_items, h->d_nz_sums.get());
+        CK(cudaGetLastError());
+        noise_mix_kernel<<<(unsigned)n_seg, NZ_THREADS, 0, s>>>(d_pcm, d_noise, n_noise, h->d_nz_items.get(), h->d_nz_seg0.get(),
+                                                                (int)n_items, h->d_nz_sums.get(), d_out,
+                                                                d_inputs ? h->d_nz_pcm.get() : nullptr);
+        CK(cudaGetLastError());
+        if (!d_inputs) return PB_OK;
+        rc = corpus_k1(h, plan, h->d_nz_pcm.get(), n_items, divisor, PB_CORPUS_LISTENER, 1, s);
+        if (rc != PB_OK) return rc;
+        const int T = h->cfg.n_features, F = h->feat;
+        const long long total = (long long)n_items * T * F;
+        vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->row_stride,
+                                                                               T, F, n_items, d_inputs);
         CK(cudaGetLastError());
         return PB_OK;
     };

@@ -28,6 +28,12 @@ Labelled clips (one network input per clip, vectorize's; statistics per pool mod
 Training (fused-family networks, many per call: pb_vectorize_clips, pb_train, pb_train_loss):
   vectorize_clips   vectorize(clip) of every clip, on the device
   TrainState, train ~ precise/model.py:57-91, scripts/train.py:159-166 (Keras fit: loss, dropout, RMSprop; val_loss)
+
+Noise augmentation (pb_add_noise):
+  NoiseSource       ~ precise/scripts/add_noise.py:56-80 (NoiseData: the noise files as one cyclic stream and its position)
+  add_noise         ~ add_noise.py:82-87 (noised_audio of each clip, on the device)
+  vectorize_noisy   vectorize of each noisy clip, without the clips leaving the device
+  Augment           fresh noisy copies of every training clip in every epoch of train
 """
 from dataclasses import dataclass
 
@@ -685,14 +691,30 @@ class TrainState:
 
 
 def train(core: PreciseB200, state: TrainState, inputs, targets, rows=None, recs=None, epochs=10, batch_size=5000,
-          sensitivity=0.2, dropout=0.2, lr=0.001, validation=None):
+          sensitivity=0.2, dropout=0.2, lr=0.001, validation=None, augment=None):
     """precise-train's fit for every network of ``state`` at once (pb_train): ``epochs`` epochs over ``inputs``
     (vectorize_clips' tensor) with labels ``targets`` (non-zero = wake word), loss_bias = 1 - sensitivity (train.py:86).
     rows / recs None: every network on every input; otherwise entry p is inputs[recs[p]] for network rows[p] (each word
     on its owner's clips plus shared negatives).  state.epoch advances by ``epochs``.  Returns the epoch losses, float64
     [k, epochs]; with validation=(inputs, targets) or (inputs, targets, rows, recs) also val_loss [k, epochs], each
-    network's loss over its validation entries without dropout after each epoch (pb_train_loss, Keras's evaluate)."""
+    network's loss over its validation entries without dropout after each epoch (pb_train_loss, Keras's evaluate).
+    augment (an Augment): ``inputs`` are then the clips themselves (as vectorize_clips takes them), and each epoch is one
+    pb_train call over entries clip-major, clip c's clean input at c (copies + 1) followed by its noisy copies; targets
+    and rows / recs pairs expand to each clip's clean and noisy entries.  Validation stays clean."""
     kw = dict(rows_of=rows, recs=recs, batch_size=batch_size, lr=lr, loss_bias=1.0 - sensitivity, dropout=dropout)
+    if augment is not None:
+        vals = []
+        step = lambda: None
+        if validation is not None:
+            v_in, v_tg = validation[0], validation[1]
+            v_rows, v_recs = (validation[2], validation[3]) if len(validation) > 2 else (None, None)
+            step = lambda: vals.append(core.train_loss(v_in, v_tg, state.rows, state.weights, v_rows, v_recs,
+                                                       loss_bias=1.0 - sensitivity))
+        kw.pop('rows_of'), kw.pop('recs')
+        loss = _train_augmented(core, state, inputs, targets, rows, recs, epochs, kw, augment, step)
+        if validation is None:
+            return loss
+        return loss, core.torch.stack(vals, 1).cpu().numpy() if vals else np.zeros((len(state.hidden), 0))
     if validation is None:
         loss = core.train(inputs, targets, state.rows, state.weights, state.rms, epochs=epochs, epoch0=state.epoch, **kw)
         state.epoch += epochs
@@ -708,3 +730,159 @@ def train(core: PreciseB200, state: TrainState, inputs, targets, rows=None, recs
     loss = core.torch.cat(losses, 1).cpu().numpy() if losses else np.zeros((k, 0))
     val = core.torch.stack(vals, 1).cpu().numpy() if vals else np.zeros((k, 0))
     return loss, val
+
+
+# ---- noise augmentation -----------------------------------------------------------------------------------------------------
+
+class NoiseSource:
+    """A noise corpus packed on the device as one int16 stream (the clips in the order given; empty ones contribute
+    nothing), and ``pos``, the position NoiseData.get_fresh_noise reads on from (add_noise.py:56-80).  add_noise and
+    vectorize_noisy advance it by the lengths of the clips they mix, modulo the corpus's length."""
+
+    def __init__(self, core: PreciseB200, noise_clips, pos=0):
+        torch = core.torch
+        clips = [_check_recording(core, c) for c in noise_clips]
+        parts = [torch.from_numpy(np.ascontiguousarray(c)) if isinstance(c, np.ndarray) else c for c in clips]
+        self.noise = torch.cat([p.to(core.device) for p in parts] + [torch.zeros(0, dtype=torch.int16, device=core.device)])
+        if self.noise.numel() == 0:
+            raise ValueError('the noise corpus is empty')
+        if not 0 <= int(pos) < self.noise.numel():
+            raise ValueError('pos = %d outside [0, %d)' % (int(pos), self.noise.numel()))
+        self.pos = int(pos)
+
+    def __len__(self):
+        return int(self.noise.numel())
+
+
+def _noise_calls(core: PreciseB200, clips, items):
+    """The library calls of a mix over items[i] = clip index, split as vectorize_clips splits clips: a list of (packed pcm,
+    offsets, the items' entries, first item, item count, samples)."""
+    clips = [_check_recording(core, c) for c in clips]
+    items = np.arange(len(clips), dtype=np.int64) if items is None else np.asarray(items, np.int64)
+    if items.ndim != 1:
+        raise ValueError('items must be a 1-D array')
+    if items.size and (items.min() < 0 or items.max() >= len(clips)):
+        raise ValueError('items must lie in [0, %d)' % len(clips))
+    calls, first = [], 0
+    for g in _call_groups([clips[i] for i in items]) if items.size else []:
+        uniq, local = np.unique(items[first:first + len(g)], return_inverse=True)
+        pcm, offsets, entry = _pack(core, [clips[i] for i in uniq])
+        calls.append((pcm, offsets, entry[local].astype(np.int32), first, len(g), sum(int(c.shape[0]) for c in g)))
+        first += len(g)
+    return calls, int(items.size)
+
+
+def _mix_calls(core: PreciseB200, calls, n_items, noise, pos, ratios, out, inputs):
+    """pb_add_noise over _noise_calls' calls, the noise position carried from call to call.  Returns (int16 tensor or None,
+    float32 tensor or None, position after the last item)."""
+    torch = core.torch
+    ratios = np.asarray(ratios, np.float64)
+    if ratios.shape != (n_items,):
+        raise ValueError('one ratio per item')
+    outs, ins = [], []
+    for pcm, offsets, entries, first, count, samples in calls:
+        o, x = core.add_noise(pcm, offsets, noise, entries, ratios[first:first + count], pos, out=out, inputs=inputs)
+        outs.append(o)
+        ins.append(x)
+        pos = (pos + samples) % int(noise.numel())
+    cat = lambda parts, empty: (parts[0] if len(parts) == 1 else torch.cat(parts)) if parts else empty
+    o = cat(outs, torch.zeros(0, dtype=torch.int16, device=core.device)) if out else None
+    x = cat(ins, torch.empty((0, core.n_features, core.feature_size), dtype=torch.float32, device=core.device)) if inputs else None
+    return o, x, pos
+
+
+def _mix_groups(core: PreciseB200, clips, noise, pos, ratios, items, out, inputs):
+    calls, n_items = _noise_calls(core, clips, items)
+    return _mix_calls(core, calls, n_items, noise, pos, ratios, out, inputs)
+
+
+def add_noise(core: PreciseB200, clips, source: NoiseSource, ratios, items=None):
+    """precise-add-noise's noised_audio on the device: item i is clips[items[i]] (items None: every clip once, in order)
+    mixed with the next stretch of ``source``'s noise at ratio ratios[i] (pb_add_noise's arithmetic; the reference's
+    differences are a silent span adding no noise and out-of-range values saturating).  Clips are 1-D int16 numpy arrays or
+    CUDA tensors read as load_audio reads them; empty ones give empty clips.  Returns (int16 CUDA tensor of the mixed clips
+    back to back, host int64 offsets [n_items + 1]) and advances source.pos; one call or many give the same clips."""
+    n = len(clips) if items is None else len(items)
+    lens = np.asarray([int(clips[i].shape[0]) for i in (range(n) if items is None else items)], np.int64)
+    o, _, source.pos = _mix_groups(core, clips, source.noise, source.pos, ratios, items, True, False)
+    return o, np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+
+
+def vectorize_noisy(core: PreciseB200, clips, source: NoiseSource, ratios, items=None):
+    """vectorize of each of add_noise's clips (none may be empty), float32 [n_items, n_features, feature_size], without the
+    mixed clips leaving the device: the rows pb_vectorize_clips makes of them when each clip's last max_samples samples start
+    at a multiple of 8 samples (so with the generic K1 forced, bit for bit vectorize_clips(add_noise(...))).  Advances
+    source.pos as add_noise does."""
+    _, x, source.pos = _mix_groups(core, clips, source.noise, source.pos, ratios, items, False, True)
+    return x
+
+
+_M64 = (1 << 64) - 1
+
+
+def _mix64(z):
+    """splitmix64's finalizer (pb_train's key, include/precise_b200.h)."""
+    z &= _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def _key(s, e, j, c):
+    return _mix64(_mix64(_mix64(_mix64(s) + e) + j) + c)
+
+
+@dataclass
+class Augment:
+    """Noise augmentation of a training run (train's ``augment``): in every epoch each clip gets ``copies`` fresh noisy
+    copies from ``source``.  In epoch e, item i (clip i // copies, copy i % copies) has ratio low + (high - low) u with
+    u = (key(seed, e, i, 0) >> 11) 2^-53, and the epoch's noise starts at (source.pos + e * copies * sum of the clip lengths)
+    mod len(source); source.pos itself is not moved.  So a resumed fit draws exactly the noise of an uninterrupted one."""
+    source: NoiseSource
+    copies: int = 1
+    low: float = 0.0
+    high: float = 0.4
+    seed: int = 0
+
+    def ratios(self, epoch, n_items):
+        u = np.asarray([(_key(int(self.seed), int(epoch), i, 0) >> 11) * 2.0 ** -53 for i in range(n_items)], np.float64)
+        return self.low + (self.high - self.low) * u
+
+    def position(self, epoch, clip_samples):
+        return (self.source.pos + int(epoch) * self.copies * int(clip_samples)) % len(self.source)
+
+
+def _train_augmented(core, state, clips, targets, rows, recs, epochs, kw, augment: Augment, validation_step):
+    """train with augment: one pb_train call per epoch over the clean clips plus each clip's noisy copies, clip-major."""
+    torch = core.torch
+    M = int(augment.copies)
+    if M < 1:
+        raise ValueError('copies must be >= 1')
+    clips = [_check_recording(core, c) for c in clips]
+    n = len(clips)
+    targets = np.asarray(targets)
+    if targets.shape != (n,):
+        raise ValueError('one target per clip')
+    clean = vectorize_clips(core, clips)
+    items = np.repeat(np.arange(n, dtype=np.int64), M)
+    calls, _ = _noise_calls(core, clips, items)                # packed once, mixed afresh every epoch
+    samples = sum(int(c.shape[0]) for c in clips)
+    tg = np.repeat(targets != 0, M + 1).astype(np.uint8)
+    if rows is not None:
+        rows = np.repeat(np.asarray(rows, np.int32), M + 1)
+        recs = (np.repeat(np.asarray(recs, np.int64), M + 1) * (M + 1) + np.tile(np.arange(M + 1), len(recs))).astype(np.int64)
+        kw = dict(kw, rows_of=rows, recs=recs)
+    losses = []
+    for _ in range(epochs):
+        e = state.epoch
+        _, noisy, _ = _mix_calls(core, calls, n * M, augment.source.noise, augment.position(e, samples),
+                                 augment.ratios(e, n * M), False, True)
+        x = torch.empty((n, M + 1, core.n_features, core.feature_size), dtype=torch.float32, device=core.device)
+        x[:, 0] = clean
+        x[:, 1:] = noisy.view(n, M, core.n_features, core.feature_size)
+        x = x.view(n * (M + 1), core.n_features, core.feature_size)
+        losses.append(core.train(x, tg, state.rows, state.weights, state.rms, epochs=1, epoch0=e, **kw))
+        state.epoch += 1
+        validation_step()
+    k = len(state.hidden)
+    return core.torch.cat(losses, 1).cpu().numpy() if losses else np.zeros((k, 0))

@@ -3,6 +3,7 @@ folder of labelled clips.
 
     python -m mycroft_precise_b200.train MODEL.npz [MODEL.npz ...] FOLDER [-e EPOCHS] [-b BATCH] [-s SENSITIVITY]
                                          [--dropout RATE] [--seed SEED] [--hidden UNITS]
+                                         [--noise-folder NOISE_FOLDER [-if N] [-nl LOW] [-nh HIGH]]
 
 FOLDER has TrainData.from_folder's layout, as precise-test reads it (test.load_folder): the clips under ``FOLDER/wake-word``
 and ``FOLDER/not-wake-word`` are trained on, and those under ``FOLDER/test/...`` give the val_loss.  An existing MODEL.npz
@@ -11,6 +12,10 @@ the i-th model) at the default ListenerParams.  Every model must share the first
 (hidden <= 24, feature size <= 16, no deltas); all of them train at once in one set of device calls (offline.train).  For
 each model, in the order given, a ``=== <model file> ===`` heading is printed, then one line per epoch with its loss and
 val_loss as Keras prints them.  Each model's weights are saved to its .npz and its .params written next to it.
+
+With ``--noise-folder``, every epoch also trains on N fresh noisy copies of each training clip (offline.Augment): noise from
+NOISE_FOLDER/*.wav (sorted, read as one cyclic stream, as precise-add-noise reads it) at ratios between LOW and HIGH drawn
+from ``--seed``.  The validation clips stay clean.
 """
 import argparse
 import os
@@ -29,6 +34,10 @@ def main(argv=None):
     ap.add_argument('--seed', type=int, default=0, help='seed of new networks (seed + i) and of every shuffle and mask')
     ap.add_argument('--hidden', type=int, default=20, help='GRU units of new networks')
     ap.add_argument('--device', type=int, default=0)
+    ap.add_argument('--noise-folder', default=None, help='folder of noise wavs: train on fresh noisy copies every epoch')
+    ap.add_argument('-if', '--inflation-factor', type=int, default=1, help='noisy copies of each clip per epoch')
+    ap.add_argument('-nl', '--noise-ratio-low', type=float, default=0.0, help='minimum ratio of noise to sample')
+    ap.add_argument('-nh', '--noise-ratio-high', type=float, default=0.4, help='maximum ratio of noise to sample')
     args = ap.parse_args(argv)
 
     from .core import PreciseB200
@@ -56,9 +65,20 @@ def main(argv=None):
         raise SystemExit('no training clips under %s' % args.folder)
     core = PreciseB200(pr, hidden=models[0][0].hidden, device=args.device, activation=models[0][0].activation,
                        recurrent_activation=models[0][0].recurrent_activation)
-    inputs = vectorize_clips(core, clips)
     state = TrainState.from_models(core, [m for m, _ in models], [args.seed + i for i in range(len(models))])
     kw = dict(epochs=args.epochs, batch_size=args.batch_size, sensitivity=args.sensitivity, dropout=args.dropout)
+    if args.noise_folder is None:
+        inputs = vectorize_clips(core, clips)
+    else:
+        import glob
+        from .offline import Augment, NoiseSource
+        from .simulate import read_wav
+        noise = [read_wav(f, pr.sample_rate) for f in sorted(glob.glob(os.path.join(args.noise_folder, '*.wav')))]
+        if sum(n.shape[0] for n in noise) == 0:
+            raise SystemExit('no noise audio in %s/*.wav' % args.noise_folder)
+        inputs = clips
+        kw['augment'] = Augment(NoiseSource(core, noise), args.inflation_factor, args.noise_ratio_low, args.noise_ratio_high,
+                                args.seed)
     if v_clips:
         loss, val = train(core, state, inputs, targets, validation=(vectorize_clips(core, v_clips), v_targets), **kw)
     else:
