@@ -23,6 +23,7 @@
 #include "../../include/precise_b200.h"
 #include "gru_kernels.cuh"
 #include "gru_bank.cuh"
+#include "gru_wg.cuh"
 #include "gru_wide.cuh"
 #include "mfcc_kernels.cuh"
 #include "mfcc_fast.cuh"
@@ -1120,12 +1121,19 @@ static void set_bank_slot(BankParams& P, int slot, const Network& net, const K2O
     P.o[slot] = o;
 }
 
+// One model runs on warpgroup MMA (gru_wg_kernel), banks of two or more on mma.sync (gru_bank_kernel).
 template <int NM, bool RING, bool KERAS_ACT>
 static int launch_bank_act(const BankParams& P, const K2In& in, int64_t n, cudaStream_t s) {
     constexpr size_t smem = (size_t)NM * BANK_MODEL_SMEM + (bank_stages(NM, RING) ? BANK_STAGE_SMEM : 0);
-    if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(gru_bank_kernel<NM, RING, KERAS_ACT>, smem));      // above the default limit
     const int per_cta = (MMA_THREADS / 32) * 16;
-    gru_bank_kernel<NM, RING, KERAS_ACT><<<(int)((n + per_cta - 1) / per_cta), MMA_THREADS, smem, s>>>(P, in, n);
+    const int grid = (int)((n + per_cta - 1) / per_cta);
+    if constexpr (NM == 1) {
+        if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(gru_wg_kernel<RING, KERAS_ACT>, smem));
+        gru_wg_kernel<RING, KERAS_ACT><<<grid, MMA_THREADS, smem, s>>>(P, in, n);
+    } else {
+        if constexpr (smem > 48 * 1024) CK(ensure_dyn_smem(gru_bank_kernel<NM, RING, KERAS_ACT>, smem));      // above the default limit
+        gru_bank_kernel<NM, RING, KERAS_ACT><<<grid, MMA_THREADS, smem, s>>>(P, in, n);
+    }
     CK(cudaGetLastError());
     return PB_OK;
 }

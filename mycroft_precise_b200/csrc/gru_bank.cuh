@@ -1,5 +1,6 @@
-// gru_bank.cuh -- K2 for the fused family of networks (H <= 24, feature_size <= 16, no deltas, any activation pair): the
-// default network's large-batch scan, and every such network of a model bank in ONE launch over the handle's shared MFCC ring.
+// gru_bank.cuh -- K2 for the fused family of networks (H <= 24, feature_size <= 16, no deltas, any activation pair): every
+// such network of a model bank in ONE launch over the handle's shared MFCC ring, routed scans and the model pool.  One model
+// alone (the default network's large-batch scan) runs the same arithmetic on warpgroup MMA in gru_wg.cuh.
 //
 // The per-step products run on the warp-level tensor cores in fp16 x 3 (hi / lo split of both operands, fp32 accumulate:
 // a_lo b_hi + a_hi b_lo + a_hi b_hi) on mma.sync m16n8k16 / m16n8k8: one k16 + one k8 MMA per n-tile and pass cover the 24
@@ -327,7 +328,7 @@ __device__ __forceinline__ void bank_scan(const PS& P, int m0, const int2* list,
 
 // Every model of P over the n items of a tick (or of pb_predict's inputs), 64 items per CTA.
 template <int NM, bool RING, bool KERAS_ACT>
-__global__ void __launch_bounds__(MMA_THREADS, NM == 1 ? 4 : 1)      // NM = 1: 128 registers (ptxas alone picks 96 and spills)
+__global__ void __launch_bounds__(MMA_THREADS, 1)                    // NM >= 2: one model runs in gru_wg_kernel (gru_wg.cuh)
 gru_bank_kernel(const __grid_constant__ BankParams P, K2In in, long long n) {
     bank_scan<NM, RING, KERAS_ACT>(P, 0, nullptr, blockIdx.x, in, n);
 }

@@ -9,6 +9,7 @@ same tick sequence, so the last tick's raw / conf / fired must be bit-identical 
 K2's floors come from what the scan has to do per update (bench.py's roofline_k2 block models an older kernel):
   bytes  K2_BYTES_PER_UPDATE = 29 ring rows x 64 B + raw (4) + conf (8) + fired (1) + trigger state (4 read + 4 written)
   FLOP   K2_MMA_FLOP_PER_UPDATE = 9 n-tiles x 3 passes x 29 steps x (m16n8k16 for x.W + m16n8k16 and m16n8k8 for h.U) / 16 streams
+         K2_WGMMA_FLOP_PER_UPDATE: the same with the k8 products run as k16 (what gru_wg_kernel executes)
 against the H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense fp16).
 
 The parent commit's library, for the default comparison:
@@ -27,6 +28,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 S, PRIME, TIMED = 131072, 30, 50
 K2_BYTES_PER_UPDATE = 29 * 64 + 4 + 8 + 1 + 4 + 4                      # 1 877
 K2_MMA_FLOP_PER_UPDATE = 9 * 3 * 29 * (2 * 16 * 8 * 16 + 2 * 16 * 8 * 16 + 2 * 16 * 8 * 8) // 16   # 501 120
+K2_WGMMA_FLOP_PER_UPDATE = 9 * 3 * 29 * (3 * 2 * 16 * 8 * 16) // 16                         # 601 344: k8 groups run as k16 on wgmma
 HBM_BPS, FP16_FLOPS = 3.35e12, 989e12
 DEFAULT_ARMS = ['parent=' + os.path.join(ROOT, 'build', 'parent', 'mycroft_precise_b200', 'csrc', 'libprecise_b200.so'),
                 'tree=' + os.path.join(ROOT, 'mycroft_precise_b200', 'csrc', 'libprecise_b200.so')]
@@ -102,7 +104,8 @@ def main():
             same = all(np.array_equal(outs[k].view(np.uint8), ref[k].view(np.uint8)) for k in outs)
             sec = r['k2_us'] * 1e-6
             r.update(arm=name, round=rnd, outputs_match_first=same,
-                     k2_GBps=S * K2_BYTES_PER_UPDATE / sec / 1e9, k2_TFLOPs=S * K2_MMA_FLOP_PER_UPDATE / sec / 1e12)
+                     k2_GBps=S * K2_BYTES_PER_UPDATE / sec / 1e9, k2_TFLOPs=S * K2_MMA_FLOP_PER_UPDATE / sec / 1e12,
+                     k2_wgmma_TFLOPs=S * K2_WGMMA_FLOP_PER_UPDATE / sec / 1e12)
             r['k2_frac_of_floor'] = max(S * K2_BYTES_PER_UPDATE / HBM_BPS, S * K2_MMA_FLOP_PER_UPDATE / FP16_FLOPS) / sec
             print('round %d %-8s K1 %6.1f us  K2 %6.1f us  tick %6.1f us | K2 %5.0f GB/s  %5.1f TFLOP/s  %.0f %% of the floor | '
                   'outputs bit-identical to the first run: %s'
@@ -116,7 +119,8 @@ def main():
     if args.out:
         with open(args.out, 'w') as f:
             json.dump(dict(card=gpu, streams=S, prime=PRIME, timed=TIMED, bytes_per_update=K2_BYTES_PER_UPDATE,
-                           mma_flop_per_update=K2_MMA_FLOP_PER_UPDATE, results=results), f, indent=1)
+                           mma_flop_per_update=K2_MMA_FLOP_PER_UPDATE,
+                           wgmma_flop_per_update=K2_WGMMA_FLOP_PER_UPDATE, results=results), f, indent=1)
     if not all(r['outputs_match_first'] for r in results):
         sys.exit('outputs differ between runs')
 
