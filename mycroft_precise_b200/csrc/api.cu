@@ -118,7 +118,7 @@ private:
 
 // One network's weights in every layout a kernel reads (load_weights builds them all at once; they never change after).
 struct NetWeights {
-    bool small_path = false;         // the default network (H = 20, F = 13, linear / hard_sigmoid): gru_warp / gru_small / gru_bank<1>
+    bool small_path = false;         // the default network (H = 20, F = 13, linear / hard_sigmoid): gru_warp / gru_small / gru_wg
     GruSmallW<20, 13> w_small;       // ... its weights as a kernel parameter
     DevArray<float> wcat, bias, wd;  // gru_tiled_kernel: [W; U], bias, dense weights (gru_wide_kernel reads wd as well)
     float bd = 0.f;
@@ -1157,7 +1157,7 @@ static int launch_gru_kernels(const Network& net, int F, const K2In& in, bool ri
         const int grid = (int)((n + 3) / 4);
         if (ring) gru_warp_kernel<20, 13, true><<<grid, 128, 0, s>>>(nw.w_small, in, n, dp, o);
         else gru_warp_kernel<20, 13, false><<<grid, 128, 0, s>>>(nw.w_small, in, n, dp, o);
-    } else if (nw.small_path && net.gru_mode != 1) {              // tensor-core scan (mma.sync fp16 x 3): the bank kernel with one model
+    } else if (nw.small_path && net.gru_mode != 1) {              // tensor-core scan (fp16 x 3): gru_wg_kernel, the one-model bank launch
         BankParams P{};
         set_bank_slot(P, 0, net, o);
         return ring ? launch_bank_nm<1, true>(P, in, n, s) : launch_bank_nm<1, false>(P, in, n, s);

@@ -2,7 +2,10 @@
 front ends and weight magnitudes it accepts.
 
 Every pool tick, bank tick, corpus call and large-batch pb_predict of a network with H <= 24, feature_size <= 16 and no
-deltas runs bank_scan.  The other test files check those paths mostly for bit identity with each other; here each one is
+deltas runs bank_scan, except that one-model launches (the default network above 8 192 streams, one-model update_models,
+a bank with one fused model) run the same arithmetic on warpgroup MMA in gru_wg_kernel (gru_wg.cuh).  Here only
+test_operand_range's 9 000-stream ticks reach gru_wg_kernel; test_gpu_wg_scan.py checks it bit for bit against the
+mma.sync kernels and against float64 on every path that reaches it.  The other test files check those paths mostly for bit identity with each other; here each one is
 anchored to oracle.gru.gru_forward in float64 on the window the GPU itself scored (read_window after each tick), which
 isolates the scan from the MFCC front end, with one end-to-end check per front end against the oracle listeners.
 
@@ -430,7 +433,7 @@ def test_operand_range(sign):
     d20, d16 = doubling(13, 20, sign), doubling(13, 16, sign)
     K = 6
     outs = {}
-    for S in (300, 9000):                     # gru_warp_kernel (fp32) and gru_bank_kernel<1> (fp16 x 3)
+    for S in (300, 9000):                     # gru_warp_kernel (fp32) and gru_wg_kernel (fp16 x 3)
         pcm = audio(64, K * 1024, seed=S)
         pcm = np.tile(pcm, (S // 64 + 1, 1))[:S].copy()
         sb = m.StreamBatch(d20, S)

@@ -6,7 +6,8 @@ Tolerances
   * GRU output on identical inputs: abs 1e-5 (BASELINE.json north_star), vs the fp32 AND fp64 oracle.  The fused
     family's fp16 x 3 scan (H <= 24, feature_size <= 16, no deltas: pools, banks, corpus calls and the default network above
     8 192 streams) is anchored to float64 over its shapes, front ends, weight magnitudes and operand range in
-    test_gpu_fused_scan.py, with oracle.gru.gru_forward_f16x3 bounding what larger weights may cost.  The other networks'
+    test_gpu_fused_scan.py, with oracle.gru.gru_forward_f16x3 bounding what larger weights may cost; its one-model form on
+    warpgroup MMA (gru_wg_kernel) is checked bit for bit against the mma.sync kernels in test_gpu_wg_scan.py.  The other networks'
     scans (gru_wide_kernel's 3 x TF32, gru_tiled_kernel) and the default network's CUDA-core scans (gru_warp_kernel,
     gru_small_kernel) are anchored the same way in test_gpu_wide_scan.py, with oracle.gru.gru_forward_tf32x3 as the wide
     kernel's reference.
@@ -202,7 +203,7 @@ def test_predict_small_path(core, scale):
 
 @pytest.mark.parametrize('mode', [0, 1, 2])
 def test_default_network_kernel_variants(core, mode):
-    """warp-per-stream (auto, small n), thread-per-stream CUDA-core (1) and tensor-core mma.sync fp16 x 3 (2) kernels."""
+    """warp-per-stream (auto, small n), thread-per-stream CUDA-core (1) and tensor-core fp16 x 3 (2, gru_wg_kernel) kernels."""
     w = og.GruWeights.random(13, 20, seed=11, scale=0.1)
     core.load_weights(w.kernel, w.recurrent, w.bias, w.dense_w, w.dense_b)
     core.gru_mode(mode)
@@ -244,9 +245,10 @@ def test_stream_tick_kernel_variants_agree():
 
 
 def test_large_batch_tensor_core_scan():
-    """n > 8192 streams: the tensor-core scan (gru_bank_kernel with one model) vs the CUDA-core kernel, including a weight
-    reload and a small-batch tick in between.  A one-model update_models arm goes through the same sequence and must score
-    bit for bit like update's scan: a window's score does not depend on the ticks before it."""
+    """n > 8192 streams: the tensor-core scan (gru_wg_kernel) vs the CUDA-core kernel, including a weight reload and a
+    small-batch tick in between.  A one-model update_models arm goes through the same sequence and must score bit for bit
+    like update's scan: a window's score does not depend on the ticks before it.  Both arms run gru_wg_kernel, so that
+    comparison is wgmma against itself; test_gpu_wg_scan.py compares it with the mma.sync kernels."""
     m = _mod()
     S, K, chunk = 9000, 36, 1024
     pcm = noise(64, K * chunk, seed=33)

@@ -1,8 +1,10 @@
-"""-m gpu: the tick's window scan (gru_bank_kernel, rows staged from the MFCC ring through shared memory) against pb_predict on
+"""-m gpu: the tick's window scan (gru_wg_kernel, rows staged from the MFCC ring through shared memory) against pb_predict on
 the same windows (the same kernel, rows loaded directly from a [n][29][13] tensor).
 
-Above 8 192 streams per tick both run the tensor-core scan with the same arithmetic, so a window scored by the tick and the
-same window read back (read_window) and scored by predict must give bit-identical raw outputs: a row staged from the wrong
+Above 8 192 streams per tick both run the tensor-core scan with the same arithmetic (gru_wg_kernel<true, true> and
+<false, true>), so a window scored by the tick and the same window read back (read_window) and scored by predict must
+give bit-identical raw outputs.  This checks staging against direct loads, wgmma against itself; test_gpu_wg_scan.py
+compares both with the mma.sync kernels.  A row staged from the wrong
 ring slot, stream or step, or a zero row staged as data (or the reverse), shows up as a difference.  The ticks use permuted
 subsets of the streams and clear some of them on the way, so windows start at every ring slot and young streams (fewer
 than 29 frames, leading zero rows) are scored beside full ones."""
