@@ -635,6 +635,52 @@ int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, i
                  int64_t n_items, int64_t noise_pos, int32_t divisor, int64_t max_samples,
                  int16_t* d_out, float* d_inputs, void* stream);
 
+/* precise-train-generated (precise/scripts/train_generated.py:118-190): clips overlaid on background recordings.
+ * Backgrounds d_bg / h_bg_offsets [n_bg + 1] and clips d_clips / h_clip_offsets [n_clips + 1] are DEVICE int16 recordings
+ * given as pb_vectorize_clips takes them.  Item i (h_items, HOST) is the first `length` samples of background `background`
+ * at gain `gain`, overlaid with segments h_segs[seg_begin .. seg_end) (HOST) laid back to back from its sample 0: segment
+ * (clip, start, length) is samples [start, start + length) of clip `clip`, or `length` samples of silence for clip = -1
+ * (start 0), at most 2^62.  The segments must cover at least the item's length; what lies beyond it is not used.  Items may
+ * share or overlap segment ranges, at any lengths: each item reads its range from its own sample 0.  With S the exact int64
+ * sum of squares of a WHOLE recording over its raw int16 samples and n its length (calc_volume sees the whole file):
+ *     rms = S > 0 ? sqrt(S / n) : 0,   vol = gain rms_background,   g = rms_clip > 0 ? vol / rms_clip : 0 (0 in silence),
+ *     y = 0.4 (gain x_background) + 0.6 (g x_clip),   out = int16(clamp(rint(y), -32768, 32767))
+ * in IEEE double, in that order, every conversion and operation rounded on its own (no FMA).  The reference mixes in float
+ * and hands the listener unrounded audio; it gives NaN for a silent clip or background.
+ *   - d_out (DEVICE int16, optional) receives the items' streams back to back, item i at the sum of the lengths before it.
+ *   - d_inputs [n_windows][n_features][feature_size] (DEVICE, optional): row w is the listener-schedule window (as
+ *     pb_score_corpus's PB_CORPUS_LISTENER windows with this chunk) after (c + 1) chunk samples of item i, for
+ *     h_windows[w] = (i, c) (HOST int64 pairs [n_windows][2], c below the item's length / chunk), its samples read as
+ *     x / divisor.  Each stream is framed from a multiple of 8 samples in a workspace, so the fast K1 applies.
+ * Asynchronous on `stream`; shares and orders itself against the corpus workspace as pb_vectorize_clips.  Every argument is
+ * checked before anything is enqueued, so a refused call changes no buffer.
+ * PB_ERR_INVALID: offsets null, negative or decreasing, a null recording pointer with samples, counts outside [0, 2^31), a
+ * null table with a positive count, divisor other than 32768 / 32767, chunk < 1, a segment's clip outside [-1, n_clips) or
+ * samples outside it (silence with start != 0), a segment length outside [0, 2^62], an item's background outside [0, n_bg), a gain that is not finite and >= 0,
+ * a length outside [0, the background's], segments outside [0, n_segs) or covering less than the length, a window's item
+ * or chunk out of range, h_windows without d_inputs, both outputs null.  PB_ERR_UNSUPPORTED: d_inputs on a front end outside
+ * the fused family.  PB_ERR_CUDA: the workspace cannot be allocated. */
+typedef struct pb_gen_item {
+    int32_t background;
+    int32_t reserved;
+    double gain;
+    int64_t length;
+    int64_t seg_begin, seg_end;
+} pb_gen_item;
+
+typedef struct pb_gen_segment {
+    int32_t clip;              /* -1: silence */
+    int32_t reserved;
+    int64_t start;
+    int64_t length;
+} pb_gen_segment;
+
+int pb_generate(pb_handle* h, const int16_t* d_bg, const int64_t* h_bg_offsets, int64_t n_bg,
+                const int16_t* d_clips, const int64_t* h_clip_offsets, int64_t n_clips,
+                const pb_gen_item* h_items, int64_t n_items, const pb_gen_segment* h_segs, int64_t n_segs,
+                const int64_t* h_windows, int64_t n_windows, int64_t chunk, int32_t divisor,
+                int16_t* d_out, float* d_inputs, void* stream);
+
 /* Floats per network of pb_train's weight and accumulator arrays.  A row holds Keras's order, flat: kernel[F][3H],
  * recurrent[H][3H], bias[3H], dense_w[H], dense_b; the tail after 3H(F + H + 1) + H + 1 floats (2 977 at H = 24, F = 16) is
  * zero and stays zero. */

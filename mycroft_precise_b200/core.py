@@ -46,6 +46,12 @@ class pb_train_row(C.Structure):
     _fields_ = [('hidden', C.c_int32), ('activation', C.c_int32), ('recurrent_activation', C.c_int32), ('seed', C.c_uint32)]
 
 
+# pb_generate's host tables (pb_gen_item, pb_gen_segment) as numpy records
+GEN_ITEM = np.dtype([('background', '<i4'), ('reserved', '<i4'), ('gain', '<f8'), ('length', '<i8'), ('seg_begin', '<i8'),
+                     ('seg_end', '<i8')])
+GEN_SEGMENT = np.dtype([('clip', '<i4'), ('reserved', '<i4'), ('start', '<i8'), ('length', '<i8')])
+
+
 class pb_train_opts(C.Structure):
     _fields_ = [('epochs', C.c_int32), ('epoch0', C.c_int32), ('batch_size', C.c_int32), ('lr', C.c_float), ('rho', C.c_float),
                 ('epsilon', C.c_float), ('loss_bias', C.c_float), ('dropout', C.c_float)]
@@ -103,6 +109,7 @@ SYMBOLS = {
                                    C.c_double, _VP, _I64, _VP, _VP]),
     'pb_vectorize_clips': (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I64, _VP, _VP]),
     'pb_add_noise': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP, _I64, _I64, _I32, _I64, _VP, _VP, _VP]),
+    'pb_generate': (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _I64, _VP, _I64, _VP, _I64, _VP, _I64, _I64, _I32, _VP, _VP, _VP]),
     'pb_train_opts_default': (C.c_int, [C.POINTER(pb_train_opts)]),
     'pb_train': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.POINTER(pb_train_opts), _VP, _VP, _VP, _VP]),
     'pb_train_loss': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.c_float, C.c_float, _I32, _VP, _VP, _VP, _VP]),
@@ -1075,6 +1082,34 @@ class PreciseB200:
         check(self.lib.pb_add_noise(self._h, _ptr(pcm), _np_ptr(offsets), n_rec, _ptr(noise), noise.numel(), _np_ptr(items),
                                     _np_ptr(ratios), n, int(noise_pos), int(divisor), int(self.params.max_samples), _ptr(d_out),
                                     _ptr(d_in), self._stream()))
+        return (None if d_out is None else d_out[:total]), d_in
+
+    def generate(self, bg, bg_offsets, clips, clip_offsets, items, segments, windows=None, chunk=2048, divisor=32767, out=True):
+        """Clips overlaid on background recordings: backgrounds bg[bg_offsets[b]:bg_offsets[b + 1]] and clips likewise (1-D
+        int16 CUDA tensors, host int64 offsets), items a GEN_ITEM array and segments a GEN_SEGMENT array (pb_gen_item /
+        pb_gen_segment), windows an int64 array [n_windows, 2] of (item, chunk index) or None.  Returns (the items' streams
+        back to back as an int16 tensor, or None with out=False; the windows' network inputs, float32
+        [n_windows, n_features, feature_size], or None without windows).  Asynchronous on the current stream.  pb_generate in
+        include/precise_b200.h."""
+        torch = self.torch
+        bg_offsets, n_bg = self._corpus_recordings(bg, bg_offsets)
+        clip_offsets, n_clips = self._corpus_recordings(clips, clip_offsets)
+        items = np.ascontiguousarray(items, dtype=GEN_ITEM)
+        segments = np.ascontiguousarray(segments, dtype=GEN_SEGMENT)
+        n = items.shape[0]
+        _check_np('items', items, GEN_ITEM, (n,), optional=False)
+        _check_np('segments', segments, GEN_SEGMENT, (segments.shape[0],), optional=False)
+        if windows is not None:
+            windows = np.ascontiguousarray(windows, dtype=np.int64).reshape(-1, 2)
+        n_win = 0 if windows is None else windows.shape[0]
+        total = int(np.maximum(items['length'], 0).sum())
+        d_out = torch.empty(max(total, 1), dtype=torch.int16, device=self.device) if out else None    # non-null when empty
+        d_in = (torch.empty((n_win, self.n_features, self.feature_size), dtype=torch.float32, device=self.device)
+                if windows is not None else None)
+        check(self.lib.pb_generate(self._h, _ptr(bg), _np_ptr(bg_offsets), n_bg, _ptr(clips), _np_ptr(clip_offsets), n_clips,
+                                   _np_ptr(items), n, _np_ptr(segments), segments.shape[0],
+                                   _np_ptr(windows) if n_win else None, n_win, int(chunk), int(divisor), _ptr(d_out),
+                                   _ptr(d_in), self._stream()))
         return (None if d_out is None else d_out[:total]), d_in
 
     def _train_args(self, inputs, targets, k, rows_of, recs, weights):

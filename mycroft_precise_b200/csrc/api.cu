@@ -41,6 +41,7 @@
 #include "pool.cuh"
 #include "train.cuh"
 #include "noise.cuh"
+#include "generate.cuh"
 
 #include <cub/device/device_segmented_sort.cuh>
 
@@ -231,6 +232,14 @@ struct pb_handle {
     DevArray<long long> d_nz_seg0;   // ... [n_items + 1] each item's first segment
     DevArray<unsigned long long> d_nz_sums;  // ... [n_items][2] (sum x^2, sum n^2)
     DevArray<int16_t> d_nz_pcm;      // ... the mixed clips' cropped tails, each at a multiple of 8 samples (K1's recordings)
+    DevArray<GenRec> d_gen_recs;     // pb_generate: [n_recs] the recordings whose sums of squares the mix needs
+    DevArray<long long> d_gen_rseg0; // ... [n_recs + 1] each recording's first CTA of the sums
+    DevArray<unsigned long long> d_gen_sums;  // ... [n_recs] their sums of squares
+    DevArray<GenItem> d_gen_items;   // ... [n_items]
+    DevArray<long long> d_gen_tile0; // ... [n_items + 1] each item's first CTA of the mix
+    DevArray<GenSeg> d_gen_segs;     // ... each item's own copy of the segments covering it
+    DevArray<long long> d_gen_wins;  // ... [n_windows] the chosen windows' places in the window table
+    DevArray<int16_t> d_gen_pcm;     // ... the generated streams, each at a multiple of 8 samples (K1's recordings)
     int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
@@ -2598,6 +2607,190 @@ PB_API int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_off
         const long long total = (long long)n_items * T * F;
         vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->row_stride,
                                                                                T, F, n_items, d_inputs);
+        CK(cudaGetLastError());
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
+}
+
+// ------------------------------------------------------------------------------------------------
+// generated training audio (generate.cuh)
+
+static int check_offsets(const char* what, const int16_t* d, const int64_t* h_off, int64_t n) {
+    if (n < 0 || n > INT32_MAX) return fail(PB_ERR_INVALID, "n_%s = %lld outside [0, 2^31)", what, (long long)n);
+    if (!h_off) return fail(PB_ERR_INVALID, "null h_%s_offsets", what);
+    if (h_off[0] < 0) return fail(PB_ERR_INVALID, "%s offset 0 = %lld is negative", what, (long long)h_off[0]);
+    for (int64_t r = 0; r < n; ++r)
+        if (h_off[r + 1] < h_off[r]) return fail(PB_ERR_INVALID, "%s offsets decrease at %lld", what, (long long)r);
+    if (h_off[n] > h_off[0] && !d) return fail(PB_ERR_INVALID, "null d_%s", what);
+    return PB_OK;
+}
+
+PB_API int pb_generate(pb_handle* h, const int16_t* d_bg, const int64_t* h_bg_offsets, int64_t n_bg, const int16_t* d_clips,
+                       const int64_t* h_clip_offsets, int64_t n_clips, const pb_gen_item* h_items, int64_t n_items,
+                       const pb_gen_segment* h_segs, int64_t n_segs, const int64_t* h_windows, int64_t n_windows, int64_t chunk,
+                       int32_t divisor, int16_t* d_out, float* d_inputs, void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = d_inputs ? check_train_front_end(h) : PB_OK;
+    if (rc != PB_OK) return rc;
+    if (!d_out && !d_inputs) return fail(PB_ERR_INVALID, "d_out and d_inputs are both null");
+    rc = check_offsets("bg", d_bg, h_bg_offsets, n_bg);
+    if (rc == PB_OK) rc = check_offsets("clip", d_clips, h_clip_offsets, n_clips);
+    if (rc != PB_OK) return rc;
+    if (divisor != 32768 && divisor != 32767) return fail(PB_ERR_INVALID, "divisor %d: 32768 (buffer_to_audio) or 32767 (load_audio)", divisor);
+    if (chunk < 1) return fail(PB_ERR_INVALID, "chunk = %lld must be >= 1", (long long)chunk);
+    if (n_items < 0 || n_items > INT32_MAX) return fail(PB_ERR_INVALID, "n_items = %lld outside [0, 2^31)", (long long)n_items);
+    if (n_segs < 0) return fail(PB_ERR_INVALID, "n_segs = %lld is negative", (long long)n_segs);
+    if (n_windows < 0 || n_windows > INT32_MAX) return fail(PB_ERR_INVALID, "n_windows = %lld outside [0, 2^31)", (long long)n_windows);
+    if ((n_items > 0 && !h_items) || (n_segs > 0 && !h_segs) || (n_windows > 0 && !h_windows))
+        return fail(PB_ERR_INVALID, "null h_items, h_segs or h_windows");
+    if (n_windows > 0 && !d_inputs) return fail(PB_ERR_INVALID, "h_windows without d_inputs");
+    for (int64_t j = 0; j < n_segs; ++j) {
+        const pb_gen_segment& g = h_segs[j];
+        if (g.clip < -1 || g.clip >= n_clips)
+            return fail(PB_ERR_INVALID, "segment %lld: clip %d outside [-1, %lld)", (long long)j, g.clip, (long long)n_clips);
+        if (g.length < 0 || g.length > GEN_MAX_SEG)
+            return fail(PB_ERR_INVALID, "segment %lld: length %lld outside [0, 2^62]", (long long)j, (long long)g.length);
+        const int64_t clen = g.clip >= 0 ? h_clip_offsets[g.clip + 1] - h_clip_offsets[g.clip] : 0;
+        if (g.clip < 0 ? g.start != 0 : (g.start < 0 || g.start > clen - g.length))
+            return fail(PB_ERR_INVALID, "segment %lld: samples [%lld, %lld + %lld) outside clip %d's %lld", (long long)j,
+                        (long long)g.start, (long long)g.start, (long long)g.length, g.clip, (long long)clen);
+    }
+    for (int64_t i = 0; i < n_items; ++i) {
+        const pb_gen_item& it = h_items[i];
+        if (it.background < 0 || it.background >= n_bg)
+            return fail(PB_ERR_INVALID, "item %lld: background %d outside [0, %lld)", (long long)i, it.background, (long long)n_bg);
+        if (!(std::isfinite(it.gain) && it.gain >= 0.0)) return fail(PB_ERR_INVALID, "item %lld: gain %g is not finite and >= 0", (long long)i, it.gain);
+        const int64_t blen = h_bg_offsets[it.background + 1] - h_bg_offsets[it.background];
+        if (it.length < 0 || it.length > blen)
+            return fail(PB_ERR_INVALID, "item %lld: length %lld outside [0, %lld] (its background)", (long long)i, (long long)it.length, (long long)blen);
+        if (it.seg_begin < 0 || it.seg_begin > it.seg_end || it.seg_end > n_segs)
+            return fail(PB_ERR_INVALID, "item %lld: segments [%lld, %lld) outside [0, %lld)", (long long)i, (long long)it.seg_begin,
+                        (long long)it.seg_end, (long long)n_segs);
+        int64_t cover = 0;
+        for (int64_t j = it.seg_begin; j < it.seg_end && cover < it.length; ++j) cover += h_segs[j].length;
+        if (cover < it.length)
+            return fail(PB_ERR_INVALID, "item %lld: its segments cover %lld of its %lld samples", (long long)i, (long long)cover, (long long)it.length);
+    }
+    for (int64_t w = 0; w < n_windows; ++w) {
+        const int64_t i = h_windows[2 * w], c = h_windows[2 * w + 1];
+        if (i < 0 || i >= n_items) return fail(PB_ERR_INVALID, "window %lld: item %lld outside [0, %lld)", (long long)w, (long long)i, (long long)n_items);
+        if (c < 0 || c >= h_items[i].length / chunk)
+            return fail(PB_ERR_INVALID, "window %lld: chunk %lld outside item %lld's %lld complete chunks", (long long)w, (long long)c,
+                        (long long)i, (long long)(h_items[i].length / chunk));
+    }
+
+    const bool vec = d_inputs && n_windows > 0;       // K1 and the gather run only for chosen windows
+    if (!d_out && !vec) return PB_OK;
+
+    // The tables: each background and clip an item uses once (GenRec, with its CTAs of the sums), the items (place in d_out,
+    // and with d_inputs in the workspace at a multiple of 8 samples), and each item's own copy of the segments that cover
+    // its length, with their positions in it: items may share or overlap segment ranges at different lengths.
+    std::vector<GenRec> recs;
+    std::vector<long long> rseg0(1, 0), tile0(1, 0);
+    std::vector<int> bg_rec((size_t)n_bg, -1), clip_rec((size_t)n_clips, -1);
+    auto rec_of = [&](std::vector<int>& ids, int r, const int64_t* off, int clip) {
+        if (ids[r] < 0) {
+            ids[r] = (int)recs.size();
+            const long long len = off[r + 1] - off[r];
+            recs.push_back(GenRec{off[r], len, clip, 0});
+            rseg0.push_back(rseg0.back() + (len + GEN_SEG - 1) / GEN_SEG);
+        }
+        return ids[r];
+    };
+    std::vector<GenItem> items((size_t)n_items);
+    std::vector<GenSeg> segs;
+    std::vector<int64_t> ws_off, ws_len;
+    long long out = 0, ws = 0;
+    for (int64_t i = 0; i < n_items; ++i) {
+        const pb_gen_item& it = h_items[i];
+        const long long len = it.length;
+        const long long seg0 = (long long)segs.size();
+        long long pos = 0;
+        for (int64_t j = it.seg_begin; j < it.seg_end && pos < len; ++j) {   // pos < len <= the background: no overflow
+            const pb_gen_segment& g = h_segs[j];
+            const bool clip = g.clip >= 0 && g.length > 0;
+            segs.push_back(GenSeg{pos, g.length, clip ? h_clip_offsets[g.clip] + g.start : 0,
+                                  clip ? rec_of(clip_rec, g.clip, h_clip_offsets, 1) : -1, 0});
+            pos += g.length;
+        }
+        items[i] = GenItem{h_bg_offsets[it.background], len, out, ws, seg0, (long long)segs.size(), it.gain, 0, 0};
+        if (len > 0) items[i].bg_rec = rec_of(bg_rec, it.background, h_bg_offsets, 0);
+        tile0.push_back(tile0.back() + (len + GEN_TILE - 1) / GEN_TILE);
+        out += len;
+        if (vec) {
+            ws_off.push_back(ws);
+            ws_len.push_back(len);
+            ws += (len + 7) / 8 * 8;
+        }
+    }
+    ws_off.push_back(ws);
+    const long long n_tiles = tile0.back(), n_rseg = rseg0.back(), n_recs = (long long)recs.size(), n_dsegs = (long long)segs.size();
+    if (n_tiles == 0) return PB_OK;                    // nothing generated, so no window either
+
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
+    DevArray<GenRec> f_recs; DevArray<long long> f_rseg0, f_tile0, f_wins; DevArray<unsigned long long> f_sums;
+    DevArray<GenItem> f_items; DevArray<GenSeg> f_segs; DevArray<int16_t> f_pcm;
+    cudaError_t e = corpus_grow(h->d_gen_recs, (size_t)n_recs, f_recs);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_rseg0, rseg0.size(), f_rseg0);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_sums, (size_t)n_recs, f_sums);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_items, (size_t)n_items, f_items);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_tile0, tile0.size(), f_tile0);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_segs, (size_t)n_dsegs, f_segs);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_wins, (size_t)n_windows, f_wins);
+    if (e == cudaSuccess) e = corpus_grow(h->d_gen_pcm, (size_t)ws, f_pcm);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(PB_ERR_CUDA, "generate workspace allocation failed (%lld items, %lld samples): %s", (long long)n_items, out,
+                    cudaGetErrorString(e));
+    }
+    if (f_recs.get() || f_rseg0.get() || f_sums.get() || f_items.get() || f_tile0.get() || f_segs.get() || f_wins.get() || f_pcm.get())
+        CK(cudaEventSynchronize(h->corpus_ev));        // the previous call may still read what is replaced
+    if (f_recs.get()) h->d_gen_recs = std::move(f_recs);
+    if (f_rseg0.get()) h->d_gen_rseg0 = std::move(f_rseg0);
+    if (f_sums.get()) h->d_gen_sums = std::move(f_sums);
+    if (f_items.get()) h->d_gen_items = std::move(f_items);
+    if (f_tile0.get()) h->d_gen_tile0 = std::move(f_tile0);
+    if (f_segs.get()) h->d_gen_segs = std::move(f_segs);
+    if (f_wins.get()) h->d_gen_wins = std::move(f_wins);
+    if (f_pcm.get()) h->d_gen_pcm = std::move(f_pcm);
+    CorpusPlan plan;
+    std::vector<long long> wins;
+    if (vec) {
+        plan = corpus_plan(h, h->d_gen_pcm.get(), ws_off.data(), n_items, PB_CORPUS_LISTENER, chunk, 0, ws_len.data());
+        wins.resize((size_t)n_windows);
+        for (int64_t w = 0; w < n_windows; ++w) wins[w] = plan.win0[h_windows[2 * w]] + h_windows[2 * w + 1];
+        rc = corpus_reserve(h, plan, n_items, CorpusPoolSizes{}, s);
+        if (rc != PB_OK) return rc;
+    } else {
+        CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
+    }
+    auto launch = [&]() -> int {
+        CK(cudaMemcpyAsync(h->d_gen_recs.get(), recs.data(), recs.size() * sizeof(GenRec), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_gen_rseg0.get(), rseg0.data(), rseg0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_gen_items.get(), items.data(), items.size() * sizeof(GenItem), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(h->d_gen_tile0.get(), tile0.data(), tile0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        if (n_dsegs > 0) CK(cudaMemcpyAsync(h->d_gen_segs.get(), segs.data(), segs.size() * sizeof(GenSeg), cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(h->d_gen_sums.get(), 0, (size_t)n_recs * sizeof(unsigned long long), s));
+        if (n_rseg > 0) {
+            gen_sums_kernel<<<(unsigned)n_rseg, GEN_THREADS, 0, s>>>(d_bg, d_clips, h->d_gen_recs.get(), h->d_gen_rseg0.get(), (int)n_recs,
+                                                                    h->d_gen_sums.get());
+            CK(cudaGetLastError());
+        }
+        gen_mix_kernel<<<(unsigned)n_tiles, GEN_THREADS, 0, s>>>(d_bg, d_clips, h->d_gen_recs.get(), h->d_gen_sums.get(), h->d_gen_items.get(),
+                                                                h->d_gen_tile0.get(), (int)n_items, h->d_gen_segs.get(), d_out,
+                                                                vec ? h->d_gen_pcm.get() : nullptr);
+        CK(cudaGetLastError());
+        if (!vec) return PB_OK;
+        rc = corpus_k1(h, plan, h->d_gen_pcm.get(), n_items, divisor, PB_CORPUS_LISTENER, chunk, s);
+        if (rc != PB_OK) return rc;
+        CK(cudaMemcpyAsync(h->d_gen_wins.get(), wins.data(), wins.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        const int T = h->cfg.n_features, F = h->feat;
+        const long long total = (long long)n_windows * T * F;
+        gen_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->d_gen_wins.get(),
+                                                                         h->row_stride, T, F, n_windows, d_inputs);
         CK(cudaGetLastError());
         return PB_OK;
     };

@@ -34,6 +34,11 @@ Noise augmentation (pb_add_noise):
   add_noise         ~ add_noise.py:82-87 (noised_audio of each clip, on the device)
   vectorize_noisy   vectorize of each noisy clip, without the clips leaving the device
   Augment           fresh noisy copies of every training clip in every epoch of train
+
+Generated training audio (pb_generate, pb_train):
+  Generator         ~ precise/scripts/train_generated.py:118-213 (wake words overlaid on backgrounds, windows labelled by
+                    vals_buffer's rule), keyed randomness, planned on the host and generated on the device
+  train_generated   ~ train_generated.py:215-226 (fit_generator over the generated windows, many networks at once)
 """
 from dataclasses import dataclass
 
@@ -886,3 +891,312 @@ def _train_augmented(core, state, clips, targets, rows, recs, epochs, kw, augmen
         validation_step()
     k = len(state.hidden)
     return core.torch.cat(losses, 1).cpu().numpy() if losses else np.zeros((k, 0))
+
+
+# ---- generated training audio (precise-train-generated) ----------------------------------------------------------------------
+
+# Samples per pb_generate call of Generator.run (items are never split: a longer item is a call of its own).  At the cap a
+# call's device memory stays under 256 MB: d_out and the aligned workspace 64 MB each (int16), the frame rows about 3 MB
+# at the default hop, and the chosen windows' inputs at most 25 MB (one 1 508-byte window per 2 048-sample chunk).
+GENERATE_CALL_SAMPLES = 1 << 25
+
+# Window-less items in a row after which Generator gives up rather than loop: the label rule keeps the window at the end of
+# any silence longer than the label buffer, so this takes a buffer longer than the longest silence (2.5 s).
+_GENERATE_IDLE = 10000
+
+
+def _unit(seed, e, j, c):
+    """A uniform double in [0, 1) from pb_train's splitmix key: (key(s, e, j, c) >> 11) 2^-53."""
+    return (_key(int(seed), int(e), int(j), int(c)) >> 11) * 2.0 ** -53
+
+
+class _LabelTail:
+    """vals_buffer (train_generated.py:176): the last ``n`` per-sample labels of the whole run, kept as the runs of ones
+    [a, b) of the label stream, which starts with n zeros.  ``end`` is the stream's length so far."""
+
+    def __init__(self, n):
+        self.n, self.end, self.runs = int(n), int(n), []
+
+    def add(self, length, one):
+        if one and length > 0:
+            if self.runs and self.runs[-1][1] == self.end:
+                self.runs[-1][1] += length
+            else:
+                self.runs.append([self.end, self.end + length])
+        self.end += length
+
+    def decide(self, p):
+        """The label rule of the window whose buffer ends at stream position p (no earlier than the last call's):
+        1, 0, or -1 for a skipped window."""
+        lo = p - self.n
+        while self.runs and self.runs[0][1] <= lo:
+            self.runs.pop(0)
+        best, last = 0, 0
+        for a, b in self.runs:
+            if a >= p:
+                break
+            best = max(best, min(b, p) - max(a, lo))
+            last = b >= p
+        frac = best / self.n
+        if not last and frac > 0.8:
+            return 1
+        return 0 if frac < 0.5 else -1
+
+    def copy(self):
+        t = _LabelTail(self.n)
+        t.end, t.runs = self.end, [list(r) for r in self.runs]
+        return t
+
+
+@dataclass
+class GeneratedItem:
+    """One background file's pass: background b at gain f, the first ``length`` samples generated, its segments
+    [(clip or -1, first sample, samples)] and its windows [(chunk index, target)] (skipped chunks left out)."""
+    background: int
+    f: float
+    length: int
+    segments: list
+    windows: list
+
+
+class Generator:
+    """precise-train-generated's sample generator (train_generated.py:118-213) with keyed randomness.
+
+    Backgrounds are taken in the order of (key(seed, 0, b, 0), b), cycled forever; pass p's item of background b draws
+    u_c = (key(seed, p + 1, b, c) >> 11) 2^-53 (pb_train's key): c = 0 the volume, f = 0.4 + 0.5 u_0; then the wake-word
+    pieces, piece k drawing u_{1 + k}: a clip (even k; a wake word if u > 0.5, the next of the wake_clips cycle, else the next
+    of other_clips) or a silence of int(sample_rate (0.5 + 2 u)) samples (odd k).  Pieces are drawn only as the chunks need
+    them, as the reference's generators draw them.  The stream is cut as chunk_audio_pieces cuts it (each ``combined`` the
+    previous piece followed by the current one: DESIGN §3 "Generated training audio"), and chunk c's window is labelled by vals_buffer's rule
+    (a run of ones over 0.8 of buffer_samples ending before the last sample: 1; under 0.5: 0; else skipped).  The clip
+    cycles and the label tail carry over items, passes and epochs, as in the reference.
+
+    plan(n) takes the next n windows; an item cut at the end of a plan continues in the next one (its stream is generated
+    again from its start).  at(epoch, entries) replays the plan, so a resumed run draws what an uninterrupted one would.
+    core None: plans only (no device data)."""
+
+    def __init__(self, core, backgrounds, wake_clips, other_clips, chunk=2048, seed=0, names=None, sample_rate=None,
+                 buffer_samples=None):
+        if not len(wake_clips) or not len(other_clips):
+            raise ValueError('the generator needs at least one wake-word and one not-wake-word clip')
+        if not len(backgrounds):
+            raise ValueError('the generator needs at least one background recording')
+        self.core, self.chunk, self.seed = core, int(chunk), int(seed)
+        if self.chunk < 1:
+            raise ValueError('chunk must be >= 1')
+        pr = core.params if core is not None else None
+        self.sample_rate = int(sample_rate if sample_rate is not None else pr.sample_rate)
+        self.buffer_samples = int(buffer_samples if buffer_samples is not None else pr.buffer_samples)
+        self.bg_lens = [int(b.shape[0]) for b in backgrounds]
+        if max(self.bg_lens) <= self.chunk:
+            raise ValueError('every background is at most one chunk (%d samples) long: none gives a window' % self.chunk)
+        self.clip_lens = [int(c.shape[0]) for c in list(wake_clips) + list(other_clips)]
+        self.n_wake, self.n_other = len(wake_clips), len(other_clips)
+        self.names = list(names) if names is not None else ['%d' % b for b in range(len(backgrounds))]
+        self.order = sorted(range(len(backgrounds)), key=lambda b: (_key(self.seed, 0, b, 0), b))
+        self._dev = None
+        if core is not None:
+            torch = core.torch
+            cat = lambda recs: torch.cat([torch.as_tensor(_check_recording(core, r)).to(core.device) for r in recs]
+                                         + [torch.zeros(0, dtype=torch.int16, device=core.device)])
+            offs = lambda lens: np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+            self._dev = (cat(backgrounds), offs(self.bg_lens), cat(list(wake_clips) + list(other_clips)), offs(self.clip_lens))
+        self._reset()
+
+    def _reset(self):
+        self.taken = 0                                        # windows planned so far
+        self.pass_, self.q = 0, 0                             # the next item: order[q] of pass pass_
+        self.next_wake = self.next_other = 0
+        self.tail = _LabelTail(self.buffer_samples)
+        self.cur, self.cur_w = None, 0                        # the item being taken and its windows taken
+        self.idle = 0                                         # items in a row without a window
+
+    def _item(self, p, b):
+        ch, seed = self.chunk, self.seed
+        n = max(0, (self.bg_lens[b] - 1) // ch)              # len(range(chunk, len, chunk))
+        f = 0.4 + 0.5 * _unit(seed, p + 1, b, 0)
+        start = self.tail.end
+        segs, need, got, prev, k = [], n * ch, 0, None, 0
+        while got < need:
+            u = _unit(seed, p + 1, b, 1 + k)
+            if k % 2 == 0:
+                wake = u > 0.5
+                if wake:
+                    piece = (self.next_wake, self.clip_lens[self.next_wake], True)
+                    self.next_wake = (self.next_wake + 1) % self.n_wake
+                else:
+                    c = self.n_wake + self.next_other
+                    piece = (c, self.clip_lens[c], False)
+                    self.next_other = (self.next_other + 1) % self.n_other
+            else:
+                piece = (-1, int(self.sample_rate * (0.5 + 2.0 * u)), False)
+            both = [piece] if prev is None or prev[1] == 0 else [prev, piece]
+            total = sum(x[1] for x in both)
+            rem = min(((total - 1) // ch if total > 0 else 0) * ch, need - got)
+            got += rem
+            for clip, length, wake in both:
+                m = min(length, rem)
+                if m > 0:
+                    segs.append((clip, 0, m))
+                    self.tail.add(m, wake)
+                rem -= m
+            prev, k = piece, k + 1
+        windows = []
+        for c in range(n):
+            t = self.tail.decide(start + (c + 1) * ch)
+            if t >= 0:
+                windows.append((c, t))
+        return GeneratedItem(b, f, n * ch, segs, windows)
+
+    def _next_item(self):
+        b = self.order[self.q]
+        item = self._item(self.pass_, b)
+        self.q += 1
+        if self.q == len(self.order):
+            self.q, self.pass_ = 0, self.pass_ + 1
+        self.idle = 0 if item.windows else self.idle + 1
+        if self.idle > _GENERATE_IDLE:
+            raise ValueError('the label rule skipped every window of %d items in a row' % _GENERATE_IDLE)
+        return item
+
+    def plan(self, n):
+        """The next n windows: a list of (GeneratedItem, first window, end window)."""
+        out, left = [], int(n)
+        while left > 0:
+            if self.cur is None or self.cur_w == len(self.cur.windows):
+                self.cur, self.cur_w = self._next_item(), 0
+            take = min(left, len(self.cur.windows) - self.cur_w)
+            if take:
+                out.append((self.cur, self.cur_w, self.cur_w + take))
+            self.cur_w += take
+            left -= take
+        self.taken += int(n)
+        return out
+
+    def seek(self, windows):
+        """Moves to the state after ``windows`` windows have been planned (replaying from the start if needed)."""
+        windows = int(windows)
+        if windows < self.taken:
+            self._reset()
+        if windows > self.taken:
+            self.plan(windows - self.taken)
+        return self
+
+    def at(self, epoch, entries):
+        """A copy of this generator at the start of ``epoch`` of ``entries`` windows per epoch."""
+        g = object.__new__(Generator)
+        g.__dict__.update(self.__dict__)
+        g._reset()
+        return g.seek(int(epoch) * int(entries))
+
+    def tables(self, plan):
+        """pb_generate's tables of a plan: (GEN_ITEM items, GEN_SEGMENT segments, int64 windows [n, 2], uint8 targets)."""
+        from .core import GEN_ITEM, GEN_SEGMENT
+        items = np.zeros(len(plan), GEN_ITEM)
+        segs, wins, tg = [], [], []
+        for i, (it, w0, w1) in enumerate(plan):
+            chosen = it.windows[w0:w1]
+            length = (chosen[-1][0] + 1) * self.chunk
+            s0 = len(segs)
+            cover = 0
+            for s in it.segments:
+                if cover >= length:
+                    break
+                segs.append(s)
+                cover += s[2]
+            items[i] = (it.background, 0, it.f, length, s0, len(segs))
+            wins += [(i, c) for c, _ in chosen]
+            tg += [t for _, t in chosen]
+        seg = np.zeros(len(segs), GEN_SEGMENT)
+        for j, (c, a, m) in enumerate(segs):
+            seg[j] = (c, 0, a, m)
+        return items, seg, np.asarray(wins, np.int64).reshape(-1, 2), np.asarray(tg, np.uint8)
+
+    def run(self, plan, out=False, divisor=32767):
+        """pb_generate over a plan, in calls of at most GENERATE_CALL_SAMPLES samples: (network inputs float32
+        [n, n_features, feature_size], targets uint8 [n], and with out=True the streams (int16 tensor) with each window's
+        end sample in them, int64 [n]; else None, None)."""
+        core = self.core
+        torch = core.torch
+        bg, bg_off, clips, clip_off = self._dev
+        groups, cur, size = [], [], 0
+        for p in plan:
+            L = (p[0].windows[p[2] - 1][0] + 1) * self.chunk
+            if cur and size + L > GENERATE_CALL_SAMPLES:
+                groups.append(cur)
+                cur, size = [], 0
+            cur.append(p)
+            size += L
+        if cur:
+            groups.append(cur)
+        ins, tgs, outs, ends, base = [], [], [], [], 0
+        for g in groups:
+            items, seg, wins, tg = self.tables(g)
+            o, x = core.generate(bg, bg_off, clips, clip_off, items, seg, wins, self.chunk, divisor, out=out)
+            ins.append(x)
+            tgs.append(tg)
+            if out:
+                starts = base + np.concatenate([[0], np.cumsum(items['length'])])[wins[:, 0]]
+                ends.append(starts + (wins[:, 1] + 1) * self.chunk)
+                outs.append(o)
+                base += int(items['length'].sum())
+        empty = torch.empty((0, core.n_features, core.feature_size), dtype=torch.float32, device=core.device)
+        x = (ins[0] if len(ins) == 1 else torch.cat(ins)) if ins else empty
+        tg = np.concatenate(tgs) if tgs else np.zeros(0, np.uint8)
+        if not out:
+            return x, tg, None, None
+        audio = torch.cat(outs) if outs else torch.zeros(0, dtype=torch.int16, device=core.device)
+        return x, tg, audio, (np.concatenate(ends) if ends else np.zeros(0, np.int64))
+
+
+def _save_generated(gen, epoch, plan, audio, ends, targets, save_prob, folder):
+    """-p: entry j of the epoch is saved when (key(seed, epoch, j, 2^32) >> 11) 2^-53 > 1 - save_prob, as
+    debug/{ww,nww}/'<background> - <chunk>.wav': the buffer_samples generated samples that end at its window (zeros before
+    its background's stream starts)."""
+    import os
+    from .add_noise import write_wav
+    B = gen.buffer_samples
+    a = audio.cpu().numpy()
+    j = 0
+    for it, w0, w1 in plan:
+        for c, t in it.windows[w0:w1]:
+            if _unit(gen.seed, epoch, j, 1 << 32) > 1.0 - save_prob:
+                e = int(ends[j])
+                s = max(e - B, e - (c + 1) * gen.chunk)
+                buf = np.zeros(B, np.int16)
+                buf[B - (e - s):] = a[s:e]
+                name = '%s - %d.wav' % (os.path.splitext(os.path.basename(gen.names[it.background]))[0], c)
+                write_wav(os.path.join(folder, 'ww' if targets[j] else 'nww', name), buf, gen.sample_rate)
+            j += 1
+
+
+def train_generated(core: PreciseB200, state: TrainState, gen: Generator, epochs, steps_per_epoch=100, batch_size=200,
+                    sensitivity=0.2, dropout=0.2, validation=None, save_prob=0.0, debug_folder='debug'):
+    """precise-train-generated's fit_generator for every network of ``state`` at once: each epoch is the generator's next
+    steps_per_epoch x batch_size windows (Generator.run: pb_generate) and one pb_train epoch over them with
+    epoch0 = state.epoch, every network on the same entries.  The generator is first moved to epoch state.epoch, so a
+    resumed run trains on what an uninterrupted one would.  pb_train shuffles the entries where fit_generator takes
+    consecutive batches.  Returns the epoch losses [k, epochs]; with validation=(inputs, targets) also val_loss
+    (pb_train_loss, as train's).  save_prob > 0 writes debug wavs of the chosen windows (_save_generated)."""
+    n = int(steps_per_epoch) * int(batch_size)
+    if n < 1:
+        raise ValueError('steps_per_epoch and batch_size must be >= 1')
+    lb = 1.0 - sensitivity
+    losses, vals = [], []
+    for _ in range(int(epochs)):
+        e = state.epoch
+        gen.seek(e * n)
+        plan = gen.plan(n)
+        x, tg, audio, ends = gen.run(plan, out=save_prob > 0)
+        losses.append(core.train(x, tg, state.rows, state.weights, state.rms, epochs=1, epoch0=e, batch_size=batch_size,
+                                 loss_bias=lb, dropout=dropout))
+        state.epoch += 1
+        if validation is not None:
+            vals.append(core.train_loss(validation[0], validation[1], state.rows, state.weights, loss_bias=lb))
+        if save_prob > 0:
+            _save_generated(gen, e, plan, audio, ends, tg, save_prob, debug_folder)
+    k = len(state.hidden)
+    loss = core.torch.cat(losses, 1).cpu().numpy() if losses else np.zeros((k, 0))
+    if validation is None:
+        return loss
+    return loss, core.torch.stack(vals, 1).cpu().numpy() if vals else np.zeros((k, 0))
