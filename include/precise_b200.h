@@ -686,7 +686,8 @@ int pb_generate(pb_handle* h, const int16_t* d_bg, const int64_t* h_bg_offsets, 
  * zero and stays zero. */
 #define PB_TRAIN_STRIDE 2980
 
-/* One trained network: hidden size (1 .. 24), PB_ACT_* and PB_RACT_* codes, and the seed of its shuffles and dropout masks. */
+/* One trained network: hidden size (1 .. 24; 1 .. 128 for pb_train_wide), PB_ACT_* and PB_RACT_* codes, and the seed of its
+ * shuffles and dropout masks. */
 typedef struct pb_train_row {
     int32_t hidden;
     int32_t activation;
@@ -742,6 +743,24 @@ int pb_train(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* 
 int pb_train_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
                   int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
                   float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream);
+
+/* Floats per network of pb_train_wide's weight and accumulator arrays: pb_train's layout for up to 128 GRU units; the tail
+ * after 3H(F + H + 1) + H + 1 floats (55 809 at H = 128, F = 16) is zero and stays zero. */
+#define PB_TRAIN_WIDE_STRIDE 55812
+
+/* pb_train and pb_train_loss for networks of up to 128 GRU units (gru_wide's limit, so the existing scans score every trained
+ * network), rows of PB_TRAIN_WIDE_STRIDE floats.  Word for word pb_train's and pb_train_loss's contracts (entries, shuffles,
+ * masks, loss, RMSprop, NaN losses, determinism, ordering, refusals) with hidden in [1, 128], one call mixing any sizes.  The
+ * matrix products run on the tensor cores with the 3xTF32 split, the elementwise work in float32, so results are close to
+ * pb_train's at H <= 24 but not bit-identical.  The batches' tiles run in launches whose state stays under 512 MB (about
+ * 4 n_features (3 F8 + 5 H8) bytes per entry, F8 and H8 rounded up to 8), on top of the 256 MB groups. */
+int pb_train_wide(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                  int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
+                  float* d_weights, float* d_rms, double* d_loss, void* stream);
+
+int pb_train_wide_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                       int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
+                       float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream);
 
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);

@@ -86,9 +86,14 @@ class StreamBatch:
         current networks or GruModel.init), on labelled ``clips`` (1-D int16, read as load_audio reads them; targets non-zero =
         wake word): rows / recs as offline.train takes them, ``opts`` its keyword arguments, seeds [k] (default 0 .. k-1).
         Each trained network is loaded into its slot through pool_load with the slot's earlier settings (those of this batch's
-        pool_load, or the defaults), which re-arms its streams as a newly loaded model does.  Returns the k trained GruModels."""
+        pool_load, or the defaults), which re-arms its streams as a newly loaded model does.  Returns the k trained GruModels.
+        The pool holds the fused family only, so networks of more than 24 units are refused before anything is trained."""
         from .offline import TrainState, train, vectorize_clips
         from .runner import _resolve_model
+        wide = [i for i, m in enumerate(models) if m.hidden > 24]
+        if wide:
+            raise ValueError('pool_train: model %d has hidden = %d; the pool holds networks of at most 24 units (train wider '
+                             'networks with offline.train)' % (wide[0], models[wide[0]].hidden))
         inputs = vectorize_clips(self.core, clips)
         state = TrainState.from_models(self.core, models, range(len(models)) if seeds is None else seeds)
         train(self.core, state, inputs, targets, rows, recs, **opts)

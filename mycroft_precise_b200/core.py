@@ -40,6 +40,7 @@ class pb_config(C.Structure):
 
 
 PB_TRAIN_STRIDE = 2980             # floats per network of pb_train's weight and accumulator rows
+PB_TRAIN_WIDE_STRIDE = 55812       # the same for pb_train_wide (up to 128 GRU units)
 
 
 class pb_train_row(C.Structure):
@@ -113,6 +114,9 @@ SYMBOLS = {
     'pb_train_opts_default': (C.c_int, [C.POINTER(pb_train_opts)]),
     'pb_train': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.POINTER(pb_train_opts), _VP, _VP, _VP, _VP]),
     'pb_train_loss': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.c_float, C.c_float, _I32, _VP, _VP, _VP, _VP]),
+    'pb_train_wide': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.POINTER(pb_train_opts), _VP, _VP, _VP, _VP]),
+    'pb_train_wide_loss': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.c_float, C.c_float, _I32, _VP, _VP, _VP,
+                                     _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -1113,7 +1117,8 @@ class PreciseB200:
         return (None if d_out is None else d_out[:total]), d_in
 
     def _train_args(self, inputs, targets, k, rows_of, recs, weights):
-        """(n_rec, targets, pair rows, pair recs, n_pairs) of a training call, checked."""
+        """(n_rec, targets, pair rows, pair recs, n_pairs, stride) of a training call, checked.  The stride is the weight
+        rows' width: PB_TRAIN_WIDE_STRIDE (pb_train_wide) when weights holds k rows of it, else PB_TRAIN_STRIDE (pb_train)."""
         torch = self.torch
         if (not isinstance(inputs, torch.Tensor) or inputs.dtype != torch.float32 or not inputs.is_contiguous()
                 or inputs.device != self.device or inputs.dim() != 3 or tuple(inputs.shape[1:]) != (self.n_features, self.feature_size)):
@@ -1123,15 +1128,17 @@ class PreciseB200:
         targets = np.ascontiguousarray(np.asarray(targets) != 0, dtype=np.uint8)
         if targets.shape != (n_rec,):
             raise ValueError('one target per input')
-        self._check_t('weights', weights, torch.float32, k * PB_TRAIN_STRIDE, optional=False)
+        wide = k > 0 and isinstance(weights, torch.Tensor) and weights.numel() == k * PB_TRAIN_WIDE_STRIDE
+        stride = PB_TRAIN_WIDE_STRIDE if wide else PB_TRAIN_STRIDE
+        self._check_t('weights', weights, torch.float32, k * stride, optional=False)
         if (rows_of is None) != (recs is None):
             raise ValueError('rows_of and recs come together')
         if rows_of is None:
-            return n_rec, targets, None, None, 0
+            return n_rec, targets, None, None, 0, stride
         pr, pc = np.ascontiguousarray(rows_of, dtype=np.int32), np.ascontiguousarray(recs, dtype=np.int32)
         if pr.ndim != 1 or pr.shape != pc.shape:
             raise ValueError('rows_of and recs must be 1-D arrays of one length')
-        return n_rec, targets, pr, pc, pr.shape[0]
+        return n_rec, targets, pr, pc, pr.shape[0], stride
 
     @staticmethod
     def train_rows(hidden, activation, recurrent_activation, seed):
@@ -1150,10 +1157,11 @@ class PreciseB200:
         tensors [k, PB_TRAIN_STRIDE]) over ``inputs`` (vectorize_clips' tensor) with labels ``targets`` (host, non-zero = wake
         word).  rows_of / recs None: every network on every input; otherwise entry p is input recs[p] of network rows_of[p].
         Returns the float64 epoch losses [k, epochs] (NaN for a network without entries) on the device.  Asynchronous on the
-        current stream.  pb_train in include/precise_b200.h."""
+        current stream.  With weights and rms [k, PB_TRAIN_WIDE_STRIDE] the call is pb_train_wide (up to 128 GRU units).
+        pb_train and pb_train_wide in include/precise_b200.h."""
         arr, k = rows
-        n_rec, targets, pr, pc, n = self._train_args(inputs, targets, k, rows_of, recs, weights)
-        self._check_t('rms', rms, self.torch.float32, k * PB_TRAIN_STRIDE, optional=False)
+        n_rec, targets, pr, pc, n, stride = self._train_args(inputs, targets, k, rows_of, recs, weights)
+        self._check_t('rms', rms, self.torch.float32, k * stride, optional=False)
         o = pb_train_opts()
         check(self.lib.pb_train_opts_default(C.byref(o)))
         o.epochs, o.epoch0, o.batch_size = int(epochs), int(epoch0), int(batch_size)
@@ -1162,25 +1170,26 @@ class PreciseB200:
         if rows_of is not None and n == 0:                     # no entry (the library reads an empty pair list as "every pair")
             loss.fill_(float('nan'))
             return loss
-        check(self.lib.pb_train(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n, C.byref(o),
-                                _ptr(weights), _ptr(rms), _ptr(loss), self._stream()))
+        fn = self.lib.pb_train_wide if stride == PB_TRAIN_WIDE_STRIDE else self.lib.pb_train
+        check(fn(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n, C.byref(o), _ptr(weights),
+                 _ptr(rms), _ptr(loss), self._stream()))
         return loss
 
     def train_loss(self, inputs, targets, rows, weights, rows_of=None, recs=None, loss_bias=0.8, dropout=0.0, epoch=0, grad=False):
         """pb_train_loss: each network's loss over all its entries as one batch (dropout 0: Keras's evaluate) -> float64
-        [k] on the device, and with grad=True also its gradient, float32 [k, PB_TRAIN_STRIDE].  Arguments as train's.
-        pb_train_loss in include/precise_b200.h."""
+        [k] on the device, and with grad=True also its gradient, float32 [k, stride] (the weights' row width).  Arguments as
+        train's; weights [k, PB_TRAIN_WIDE_STRIDE] make it pb_train_wide_loss.  pb_train_loss in include/precise_b200.h."""
         arr, k = rows
-        n_rec, targets, pr, pc, n = self._train_args(inputs, targets, k, rows_of, recs, weights)
+        n_rec, targets, pr, pc, n, stride = self._train_args(inputs, targets, k, rows_of, recs, weights)
         torch = self.torch
         loss = torch.empty(k, dtype=torch.float64, device=self.device)
-        g = torch.zeros((k, PB_TRAIN_STRIDE), dtype=torch.float32, device=self.device) if grad else None
+        g = torch.zeros((k, stride), dtype=torch.float32, device=self.device) if grad else None
         if rows_of is not None and n == 0:
             loss.fill_(float('nan'))
             return (loss, g) if grad else loss
-        check(self.lib.pb_train_loss(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n,
-                                     float(loss_bias), float(dropout), int(epoch), _ptr(weights), _ptr(loss), _ptr(g),
-                                     self._stream()))
+        fn = self.lib.pb_train_wide_loss if stride == PB_TRAIN_WIDE_STRIDE else self.lib.pb_train_loss
+        check(fn(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n, float(loss_bias),
+                 float(dropout), int(epoch), _ptr(weights), _ptr(loss), _ptr(g), self._stream()))
         return (loss, g) if grad else loss
 
     def corpus_pairs_batch(self, windows):

@@ -40,6 +40,7 @@
 #include "dataset.cuh"
 #include "pool.cuh"
 #include "train.cuh"
+#include "train_wide.cuh"
 #include "noise.cuh"
 #include "generate.cuh"
 
@@ -227,7 +228,8 @@ struct pb_handle {
     DevArray<PairTile> d_pp_tiles;   // ... the batch's scan tiles, one activation class after the other
     DevArray<float> d_ds_thr;        // pb_score_dataset: the histogram's float32 thresholds
     DevArray<uint8_t> d_ds_targets;  // ... [n_rec] the recordings' labels
-    DevArray<uint8_t> d_tr_ws;       // pb_train / pb_train_loss: one arena, carved per call (at most TRAIN_WS_CAP bytes per group)
+    DevArray<uint8_t> d_tr_ws;       // pb_train(_wide) / pb_train(_wide)_loss: one arena, carved per call (at most TRAIN_WS_CAP
+                                     // bytes per group, plus TW_STATE_CAP of tile state for the wide calls)
     DevArray<NoiseItem> d_nz_items;  // pb_add_noise: [n_items] the items
     DevArray<long long> d_nz_seg0;   // ... [n_items + 1] each item's first segment
     DevArray<unsigned long long> d_nz_sums;  // ... [n_items][2] (sum x^2, sum n^2)
@@ -2812,7 +2814,9 @@ struct TrainEntries {
 };
 
 // A group of consecutive rows with entries, trained together, and its tile tables: batch b's gradient tiles are
-// tiles[tile0[b] .. tile0[b + 1]), its row updates steps[step0[b] .. step0[b + 1]).
+// tiles[tile0[b] .. tile0[b + 1]), its row updates steps[step0[b] .. step0[b + 1]).  Wide calls also cut each batch's tiles
+// into launches: launch c runs tiles [launch0[c], launch0[c + 1]), batch b's launches are [blaunch0[b], blaunch0[b + 1]), and
+// soff[i] is tile i's state offset (floats) within its launch's state.
 struct TrainGroup {
     std::vector<int> rows;
     int64_t e0 = 0, n = 0;           // entries [e0, e0 + n) of TrainEntries::ent
@@ -2822,18 +2826,21 @@ struct TrainGroup {
     std::vector<int64_t> tile0, step0;
     int64_t max_tiles = 0;
     size_t sort_bytes = 0;
+    std::vector<long long> soff;
+    std::vector<int64_t> launch0, blaunch0;
+    size_t state_floats = 0;         // the largest launch's state
 };
 
 // Checks the arguments both training calls share and lists the entries.
 static int check_train(const pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
-                       int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, TrainEntries& te) {
+                       int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, int max_h, TrainEntries& te) {
     int rc = check_train_front_end(h);
     if (rc != PB_OK) return rc;
     if (k < 0 || k > INT32_MAX / 2) return fail(PB_ERR_INVALID, "k = %lld outside [0, 2^30)", (long long)k);
     if (k > 0 && !h_rows) return fail(PB_ERR_INVALID, "null h_rows");
     for (int64_t i = 0; i < k; ++i) {
         const pb_train_row& r = h_rows[i];
-        if (r.hidden < 1 || r.hidden > TR_MAX_H) return fail(PB_ERR_INVALID, "row %lld: hidden = %d outside [1, %d]", (long long)i, r.hidden, TR_MAX_H);
+        if (r.hidden < 1 || r.hidden > max_h) return fail(PB_ERR_INVALID, "row %lld: hidden = %d outside [1, %d]", (long long)i, r.hidden, max_h);
         if ((r.activation != PB_ACT_LINEAR && r.activation != PB_ACT_TANH) ||
             (r.recurrent_activation != PB_RACT_HARD_SIGMOID && r.recurrent_activation != PB_RACT_SIGMOID))
             return fail(PB_ERR_INVALID, "row %lld: unknown activation codes (%d, %d)", (long long)i, r.activation, r.recurrent_activation);
@@ -2882,15 +2889,16 @@ static int64_t train_tiles(int64_t n, int64_t bs) {
     return t;
 }
 
-// Groups of consecutive rows with entries whose workspace stays under TRAIN_WS_CAP, with their tile tables.
-static std::vector<TrainGroup> train_groups(const TrainEntries& te, int64_t k, int64_t bs) {
+// Groups of consecutive rows with entries whose workspace (partial rows of `stride` floats) stays under TRAIN_WS_CAP, with
+// their tile tables.
+static std::vector<TrainGroup> train_groups(const TrainEntries& te, int64_t k, int64_t bs, size_t stride) {
     std::vector<TrainGroup> out;
     size_t bytes = 0;
     for (int64_t r = 0; r < k; ++r) {
         const int64_t n = te.off[(size_t)r + 1] - te.off[(size_t)r];
         if (n == 0) continue;
         const int64_t b = std::min(bs, n), nb = (n + bs - 1) / bs;
-        const size_t cost = (size_t)n * 40 + (size_t)((b + TR_TILE - 1) / TR_TILE) * (TR_STRIDE * 4 + 8) +
+        const size_t cost = (size_t)n * 40 + (size_t)((b + TR_TILE - 1) / TR_TILE) * (stride * 4 + 8) +
                             (size_t)train_tiles(n, bs) * sizeof(TrainTile) + (size_t)nb * sizeof(TrainStep) + 64;
         if (out.empty() || bytes + cost > TRAIN_WS_CAP || out.back().rows.size() >= 65535) {
             out.emplace_back();
@@ -2944,10 +2952,11 @@ struct TrainWs {
     TrainRowDev* rows; uint8_t* targets; double* loss_acc;
     int* ent; int* order; int* vals; uint64_t* keys; uint64_t* keys2; int* seg; int* seg_row;
     TrainTile* tiles; TrainStep* steps; float* part; double* part_loss; void* sort_tmp;
+    long long* soff; float* state;   // wide calls only (state_floats > 0)
 };
 
 static TrainWs train_layout(uint8_t* base, int64_t k, int64_t n_rec, int64_t n, int64_t rows, int64_t tiles, int64_t steps,
-                            int64_t max_tiles, size_t sort_bytes, size_t* bytes) {
+                            int64_t max_tiles, size_t sort_bytes, size_t stride, size_t state_floats, size_t* bytes) {
     TrainCarve c{base};
     TrainWs w{};
     w.rows = c.take<TrainRowDev>((size_t)k); w.targets = c.take<uint8_t>((size_t)n_rec); w.loss_acc = c.take<double>((size_t)k);
@@ -2955,22 +2964,44 @@ static TrainWs train_layout(uint8_t* base, int64_t k, int64_t n_rec, int64_t n, 
     w.keys = c.take<uint64_t>((size_t)n); w.keys2 = c.take<uint64_t>((size_t)n);
     w.seg = c.take<int>((size_t)rows + 1); w.seg_row = c.take<int>((size_t)rows);
     w.tiles = c.take<TrainTile>((size_t)tiles); w.steps = c.take<TrainStep>((size_t)steps);
-    w.part = c.take<float>((size_t)max_tiles * TR_STRIDE); w.part_loss = c.take<double>((size_t)max_tiles);
+    w.part = c.take<float>((size_t)max_tiles * stride); w.part_loss = c.take<double>((size_t)max_tiles);
     w.sort_tmp = c.take<uint8_t>(sort_bytes);
+    if (state_floats) { w.soff = c.take<long long>((size_t)tiles); w.state = c.take<float>(state_floats); }
     if (bytes) *bytes = c.at;
     return w;
 }
 
-// Shared body of pb_train (train = true: shuffle, batches, RMSprop) and pb_train_loss (one batch per row in request order,
-// the gradient to d_grad).
+// The wide calls' launches: each batch's tiles in order, cut where a launch's state would pass TW_STATE_CAP.
+static void train_wide_launches(TrainGroup& g, const pb_train_row* h_rows, int T, int F) {
+    g.soff.assign(g.tiles.size(), 0);
+    g.launch0.clear();
+    g.blaunch0.assign(1, 0);
+    const size_t cap = TW_STATE_CAP / sizeof(float);
+    for (size_t b = 0; b + 1 < g.tile0.size(); ++b) {
+        size_t at = cap;                                             // full: the batch starts a launch
+        for (int64_t i = g.tile0[b]; i < g.tile0[b + 1]; ++i) {
+            const size_t f = (size_t)tw_tile_floats(T, F, h_rows[g.tiles[(size_t)i].row].hidden);
+            if (at + f > cap) { g.launch0.push_back(i); at = 0; }
+            g.soff[(size_t)i] = (long long)at;
+            at += f;
+            g.state_floats = std::max(g.state_floats, at);
+        }
+        g.blaunch0.push_back((int64_t)g.launch0.size());
+    }
+    g.launch0.push_back((int64_t)g.tiles.size());
+}
+
+// Shared body of pb_train(_wide) (train = true: shuffle, batches, RMSprop) and pb_train(_wide)_loss (one batch per row in
+// request order, the gradient to d_grad); wide: rows of TW_STRIDE floats on train_wide.cuh's kernels.
 static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
                      int64_t k, const TrainEntries& te, bool train, int epochs, int epoch0, int64_t bs, float lr, float rho,
                      float eps, float loss_bias, float dropout, const float* d_weights_in, float* d_weights, float* d_rms,
-                     double* d_loss, float* d_grad, cudaStream_t s) {
+                     double* d_loss, float* d_grad, bool wide, cudaStream_t s) {
     CK(cudaSetDevice(h->cfg.device));
-    std::vector<TrainGroup> groups = train_groups(te, k, train ? bs : std::numeric_limits<int64_t>::max() / 2);
+    const size_t stride = wide ? TW_STRIDE : TR_STRIDE;
+    std::vector<TrainGroup> groups = train_groups(te, k, train ? bs : std::numeric_limits<int64_t>::max() / 2, stride);
     int64_t rows_max = 0, n_max = 0, tiles_max = 0, steps_max = 0, ptiles_max = 0;
-    size_t sort_max = 0;
+    size_t sort_max = 0, state_max = 0;
     for (TrainGroup& g : groups) {
         if (train) {
             size_t sb = 0;
@@ -2979,15 +3010,17 @@ static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const u
                                                          (const int*)nullptr, s));
             g.sort_bytes = sb;
         }
+        if (wide) train_wide_launches(g, h_rows, h->cfg.n_features, h->feat);
         rows_max = std::max<int64_t>(rows_max, (int64_t)g.rows.size());
         n_max = std::max(n_max, g.n);
         tiles_max = std::max<int64_t>(tiles_max, (int64_t)g.tiles.size());
         steps_max = std::max<int64_t>(steps_max, (int64_t)g.steps.size());
         ptiles_max = std::max(ptiles_max, g.max_tiles);
         sort_max = std::max(sort_max, g.sort_bytes);
+        state_max = std::max(state_max, g.state_floats);
     }
     size_t bytes = 0;
-    train_layout(nullptr, k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, &bytes);
+    train_layout(nullptr, k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, stride, state_max, &bytes);
     if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
     if (h->d_tr_ws.size() < bytes) {
         DevArray<uint8_t> fresh;
@@ -2999,9 +3032,10 @@ static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const u
         CK(cudaEventSynchronize(h->corpus_ev));                     // the previous call may still use the arena
         h->d_tr_ws = std::move(fresh);
     }
-    CK(ensure_dyn_smem(train_grad_kernel, train_smem(h->cfg.n_features)));
+    if (!wide) CK(ensure_dyn_smem(train_grad_kernel, train_smem(h->cfg.n_features)));
     CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
-    const TrainWs w = train_layout(h->d_tr_ws.get(), k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, nullptr);
+    const TrainWs w = train_layout(h->d_tr_ws.get(), k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, stride,
+                                   state_max, nullptr);
     auto launch = [&]() -> int {
         const int n_loss = train ? epochs : 1;
         if (d_loss) {
@@ -3023,6 +3057,7 @@ static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const u
             CK(cudaMemcpyAsync(w.seg_row, g.rows.data(), g.rows.size() * sizeof(int), cudaMemcpyHostToDevice, s));
             CK(cudaMemcpyAsync(w.tiles, g.tiles.data(), g.tiles.size() * sizeof(TrainTile), cudaMemcpyHostToDevice, s));
             CK(cudaMemcpyAsync(w.steps, g.steps.data(), g.steps.size() * sizeof(TrainStep), cudaMemcpyHostToDevice, s));
+            if (wide) CK(cudaMemcpyAsync(w.soff, g.soff.data(), g.soff.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
             int64_t seg_max = 0;
             for (size_t i = 0; i < g.rows.size(); ++i) seg_max = std::max<int64_t>(seg_max, g.seg[i + 1] - g.seg[i]);
             for (int ep = 0; ep < (train ? epochs : 1); ++ep) {
@@ -3036,21 +3071,42 @@ static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const u
                                                                  (int)g.rows.size(), w.seg, w.seg + 1, s));
                 }
                 for (size_t b = 0; b + 1 < g.tile0.size(); ++b) {
-                    TrainGrad G{};
-                    G.weights = train ? d_weights : d_weights_in; G.rows = w.rows; G.inputs = d_inputs; G.targets = w.targets;
-                    G.ent = w.ent; G.order = train ? w.order : nullptr; G.tiles = w.tiles + g.tile0[b];
-                    G.part = w.part; G.part_loss = w.part_loss;
-                    G.T = h->cfg.n_features; G.F = h->feat; G.epoch = epoch;
-                    G.rate = dropout; G.scale = scale; G.loss_bias = loss_bias;
-                    const unsigned nt = (unsigned)(g.tile0[b + 1] - g.tile0[b]);
-                    train_grad_kernel<<<nt, TR_THREADS, train_smem(G.T), s>>>(G);
-                    CK(cudaGetLastError());
+                    if (wide) {
+                        for (int64_t c = g.blaunch0[b]; c < g.blaunch0[b + 1]; ++c) {
+                            const int64_t t0 = g.launch0[(size_t)c], nt = g.launch0[(size_t)c + 1] - t0;
+                            TrainWideScan S{};
+                            S.weights = train ? d_weights : d_weights_in; S.rows = w.rows; S.inputs = d_inputs; S.targets = w.targets;
+                            S.ent = w.ent; S.order = train ? w.order : nullptr; S.tiles = w.tiles + t0; S.soff = w.soff + t0;
+                            S.state = w.state; S.T = h->cfg.n_features; S.F = h->feat; S.epoch = epoch;
+                            S.rate = dropout; S.scale = scale; S.loss_bias = loss_bias;
+                            train_wide_scan_kernel<<<dim3((unsigned)nt, TR_TILE / TW_SUB), TW_THREADS, 0, s>>>(S);
+                            CK(cudaGetLastError());
+                            TrainWideGrad Q{};
+                            Q.rows = w.rows; Q.tiles = w.tiles + t0; Q.soff = w.soff + t0; Q.state = w.state;
+                            Q.part = w.part; Q.part_loss = w.part_loss; Q.p0 = (int)(t0 - g.tile0[b]);
+                            Q.T = h->cfg.n_features; Q.F = h->feat;
+                            train_wide_grad_kernel<<<dim3((unsigned)nt, TW_MBLOCKS, 3), TW_THREADS, 0, s>>>(Q);
+                            CK(cudaGetLastError());
+                        }
+                    } else {
+                        TrainGrad G{};
+                        G.weights = train ? d_weights : d_weights_in; G.rows = w.rows; G.inputs = d_inputs; G.targets = w.targets;
+                        G.ent = w.ent; G.order = train ? w.order : nullptr; G.tiles = w.tiles + g.tile0[b];
+                        G.part = w.part; G.part_loss = w.part_loss;
+                        G.T = h->cfg.n_features; G.F = h->feat; G.epoch = epoch;
+                        G.rate = dropout; G.scale = scale; G.loss_bias = loss_bias;
+                        const unsigned nt = (unsigned)(g.tile0[b + 1] - g.tile0[b]);
+                        train_grad_kernel<<<nt, TR_THREADS, train_smem(G.T), s>>>(G);
+                        CK(cudaGetLastError());
+                    }
                     TrainUpdate P{};
                     P.steps = w.steps + g.step0[b]; P.rows = w.rows; P.part = w.part; P.part_loss = w.part_loss;
                     P.weights = train ? d_weights : nullptr; P.rms = d_rms; P.grad = train ? nullptr : d_grad;
                     P.loss_acc = w.loss_acc; P.loss = d_loss; P.n_loss = n_loss; P.loss_col = ep; P.F = h->feat;
                     P.lr = lr; P.rho = rho; P.eps = eps;
-                    train_update_kernel<<<(unsigned)(g.step0[b + 1] - g.step0[b]), TR_UPDATE_THREADS, 0, s>>>(P);
+                    const unsigned ns = (unsigned)(g.step0[b + 1] - g.step0[b]);
+                    if (wide) train_update_kernel<TW_STRIDE><<<ns, TR_UPDATE_THREADS, 0, s>>>(P);
+                    else train_update_kernel<TR_STRIDE><<<ns, TR_UPDATE_THREADS, 0, s>>>(P);
                     CK(cudaGetLastError());
                 }
             }
@@ -3060,9 +3116,9 @@ static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const u
     return corpus_done(h, s, launch());
 }
 
-PB_API int pb_train(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows, int64_t k,
-                    const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
-                    float* d_weights, float* d_rms, double* d_loss, void* stream) {
+static int train_call(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows, int64_t k,
+                      const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
+                      float* d_weights, float* d_rms, double* d_loss, bool wide, void* stream) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (!opts) return fail(PB_ERR_INVALID, "null opts");
     const pb_train_opts o = *opts;
@@ -3075,29 +3131,57 @@ PB_API int pb_train(pb_handle* h, const float* d_inputs, int64_t n_rec, const ui
     if (!(o.loss_bias >= 0.f && o.loss_bias <= 1.f)) return fail(PB_ERR_INVALID, "loss_bias = %g outside [0, 1]", o.loss_bias);
     if (!(o.dropout >= 0.f && o.dropout < 1.f)) return fail(PB_ERR_INVALID, "dropout = %g outside [0, 1)", o.dropout);
     TrainEntries te;
-    const int rc = check_train(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, te);
+    const int rc = check_train(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, wide ? TW_MAX_H : TR_MAX_H, te);
     if (rc != PB_OK) return rc;
     if (k > 0 && (!d_weights || !d_rms)) return fail(PB_ERR_INVALID, "null d_weights or d_rms");
     if (k == 0) return PB_OK;
     return train_run(h, d_inputs, n_rec, h_targets, h_rows, k, te, true, o.epochs, o.epoch0, o.batch_size, o.lr, o.rho, o.epsilon,
-                     o.loss_bias, o.dropout, nullptr, d_weights, d_rms, d_loss, nullptr, (cudaStream_t)stream);
+                     o.loss_bias, o.dropout, nullptr, d_weights, d_rms, d_loss, nullptr, wide, (cudaStream_t)stream);
 }
 
-PB_API int pb_train_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
-                         int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
-                         float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream) {
+static int train_loss_call(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                           int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
+                           float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, bool wide, void* stream) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (!(loss_bias >= 0.f && loss_bias <= 1.f)) return fail(PB_ERR_INVALID, "loss_bias = %g outside [0, 1]", loss_bias);
     if (!(dropout >= 0.f && dropout < 1.f)) return fail(PB_ERR_INVALID, "dropout = %g outside [0, 1)", dropout);
     if (epoch < 0) return fail(PB_ERR_INVALID, "epoch = %d is negative", epoch);
     TrainEntries te;
-    const int rc = check_train(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, te);
+    const int rc = check_train(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, wide ? TW_MAX_H : TR_MAX_H, te);
     if (rc != PB_OK) return rc;
     if (k > 0 && !d_weights) return fail(PB_ERR_INVALID, "null d_weights");
     if (!d_loss && !d_grad) return fail(PB_ERR_INVALID, "d_loss and d_grad are both null");
     if (k == 0) return PB_OK;
     return train_run(h, d_inputs, n_rec, h_targets, h_rows, k, te, false, 1, epoch, 0, 0.f, 0.f, 0.f, loss_bias, dropout, d_weights,
-                     nullptr, nullptr, d_loss, d_grad, (cudaStream_t)stream);
+                     nullptr, nullptr, d_loss, d_grad, wide, (cudaStream_t)stream);
+}
+
+PB_API int pb_train(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows, int64_t k,
+                    const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
+                    float* d_weights, float* d_rms, double* d_loss, void* stream) {
+    return train_call(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, opts, d_weights, d_rms, d_loss,
+                      false, stream);
+}
+
+PB_API int pb_train_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                         int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
+                         float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream) {
+    return train_loss_call(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, loss_bias, dropout, epoch,
+                           d_weights, d_loss, d_grad, false, stream);
+}
+
+PB_API int pb_train_wide(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                         int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, const pb_train_opts* opts,
+                         float* d_weights, float* d_rms, double* d_loss, void* stream) {
+    return train_call(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, opts, d_weights, d_rms, d_loss,
+                      true, stream);
+}
+
+PB_API int pb_train_wide_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets, const pb_train_row* h_rows,
+                              int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
+                              float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream) {
+    return train_loss_call(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, loss_bias, dropout, epoch,
+                           d_weights, d_loss, d_grad, true, stream);
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {

@@ -13,7 +13,7 @@
 //                            and the weight gradient is accumulated in the warp's own shared gradient row (a lane writes
 //                            only its own columns: no atomics).  The warps' rows are summed in warp order into the
 //                            tile's partial gradient, with the tile's loss sum beside it.
-//   train_update_kernel      one CTA per row of a batch: the row's partials summed in tile order, then RMSprop (pb_train)
+//   train_update_kernel      (templated on the row stride; train_wide.cuh reuses it) one CTA per row of a batch: the row's partials summed in tile order, then RMSprop (pb_train)
 //                            or the gradient written out (pb_train_loss).  The fixed orders make every result independent
 //                            of the other rows of the call, of the grouping of rows and of the launch configuration.
 //
@@ -260,9 +260,9 @@ struct TrainUpdate {
     const TrainRowDev* rows;
     const float* part;
     const double* part_loss;
-    float* weights;                  // [k][TR_STRIDE]: RMSprop (pb_train), or null
+    float* weights;                  // [k][STRIDE]: RMSprop (pb_train), or null
     float* rms;
-    float* grad;                     // [k][TR_STRIDE]: the summed gradient instead (pb_train_loss), or null
+    float* grad;                     // [k][STRIDE]: the summed gradient instead (pb_train_loss), or null
     double* loss_acc;                // [k] the epoch's running loss sum
     double* loss;                    // [k][n_loss] or null
     int n_loss, loss_col;
@@ -270,13 +270,15 @@ struct TrainUpdate {
     float lr, rho, eps;
 };
 
+// STRIDE: floats per row and per partial row (TR_STRIDE here, TW_STRIDE for train_wide.cuh).
+template <int STRIDE>
 __global__ void __launch_bounds__(TR_UPDATE_THREADS) train_update_kernel(const __grid_constant__ TrainUpdate P) {
     const TrainStep st = P.steps[blockIdx.x];
     const int n_w = tr_row_size(P.F, P.rows[st.row].hidden);
-    const size_t off = (size_t)st.row * TR_STRIDE;
+    const size_t off = (size_t)st.row * STRIDE;
     for (int i = threadIdx.x; i < n_w; i += TR_UPDATE_THREADS) {
         float g = 0.f;
-        for (int t = st.t0; t < st.t1; ++t) g += P.part[(size_t)t * TR_STRIDE + i];
+        for (int t = st.t0; t < st.t1; ++t) g += P.part[(size_t)t * STRIDE + i];
         if (P.grad) {
             P.grad[off + i] = g;
         } else if (P.weights) {

@@ -25,7 +25,8 @@ Labelled clips (one network input per clip, vectorize's; statistics per pool mod
   graph_thresholds, roc ~ precise/scripts/graph.py:147-152 (the thresholds and the curve precise-graph plots)
   calc_threshold    ~ precise/scripts/calc_threshold.py:66-83 (a model's threshold_config from its positive clips)
 
-Training (fused-family networks, many per call: pb_vectorize_clips, pb_train, pb_train_loss):
+Training (up to 128 GRU units, many per call: pb_vectorize_clips, pb_train / pb_train_loss up to 24 units, pb_train_wide /
+pb_train_wide_loss beyond):
   vectorize_clips   vectorize(clip) of every clip, on the device
   TrainState, train ~ precise/model.py:57-91, scripts/train.py:159-166 (Keras fit: loss, dropout, RMSprop; val_loss)
 
@@ -44,7 +45,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from .core import PB_TRAIN_STRIDE, PreciseB200, threshold_encode
+from .core import PB_TRAIN_STRIDE, PB_TRAIN_WIDE_STRIDE, PreciseB200, threshold_encode
 from .model_io import GruModel
 
 
@@ -654,8 +655,10 @@ def vectorize_clips(core: PreciseB200, clips, divisor=32767):
 
 class TrainState:
     """Networks being trained on one handle's front end: their weights and RMSprop accumulators as device rows
-    [k, PB_TRAIN_STRIDE] (Keras's order: kernel, recurrent, bias, dense_w, dense_b), each row's hidden size, activations and
-    seed, and the next epoch's number (the shuffles and dropout masks of a resumed fit continue from it)."""
+    [k, stride] (Keras's order: kernel, recurrent, bias, dense_w, dense_b), each row's hidden size, activations and
+    seed, and the next epoch's number (the shuffles and dropout masks of a resumed fit continue from it).  ``stride`` is the
+    layout: PB_TRAIN_STRIDE (pb_train) when every network has at most 24 units, else PB_TRAIN_WIDE_STRIDE (pb_train_wide, up
+    to 128 units); the training calls follow the rows' width."""
 
     def __init__(self, core: PreciseB200, weights, rms, hidden, activation, recurrent_activation, seeds, epoch=0):
         self.core = core
@@ -664,12 +667,21 @@ class TrainState:
         self.seeds = [int(s) for s in seeds]
         self.epoch = int(epoch)
         self.rows = core.train_rows(self.hidden, self.activation, self.recurrent_activation, self.seeds)
+        k = len(self.hidden)
+        self.stride = PB_TRAIN_WIDE_STRIDE if k and weights.numel() == k * PB_TRAIN_WIDE_STRIDE else PB_TRAIN_STRIDE
+
+    @property
+    def wide(self):
+        """Whether the rows have pb_train_wide's layout."""
+        return self.stride == PB_TRAIN_WIDE_STRIDE
 
     @staticmethod
     def from_models(core: PreciseB200, models, seeds):
-        """One row per GruModel (feature size core.feature_size, hidden <= 24), accumulators at zero."""
+        """One row per GruModel (feature size core.feature_size, hidden <= 128), accumulators at zero; the wide layout when
+        any network has more than 24 units."""
         torch = core.torch
-        w = np.zeros((len(models), PB_TRAIN_STRIDE), np.float32)
+        wide = any(m.hidden > 24 for m in models)
+        w = np.zeros((len(models), PB_TRAIN_WIDE_STRIDE if wide else PB_TRAIN_STRIDE), np.float32)
         for i, m in enumerate(models):
             if m.feature_size != core.feature_size:
                 raise ValueError('model %d has feature size %d, the handle %d' % (i, m.feature_size, core.feature_size))

@@ -99,6 +99,21 @@ def check_pool_models(names, models):
                              % (name, model.hidden, model.feature_size, ', deltas' if pr.use_delta else ''))
 
 
+def check_train_models(names, models):
+    """Networks trained together: each must share the first one's front end, which training covers for feature size <= 16
+    without deltas, and have at most 128 units (pb_train up to 24, pb_train_wide beyond)."""
+    from .core import FRONT_END_FIELDS
+    pr0 = models[0][1]
+    for name, (model, pr) in zip(names, models):
+        diff = [f for f in FRONT_END_FIELDS if getattr(pr, f) != getattr(pr0, f)]
+        if diff:
+            raise ValueError('%s: front end differs from %s in %s; models trained together share one MFCC front end'
+                             % (name, names[0], ', '.join(diff)))
+        if model.hidden > 128 or model.feature_size > 16 or pr.use_delta:
+            raise ValueError('%s: training covers hidden <= 128, feature size <= 16 and no deltas; this one has hidden = %d, '
+                             'feature size = %d%s' % (name, model.hidden, model.feature_size, ', deltas' if pr.use_delta else ''))
+
+
 def print_metrics(files, metrics, total):
     for f, m in zip(files, metrics):
         if m is None:

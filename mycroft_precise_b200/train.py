@@ -8,8 +8,9 @@ folder of labelled clips.
 FOLDER has TrainData.from_folder's layout, as precise-test reads it (test.load_folder): the clips under ``FOLDER/wake-word``
 and ``FOLDER/not-wake-word`` are trained on, and those under ``FOLDER/test/...`` give the val_loss.  An existing MODEL.npz
 (with its .params) is fine-tuned; a missing one is created with GruModel.init (``--hidden`` units, seed ``--seed`` + i for
-the i-th model) at the default ListenerParams.  Every model must share the first one's front end and be of the fused family
-(hidden <= 24, feature size <= 16, no deltas); all of them train at once in one set of device calls (offline.train).  For
+the i-th model) at the default ListenerParams.  Every model must share the first one's front end (feature size <= 16, no
+deltas) and have at most 128 GRU units; all of them train at once in one set of device calls (offline.train: pb_train when
+every model has at most 24 units, pb_train_wide on the tensor cores when any has more).  For
 each model, in the order given, a ``=== <model file> ===`` heading is printed, then one line per epoch with its loss and
 val_loss as Keras prints them.  Each model's weights are saved to its .npz and its .params written next to it.
 
@@ -32,7 +33,7 @@ def main(argv=None):
     ap.add_argument('-s', '--sensitivity', type=float, default=0.2, help='weighted loss bias: higher = more false negatives')
     ap.add_argument('--dropout', type=float, default=0.2, help='input dropout rate of the GRU')
     ap.add_argument('--seed', type=int, default=0, help='seed of new networks (seed + i) and of every shuffle and mask')
-    ap.add_argument('--hidden', type=int, default=20, help='GRU units of new networks')
+    ap.add_argument('--hidden', type=int, default=20, help='GRU units of new networks (1 to 128)')
     ap.add_argument('--device', type=int, default=0)
     ap.add_argument('--noise-folder', default=None, help='folder of noise wavs: train on fresh noisy copies every epoch')
     ap.add_argument('-if', '--inflation-factor', type=int, default=1, help='noisy copies of each clip per epoch')
@@ -44,7 +45,7 @@ def main(argv=None):
     from .model_io import GruModel, load_weights, save_weights
     from .offline import TrainState, train, vectorize_clips
     from .params import ListenerParams, load_params, save_params
-    from .simulate import check_pool_models
+    from .simulate import check_train_models
     from .test import load_folder
     names = args.model
     for n in names:
@@ -57,7 +58,7 @@ def main(argv=None):
         else:
             pr = ListenerParams()
             models.append((GruModel.init(pr.feature_size, args.hidden, args.seed + i), pr))
-    check_pool_models(names, models)
+    check_train_models(names, models)
     pr = models[0][1]
     _, clips, targets = load_folder(args.folder, True, pr.sample_rate)
     _, v_clips, v_targets = load_folder(args.folder, False, pr.sample_rate)

@@ -7,7 +7,8 @@ wake words overlaid on background recordings, generated and labelled on the devi
 
 FOLDER has TrainData.from_folder's layout, as train reads it: the clips under FOLDER/wake-word and FOLDER/not-wake-word are
 overlaid (each list sorted by path and cycled), and those under FOLDER/test/... give the val_loss.  RANDOM_FOLDER's wavs
-(searched recursively, sorted) are the backgrounds.  Models are created or fine-tuned as train does them.  Each epoch is
+(searched recursively, sorted) are the backgrounds.  Models are created or fine-tuned as train does them, with up to 128 GRU
+units (feature size <= 16, no deltas).  Each epoch is
 STEPS x BATCH generated windows (offline.Generator, keyed by --seed) and one training epoch over them (pb_train shuffles
 them, where Keras's fit_generator takes consecutive batches).  Per model a ``=== <model file> ===`` heading and one
 Keras-style line per epoch are printed.  The weights go to each .npz (with -sb only when the epoch's loss is the model's best
@@ -57,7 +58,7 @@ def main(argv=None):
     ap.add_argument('-s', '--sensitivity', type=float, default=0.2, help='weighted loss bias: higher = more false negatives')
     ap.add_argument('--dropout', type=float, default=0.2, help='input dropout rate of the GRU')
     ap.add_argument('--seed', type=int, default=0, help='seed of new networks (seed + i), of the generator and of every shuffle')
-    ap.add_argument('--hidden', type=int, default=20, help='GRU units of new networks')
+    ap.add_argument('--hidden', type=int, default=20, help='GRU units of new networks (1 to 128)')
     ap.add_argument('-sb', '--save-best', action='store_true', help="save a model only when its epoch's loss improves")
     ap.add_argument('-p', '--save-prob', type=float, default=0.0, help='probability of saving a window into debug/ww or debug/nww')
     ap.add_argument('--device', type=int, default=0)
@@ -67,7 +68,7 @@ def main(argv=None):
     from .model_io import GruModel, load_weights, save_weights
     from .offline import Generator, TrainState, train_generated, vectorize_clips
     from .params import ListenerParams, load_params, save_params
-    from .simulate import check_pool_models, read_wav
+    from .simulate import check_train_models, read_wav
     from .test import find_wavs, load_folder
     names = args.model
     for n in names:
@@ -84,7 +85,7 @@ def main(argv=None):
         else:
             pr = ListenerParams()
             models.append((GruModel.init(pr.feature_size, args.hidden, args.seed + i), pr))
-    check_pool_models(names, models)
+    check_train_models(names, models)
     pr = models[0][1]
     ww, nww = (sorted(f) for f in find_wavs(args.folder))
     wake = [read_wav(f, pr.sample_rate) for f in ww]
