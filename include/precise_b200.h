@@ -762,6 +762,42 @@ int pb_train_wide_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const
                        int64_t k, const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs, float loss_bias,
                        float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream);
 
+/* precise-test, precise-graph and precise-calc-threshold's statistics (pb_score_dataset's) for k networks given as weight rows,
+ * over labelled network inputs: networks of up to 128 GRU units straight from pb_train(_wide)'s rows, with no pool slot, slot-0
+ * weights or decoder involved (every statistic is over raw).
+ *   - Networks: rows of d_weights [k][stride] (DEVICE) in pb_train's layout (kernel, recurrent, bias, dense_w, dense_b, flat in
+ *     Keras order), stride PB_TRAIN_STRIDE (hidden 1 .. 24) or PB_TRAIN_WIDE_STRIDE (hidden 1 .. 128); hidden and activation
+ *     codes from h_rows (HOST, the seed is ignored).  F is the handle's feature size, as for pb_train.
+ *   - Inputs: d_inputs [n_rec][n_features][F] (DEVICE), pb_vectorize_clips' rows, labels h_targets [n_rec] (HOST).
+ *   - Entries, statistics (d_count, d_hist, d_fit, the miss list), optional outputs and their limits: word for word
+ *     pb_score_dataset's, with network i in place of pool model h_model_ids[i] and clip r in place of recording r.  Every
+ *     statistic is zeroed by the call and is an exact int64 sum, so calls add.
+ *   - Raw: entry (i, r) is bit-identical to pb_predict's d_out[r] for the same inputs on a handle whose slot 0 holds network i
+ *     (same H, F and activations, default gru_mode) wherever pb_predict runs gru_wide's scan, i.e. for every network but the
+ *     default one (H 20, F 13, linear / hard_sigmoid), which pb_predict scores on its own kernels: raw here is always
+ *     gru_wide's 3xTF32 scan.  Pair p's raw is bit-identical to the cross product's entry (h_pair_rows[p], h_pair_recs[p]).
+ *     A row's outputs do not depend on the other rows, their order, the order of the pairs, or how the call cuts them into
+ *     groups and batches.  Like pb_predict's, the last bit of entry r follows r's place in a 16-row block (r mod 16 < 8 or
+ *     not), so two calls over consecutive parts of the clips add up to one call exactly when cut at a multiple of 16 clips.
+ *   - Networks are split into gru_wide's fragments on the device in groups whose fragments stay under 256 MB (about 444 KB per
+ *     network at H = 128, F = 16) and scanned by one launch per batch; without d_raw, raw of a batch (whole rows under
+ *     256 MB, or 2^25 pairs) stays in the arena.
+ *   - Reads and writes no stream state, pool slot or detector.  Asynchronous on `stream`; uses the training arena and orders
+ *     itself against the corpus and training calls as pb_train.  Profile slot 1 counts the scans and statistics.  Every
+ *     argument is checked before anything is enqueued, so a refused call writes nothing.
+ * PB_ERR_INVALID: a null handle, stride other than PB_TRAIN_STRIDE or PB_TRAIN_WIDE_STRIDE, k outside [0, 2^30), a null h_rows
+ * (k > 0), hidden outside [1, 24] (PB_TRAIN_STRIDE) or [1, 128], an unknown activation code, n_rec outside [0, 2^31), every
+ * output null, a null h_targets (n_rec > 0), d_weights (k > 0) or d_inputs (with entries), and pb_score_dataset's refusals of
+ * pairs, thresholds, the miss list and the fit's 2^24 entries per (row, label).  PB_ERR_UNSUPPORTED: a front end outside the
+ * fused family (deltas, feature size > 16, n_features > 112).  PB_ERR_CUDA: the workspace cannot be allocated. */
+int pb_score_rows(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets,
+                  const pb_train_row* h_rows, int64_t k, const float* d_weights, int32_t stride,
+                  const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs,
+                  const double* h_thresholds, int32_t n_thr,
+                  float* d_raw, int64_t* d_count, int64_t* d_hist, int64_t* d_fit,
+                  double miss_threshold, int64_t* d_miss, int64_t miss_capacity, unsigned long long* d_n_miss,
+                  void* stream);
+
 /* Pinned host memory for pb_update_host / benchmarks. */
 int pb_host_alloc(void** out, uint64_t bytes);
 int pb_host_free(void* p);
@@ -811,6 +847,10 @@ int pb_debug_corpus_pool_scan(pb_handle* h, int32_t nm, int32_t groups_fast);
 /* Test hook for pb_score_corpus_pairs: at most `windows` pair-windows per batch (a larger pair still forms one batch), so that
  * small corpora reach the multi-batch path; 0 restores the default (2^25).  PB_ERR_INVALID: null handle, windows < 0. */
 int pb_debug_corpus_pairs_batch(pb_handle* h, int64_t windows);
+/* Test hook for pb_score_rows: at most `networks` networks per group and `entries` entries per batch (the cross product keeps
+ * whole rows, at least one), so that small calls reach several groups and batches; 0 restores each default.  Every cut
+ * scores bit-identical outputs.  PB_ERR_INVALID: null handle, a negative value. */
+int pb_debug_rows_groups(pb_handle* h, int32_t networks, int64_t entries);
 /* CPU model of a tensor-core formulation of the DFT (csrc/mfcc_tc.cuh: radix-16 butterflies, second stage as an fp16 hi / lo
  * matrix product) for one frame of 512 int16 samples -> |X[k]|^2, k = 0..256.  No device needed.  Test hook. */
 int pb_debug_tc_dft_power(const int16_t* x512, double* power257);

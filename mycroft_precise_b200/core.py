@@ -117,6 +117,8 @@ SYMBOLS = {
     'pb_train_wide': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.POINTER(pb_train_opts), _VP, _VP, _VP, _VP]),
     'pb_train_wide_loss': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _VP, _I64, C.c_float, C.c_float, _I32, _VP, _VP, _VP,
                                      _VP]),
+    'pb_score_rows': (C.c_int, [_VP, _VP, _I64, _VP, _VP, _I64, _VP, _I32, _VP, _VP, _I64, _VP, _I32, _VP, _VP, _VP, _VP,
+                                C.c_double, _VP, _I64, _VP, _VP]),
     'pb_host_alloc': (C.c_int, [C.POINTER(_VP), C.c_uint64]),
     'pb_host_free': (C.c_int, [_VP]),
     'pb_profile_enable': (C.c_int, [_VP, C.c_int]),
@@ -132,6 +134,7 @@ SYMBOLS = {
     'pb_debug_corpus_pool_rows': (C.c_int, [_VP, _I64]),
     'pb_debug_corpus_pool_scan': (C.c_int, [_VP, _I32, _I32]),
     'pb_debug_corpus_pairs_batch': (C.c_int, [_VP, _I64]),
+    'pb_debug_rows_groups': (C.c_int, [_VP, _I32, _I64]),
     'pb_debug_tc_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_mma_dft_power': (C.c_int, [_VP, _VP]),
     'pb_debug_tc_mfcc_frame': (C.c_int, [_VP, _VP, _VP]),
@@ -1191,6 +1194,59 @@ class PreciseB200:
         check(fn(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _np_ptr(pr), _np_ptr(pc), n, float(loss_bias),
                  float(dropout), int(epoch), _ptr(weights), _ptr(loss), _ptr(g), self._stream()))
         return (loss, g) if grad else loss
+
+    def score_rows(self, inputs, targets, rows, weights, pair_rows=None, pair_recs=None, thresholds=(0.5,), per_entry=True,
+                   miss_threshold=None, miss_capacity=None):
+        """score_dataset's statistics for the k networks of ``rows`` (train_rows' array) given as weight rows ``weights``
+        (float32 CUDA tensor [k, stride]: PB_TRAIN_STRIDE up to 24 units, PB_TRAIN_WIDE_STRIDE up to 128, read from its
+        width), over ``inputs`` (vectorize_clips' tensor) with labels ``targets`` (host, non-zero = wake word).  pair_rows /
+        pair_recs None: every network over every input, raw [k, n_rec]; otherwise entry p is network pair_rows[p] over input
+        pair_recs[p], raw [n_pairs].  Returns score_dataset's dict, misses included.  Asynchronous on the current stream (a
+        miss list that overflows miss_capacity waits, as in score_dataset).  pb_score_rows in include/precise_b200.h."""
+        torch = self.torch
+        arr, k = rows
+        n_rec, targets, pr, pc, n, stride = self._train_args(inputs, targets, k, pair_rows, pair_recs, weights)
+        thr = np.ascontiguousarray(thresholds, dtype=np.float64)
+        if thr.ndim != 1:
+            raise ValueError('thresholds must be a 1-D list')
+        n_thr = thr.shape[0]
+        f = lambda shape, dt: torch.empty(shape, dtype=dt, device=self.device)
+        out = dict(raw=None, count=f((k, 2), torch.int64), hist=f((k, 2, 2 * n_thr + 1), torch.int64),
+                   fit=f((k, 2, 3), torch.int64), thresholds=thr.astype(np.float32))
+        if per_entry:
+            out['raw'] = f((n,), torch.float32) if pr is not None else f((k, n_rec), torch.float32)
+        misses = miss_threshold is not None
+        n_miss = f((1,), torch.int64) if misses else None
+        cap = self._int('miss_capacity', 1 << 16 if miss_capacity is None else miss_capacity) if misses else 0
+
+        def run(cap):
+            d_miss = f((max(cap, 1),), torch.int64) if misses else None
+            check(self.lib.pb_score_rows(self._h, _ptr(inputs), n_rec, _np_ptr(targets), arr, k, _ptr(weights), stride,
+                                         _np_ptr(pr) if n else None, _np_ptr(pc) if n else None, n, _np_ptr(thr), n_thr,
+                                         _ptr(out['raw']), _ptr(out['count']), _ptr(out['hist']), _ptr(out['fit']),
+                                         float(miss_threshold) if misses else 0.0, _ptr(d_miss) if cap else None, cap,
+                                         _ptr(n_miss), self._stream()))
+            return d_miss
+
+        if k == 0 or (pr is not None and n == 0):             # no entry (the library reads an empty pair list as "every pair")
+            for key in ('count', 'hist', 'fit'):
+                out[key].zero_()
+            if misses:
+                out['misses'] = f((0,), torch.int64)
+            return out
+        d_miss = run(cap)
+        if misses:
+            total = int(n_miss.item())
+            if total > cap:
+                cap = total
+                d_miss = run(cap)
+            out['misses'] = torch.sort(d_miss[:total])[0]
+        return out
+
+    def rows_groups(self, networks=0, entries=0):
+        """Test hook: score_rows splits at most ``networks`` networks per group and scans at most ``entries`` entries per
+        batch (whole rows in the cross product); 0 = the default."""
+        check(self.lib.pb_debug_rows_groups(self._h, int(networks), int(entries)))
 
     def corpus_pairs_batch(self, windows):
         """Test hook: score_corpus_pairs scans at most ``windows`` pair-windows per batch (0 = the default)."""

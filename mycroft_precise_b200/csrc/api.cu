@@ -43,6 +43,7 @@
 #include "train_wide.cuh"
 #include "noise.cuh"
 #include "generate.cuh"
+#include "rows.cuh"
 
 #include <cub/device/device_segmented_sort.cuh>
 
@@ -243,6 +244,8 @@ struct pb_handle {
     DevArray<long long> d_gen_wins;  // ... [n_windows] the chosen windows' places in the window table
     DevArray<int16_t> d_gen_pcm;     // ... the generated streams, each at a multiple of 8 samples (K1's recordings)
     int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
+    int32_t rows_group_nets = 0;     // pb_debug_rows_groups: at most this many networks per group (0 = the 256 MB cap's)
+    int64_t rows_batch_entries = 0;  // ... at most this many entries per batch (0 = ROWS_RAW_CAP's, or ROWS_PAIRS_BATCH)
     // model pool (pb_set_pool, pool.cuh); a handle without one keeps pool = false and launches none of this
     bool pool = false;               // a pool exists
     int32_t pool_models = 0;         // max_models
@@ -800,6 +803,46 @@ static int upload_wide(NetWeights& w, int H, int F, const float* kernel, const f
     CK(w.wg_b2.upload(b2));
     CK(w.wg_bias.upload(wb));
     return PB_OK;
+}
+
+// upload_wide's layout written on the device (pb_score_rows): both write one layout with the same arithmetic -- the TF32
+// rounding on the integer bits, then one exact float subtraction for lo -- so a network's fragments are bit-identical
+// whichever wrote them.  Block y splits network y of a group from its pb_train weight row weights[rows[y]] (kernel,
+// recurrent, bias, dense_w, dense_b) into b1, b2 and bias at the pointers of nets[y] (H, F, FP and HP set), and fills its bd.
+__global__ void rows_split_kernel(const float* __restrict__ weights, long long stride, const int* __restrict__ rows, GruWideW* nets) {
+    GruWideW& N = nets[blockIdx.y];
+    const int H = N.H, F = N.F, FP = N.FP, HP = N.HP, H3 = 3 * H, KS = (FP + HP) / 8;
+    const float* kernel = weights + rows[blockIdx.y] * stride;
+    const float* recurrent = kernel + (size_t)F * H3;
+    const float* bias = recurrent + (size_t)H * H3;
+    auto tf32 = [](float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); };
+    auto wv = [&](int k, int gate, int unit) -> float {
+        if (unit >= H) return 0.f;
+        if (k < FP) return k < F ? kernel[(size_t)k * H3 + gate * H + unit] : 0.f;
+        const int hu = k - FP;
+        return hu < H ? recurrent[(size_t)hu * H3 + gate * H + unit] : 0.f;
+    };
+    auto frag = [&](int s, int lane, int gate, int unit) {
+        const int t = lane & 3;
+        const float v0 = wv(8 * s + t, gate, unit), v1 = wv(8 * s + t + 4, gate, unit);
+        const float h0 = tf32(v0), h1 = tf32(v1), l0 = tf32(__fsub_rn(v0, h0)), l1 = tf32(__fsub_rn(v1, h1));
+        return make_uint4(__float_as_uint(h0), __float_as_uint(h1), __float_as_uint(l0), __float_as_uint(l1));
+    };
+    const long long n1 = (long long)KS * (HP / 4) * 32, n2 = (long long)KS * (HP / 8) * 32, nb = 3 * HP;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n1 + n2 + nb; e += (long long)gridDim.x * blockDim.x) {
+        if (e < n1) {
+            const int lane = (int)(e & 31), nt = (int)((e >> 5) % (HP / 4)), s = (int)((e >> 5) / (HP / 4)), c = 8 * nt + (lane >> 2);
+            const_cast<uint4*>(N.b1)[e] = frag(s, lane, c < HP ? 0 : 1, c % HP);
+        } else if (e < n1 + n2) {
+            const long long q = e - n1;
+            const int lane = (int)(q & 31), nt = (int)((q >> 5) % (HP / 8)), s = (int)((q >> 5) / (HP / 8));
+            const_cast<uint4*>(N.b2)[q] = frag(s, lane, 2, 8 * nt + (lane >> 2));
+        } else {
+            const int j = (int)(e - n1 - n2), g3 = j / HP, u = j - g3 * HP;
+            const_cast<float*>(N.bias)[j] = u < H ? bias[g3 * H + u] : 0.f;
+        }
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) N.bd = bias[H3 + H];
 }
 
 // [W; U] of gru_tiled_kernel, its bias and the dense weights.
@@ -2281,6 +2324,51 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
 // ------------------------------------------------------------------------------------------------
 // pool models over labelled clips (dataset.cuh)
 
+// The refusals pb_score_dataset and pb_score_rows share beyond their networks: pairs (rows of k, clips of n_rec), thresholds,
+// the miss list and the fit's 2^24 entries per (row, label).  thr receives the thresholds rounded to float32.
+static int check_dataset_stats(int64_t k, int64_t n_rec, const uint8_t* h_targets, const int32_t* h_pair_rows,
+                               const int32_t* h_pair_recs, int64_t n_pairs, const double* h_thresholds, int32_t n_thr,
+                               const int64_t* d_hist, const int64_t* d_fit, const int64_t* d_miss, int64_t miss_capacity,
+                               const unsigned long long* d_n_miss, std::vector<float>& thr) {
+    if (n_pairs < 0 || n_pairs > INT32_MAX) return fail(PB_ERR_INVALID, "n_pairs = %lld outside [0, 2^31)", (long long)n_pairs);
+    const bool by_pairs = n_pairs > 0, misses = d_n_miss != nullptr;
+    if (by_pairs && (!h_pair_rows || !h_pair_recs)) return fail(PB_ERR_INVALID, "null h_pair_rows or h_pair_recs");
+    for (int64_t i = 0; i < n_pairs; ++i) {
+        const int32_t row = h_pair_rows[i], r = h_pair_recs[i];
+        if (row < 0 || row >= k) return fail(PB_ERR_INVALID, "row %d (pair %lld) outside [0, k = %lld)", row, (long long)i, (long long)k);
+        if (r < 0 || r >= n_rec)
+            return fail(PB_ERR_INVALID, "recording id %d (pair %lld) outside [0, n_rec = %lld)", r, (long long)i, (long long)n_rec);
+    }
+    if (n_thr < 0 || n_thr > DS_MAX_THR) return fail(PB_ERR_INVALID, "n_thr = %d outside [0, %d]", n_thr, DS_MAX_THR);
+    if (d_hist && n_thr < 1) return fail(PB_ERR_INVALID, "d_hist needs at least one threshold");
+    if (n_thr > 0 && !h_thresholds) return fail(PB_ERR_INVALID, "null h_thresholds");
+    thr.assign((size_t)n_thr, 0.f);
+    for (int i = 0; i < n_thr; ++i) {
+        thr[i] = (float)h_thresholds[i];
+        if (!(i == 0 ? thr[i] == thr[i] : thr[i] > thr[i - 1]))
+            return fail(PB_ERR_INVALID, "threshold %d = %g: rounded to float32, thresholds must be strictly ascending", i, h_thresholds[i]);
+    }
+    if (miss_capacity < 0) return fail(PB_ERR_INVALID, "miss_capacity = %lld is negative", (long long)miss_capacity);
+    if (miss_capacity > 0 && !d_miss) return fail(PB_ERR_INVALID, "null d_miss with miss_capacity = %lld", (long long)miss_capacity);
+    if (d_miss && !misses) return fail(PB_ERR_INVALID, "d_miss without d_n_miss");
+    if (d_fit) {
+        // the fit's int64 sums hold 2^24 entries of one (row, label)
+        const int64_t limit = 1ll << 24;
+        if (by_pairs) {
+            std::vector<int64_t> per((size_t)k * 2, 0);
+            for (int64_t i = 0; i < n_pairs; ++i)
+                if (++per[(size_t)h_pair_rows[i] * 2 + (h_targets[h_pair_recs[i]] != 0)] > limit)
+                    return fail(PB_ERR_INVALID, "row %d has more than 2^24 entries of one label: split the call", h_pair_rows[i]);
+        } else {
+            int64_t pos = 0;
+            for (int64_t r = 0; r < n_rec; ++r) pos += h_targets[r] != 0;
+            if (k > 0 && std::max(pos, n_rec - pos) > limit)
+                return fail(PB_ERR_INVALID, "%lld recordings of one label, more than 2^24: split the call", (long long)std::max(pos, n_rec - pos));
+        }
+    }
+    return PB_OK;
+}
+
 PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
                             const uint8_t* h_targets, const int32_t* h_model_ids, int64_t k,
                             const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs,
@@ -2307,42 +2395,11 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
         if (h->pool_cd_of[m] == h->pool_cd.end())
             return fail(PB_ERR_INVALID, "pool slot %d (entry %lld) holds no model: pb_pool_load it first", m, (long long)i);
     }
-    if (n_pairs < 0 || n_pairs > INT32_MAX) return fail(PB_ERR_INVALID, "n_pairs = %lld outside [0, 2^31)", (long long)n_pairs);
+    std::vector<float> thr;
+    rc = check_dataset_stats(k, n_rec, h_targets, h_pair_rows, h_pair_recs, n_pairs, h_thresholds, n_thr, d_hist, d_fit, d_miss,
+                             miss_capacity, d_n_miss, thr);
+    if (rc != PB_OK) return rc;
     const bool by_pairs = n_pairs > 0;
-    if (by_pairs && (!h_pair_rows || !h_pair_recs)) return fail(PB_ERR_INVALID, "null h_pair_rows or h_pair_recs");
-    for (int64_t i = 0; i < n_pairs; ++i) {
-        const int32_t row = h_pair_rows[i], r = h_pair_recs[i];
-        if (row < 0 || row >= k) return fail(PB_ERR_INVALID, "row %d (pair %lld) outside [0, k = %lld)", row, (long long)i, (long long)k);
-        if (r < 0 || r >= n_rec)
-            return fail(PB_ERR_INVALID, "recording id %d (pair %lld) outside [0, n_rec = %lld)", r, (long long)i, (long long)n_rec);
-    }
-    if (n_thr < 0 || n_thr > DS_MAX_THR) return fail(PB_ERR_INVALID, "n_thr = %d outside [0, %d]", n_thr, DS_MAX_THR);
-    if (d_hist && n_thr < 1) return fail(PB_ERR_INVALID, "d_hist needs at least one threshold");
-    if (n_thr > 0 && !h_thresholds) return fail(PB_ERR_INVALID, "null h_thresholds");
-    std::vector<float> thr((size_t)n_thr);
-    for (int i = 0; i < n_thr; ++i) {
-        thr[i] = (float)h_thresholds[i];
-        if (!(i == 0 ? thr[i] == thr[i] : thr[i] > thr[i - 1]))
-            return fail(PB_ERR_INVALID, "threshold %d = %g: rounded to float32, thresholds must be strictly ascending", i, h_thresholds[i]);
-    }
-    if (miss_capacity < 0) return fail(PB_ERR_INVALID, "miss_capacity = %lld is negative", (long long)miss_capacity);
-    if (miss_capacity > 0 && !d_miss) return fail(PB_ERR_INVALID, "null d_miss with miss_capacity = %lld", (long long)miss_capacity);
-    if (d_miss && !misses) return fail(PB_ERR_INVALID, "d_miss without d_n_miss");
-    if (d_fit) {
-        // the fit's int64 sums hold 2^24 entries of one (row, label)
-        const int64_t limit = 1ll << 24;
-        if (by_pairs) {
-            std::vector<int64_t> per((size_t)k * 2, 0);
-            for (int64_t i = 0; i < n_pairs; ++i)
-                if (++per[(size_t)h_pair_rows[i] * 2 + (h_targets[h_pair_recs[i]] != 0)] > limit)
-                    return fail(PB_ERR_INVALID, "row %d has more than 2^24 entries of one label: split the call", h_pair_rows[i]);
-        } else {
-            int64_t pos = 0;
-            for (int64_t r = 0; r < n_rec; ++r) pos += h_targets[r] != 0;
-            if (k > 0 && std::max(pos, n_rec - pos) > limit)
-                return fail(PB_ERR_INVALID, "%lld recordings of one label, more than 2^24: split the call", (long long)std::max(pos, n_rec - pos));
-        }
-    }
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     const int bins = 2 * n_thr + 1;
@@ -3182,6 +3239,255 @@ PB_API int pb_train_wide_loss(pb_handle* h, const float* d_inputs, int64_t n_rec
                               float dropout, int32_t epoch, const float* d_weights, double* d_loss, float* d_grad, void* stream) {
     return train_loss_call(h, d_inputs, n_rec, h_targets, h_rows, k, h_pair_rows, h_pair_recs, n_pairs, loss_bias, dropout, epoch,
                            d_weights, d_loss, d_grad, true, stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// networks from weight rows over labelled clips (rows.cuh)
+
+constexpr size_t ROWS_FRAG_CAP = size_t(256) << 20;   // fragments of one group of networks
+constexpr int64_t ROWS_RAW_CAP = 256ll << 20;         // raw of one cross-product batch kept in the arena (no d_raw)
+constexpr int64_t ROWS_PAIRS_BATCH = 1ll << 25;       // pairs per batch: 8 B of window start and 4 B of raw each
+constexpr int ROWS_MAX_NETS = 65535;                  // networks per group (gridDim.y of the split and the scan)
+
+// Arena bytes of one network's fragments, bias and table entry at feature size F (upload_wide's sizes, each part aligned).
+static size_t rows_net_bytes(int H, int F) {
+    const size_t FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
+    auto al = [](size_t b) { return (b + TRAIN_ALIGN - 1) / TRAIN_ALIGN * TRAIN_ALIGN; };
+    return al(KS * (HP / 4) * 32 * sizeof(uint4)) + al(KS * (HP / 8) * 32 * sizeof(uint4)) + al(3 * HP * sizeof(float)) +
+           sizeof(GruWideW) + sizeof(int);
+}
+
+PB_API int pb_debug_rows_groups(pb_handle* h, int32_t networks, int64_t entries) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    if (networks < 0 || entries < 0) return fail(PB_ERR_INVALID, "networks = %d and entries = %lld must be >= 0", networks, (long long)entries);
+    h->rows_group_nets = networks;
+    h->rows_batch_entries = entries;
+    return PB_OK;
+}
+
+PB_API int pb_score_rows(pb_handle* h, const float* d_inputs, int64_t n_rec, const uint8_t* h_targets,
+                         const pb_train_row* h_rows, int64_t k, const float* d_weights, int32_t stride,
+                         const int32_t* h_pair_rows, const int32_t* h_pair_recs, int64_t n_pairs,
+                         const double* h_thresholds, int32_t n_thr,
+                         float* d_raw, int64_t* d_count, int64_t* d_hist, int64_t* d_fit,
+                         double miss_threshold, int64_t* d_miss, int64_t miss_capacity, unsigned long long* d_n_miss,
+                         void* stream) {
+    if (!h) return fail(PB_ERR_INVALID, "null handle");
+    int rc = check_train_front_end(h);
+    if (rc != PB_OK) return rc;
+    if (stride != TR_STRIDE && stride != TW_STRIDE)
+        return fail(PB_ERR_INVALID, "stride = %d must be PB_TRAIN_STRIDE (%d) or PB_TRAIN_WIDE_STRIDE (%d)", stride, TR_STRIDE, TW_STRIDE);
+    const int max_h = stride == TR_STRIDE ? TR_MAX_H : TW_MAX_H;
+    if (k < 0 || k > INT32_MAX / 2) return fail(PB_ERR_INVALID, "k = %lld outside [0, 2^30)", (long long)k);
+    if (k > 0 && !h_rows) return fail(PB_ERR_INVALID, "null h_rows");
+    for (int64_t i = 0; i < k; ++i) {
+        const pb_train_row& r = h_rows[i];
+        if (r.hidden < 1 || r.hidden > max_h) return fail(PB_ERR_INVALID, "row %lld: hidden = %d outside [1, %d]", (long long)i, r.hidden, max_h);
+        if ((r.activation != PB_ACT_LINEAR && r.activation != PB_ACT_TANH) ||
+            (r.recurrent_activation != PB_RACT_HARD_SIGMOID && r.recurrent_activation != PB_RACT_SIGMOID))
+            return fail(PB_ERR_INVALID, "row %lld: unknown activation codes (%d, %d)", (long long)i, r.activation, r.recurrent_activation);
+    }
+    if (n_rec < 0 || n_rec > INT32_MAX) return fail(PB_ERR_INVALID, "n_rec = %lld outside [0, 2^31)", (long long)n_rec);
+    const bool misses = d_n_miss != nullptr, stats = d_count || d_hist || d_fit || misses;
+    if (!d_raw && !stats) return fail(PB_ERR_INVALID, "every output is null");
+    if (n_rec > 0 && !h_targets) return fail(PB_ERR_INVALID, "null h_targets");
+    if (k > 0 && !d_weights) return fail(PB_ERR_INVALID, "null d_weights");
+    if (k > 0 && n_rec > 0 && !d_inputs) return fail(PB_ERR_INVALID, "null d_inputs");
+    std::vector<float> thr;
+    rc = check_dataset_stats(k, n_rec, h_targets, h_pair_rows, h_pair_recs, n_pairs, h_thresholds, n_thr, d_hist, d_fit, d_miss,
+                             miss_capacity, d_n_miss, thr);
+    if (rc != PB_OK) return rc;
+    const bool by_pairs = n_pairs > 0;
+    CK(cudaSetDevice(h->cfg.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int bins = 2 * n_thr + 1;
+    auto zero = [&]() -> int {
+        if (d_count) CK(cudaMemsetAsync(d_count, 0, (size_t)k * 2 * sizeof(int64_t), s));
+        if (d_hist) CK(cudaMemsetAsync(d_hist, 0, (size_t)k * 2 * bins * sizeof(int64_t), s));
+        if (d_fit) CK(cudaMemsetAsync(d_fit, 0, (size_t)k * 6 * sizeof(int64_t), s));
+        if (misses) CK(cudaMemsetAsync(d_n_miss, 0, sizeof(unsigned long long), s));
+        return PB_OK;
+    };
+    if (n_rec == 0 || k == 0) return zero();
+
+    const int T = h->cfg.n_features, F = h->feat;
+    const int net_cap = h->rows_group_nets > 0 ? std::min(h->rows_group_nets, ROWS_MAX_NETS) : ROWS_MAX_NETS;
+    // A group: networks whose fragments are split together (under ROWS_FRAG_CAP, at most net_cap) and its batches.  Cross
+    // product: consecutive rows nets[0 ..), batches of consecutive rows b0 .. b1 - 1 (whole rows of raw).  Pairs: one batch of
+    // consecutive pairs p0 .. p1 - 1, the group the networks they name (in order of first appearance), and its slots
+    // (rows.cuh): tiles of 128 slots on one network (tile_net), slot_pair the batch-local pair in each slot or -1.
+    struct RowsGroup { std::vector<int> nets; std::vector<int64_t> b; std::vector<int> slot_pair, tile_net; size_t bytes = 0; };
+    std::vector<RowsGroup> groups;
+    int64_t batch_rows = 0, batch_cap = 0;
+    size_t net_max = 0, bytes_max = 0, smem_max = 0, slots_max = 0;
+    for (int64_t i = 0; i < k; ++i) {
+        const int HP = (h_rows[i].hidden + 15) & ~15;
+        smem_max = std::max(smem_max, wg_smem((F + 7) & ~7, HP));
+    }
+    if (!by_pairs) {
+        const int64_t E = h->rows_batch_entries > 0 ? h->rows_batch_entries : d_raw ? INT64_MAX : ROWS_RAW_CAP / 4;
+        batch_rows = std::max<int64_t>(1, std::min<int64_t>(E / n_rec, ROWS_MAX_NETS));
+        for (int64_t i = 0; i < k; ++i) {
+            const size_t b = rows_net_bytes(h_rows[i].hidden, F);
+            if (groups.empty() || groups.back().bytes + b > ROWS_FRAG_CAP || (int)groups.back().nets.size() >= net_cap) groups.emplace_back();
+            groups.back().nets.push_back((int)i);
+            groups.back().bytes += b;
+        }
+        for (RowsGroup& g : groups) {
+            const int64_t r0 = g.nets.front(), r1 = r0 + (int64_t)g.nets.size();
+            for (int64_t b0 = r0; b0 < r1; b0 += batch_rows) g.b.push_back(b0);
+            g.b.push_back(r1);
+            net_max = std::max(net_max, g.nets.size());
+            bytes_max = std::max(bytes_max, g.bytes);
+        }
+        batch_rows = std::min<int64_t>(batch_rows, (int64_t)net_max);
+    } else {
+        batch_cap = std::min<int64_t>(n_pairs, h->rows_batch_entries > 0 ? std::min(h->rows_batch_entries, ROWS_PAIRS_BATCH) : ROWS_PAIRS_BATCH);
+        std::vector<int> local((size_t)k, -1);
+        for (int64_t p0 = 0; p0 < n_pairs;) {
+            RowsGroup g;
+            int64_t p1 = p0;
+            while (p1 < n_pairs && p1 - p0 < batch_cap) {
+                const int r = h_pair_rows[p1];
+                if (local[r] < 0) {
+                    const size_t b = rows_net_bytes(h_rows[r].hidden, F);
+                    if (!g.nets.empty() && (g.bytes + b > ROWS_FRAG_CAP || (int)g.nets.size() >= net_cap)) break;
+                    local[r] = (int)g.nets.size();
+                    g.nets.push_back(r);
+                    g.bytes += b;
+                }
+                ++p1;
+            }
+            // each network's pairs, by the class of their clip's row in a 16-row block, into tiles of 64 slots of each class
+            std::vector<std::vector<int>> cls(2 * g.nets.size());
+            for (int64_t q = p0; q < p1; ++q) cls[2 * local[h_pair_rows[q]] + ((h_pair_recs[q] & 15) >= 8)].push_back((int)(q - p0));
+            for (size_t j = 0; j < g.nets.size(); ++j) {
+                const std::vector<int>& lo = cls[2 * j];
+                const std::vector<int>& hi = cls[2 * j + 1];
+                for (size_t a = 0; a < std::max(lo.size(), hi.size()); a += 64) {
+                    g.tile_net.push_back((int)j);
+                    for (int sl = 0; sl < WG_STREAMS; ++sl) {
+                        const std::vector<int>& v = (sl & 15) >= 8 ? hi : lo;
+                        const size_t at = a + (size_t)(sl >> 4) * 8 + (sl & 7);
+                        g.slot_pair.push_back(at < v.size() ? v[at] : -1);
+                    }
+                }
+            }
+            for (int r : g.nets) local[r] = -1;
+            slots_max = std::max(slots_max, g.slot_pair.size());
+            g.b = {p0, p1};
+            net_max = std::max(net_max, g.nets.size());
+            bytes_max = std::max(bytes_max, g.bytes);
+            groups.push_back(std::move(g));
+            p0 = p1;
+        }
+    }
+    struct RowsWs {
+        GruWideW* nets; int* rows; uint8_t* frag; uint8_t* targets; float* thr; int2* pairs; int* slot_pair; int* tile_net;
+        long long* starts; float* raw_slot; float* raw;
+    };
+    const size_t raw_n = d_raw ? 0 : by_pairs ? (size_t)batch_cap : (size_t)(batch_rows * n_rec);
+    auto layout = [&](uint8_t* base, size_t* bytes) {
+        TrainCarve c{base};
+        RowsWs w{};
+        w.nets = c.take<GruWideW>(net_max); w.rows = c.take<int>(net_max); w.frag = c.take<uint8_t>(bytes_max);
+        w.targets = c.take<uint8_t>(stats ? (size_t)n_rec : 0); w.thr = c.take<float>((size_t)n_thr);
+        w.pairs = c.take<int2>((size_t)n_pairs); w.slot_pair = c.take<int>(slots_max); w.tile_net = c.take<int>(slots_max / WG_STREAMS);
+        w.starts = c.take<long long>(slots_max); w.raw_slot = c.take<float>(slots_max); w.raw = c.take<float>(raw_n);
+        if (bytes) *bytes = c.at;
+        return w;
+    };
+    size_t bytes = 0;
+    layout(nullptr, &bytes);
+    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
+    if (h->d_tr_ws.size() < bytes) {
+        DevArray<uint8_t> fresh;
+        const cudaError_t e = fresh.alloc(bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(PB_ERR_CUDA, "workspace allocation failed (%zu bytes): %s", bytes, cudaGetErrorString(e));
+        }
+        CK(cudaEventSynchronize(h->corpus_ev));                     // the previous call may still use the arena
+        h->d_tr_ws = std::move(fresh);
+    }
+    CK(ensure_dyn_smem(gru_wide_rows_kernel, smem_max));
+    CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
+    const RowsWs w = layout(h->d_tr_ws.get(), nullptr);
+    auto launch = [&]() -> int {
+        rc = zero();
+        if (rc != PB_OK) return rc;
+        if (d_hist) CK(cudaMemcpyAsync(w.thr, thr.data(), thr.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (stats) CK(cudaMemcpyAsync(w.targets, h_targets, (size_t)n_rec, cudaMemcpyHostToDevice, s));
+        if (by_pairs) {
+            std::vector<int2> pairs((size_t)n_pairs);
+            for (int64_t i = 0; i < n_pairs; ++i) pairs[i] = make_int2(h_pair_rows[i], h_pair_recs[i]);
+            CK(cudaMemcpyAsync(w.pairs, pairs.data(), pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        }
+        ProfScope prof(h, 1, s);
+        K2In in{};
+        in.inputs = d_inputs; in.row_stride = F; in.T = T; in.F_base = h->n_out; in.use_delta = 0;
+        DatasetStats D{};
+        D.targets = w.targets; D.thr = d_hist ? w.thr : nullptr; D.n_thr = n_thr;
+        D.count = d_count; D.hist = d_hist; D.fit = d_fit;
+        D.miss_thr = (float)miss_threshold; D.miss = d_miss; D.capacity = miss_capacity; D.n_miss = d_n_miss;
+        std::vector<GruWideW> table;
+        for (const RowsGroup& g : groups) {
+            // the group's table: fragment pointers into the arena (rows_split_kernel fills them and bd), dense_w in the row; the
+            // host buffers are staged by the copies, so the next group may refill them
+            table.assign(g.nets.size(), GruWideW{});
+            TrainCarve c{w.frag};
+            for (size_t j = 0; j < g.nets.size(); ++j) {
+                const int H = h_rows[g.nets[j]].hidden, FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
+                GruWideW& n = table[j];
+                n.b1 = c.take<uint4>((size_t)KS * (HP / 4) * 32); n.b2 = c.take<uint4>((size_t)KS * (HP / 8) * 32);
+                n.bias = c.take<float>((size_t)3 * HP);
+                n.wd = d_weights + (size_t)g.nets[j] * stride + (size_t)3 * H * (F + H + 1);
+                n.H = H; n.F = F; n.FP = FP; n.HP = HP; n.act = h_rows[g.nets[j]].activation; n.ract = h_rows[g.nets[j]].recurrent_activation;
+            }
+            CK(cudaMemcpyAsync(w.nets, table.data(), table.size() * sizeof(GruWideW), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(w.rows, g.nets.data(), g.nets.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+            const int HPm = (max_h + 15) & ~15, KSm = (((F + 7) & ~7) + HPm) / 8;
+            const unsigned gx = (unsigned)std::min<int64_t>(((int64_t)KSm * (3 * HPm / 8) * 32 + 3 * HPm + 255) / 256, 128);
+            rows_split_kernel<<<dim3(gx, (unsigned)g.nets.size()), 256, 0, s>>>(d_weights, stride, w.rows, w.nets);
+            CK(cudaGetLastError());
+            if (!by_pairs) {
+                for (size_t b = 0; b + 1 < g.b.size(); ++b) {
+                    const int64_t b0 = g.b[b], nb = g.b[b + 1] - b0;
+                    float* raw = d_raw ? d_raw + b0 * n_rec : w.raw;
+                    RowsScan S{};
+                    S.nets = w.nets + (b0 - g.nets.front()); S.raw = raw; S.n = n_rec;
+                    gru_wide_rows_kernel<<<dim3((unsigned)((n_rec + WG_STREAMS - 1) / WG_STREAMS), (unsigned)nb), WG_THREADS, smem_max, s>>>(S, in);
+                    CK(cudaGetLastError());
+                    if (!stats) continue;
+                    D.raw = raw; D.row0 = (int)b0; D.n = n_rec;
+                    const unsigned sx = (unsigned)((n_rec + DS_THREADS * DS_ITERS - 1) / (DS_THREADS * DS_ITERS));
+                    dataset_stats_kernel<false><<<dim3(sx, (unsigned)nb), DS_THREADS, 0, s>>>(D);
+                    CK(cudaGetLastError());
+                }
+            } else {
+                const int64_t p0 = g.b[0], nb = g.b[1] - p0, ns = (int64_t)g.slot_pair.size();
+                float* raw = d_raw ? d_raw + p0 : w.raw;
+                CK(cudaMemcpyAsync(w.slot_pair, g.slot_pair.data(), (size_t)ns * sizeof(int), cudaMemcpyHostToDevice, s));
+                CK(cudaMemcpyAsync(w.tile_net, g.tile_net.data(), g.tile_net.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+                rows_slots_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, s>>>(w.slot_pair, w.pairs + p0, ns, T, w.starts);
+                CK(cudaGetLastError());
+                RowsScan S{};
+                S.nets = w.nets; S.tile_net = w.tile_net; S.raw = w.raw_slot; S.n = ns;
+                K2In pin = in;
+                pin.starts = w.starts;
+                gru_wide_rows_kernel<<<(unsigned)g.tile_net.size(), WG_THREADS, smem_max, s>>>(S, pin);
+                CK(cudaGetLastError());
+                rows_scatter_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, s>>>(w.slot_pair, w.raw_slot, ns, raw);
+                CK(cudaGetLastError());
+                if (!stats) continue;
+                D.raw = raw; D.pairs = w.pairs + p0; D.n = nb; D.base = p0;
+                dataset_stats_kernel<true><<<(unsigned)((nb + DS_THREADS - 1) / DS_THREADS), DS_THREADS, 0, s>>>(D);
+                CK(cudaGetLastError());
+            }
+        }
+        return PB_OK;
+    };
+    return corpus_done(h, s, launch());
 }
 
 __global__ void read_window_kernel(K2In in, const int* ids, long long n, float* out) {

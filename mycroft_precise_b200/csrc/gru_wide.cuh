@@ -36,9 +36,14 @@ __device__ __forceinline__ void wg_afrag(const float* base, int stride, int row,
     split_tf32(v, hi, lo);
 }
 
-template <bool RING>
-__global__ void __launch_bounds__(WG_THREADS, 1)
-gru_wide_kernel(GruWideW W, K2In in, long long n, DecodeParams dp, K2Out out) {
+// The scan of one tile: items base .. base + 127 (those below n) of `in`, base = tile_base(), network W, Dense and epilogue
+// into out.  Shared by gru_wide_kernel (W a kernel parameter, one tile per CTA) and gru_wide_rows_kernel (rows.cuh: W from a
+// per-network table).  tile_base is called where the kernel always computed its base, which keeps gru_wide_kernel's SASS.
+// PIN_FMA: the state update z h + (1 - z) a with gru_wide_kernel's contractions spelled out (see below), for kernels that
+// must reproduce its bits; gru_wide_kernel itself leaves the choice to the compiler.
+template <bool RING, bool PIN_FMA, typename TileBase>
+__device__ __forceinline__ void gru_wide_tile(const GruWideW& W, const K2In& in, TileBase tile_base, long long n, const DecodeParams& dp,
+                                              const K2Out& out) {
     extern __shared__ __align__(16) float wg_sm[];
     const int F = W.F, H = W.H, FP = W.FP, HP = W.HP;
     const int AS = wg_as(FP, HP), RS = wg_rs(HP);
@@ -48,7 +53,7 @@ gru_wide_kernel(GruWideW W, K2In in, long long n, DecodeParams dp, K2Out out) {
     __shared__ int s_sid[WG_STREAMS];
     __shared__ long long s_rel[WG_STREAMS];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
-    const long long base = (long long)blockIdx.x * WG_STREAMS;
+    const long long base = tile_base();
     if (tid < WG_STREAMS) {
         const long long i = base + tid;
         int sid = 0; long long rel = 0;
@@ -173,7 +178,15 @@ gru_wide_kernel(GruWideW W, K2In in, long long n, DecodeParams dp, K2Out out) {
                         for (int e = 0; e < 4; ++e) {
                             const int row = 16 * (4 * mh + m) + g + 8 * (e >> 1), u = 16 * warp + 8 * q + 2 * t + (e & 1);
                             const float zz = Z[row * RS + u], hp = A[row * AS + FP + u];
-                            A[row * AS + FP + u] = zz * hp + (1.f - zz) * apply_act(acc[m][q][e], W.act);
+                            if constexpr (PIN_FMA) {
+                                // gru_wide_kernel's SASS computes (q, e) = (0, 0) as fma(1 - z, a, z h) (it takes z h before
+                                // the activation's branch) and every other (m, q, e) as fma(z, h, (1 - z) a), on both branches
+                                const float a = apply_act(acc[m][q][e], W.act), om = __fsub_rn(1.f, zz);
+                                A[row * AS + FP + u] = q == 0 && e == 0 ? __fmaf_rn(om, a, __fmul_rn(zz, hp))
+                                                                        : __fmaf_rn(zz, hp, __fmul_rn(om, a));
+                            } else {
+                                A[row * AS + FP + u] = zz * hp + (1.f - zz) * apply_act(acc[m][q][e], W.act);
+                            }
                         }
             }
         }
@@ -186,6 +199,12 @@ gru_wide_kernel(GruWideW W, K2In in, long long n, DecodeParams dp, K2Out out) {
         for (int j = 0; j < H; ++j) logit = fmaf(A[tid * AS + FP + j], __ldg(W.wd + j), logit);
         epilogue(logit, i < n, i, s_sid[tid], dp, out);
     }
+}
+
+template <bool RING>
+__global__ void __launch_bounds__(WG_THREADS, 1)
+gru_wide_kernel(GruWideW W, K2In in, long long n, DecodeParams dp, K2Out out) {
+    gru_wide_tile<RING, false>(W, in, [] { return (long long)blockIdx.x * WG_STREAMS; }, n, dp, out);
 }
 
 }  // namespace pb

@@ -29,6 +29,8 @@ Training (up to 128 GRU units, many per call: pb_vectorize_clips, pb_train / pb_
 pb_train_wide_loss beyond):
   vectorize_clips   vectorize(clip) of every clip, on the device
   TrainState, train ~ precise/model.py:57-91, scripts/train.py:159-166 (Keras fit: loss, dropout, RMSprop; val_loss)
+  test_rows         test_pool for the networks of a TrainState (up to 128 units), scored from their weight rows
+                    (pb_score_rows) over vectorize_clips' inputs
 
 Noise augmentation (pb_add_noise):
   NoiseSource       ~ precise/scripts/add_noise.py:56-80 (NoiseData: the noise files as one cyclic stream and its position)
@@ -705,6 +707,63 @@ class TrainState:
             out.append(GruModel(parts[0].reshape(F, 3 * H), parts[1].reshape(H, 3 * H), parts[2], parts[3], parts[4],
                                 self.activation[i], self.recurrent_activation[i]))
         return out
+
+
+# Clips per pb_score_rows call of test_rows: the fit's sums hold 2^24 entries of one (row, label).
+ROWS_CALL_CLIPS = 1 << 24
+
+
+def test_rows(core: PreciseB200, state: TrainState, inputs, targets, rows=None, recs=None, thresholds=(0.5,), misses=False,
+              miss_threshold=0.5):
+    """test_pool for the networks of ``state`` (a TrainState, or TrainState.from_models(core, models, seeds) for models on
+    disk; up to 128 units), scored straight from its weight rows (pb_score_rows) over ``inputs`` (vectorize_clips' tensor)
+    with labels ``targets`` (non-zero = wake word).  rows / recs None: every network over every input; otherwise entry p is
+    network rows[p] over inputs[recs[p]].  Inputs are split into calls of at most ROWS_CALL_CLIPS clips and the calls'
+    statistics are added.  Returns a list of k DatasetStats, and with misses=True also a list of k sorted arrays of the
+    input indices network i misclassifies at ``miss_threshold``, as test_pool does."""
+    targets = np.ascontiguousarray(np.asarray(targets) != 0, dtype=np.uint8)
+    n_rec, k = int(inputs.shape[0]), len(state.hidden)
+    if targets.shape != (n_rec,):
+        raise ValueError('one target per input')
+    if (rows is None) != (recs is None):
+        raise ValueError('rows and recs come together')
+    if rows is not None:
+        rows, recs = np.ascontiguousarray(rows, dtype=np.int32), np.ascontiguousarray(recs, dtype=np.int64)
+        if rows.ndim != 1 or rows.shape != recs.shape:
+            raise ValueError('rows and recs must be 1-D arrays of one length')
+        if rows.size and (recs.min() < 0 or recs.max() >= n_rec or rows.min() < 0 or rows.max() >= k):
+            raise ValueError('rows must lie in [0, %d) and recs in [0, %d)' % (k, n_rec))
+    thr = np.unique(np.asarray(thresholds, np.float32))
+    n_thr = thr.shape[0]
+    count, hist, fit = np.zeros((k, 2), np.int64), np.zeros((k, 2, 2 * n_thr + 1), np.int64), np.zeros((k, 2, 3), np.int64)
+    missed = [[] for _ in range(k)]
+    kw = dict(thresholds=thr.astype(np.float64), per_entry=False, miss_threshold=miss_threshold if misses else None)
+    for c0 in range(0, n_rec, ROWS_CALL_CLIPS):
+        c1 = min(n_rec, c0 + ROWS_CALL_CLIPS)
+        if rows is None:
+            res = core.score_rows(inputs[c0:c1], targets[c0:c1], state.rows, state.weights, **kw)
+        else:
+            sel = np.nonzero((recs >= c0) & (recs < c1))[0]
+            res = core.score_rows(inputs[c0:c1], targets[c0:c1], state.rows, state.weights, rows[sel],
+                                  (recs[sel] - c0).astype(np.int32), **kw)
+        count += res['count'].cpu().numpy()
+        hist += res['hist'].cpu().numpy()
+        fit += res['fit'].cpu().numpy()
+        if misses:
+            q = res['misses'].cpu().numpy()
+            if rows is None:
+                for i, r in zip((q // (c1 - c0)).tolist(), (q % (c1 - c0)).tolist()):
+                    missed[i].append(c0 + r)
+            else:
+                for p in sel[q].tolist():
+                    missed[int(rows[p])].append(int(recs[p]))
+    stats = [DatasetStats(thr, count[i], hist[i], fit[i]) for i in range(k)]
+    if misses:
+        return stats, [np.asarray(sorted(m), np.int64) for m in missed]
+    return stats
+
+
+test_rows.__test__ = False        # not a pytest test, whatever module imports it
 
 
 def train(core: PreciseB200, state: TrainState, inputs, targets, rows=None, recs=None, epochs=10, batch_size=5000,

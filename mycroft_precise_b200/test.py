@@ -9,8 +9,11 @@ FOLDER has TrainData.from_folder's layout (precise/train_data.py:53-67): ``FOLDE
 (simulate.read_wav: 16-bit mono PCM at the model's sample rate, samples / 32767); an empty or unreadable file is skipped.
 Each clip is scored once, on its last buffer_t seconds, as the reference's vectorize + Runner.predict score it.
 
-All models are loaded into one model pool and scored over the clips in one pass (offline.test_pool), so every model must
-share the first one's front end and be of the fused family (hidden <= 24, feature size <= 16, no deltas).  For each model,
+Every model must share the first one's front end.  When all are of the fused family (hidden <= 24, feature size <= 16, no
+deltas), they are loaded into one model pool and scored over the clips in one pass (offline.test_pool).  When any has more
+than 24 units, every model must have at most 128 units, feature size <= 16 and no deltas: the clips are vectorized once
+(offline.vectorize_clips), the networks packed as weight rows (offline.TrainState.from_models) and scored from them in one
+pass (offline.test_rows).  Both print the same blocks.  For each model,
 in the order given, a ``=== <model file> ===`` heading is printed, then (unless ``-nf``) the false-positive and
 false-negative file lists, then Stats.counts_str and Stats.summary_str as precise-test prints them.  With
 ``--calc-threshold`` the ``Peak: ... mu, ... std`` line of precise-calc-threshold follows (offline.calc_threshold); the
@@ -62,22 +65,28 @@ def main(argv=None):
     args = ap.parse_args(argv)
 
     from .core import PreciseB200
-    from .offline import calc_threshold, test_pool
+    from .offline import TrainState, calc_threshold, test_pool, test_rows, vectorize_clips
     from .params import ListenerParams
     from .runner import _resolve_model
-    from .simulate import check_pool_models
+    from .simulate import check_pool_models, check_train_models
     models = [_resolve_model(m) for m in args.model]
     models = [(model, pr or ListenerParams()) for model, pr in models]
-    check_pool_models(args.model, models)
+    wide = any(m.hidden > 24 for m, _ in models)
+    (check_train_models if wide else check_pool_models)(args.model, models)
     model, pr = models[0]
     files, clips, targets = load_folder(args.folder, args.use_train, pr.sample_rate)
     core = PreciseB200(pr, hidden=model.hidden, device=args.device, activation=model.activation,
                        recurrent_activation=model.recurrent_activation)
-    core.set_pool(len(models))
-    for i, (m, p) in enumerate(models):
-        core.pool_load(i, m, p)
-    stats, missed = test_pool(core, clips, targets, np.arange(len(models), dtype=np.int32), thresholds=(args.threshold,),
-                              misses=True, miss_threshold=args.threshold)
+    kw = dict(thresholds=(args.threshold,), misses=True, miss_threshold=args.threshold)
+    if wide:
+        inputs = vectorize_clips(core, clips)
+        state = TrainState.from_models(core, [m for m, _ in models], [0] * len(models))
+        stats, missed = test_rows(core, state, inputs, targets, **kw)
+    else:
+        core.set_pool(len(models))
+        for i, (m, p) in enumerate(models):
+            core.pool_load(i, m, p)
+        stats, missed = test_pool(core, clips, targets, np.arange(len(models), dtype=np.int32), **kw)
     for name, st, miss in zip(args.model, stats, missed):
         print('=== %s ===' % name)
         if not args.no_filenames:
