@@ -474,10 +474,10 @@ int64_t pb_corpus_windows(const pb_config* cfg, int32_t schedule, int64_t chunk,
  *   d_raw [M][W_total] float32 (required), d_conf [M][W_total] float64, d_fired [M][W_total] uint8,
  *   d_activations, d_above [M][n_rec] int64, d_sum [M][n_rec] float64 -- all but d_raw optional (NULL).
  * Asynchronous on `stream`; h_offsets may be reused once the call returns.  The frames, window table and device offsets live
- * in a handle-owned workspace that grows on demand (about one row_stride-float row per hop of audio, 4 % of the int16
- * bytes at the defaults) and is freed by pb_destroy.  Two corpus calls on different CUDA streams are ordered by the library
- * (an event recorded after every call, failed ones included); the host waits for the previous call only when the workspace
- * must grow.
+ * in the handle's workspace, which every offline call shares (the corpus, labelled-clip, noise, generation and training
+ * calls); it grows on demand (about one row_stride-float row per hop of audio, 4 % of the int16 bytes at the defaults) and
+ * is freed by pb_destroy.  Two such calls on different CUDA streams are ordered by the library (an event recorded after
+ * every call, failed ones included); the host waits for the previous call only when the workspace must grow.
  * Profile slot 0 counts the MFCC kernels, slot 1 the network and trigger kernels.
  * At the aligned default geometry, recordings whose offset is a multiple of 8 samples (and d_pcm 16-byte aligned) take the
  * per-frame arithmetic of pb_mfcc's fast kernel, the others its generic kernel: frames are bit-identical to pb_mfcc of the
@@ -579,7 +579,7 @@ int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64_t* h_o
  *     (raw > (float)miss_threshold) != label, and the first min(total, miss_capacity) of them go to d_miss [miss_capacity] as
  *     i * n_rec + r (cross product) or p (pairs), in no particular order; the set is exact.
  *   - Every output is optional, d_raw included, but not all of them at once.  Without d_raw, raw of a batch (rows of at most
- *     256 MB, or 2^25 pairs) is kept in the corpus workspace, each batch followed by its statistics pass.
+ *     256 MB, or 2^25 pairs) is kept in the workspace, each batch followed by its statistics pass.
  *   - Reads and writes no stream state, pool assignment or detector; needs no slot-0 weights.  Asynchronous on `stream`,
  *     ordered against the corpus calls as pb_score_corpus (it shares their workspace).  Profile slot 0 counts K1, slot 1 the
  *     scans and statistics.  Every argument is checked before anything is enqueued, so a refused call changes no state.
@@ -623,13 +623,13 @@ int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offs
  *   - d_inputs [n_items][n_features][feature_size] (DEVICE, optional) receives vectorize(mixed clip), bit-identical to
  *     pb_vectorize_clips' rows of the mixed clips when each clip's last max_samples samples start at a multiple of 8 samples
  *     (the fast K1 at the default geometry, or the generic one under pb_debug_force_generic).
- * Asynchronous on `stream`; shares and orders itself against the corpus workspace as pb_vectorize_clips.  Every argument is
+ * Asynchronous on `stream`; shares the workspace and orders itself against the other offline calls as pb_vectorize_clips.  Every argument is
  * checked before anything is enqueued, so a refused call changes no buffer.
  * PB_ERR_INVALID: pb_vectorize_clips' refusals of the clips (null or decreasing offsets, divisor, max_samples < 1), a null
  * d_noise, n_noise < 1, noise_pos outside [0, n_noise), n_items outside [0, 2^31), null item or ratio arrays with
  * n_items > 0, an item outside [0, n_rec), a ratio that is NaN or outside [0, 1], both outputs null, an empty item with
  * d_inputs (empty items are fine with d_out alone: their clips are empty).  PB_ERR_UNSUPPORTED: d_inputs on a front end
- * outside the fused family.  PB_ERR_CUDA: the workspace cannot be allocated. */
+ * outside the fused family.  PB_ERR_CUDA: the workspace cannot be allocated (the handle is then unchanged). */
 int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec,
                  const int16_t* d_noise, int64_t n_noise, const int32_t* h_items, const double* h_ratios,
                  int64_t n_items, int64_t noise_pos, int32_t divisor, int64_t max_samples,
@@ -652,14 +652,14 @@ int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, i
  *     pb_score_corpus's PB_CORPUS_LISTENER windows with this chunk) after (c + 1) chunk samples of item i, for
  *     h_windows[w] = (i, c) (HOST int64 pairs [n_windows][2], c below the item's length / chunk), its samples read as
  *     x / divisor.  Each stream is framed from a multiple of 8 samples in a workspace, so the fast K1 applies.
- * Asynchronous on `stream`; shares and orders itself against the corpus workspace as pb_vectorize_clips.  Every argument is
+ * Asynchronous on `stream`; shares the workspace and orders itself against the other offline calls as pb_vectorize_clips.  Every argument is
  * checked before anything is enqueued, so a refused call changes no buffer.
  * PB_ERR_INVALID: offsets null, negative or decreasing, a null recording pointer with samples, counts outside [0, 2^31), a
  * null table with a positive count, divisor other than 32768 / 32767, chunk < 1, a segment's clip outside [-1, n_clips) or
  * samples outside it (silence with start != 0), a segment length outside [0, 2^62], an item's background outside [0, n_bg), a gain that is not finite and >= 0,
  * a length outside [0, the background's], segments outside [0, n_segs) or covering less than the length, a window's item
  * or chunk out of range, h_windows without d_inputs, both outputs null.  PB_ERR_UNSUPPORTED: d_inputs on a front end outside
- * the fused family.  PB_ERR_CUDA: the workspace cannot be allocated. */
+ * the fused family.  PB_ERR_CUDA: the workspace cannot be allocated (the handle is then unchanged). */
 typedef struct pb_gen_item {
     int32_t background;
     int32_t reserved;
@@ -781,9 +781,9 @@ int pb_train_wide_loss(pb_handle* h, const float* d_inputs, int64_t n_rec, const
  *     not), so two calls over consecutive parts of the clips add up to one call exactly when cut at a multiple of 16 clips.
  *   - Networks are split into gru_wide's fragments on the device in groups whose fragments stay under 256 MB (about 444 KB per
  *     network at H = 128, F = 16) and scanned by one launch per batch; without d_raw, raw of a batch (whole rows under
- *     256 MB, or 2^25 pairs) stays in the arena.
- *   - Reads and writes no stream state, pool slot or detector.  Asynchronous on `stream`; uses the training arena and orders
- *     itself against the corpus and training calls as pb_train.  Profile slot 1 counts the scans and statistics.  Every
+ *     256 MB, or 2^25 pairs) stays in the workspace.
+ *   - Reads and writes no stream state, pool slot or detector.  Asynchronous on `stream`; shares the workspace and orders
+ *     itself against the other offline calls as pb_train.  Profile slot 1 counts the scans and statistics.  Every
  *     argument is checked before anything is enqueued, so a refused call writes nothing.
  * PB_ERR_INVALID: a null handle, stride other than PB_TRAIN_STRIDE or PB_TRAIN_WIDE_STRIDE, k outside [0, 2^30), a null h_rows
  * (k > 0), hidden outside [1, 24] (PB_TRAIN_STRIDE) or [1, 128], an unknown activation code, n_rec outside [0, 2^31), every

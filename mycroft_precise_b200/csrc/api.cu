@@ -209,40 +209,13 @@ struct pb_handle {
     DevArray<long long> d_hist_start;  // [max_streams] history start
     std::vector<int> hist_row;       // host mirror of d_hist_row
     std::vector<int> hist_free;      // rows no stream owns
-    // recorded corpora (pb_score_corpus): a workspace that grows on demand and never shrinks
-    DevArray<float> d_cw_rows;       // the frame buffer (corpus.cuh)
-    DevArray<CorpusPair> d_cw_pairs; // K1's pair list
-    DevArray<long long> d_cw_starts; // [windows] first row of each window
-    DevArray<long long> d_cw_win0;   // [n_rec + 1] window prefix
-    DevArray<long long> d_cw_frow;   // [n_rec] row of each recording's frame 0
-    DevArray<CorpusRec> d_cw_recs;   // [n_rec + 1] recordings in pair-list order
-    cudaEvent_t corpus_ev = nullptr; // recorded after each corpus call; the next one waits on it before reusing the workspace
-    DevArray<int2> d_cp_groups;      // pb_score_corpus_pool: the scan's model groups, (pool slot, output row) entries
-    DevArray<int> d_cp_ids;          // ... the requested pool slots, one per output row
-    DevArray<float> d_cp_raw;        // ... raw of one batch of rows when the caller passes no d_raw (at most CORPUS_POOL_RAW_CAP bytes)
+    // offline calls (pb_score_corpus .. pb_score_rows, pb_vectorize_clips, pb_add_noise, pb_generate, the training calls): one
+    // workspace, carved per call (reserve_workspace), that grows on demand and never shrinks
+    DevArray<uint8_t> ws;
+    cudaEvent_t ws_ev = nullptr;     // recorded after each offline call; the next one waits on it before reusing the workspace
     int64_t corpus_pool_rows = 0;    // pb_debug_corpus_pool_rows: at most this many rows per batch (0 = the cap's)
     int corpus_pool_nm = 0;          // pb_debug_corpus_pool_scan: models per group (0 = CORPUS_POOL_NM)
     int corpus_pool_order = -1;      // ... grid order (-1 = CORPUS_POOL_GROUPS_FAST)
-    DevArray<int2> d_pp_pairs;       // pb_score_corpus_pairs: [n_pairs] (pool slot, recording); raw of a batch goes to d_cp_raw
-    DevArray<long long> d_pp_pw0;    // ... each batch's pair-window prefix, batch b's at [p0 + b, p1 + b]
-    DevArray<long long> d_pp_starts; // ... [batch pair-windows] the batch's window table
-    DevArray<PairTile> d_pp_tiles;   // ... the batch's scan tiles, one activation class after the other
-    DevArray<float> d_ds_thr;        // pb_score_dataset: the histogram's float32 thresholds
-    DevArray<uint8_t> d_ds_targets;  // ... [n_rec] the recordings' labels
-    DevArray<uint8_t> d_tr_ws;       // pb_train(_wide) / pb_train(_wide)_loss: one arena, carved per call (at most TRAIN_WS_CAP
-                                     // bytes per group, plus TW_STATE_CAP of tile state for the wide calls)
-    DevArray<NoiseItem> d_nz_items;  // pb_add_noise: [n_items] the items
-    DevArray<long long> d_nz_seg0;   // ... [n_items + 1] each item's first segment
-    DevArray<unsigned long long> d_nz_sums;  // ... [n_items][2] (sum x^2, sum n^2)
-    DevArray<int16_t> d_nz_pcm;      // ... the mixed clips' cropped tails, each at a multiple of 8 samples (K1's recordings)
-    DevArray<GenRec> d_gen_recs;     // pb_generate: [n_recs] the recordings whose sums of squares the mix needs
-    DevArray<long long> d_gen_rseg0; // ... [n_recs + 1] each recording's first CTA of the sums
-    DevArray<unsigned long long> d_gen_sums;  // ... [n_recs] their sums of squares
-    DevArray<GenItem> d_gen_items;   // ... [n_items]
-    DevArray<long long> d_gen_tile0; // ... [n_items + 1] each item's first CTA of the mix
-    DevArray<GenSeg> d_gen_segs;     // ... each item's own copy of the segments covering it
-    DevArray<long long> d_gen_wins;  // ... [n_windows] the chosen windows' places in the window table
-    DevArray<int16_t> d_gen_pcm;     // ... the generated streams, each at a multiple of 8 samples (K1's recordings)
     int64_t corpus_pairs_batch = 0;  // pb_debug_corpus_pairs_batch: at most this many pair-windows per batch (0 = CORPUS_PAIRS_BATCH)
     int32_t rows_group_nets = 0;     // pb_debug_rows_groups: at most this many networks per group (0 = the 256 MB cap's)
     int64_t rows_batch_entries = 0;  // ... at most this many entries per batch (0 = ROWS_RAW_CAP's, or ROWS_PAIRS_BATCH)
@@ -296,7 +269,7 @@ struct pb_handle {
         for (auto& p : prof)
             for (auto e : p.ev) cudaEventDestroy(e);
         if (route_ev) cudaEventDestroy(route_ev);
-        if (corpus_ev) cudaEventDestroy(corpus_ev);
+        if (ws_ev) cudaEventDestroy(ws_ev);
         if (pool_ev) cudaEventDestroy(pool_ev);
     }
 };
@@ -1725,11 +1698,52 @@ PB_API int64_t pb_corpus_windows(const pb_config* cfg, int32_t schedule, int64_t
     return rc != PB_OK ? rc : corpus_windows(*cfg, schedule, chunk, n_samples);
 }
 
-// Grows a workspace array to n elements.  The replaced array is freed only after the previous corpus call is done with it.
-template <typename T>
-static cudaError_t corpus_grow(const DevArray<T>& a, size_t n, DevArray<T>& fresh) {
-    if (a.size() >= n) return cudaSuccess;
-    return fresh.alloc(n + n / 4);
+constexpr size_t WS_ALIGN = 256;
+
+// Carves typed arrays out of the workspace, each at a multiple of WS_ALIGN bytes (a null base only measures).
+struct Carve {
+    uint8_t* base;
+    size_t at = 0;
+    template <typename T> T* take(size_t n) {
+        at = (at + WS_ALIGN - 1) / WS_ALIGN * WS_ALIGN;
+        T* p = base ? reinterpret_cast<T*>(base + at) : nullptr;
+        at += std::max<size_t>(n, 1) * sizeof(T);
+        return p;
+    }
+};
+
+// Reserves the workspace for one offline call and carves it: layout(Carve&) takes the call's arrays, first from a null base to
+// measure them, then from the workspace.  The workspace grows to the request plus a quarter; the new memory is allocated
+// before the old is freed, so a failed allocation leaves the handle unchanged, and the host waits for the previous call only
+// when it replaces memory that call may still use.  Then s waits for the previous call, whatever its stream.
+template <typename L>
+static int reserve_workspace(pb_handle* h, cudaStream_t s, L&& layout) {
+    Carve m{nullptr};
+    layout(m);
+    if (!h->ws_ev) CK(cudaEventCreateWithFlags(&h->ws_ev, cudaEventDisableTiming));
+    if (h->ws.size() < m.at) {
+        DevArray<uint8_t> fresh;
+        const cudaError_t e = fresh.alloc(m.at + m.at / 4);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(PB_ERR_CUDA, "workspace allocation failed (%zu bytes): %s", m.at, cudaGetErrorString(e));
+        }
+        CK(cudaEventSynchronize(h->ws_ev));
+        h->ws = std::move(fresh);
+    }
+    CK(cudaStreamWaitEvent(s, h->ws_ev, 0));
+    Carve c{h->ws.get()};
+    layout(c);
+    return PB_OK;
+}
+
+// Records ws_ev after an offline call's work, even when a launch failed, so the next call orders itself after whatever this
+// one queued.
+static int corpus_done(pb_handle* h, cudaStream_t s, int rc) {
+    const cudaError_t er = cudaEventRecord(h->ws_ev, s);
+    if (rc != PB_OK) return rc;
+    if (er != cudaSuccess) return fail(PB_ERR_CUDA, "cudaEventRecord failed: %s", cudaGetErrorString(er));
+    return PB_OK;
 }
 
 // The checks every corpus call shares (pb_score_corpus, pb_score_corpus_pool); raw_required: d_raw may not be null.
@@ -1762,12 +1776,13 @@ struct CorpusPlan {
 // crop > 0 (labelled clips, vectorization.py:73-82): each recording is its last `crop` samples, framed from the first of
 // them, and has one window, the n_features rows ending at its last frame (row 0's zeros when it has no frame).
 // h_lens (pb_add_noise's workspace, where recordings have gaps between them): recording r is h_lens[r] samples from
-// h_offsets[r]; without it, recording r ends where r + 1 starts.
-static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t schedule,
+// h_offsets[r]; without it, recording r ends where r + 1 starts.  aligned: the audio starts at a multiple of 16 bytes, so a
+// recording at a multiple of 8 samples may take the fast K1.
+static CorpusPlan corpus_plan(const pb_handle* h, bool aligned, const int64_t* h_offsets, int64_t n_rec, int32_t schedule,
                               int64_t chunk, int64_t crop = 0, const int64_t* h_lens = nullptr) {
     const pb_config& c = h->cfg;
     const int T = c.n_features;
-    const bool fast = h->fast_ok && !h->force_generic && (uintptr_t)d_pcm % 16 == 0;
+    const bool fast = h->fast_ok && !h->force_generic && aligned;
     CorpusPlan p;
     p.win0.resize((size_t)n_rec + 1);
     p.frow.resize((size_t)n_rec);
@@ -1795,127 +1810,79 @@ static CorpusPlan corpus_plan(const pb_handle* h, const int16_t* d_pcm, const in
     return p;
 }
 
-// Sizes of pb_score_corpus_pool's and pb_score_corpus_pairs's own workspace arrays (0 for pb_score_corpus).
-struct CorpusPoolSizes {
-    size_t groups = 0, ids = 0, raw = 0;
-    size_t pairs = 0, pw0 = 0, starts = 0, tiles = 0;
-    size_t thr = 0, targets = 0;     // pb_score_dataset
+// A corpus call's part of the workspace, sized by its plan.
+struct CorpusWs {
+    float* rows;                     // the frame buffer (corpus.cuh)
+    CorpusPair* pairs;               // K1's pair list
+    long long* starts;               // [windows] first row of each window
+    long long* win0;                 // [n_rec + 1] window prefix
+    long long* frow;                 // [n_rec] row of each recording's frame 0
+    CorpusRec* recs;                 // [n_rec + 1] recordings in pair-list order
 };
 
-// Grows the workspace for plan p, all at once, so that a failed allocation leaves the handle as it was; then orders s after
-// the previous corpus call.
-static int corpus_reserve(pb_handle* h, const CorpusPlan& p, int64_t n_rec, const CorpusPoolSizes& ps, cudaStream_t s) {
-    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
-    DevArray<float> f_rows, f_raw; DevArray<CorpusPair> f_pairs; DevArray<long long> f_starts, f_win0, f_frow; DevArray<CorpusRec> f_recs;
-    DevArray<int2> f_groups; DevArray<int> f_ids;
-    DevArray<int2> f_ppairs; DevArray<long long> f_pw0, f_pstarts; DevArray<PairTile> f_tiles;
-    DevArray<float> f_thr; DevArray<uint8_t> f_targets;
-    cudaError_t e = corpus_grow(h->d_cw_rows, (size_t)p.rows * h->row_stride, f_rows);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cw_pairs, (size_t)p.n_pairs, f_pairs);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cw_starts, (size_t)p.W, f_starts);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cw_win0, (size_t)n_rec + 1, f_win0);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cw_frow, (size_t)n_rec, f_frow);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cw_recs, p.recs.size(), f_recs);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cp_groups, ps.groups, f_groups);
-    if (e == cudaSuccess) e = corpus_grow(h->d_cp_ids, ps.ids, f_ids);
-    if (e == cudaSuccess && h->d_cp_raw.size() < ps.raw) e = f_raw.alloc(ps.raw);     // capped: no headroom
-    if (e == cudaSuccess) e = corpus_grow(h->d_pp_pairs, ps.pairs, f_ppairs);
-    if (e == cudaSuccess) e = corpus_grow(h->d_pp_pw0, ps.pw0, f_pw0);
-    if (e == cudaSuccess && h->d_pp_starts.size() < ps.starts) e = f_pstarts.alloc(ps.starts);   // capped: no headroom
-    if (e == cudaSuccess) e = corpus_grow(h->d_pp_tiles, ps.tiles, f_tiles);
-    if (e == cudaSuccess) e = corpus_grow(h->d_ds_thr, ps.thr, f_thr);
-    if (e == cudaSuccess) e = corpus_grow(h->d_ds_targets, ps.targets, f_targets);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return fail(PB_ERR_CUDA, "corpus workspace allocation failed (%lld frame rows, %lld windows): %s", p.rows, p.W, cudaGetErrorString(e));
-    }
-    const bool grows = f_rows.get() || f_pairs.get() || f_starts.get() || f_win0.get() || f_frow.get() || f_recs.get() ||
-                       f_groups.get() || f_ids.get() || f_raw.get() || f_ppairs.get() || f_pw0.get() || f_pstarts.get() ||
-                       f_tiles.get() || f_thr.get() || f_targets.get();
-    if (grows) CK(cudaEventSynchronize(h->corpus_ev));            // the previous call may still read what is replaced
-    if (f_rows.get()) h->d_cw_rows = std::move(f_rows);
-    if (f_pairs.get()) h->d_cw_pairs = std::move(f_pairs);
-    if (f_starts.get()) h->d_cw_starts = std::move(f_starts);
-    if (f_win0.get()) h->d_cw_win0 = std::move(f_win0);
-    if (f_frow.get()) h->d_cw_frow = std::move(f_frow);
-    if (f_recs.get()) h->d_cw_recs = std::move(f_recs);
-    if (f_groups.get()) h->d_cp_groups = std::move(f_groups);
-    if (f_ids.get()) h->d_cp_ids = std::move(f_ids);
-    if (f_raw.get()) h->d_cp_raw = std::move(f_raw);
-    if (f_ppairs.get()) h->d_pp_pairs = std::move(f_ppairs);
-    if (f_pw0.get()) h->d_pp_pw0 = std::move(f_pw0);
-    if (f_pstarts.get()) h->d_pp_starts = std::move(f_pstarts);
-    if (f_tiles.get()) h->d_pp_tiles = std::move(f_tiles);
-    if (f_thr.get()) h->d_ds_thr = std::move(f_thr);
-    if (f_targets.get()) h->d_ds_targets = std::move(f_targets);
-    CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));                      // a corpus call on another stream may still use it
-    return PB_OK;
+static CorpusWs corpus_ws(Carve& c, const pb_handle* h, const CorpusPlan& p) {
+    CorpusWs w;
+    w.rows = c.take<float>((size_t)p.rows * h->row_stride); w.pairs = c.take<CorpusPair>((size_t)p.n_pairs);
+    w.starts = c.take<long long>((size_t)p.W); w.win0 = c.take<long long>(p.win0.size());
+    w.frow = c.take<long long>(p.frow.size()); w.recs = c.take<CorpusRec>(p.recs.size());
+    return w;
 }
 
 // K1 of a corpus call: the plan's device copies, the frame buffer and the window table (profile slot 0).
-static int corpus_k1(pb_handle* h, const CorpusPlan& p, const int16_t* d_pcm, int64_t n_rec, int32_t divisor, int32_t schedule,
-                     int64_t chunk, cudaStream_t s) {
+static int corpus_k1(pb_handle* h, const CorpusPlan& p, const CorpusWs& w, const int16_t* d_pcm, int64_t n_rec, int32_t divisor,
+                     int32_t schedule, int64_t chunk, cudaStream_t s) {
     const pb_config& c = h->cfg;
-    CK(cudaMemcpyAsync(h->d_cw_win0.get(), p.win0.data(), p.win0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->d_cw_frow.get(), p.frow.data(), p.frow.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->d_cw_recs.get(), p.recs.data(), p.recs.size() * sizeof(CorpusRec), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(w.win0, p.win0.data(), p.win0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(w.frow, p.frow.data(), p.frow.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(w.recs, p.recs.data(), p.recs.size() * sizeof(CorpusRec), cudaMemcpyHostToDevice, s));
     if (p.n_pairs == 0 && p.W == 0) return PB_OK;
-    float* frames = h->d_cw_rows.get();
+    float* frames = w.rows;
     ProfScope ps(h, 0, s);
     CK(cudaMemsetAsync(frames, 0, (size_t)p.rows * h->row_stride * sizeof(float), s));
     const float inv = 1.0f / (float)divisor, scale = inv * inv / (float)c.n_fft;
     if (p.n_pairs > 0) {
-        corpus_pairs_kernel<<<(unsigned)((p.n_pairs + 255) / 256), 256, 0, s>>>(h->d_cw_recs.get(), (int)p.recs.size() - 1, p.n_pairs,
-                                                                              c.hop_samples, h->d_cw_pairs.get());
+        corpus_pairs_kernel<<<(unsigned)((p.n_pairs + 255) / 256), 256, 0, s>>>(w.recs, (int)p.recs.size() - 1, p.n_pairs,
+                                                                              c.hop_samples, w.pairs);
         CK(cudaGetLastError());
     }
     if (p.n_fast_pairs > 0) {
         const int grid = (int)std::min<int64_t>((p.n_fast_pairs + K1F_WARPS - 1) / K1F_WARPS, (int64_t)h->sm_count * 4);
-        mfcc_fast_corpus_kernel<<<grid, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, h->d_cw_pairs.get(), p.n_fast_pairs, c.hop_samples, scale,
+        mfcc_fast_corpus_kernel<<<grid, K1F_THREADS, h->k1_fast_smem, s>>>(d_pcm, w.pairs, p.n_fast_pairs, c.hop_samples, scale,
                                                                           mel_tables(h), fast_tables(h), frames, h->row_stride);
         CK(cudaGetLastError());
     }
     if (p.n_pairs > p.n_fast_pairs) {
         const int64_t tiles = (p.n_pairs - p.n_fast_pairs + K1_TILE / 2 - 1) / (K1_TILE / 2);
         const int grid = (int)std::min<int64_t>(tiles, (int64_t)h->sm_count * 4);
-        mfcc_corpus_kernel<<<grid, K1_THREADS, h->k1_batch_smem, s>>>(d_pcm, h->d_cw_pairs.get() + p.n_fast_pairs, p.n_pairs - p.n_fast_pairs,
+        mfcc_corpus_kernel<<<grid, K1_THREADS, h->k1_batch_smem, s>>>(d_pcm, w.pairs + p.n_fast_pairs, p.n_pairs - p.n_fast_pairs,
                                                                      c.hop_samples, h->used, scale, mel_tables(h), frames, h->row_stride);
         CK(cudaGetLastError());
     }
     if (!p.starts.empty()) {
-        CK(cudaMemcpyAsync(h->d_cw_starts.get(), p.starts.data(), p.starts.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(w.starts, p.starts.data(), p.starts.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
     } else if (p.W > 0) {
-        corpus_windows_kernel<<<(unsigned)((p.W + 255) / 256), 256, 0, s>>>(h->d_cw_win0.get(), h->d_cw_frow.get(), (int)n_rec, p.W, schedule, chunk,
-                                                                          h->rel_window, c.hop_samples, c.n_features, h->d_cw_starts.get());
+        corpus_windows_kernel<<<(unsigned)((p.W + 255) / 256), 256, 0, s>>>(w.win0, w.frow, (int)n_rec, p.W, schedule, chunk,
+                                                                          h->rel_window, c.hop_samples, c.n_features, w.starts);
         CK(cudaGetLastError());
     }
     return PB_OK;
 }
 
 // Predict-mode input of a corpus call's scans: the windows in place in the frame buffer.
-static K2In corpus_k2in(const pb_handle* h) {
+static K2In corpus_k2in(const pb_handle* h, const CorpusWs& w) {
     K2In in{};
-    in.inputs = h->d_cw_rows.get(); in.starts = h->d_cw_starts.get(); in.row_stride = h->row_stride;
+    in.inputs = w.rows; in.starts = w.starts; in.row_stride = h->row_stride;
     in.T = h->cfg.n_features; in.F_base = h->n_out; in.use_delta = h->cfg.use_delta;
     return in;
 }
 
 // The trigger pass's fields shared by every row.
-static CorpusTrig corpus_trig(const pb_handle* h, int64_t n_rec, int64_t W, int32_t schedule, int64_t chunk, double threshold) {
+static CorpusTrig corpus_trig(const CorpusWs& w, int64_t n_rec, int64_t W, int32_t schedule, int64_t chunk, double threshold) {
     CorpusTrig t{};
-    t.win0 = h->d_cw_win0.get(); t.W = W; t.n_rec = (int)n_rec; t.schedule = schedule;
+    t.win0 = w.win0; t.W = W; t.n_rec = (int)n_rec; t.schedule = schedule;
     t.hot_f = (float)(1.0 - threshold); t.above_f = (float)threshold;
     t.sim_reset = trigger_reset(chunk);
     return t;
-}
-
-// Records corpus_ev after the call's work, even when a launch failed, so the next call orders itself after whatever this
-// one queued.
-static int corpus_done(pb_handle* h, cudaStream_t s, int rc) {
-    const cudaError_t er = cudaEventRecord(h->corpus_ev, s);
-    if (rc != PB_OK) return rc;
-    if (er != cudaSuccess) return fail(PB_ERR_CUDA, "cudaEventRecord failed: %s", cudaGetErrorString(er));
-    return PB_OK;
 }
 
 PB_API int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
@@ -1929,19 +1896,20 @@ PB_API int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
     const int M = (int)h->models.size();
-    const CorpusPlan p = corpus_plan(h, d_pcm, h_offsets, n_rec, schedule, chunk);
+    const CorpusPlan p = corpus_plan(h, (uintptr_t)d_pcm % 16 == 0, h_offsets, n_rec, schedule, chunk);
     const long long W = p.W;
-    rc = corpus_reserve(h, p, n_rec, CorpusPoolSizes{}, s);
+    CorpusWs w;
+    rc = reserve_workspace(h, s, [&](Carve& c) { w = corpus_ws(c, h, p); });
     if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        rc = corpus_k1(h, p, d_pcm, n_rec, divisor, schedule, chunk, s);
+        rc = corpus_k1(h, p, w, d_pcm, n_rec, divisor, schedule, chunk, s);
         if (rc != PB_OK) return rc;
         ProfScope ps(h, 1, s);
         if (W > 0) {
             // every model scans the windows in place.  One model runs pb_predict's dispatch (the warp-per-window kernel up to
             // 8 192 windows for the default network); a bank runs its fused family in one predict-mode bank launch, the others
             // one launch each
-            const K2In in = corpus_k2in(h);
+            const K2In in = corpus_k2in(h, w);
             BankParams P{};
             int nm = 0;
             for (int m = 0; m < M; ++m) {
@@ -1962,7 +1930,7 @@ PB_API int pb_score_corpus(pb_handle* h, const int16_t* d_pcm, const int64_t* h_
             }
         }
         if (d_fired || d_activations || d_above || d_sum) {
-            CorpusTrig t = corpus_trig(h, n_rec, W, schedule, chunk, threshold);
+            CorpusTrig t = corpus_trig(w, n_rec, W, schedule, chunk, threshold);
             t.raw = d_raw; t.conf = d_conf; t.fired = d_fired; t.activations = d_activations; t.above = d_above; t.sum = d_sum;
             CorpusBankDP dp{};
             for (int m = 0; m < M; ++m) {
@@ -2036,6 +2004,18 @@ static void pool_corpus_groups(const pb_handle* h, const int32_t* h_model_ids, i
     g0[2 * n_batches] = (int64_t)groups.size() / NM;
 }
 
+// Refuses a pool slot id outside [0, max_models) or naming an empty slot; `noun` names the ids' places in the messages.
+static int check_pool_ids(const pb_handle* h, const int32_t* ids, int64_t n, const char* noun) {
+    for (int64_t i = 0; i < n; ++i) {
+        const int32_t m = ids[i];
+        if (m < 0 || m >= h->pool_models)
+            return fail(PB_ERR_INVALID, "model id %d (%s %lld) outside [0, max_models = %d)", m, noun, (long long)i, h->pool_models);
+        if (h->pool_cd_of[m] == h->pool_cd.end())
+            return fail(PB_ERR_INVALID, "pool slot %d (%s %lld) holds no model: pb_pool_load it first", m, noun, (long long)i);
+    }
+    return PB_OK;
+}
+
 PB_API int pb_debug_corpus_pool_rows(pb_handle* h, int64_t rows) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (rows < 0) return fail(PB_ERR_INVALID, "rows = %lld is negative", (long long)rows);
@@ -2064,17 +2044,12 @@ PB_API int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_
     if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
     if (k < 0) return fail(PB_ERR_INVALID, "k = %lld is negative", (long long)k);
     if (k > 0 && !h_model_ids) return fail(PB_ERR_INVALID, "null h_model_ids");
-    for (int64_t i = 0; i < k; ++i) {
-        const int32_t m = h_model_ids[i];
-        if (m < 0 || m >= h->pool_models)
-            return fail(PB_ERR_INVALID, "model id %d (entry %lld) outside [0, max_models = %d)", m, (long long)i, h->pool_models);
-        if (h->pool_cd_of[m] == h->pool_cd.end())
-            return fail(PB_ERR_INVALID, "pool slot %d (entry %lld) holds no model: pb_pool_load it first", m, (long long)i);
-    }
+    rc = check_pool_ids(h, h_model_ids, k, "entry");
+    if (rc != PB_OK) return rc;
     if (n_rec == 0 || k == 0) return PB_OK;
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    const CorpusPlan p = corpus_plan(h, d_pcm, h_offsets, n_rec, schedule, chunk);
+    const CorpusPlan p = corpus_plan(h, (uintptr_t)d_pcm % 16 == 0, h_offsets, n_rec, schedule, chunk);
     const long long W = p.W;
     // rows per batch: all of them when the caller's d_raw holds raw (or no trigger pass needs it), else as many as the cap holds
     const bool own_raw = !d_raw && reduce && W > 0;
@@ -2090,30 +2065,36 @@ PB_API int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_
     std::vector<int2> groups;
     std::vector<int64_t> g0;
     pool_corpus_groups(h, h_model_ids, k, rows, NM, groups, g0);
-    CorpusPoolSizes ps;
-    ps.groups = groups.size();
-    ps.ids = (size_t)k;
-    ps.raw = own_raw ? (size_t)(rows * W) : 0;
-    rc = corpus_reserve(h, p, n_rec, ps, s);
+    // the scan's model groups, (pool slot, output row) entries; the requested slots, one per output row; raw of one batch of
+    // rows when the caller passes no d_raw
+    CorpusWs w;
+    int2* d_groups;
+    int* d_ids;
+    float* d_own_raw;
+    rc = reserve_workspace(h, s, [&](Carve& c) {
+        w = corpus_ws(c, h, p);
+        d_groups = c.take<int2>(groups.size()); d_ids = c.take<int>((size_t)k);
+        d_own_raw = c.take<float>(own_raw ? (size_t)(rows * W) : 0);
+    });
     if (rc != PB_OK) return rc;
     const int order = h->corpus_pool_order >= 0 ? h->corpus_pool_order : CORPUS_POOL_GROUPS_FAST;
     auto launch = [&]() -> int {
-        rc = corpus_k1(h, p, d_pcm, n_rec, divisor, schedule, chunk, s);
+        rc = corpus_k1(h, p, w, d_pcm, n_rec, divisor, schedule, chunk, s);
         if (rc != PB_OK) return rc;
         if (W == 0 && !reduce) return PB_OK;
-        CK(cudaMemcpyAsync(h->d_cp_groups.get(), groups.data(), groups.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_cp_ids.get(), h_model_ids, (size_t)k * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_groups, groups.data(), groups.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_ids, h_model_ids, (size_t)k * sizeof(int32_t), cudaMemcpyHostToDevice, s));
         ProfScope ps(h, 1, s);
-        const K2In in = corpus_k2in(h);
+        const K2In in = corpus_k2in(h, w);
         for (int64_t b = 0; b < n_batches; ++b) {
             const int64_t b0 = b * rows, nb = std::min<int64_t>(k, b0 + rows) - b0;
-            float* raw = own_raw ? h->d_cp_raw.get() : d_raw ? d_raw + b0 * W : nullptr;
+            float* raw = own_raw ? d_own_raw : d_raw ? d_raw + b0 * W : nullptr;
             if (W > 0) {
                 PoolCorpus c{};
                 c.slots = h->d_pool_slots.get(); c.n_tiles = (W + 63) / 64; c.raw = raw;
                 c.conf = d_conf ? d_conf + b0 * W : nullptr; c.W = W; c.groups_fast = order;
                 for (int ka = 0; ka < 2; ++ka) {
-                    c.groups = h->d_cp_groups.get() + g0[2 * b + ka] * NM;
+                    c.groups = d_groups + g0[2 * b + ka] * NM;
                     c.n_groups = g0[2 * b + ka + 1] - g0[2 * b + ka];
                     rc = launch_pool_corpus_nm(NM, split && ka == 1, c, in, s);
                     if (rc != PB_OK) return rc;
@@ -2123,14 +2104,14 @@ PB_API int pb_score_corpus_pool(pb_handle* h, const int16_t* d_pcm, const int64_
             // rows b0 .. b0 + nb - 1, at most 65 535 per launch (gridDim.y)
             for (int64_t y0 = 0; y0 < nb; y0 += 65535) {
                 const int64_t r0 = b0 + y0, ny = std::min<int64_t>(65535, nb - y0);
-                CorpusTrig t = corpus_trig(h, n_rec, W, schedule, chunk, threshold);
+                CorpusTrig t = corpus_trig(w, n_rec, W, schedule, chunk, threshold);
                 t.raw = raw ? raw + y0 * W : nullptr;
                 t.conf = d_conf ? d_conf + r0 * W : nullptr;
                 t.fired = d_fired ? d_fired + r0 * W : nullptr;
                 t.activations = d_activations ? d_activations + r0 * n_rec : nullptr;
                 t.above = d_above ? d_above + r0 * n_rec : nullptr;
                 t.sum = d_sum ? d_sum + r0 * n_rec : nullptr;
-                CorpusPoolDP dp{h->d_pool_slots.get(), h->d_cp_ids.get() + r0, trigger_reset(2 * chunk)};
+                CorpusPoolDP dp{h->d_pool_slots.get(), d_ids + r0, trigger_reset(2 * chunk)};
                 const unsigned per = CORPUS_TRIG_THREADS / 32;
                 corpus_trigger_kernel<<<dim3((unsigned)((n_rec + per - 1) / per), (unsigned)ny), CORPUS_TRIG_THREADS, 0, s>>>(t, dp);
                 CK(cudaGetLastError());
@@ -2176,6 +2157,22 @@ static int64_t pair_tiles(const pb_handle* h, const std::vector<int2>& pairs, co
     return n_keras;
 }
 
+// The pair tables pb_score_corpus_pairs and pb_score_dataset (by pairs) carve after their CorpusWs.
+struct PairsWs {
+    int2* pairs;                     // [n_pairs] (pool slot, recording), or (row, recording) for pb_score_dataset
+    long long* pw0;                  // each batch's pair-window prefix
+    long long* starts;               // the largest batch's window table
+    PairTile* tiles;                 // ... its scan tiles, one activation class after the other
+    float* raw;                      // ... its raw when the caller passes no d_raw
+};
+
+static PairsWs pairs_ws(Carve& c, size_t pairs, size_t pw0, size_t starts, size_t tiles, size_t raw) {
+    PairsWs w;
+    w.pairs = c.take<int2>(pairs); w.pw0 = c.take<long long>(pw0); w.starts = c.take<long long>(starts);
+    w.tiles = c.take<PairTile>(tiles); w.raw = c.take<float>(raw);
+    return w;
+}
+
 PB_API int pb_debug_corpus_pairs_batch(pb_handle* h, int64_t windows) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
     if (windows < 0) return fail(PB_ERR_INVALID, "windows = %lld is negative", (long long)windows);
@@ -2198,12 +2195,10 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
     if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
     if (n_pairs < 0 || n_pairs > INT32_MAX) return fail(PB_ERR_INVALID, "n_pairs = %lld outside [0, 2^31)", (long long)n_pairs);
     if (n_pairs > 0 && (!h_pair_models || !h_pair_recs)) return fail(PB_ERR_INVALID, "null h_pair_models or h_pair_recs");
+    rc = check_pool_ids(h, h_pair_models, n_pairs, "pair");
+    if (rc != PB_OK) return rc;
     for (int64_t i = 0; i < n_pairs; ++i) {
-        const int32_t m = h_pair_models[i], r = h_pair_recs[i];
-        if (m < 0 || m >= h->pool_models)
-            return fail(PB_ERR_INVALID, "model id %d (pair %lld) outside [0, max_models = %d)", m, (long long)i, h->pool_models);
-        if (h->pool_cd_of[m] == h->pool_cd.end())
-            return fail(PB_ERR_INVALID, "pool slot %d (pair %lld) holds no model: pb_pool_load it first", m, (long long)i);
+        const int32_t r = h_pair_recs[i];
         if (r < 0 || r >= n_rec)
             return fail(PB_ERR_INVALID, "recording id %d (pair %lld) outside [0, n_rec = %lld)", r, (long long)i, (long long)n_rec);
     }
@@ -2217,7 +2212,7 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
         if (hits) CK(cudaMemsetAsync(d_n_hits, 0, sizeof(unsigned long long), s));
         return PB_OK;
     }
-    const CorpusPlan plan = corpus_plan(h, d_pcm, h_offsets, n_rec, schedule, chunk);
+    const CorpusPlan plan = corpus_plan(h, (uintptr_t)d_pcm % 16 == 0, h_offsets, n_rec, schedule, chunk);
     // pair p's windows are P[p] .. P[p + 1] - 1 of every per-window output
     std::vector<long long> P((size_t)n_pairs + 1);
     std::vector<int2> pairs((size_t)n_pairs);
@@ -2253,40 +2248,39 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
     const int64_t n_batches = (int64_t)bp.size() - 1;
     const long long Wp = P[n_pairs];
     const bool own_raw = !d_raw && (reduce || hits) && Wp > 0;
-    CorpusPoolSizes ps;
-    ps.raw = own_raw ? (size_t)max_bw : 0;
-    ps.pairs = (size_t)n_pairs;
-    ps.pw0 = pw0.size();
-    ps.starts = (size_t)max_bw;
-    ps.tiles = (size_t)max_tiles;
-    rc = corpus_reserve(h, plan, n_rec, ps, s);
+    // batch b's pair-window prefix is pw0[p0 + b .. p1 + b]
+    CorpusWs w;
+    PairsWs pw;
+    rc = reserve_workspace(h, s, [&](Carve& c) {
+        w = corpus_ws(c, h, plan);
+        pw = pairs_ws(c, (size_t)n_pairs, pw0.size(), (size_t)max_bw, (size_t)max_tiles, own_raw ? (size_t)max_bw : 0);
+    });
     if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        rc = corpus_k1(h, plan, d_pcm, n_rec, divisor, schedule, chunk, s);
+        rc = corpus_k1(h, plan, w, d_pcm, n_rec, divisor, schedule, chunk, s);
         if (rc != PB_OK) return rc;
         if (hits) CK(cudaMemsetAsync(d_n_hits, 0, sizeof(unsigned long long), s));
-        CK(cudaMemcpyAsync(h->d_pp_pairs.get(), pairs.data(), pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_pp_pw0.get(), pw0.data(), pw0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(pw.pairs, pairs.data(), pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(pw.pw0, pw0.data(), pw0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
         ProfScope prof(h, 1, s);
-        const K2In in = corpus_k2in(h);
+        const K2In in = corpus_k2in(h, w);
         const uint4* slots = h->d_pool_slots.get();
         std::vector<PairTile> tiles;
         for (int64_t b = 0; b < n_batches; ++b) {
             const int64_t p0 = bp[b], p1 = bp[b + 1], nb = p1 - p0;
             const long long q0 = P[p0], nw = P[p1] - q0;
-            const long long* bpw0 = h->d_pp_pw0.get() + p0 + b;
-            const int2* bpairs = h->d_pp_pairs.get() + p0;
-            float* raw = own_raw ? h->d_cp_raw.get() : d_raw ? d_raw + q0 : nullptr;
+            const long long* bpw0 = pw.pw0 + p0 + b;
+            const int2* bpairs = pw.pairs + p0;
+            float* raw = own_raw ? pw.raw : d_raw ? d_raw + q0 : nullptr;
             double* conf = d_conf ? d_conf + q0 : nullptr;
             if (nw > 0) {
-                pairs_windows_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(bpw0, bpairs, (int)nb, nw, h->d_cw_win0.get(),
-                                                                                 h->d_cw_starts.get(), h->d_pp_starts.get());
+                pairs_windows_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(bpw0, bpairs, (int)nb, nw, w.win0, w.starts, pw.starts);
                 CK(cudaGetLastError());
                 const int64_t n_keras = pair_tiles(h, pairs, P, p0, p1, tiles);
-                CK(cudaMemcpyAsync(h->d_pp_tiles.get(), tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
+                CK(cudaMemcpyAsync(pw.tiles, tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
                 PairsCorpus c{};
-                c.slots = slots; c.starts = h->d_pp_starts.get(); c.raw = raw; c.conf = conf;
-                c.tiles = h->d_pp_tiles.get(); c.n_tiles = n_keras;
+                c.slots = slots; c.starts = pw.starts; c.raw = raw; c.conf = conf;
+                c.tiles = pw.tiles; c.n_tiles = n_keras;
                 rc = launch_pairs_corpus<true>(c, in, s);
                 if (rc != PB_OK) return rc;
                 c.tiles += n_keras; c.n_tiles = (int64_t)tiles.size() - n_keras;
@@ -2295,7 +2289,7 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
             }
             if (reduce) {
                 // one "recording" per pair of the batch, one row
-                CorpusTrig t = corpus_trig(h, nb, nw, schedule, chunk, threshold);
+                CorpusTrig t = corpus_trig(w, nb, nw, schedule, chunk, threshold);
                 t.win0 = bpw0;
                 t.raw = raw; t.conf = conf;
                 t.fired = d_fired ? d_fired + q0 : nullptr;
@@ -2323,6 +2317,23 @@ PB_API int pb_score_corpus_pairs(pb_handle* h, const int16_t* d_pcm, const int64
 
 // ------------------------------------------------------------------------------------------------
 // pool models over labelled clips (dataset.cuh)
+
+// Refuses an empty recording: labelled clips are vectorized, and empty audio has no vector.
+static int check_nonempty(const int64_t* h_offsets, int64_t n_rec) {
+    for (int64_t r = 0; r < n_rec; ++r)
+        if (h_offsets[r + 1] == h_offsets[r]) return fail(PB_ERR_INVALID, "recording %lld is empty: cannot vectorize empty audio", (long long)r);
+    return PB_OK;
+}
+
+// Zeroes the statistics pb_score_dataset and pb_score_rows add up (the outputs that are not null).
+static int zero_stats(int64_t k, int32_t n_thr, int64_t* d_count, int64_t* d_hist, int64_t* d_fit, unsigned long long* d_n_miss,
+                      cudaStream_t s) {
+    if (d_count) CK(cudaMemsetAsync(d_count, 0, (size_t)k * 2 * sizeof(int64_t), s));
+    if (d_hist) CK(cudaMemsetAsync(d_hist, 0, (size_t)k * 2 * (2 * n_thr + 1) * sizeof(int64_t), s));
+    if (d_fit) CK(cudaMemsetAsync(d_fit, 0, (size_t)k * 6 * sizeof(int64_t), s));
+    if (d_n_miss) CK(cudaMemsetAsync(d_n_miss, 0, sizeof(unsigned long long), s));
+    return PB_OK;
+}
 
 // The refusals pb_score_dataset and pb_score_rows share beyond their networks: pairs (rows of k, clips of n_rec), thresholds,
 // the miss list and the fit's 2^24 entries per (row, label).  thr receives the thresholds rounded to float32.
@@ -2384,17 +2395,12 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
     if (!h->pool) return fail(PB_ERR_STATE, "no model pool: call pb_set_pool first");
     if (max_samples < 1) return fail(PB_ERR_INVALID, "max_samples = %lld must be >= 1", (long long)max_samples);
     if (n_rec > 0 && !h_targets) return fail(PB_ERR_INVALID, "null h_targets");
-    for (int64_t r = 0; r < n_rec; ++r)
-        if (h_offsets[r + 1] == h_offsets[r]) return fail(PB_ERR_INVALID, "recording %lld is empty: cannot vectorize empty audio", (long long)r);
+    rc = check_nonempty(h_offsets, n_rec);
+    if (rc != PB_OK) return rc;
     if (k < 0 || k > INT32_MAX / 2) return fail(PB_ERR_INVALID, "k = %lld outside [0, 2^30)", (long long)k);
     if (k > 0 && !h_model_ids) return fail(PB_ERR_INVALID, "null h_model_ids");
-    for (int64_t i = 0; i < k; ++i) {
-        const int32_t m = h_model_ids[i];
-        if (m < 0 || m >= h->pool_models)
-            return fail(PB_ERR_INVALID, "model id %d (entry %lld) outside [0, max_models = %d)", m, (long long)i, h->pool_models);
-        if (h->pool_cd_of[m] == h->pool_cd.end())
-            return fail(PB_ERR_INVALID, "pool slot %d (entry %lld) holds no model: pb_pool_load it first", m, (long long)i);
-    }
+    rc = check_pool_ids(h, h_model_ids, k, "entry");
+    if (rc != PB_OK) return rc;
     std::vector<float> thr;
     rc = check_dataset_stats(k, n_rec, h_targets, h_pair_rows, h_pair_recs, n_pairs, h_thresholds, n_thr, d_hist, d_fit, d_miss,
                              miss_capacity, d_n_miss, thr);
@@ -2402,16 +2408,8 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
     const bool by_pairs = n_pairs > 0;
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    const int bins = 2 * n_thr + 1;
-    auto zero = [&]() -> int {
-        if (d_count) CK(cudaMemsetAsync(d_count, 0, (size_t)k * 2 * sizeof(int64_t), s));
-        if (d_hist) CK(cudaMemsetAsync(d_hist, 0, (size_t)k * 2 * bins * sizeof(int64_t), s));
-        if (d_fit) CK(cudaMemsetAsync(d_fit, 0, (size_t)k * 6 * sizeof(int64_t), s));
-        if (misses) CK(cudaMemsetAsync(d_n_miss, 0, sizeof(unsigned long long), s));
-        return PB_OK;
-    };
-    if (n_rec == 0 || k == 0) return zero();
-    const CorpusPlan plan = corpus_plan(h, d_pcm, h_offsets, n_rec, PB_CORPUS_LISTENER, 1, max_samples);
+    if (n_rec == 0 || k == 0) return zero_stats(k, n_thr, d_count, d_hist, d_fit, d_n_miss, s);
+    const CorpusPlan plan = corpus_plan(h, (uintptr_t)d_pcm % 16 == 0, h_offsets, n_rec, PB_CORPUS_LISTENER, 1, max_samples);
     // entries per batch: all of them into the caller's d_raw, else as many as the capped raw buffer holds; the cross product
     // in whole rows, pairs in runs of consecutive pairs
     const int NM = h->corpus_pool_nm ? h->corpus_pool_nm : CORPUS_POOL_NM;
@@ -2419,9 +2417,7 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
     std::vector<int2> groups, slot_pairs, row_pairs;
     std::vector<int64_t> g0;
     std::vector<long long> P;
-    CorpusPoolSizes ps;
-    ps.thr = d_hist ? (size_t)n_thr : 0;
-    ps.targets = stats ? (size_t)n_rec : 0;
+    size_t max_tiles = 0;
     if (by_pairs) {
         cap = std::min<int64_t>(n_pairs, h->corpus_pairs_batch > 0 ? h->corpus_pairs_batch : CORPUS_PAIRS_BATCH);
         slot_pairs.resize((size_t)n_pairs);
@@ -2433,10 +2429,6 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
             P[i] = i;
         }
         P[n_pairs] = n_pairs;
-        ps.raw = !d_raw ? (size_t)cap : 0;
-        ps.pairs = (size_t)n_pairs;
-        ps.pw0 = (size_t)cap + 1;
-        ps.starts = (size_t)cap;
         for (int64_t p0 = 0; p0 < n_pairs; p0 += cap) {               // the scan tiles of the largest batch
             const int64_t p1 = std::min(n_pairs, p0 + cap);
             size_t tiles = 0;
@@ -2444,7 +2436,7 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
                 for (e = a + 1; e < p1 && slot_pairs[e].x == slot_pairs[a].x;) ++e;
                 tiles += (size_t)((e - a + 63) / 64);
             }
-            ps.tiles = std::max(ps.tiles, tiles);
+            max_tiles = std::max(max_tiles, tiles);
         }
     } else {
         if (!d_raw) {
@@ -2453,35 +2445,49 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
             rows = std::min<int64_t>(rows, k);
         }
         pool_corpus_groups(h, h_model_ids, k, rows, NM, groups, g0);
-        ps.groups = groups.size();
-        ps.raw = !d_raw ? (size_t)(rows * n_rec) : 0;
     }
-    rc = corpus_reserve(h, plan, n_rec, ps, s);
+    // the histogram's float32 thresholds and the recordings' labels; then the pair tables, or the cross product's model groups
+    // and raw of one batch of rows when the caller passes no d_raw
+    CorpusWs w;
+    float* d_thr;
+    uint8_t* d_targets;
+    PairsWs pw{};
+    int2* d_groups = nullptr;
+    float* d_own_raw = nullptr;
+    rc = reserve_workspace(h, s, [&](Carve& c) {
+        w = corpus_ws(c, h, plan);
+        d_thr = c.take<float>(d_hist ? (size_t)n_thr : 0); d_targets = c.take<uint8_t>(stats ? (size_t)n_rec : 0);
+        if (by_pairs) {
+            pw = pairs_ws(c, (size_t)n_pairs, (size_t)cap + 1, (size_t)cap, max_tiles, !d_raw ? (size_t)cap : 0);
+        } else {
+            d_groups = c.take<int2>(groups.size()); d_own_raw = c.take<float>(!d_raw ? (size_t)(rows * n_rec) : 0);
+        }
+    });
     if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        rc = corpus_k1(h, plan, d_pcm, n_rec, divisor, PB_CORPUS_LISTENER, 1, s);
+        rc = corpus_k1(h, plan, w, d_pcm, n_rec, divisor, PB_CORPUS_LISTENER, 1, s);
         if (rc != PB_OK) return rc;
-        rc = zero();
+        rc = zero_stats(k, n_thr, d_count, d_hist, d_fit, d_n_miss, s);
         if (rc != PB_OK) return rc;
-        if (d_hist) CK(cudaMemcpyAsync(h->d_ds_thr.get(), thr.data(), thr.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-        if (stats) CK(cudaMemcpyAsync(h->d_ds_targets.get(), h_targets, (size_t)n_rec, cudaMemcpyHostToDevice, s));
+        if (d_hist) CK(cudaMemcpyAsync(d_thr, thr.data(), thr.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        if (stats) CK(cudaMemcpyAsync(d_targets, h_targets, (size_t)n_rec, cudaMemcpyHostToDevice, s));
         ProfScope prof(h, 1, s);
-        const K2In in = corpus_k2in(h);
+        const K2In in = corpus_k2in(h, w);
         DatasetStats D{};
-        D.targets = h->d_ds_targets.get(); D.thr = d_hist ? h->d_ds_thr.get() : nullptr; D.n_thr = n_thr;
+        D.targets = d_targets; D.thr = d_hist ? d_thr : nullptr; D.n_thr = n_thr;
         D.count = d_count; D.hist = d_hist; D.fit = d_fit;
         D.miss_thr = (float)miss_threshold; D.miss = d_miss; D.capacity = miss_capacity; D.n_miss = d_n_miss;
         if (!by_pairs) {
-            CK(cudaMemcpyAsync(h->d_cp_groups.get(), groups.data(), groups.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(d_groups, groups.data(), groups.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
             const bool split = pool_corpus_keras(NM);
             const int order = h->corpus_pool_order >= 0 ? h->corpus_pool_order : CORPUS_POOL_GROUPS_FAST;
             for (int64_t b0 = 0, b = 0; b0 < k; b0 += rows, ++b) {
                 const int64_t nb = std::min<int64_t>(k, b0 + rows) - b0;
-                float* raw = d_raw ? d_raw + b0 * n_rec : h->d_cp_raw.get();
+                float* raw = d_raw ? d_raw + b0 * n_rec : d_own_raw;
                 PoolCorpus c{};
                 c.slots = h->d_pool_slots.get(); c.n_tiles = (n_rec + 63) / 64; c.raw = raw; c.W = n_rec; c.groups_fast = order;
                 for (int ka = 0; ka < 2; ++ka) {
-                    c.groups = h->d_cp_groups.get() + g0[2 * b + ka] * NM;
+                    c.groups = d_groups + g0[2 * b + ka] * NM;
                     c.n_groups = g0[2 * b + ka + 1] - g0[2 * b + ka];
                     rc = launch_pool_corpus_nm(NM, split && ka == 1, c, in, s);
                     if (rc != PB_OK) return rc;
@@ -2496,22 +2502,21 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
             }
             return PB_OK;
         }
-        CK(cudaMemcpyAsync(h->d_pp_pairs.get(), row_pairs.data(), row_pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_pp_pw0.get(), P.data(), (size_t)(cap + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(pw.pairs, row_pairs.data(), row_pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(pw.pw0, P.data(), (size_t)(cap + 1) * sizeof(long long), cudaMemcpyHostToDevice, s));
         std::vector<PairTile> tiles;
         for (int64_t p0 = 0; p0 < n_pairs; p0 += cap) {
             const int64_t p1 = std::min(n_pairs, p0 + cap), nb = p1 - p0;
-            const int2* bpairs = h->d_pp_pairs.get() + p0;
-            float* raw = d_raw ? d_raw + p0 : h->d_cp_raw.get();
+            const int2* bpairs = pw.pairs + p0;
+            float* raw = d_raw ? d_raw + p0 : pw.raw;
             // one pair-window per pair: the batch's prefix is 0 .. nb
-            pairs_windows_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, s>>>(h->d_pp_pw0.get(), bpairs, (int)nb, nb, h->d_cw_win0.get(),
-                                                                             h->d_cw_starts.get(), h->d_pp_starts.get());
+            pairs_windows_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, s>>>(pw.pw0, bpairs, (int)nb, nb, w.win0, w.starts, pw.starts);
             CK(cudaGetLastError());
             const int64_t n_keras = pair_tiles(h, slot_pairs, P, p0, p1, tiles);
-            CK(cudaMemcpyAsync(h->d_pp_tiles.get(), tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(pw.tiles, tiles.data(), tiles.size() * sizeof(PairTile), cudaMemcpyHostToDevice, s));
             PairsCorpus c{};
-            c.slots = h->d_pool_slots.get(); c.starts = h->d_pp_starts.get(); c.raw = raw;
-            c.tiles = h->d_pp_tiles.get(); c.n_tiles = n_keras;
+            c.slots = h->d_pool_slots.get(); c.starts = pw.starts; c.raw = raw;
+            c.tiles = pw.tiles; c.n_tiles = n_keras;
             rc = launch_pairs_corpus<true>(c, in, s);
             if (rc != PB_OK) return rc;
             c.tiles += n_keras; c.n_tiles = (int64_t)tiles.size() - n_keras;
@@ -2531,7 +2536,6 @@ PB_API int pb_score_dataset(pb_handle* h, const int16_t* d_pcm, const int64_t* h
 // training (train.cuh)
 
 constexpr size_t TRAIN_WS_CAP = size_t(256) << 20;     // workspace of one group of rows
-constexpr size_t TRAIN_ALIGN = 256;
 
 // The fused family's front end, which pb_vectorize_clips and the training kernels cover.
 static int check_train_front_end(const pb_handle* h) {
@@ -2543,6 +2547,18 @@ static int check_train_front_end(const pb_handle* h) {
     return PB_OK;
 }
 
+// K1 over labelled clips (one window each, crop > 0 in the plan) and their windows gathered into d_inputs.
+static int vectorize(pb_handle* h, const CorpusPlan& p, const CorpusWs& w, const int16_t* d_pcm, int64_t n_rec, int32_t divisor,
+                     float* d_inputs, cudaStream_t s) {
+    const int rc = corpus_k1(h, p, w, d_pcm, n_rec, divisor, PB_CORPUS_LISTENER, 1, s);
+    if (rc != PB_OK) return rc;
+    const int T = h->cfg.n_features, F = h->feat;
+    const long long total = (long long)n_rec * T * F;
+    vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w.rows, w.starts, h->row_stride, T, F, n_rec, d_inputs);
+    CK(cudaGetLastError());
+    return PB_OK;
+}
+
 PB_API int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t* h_offsets, int64_t n_rec, int32_t divisor,
                               int64_t max_samples, float* d_inputs, void* stream) {
     if (!h) return fail(PB_ERR_INVALID, "null handle");
@@ -2551,25 +2567,16 @@ PB_API int pb_vectorize_clips(pb_handle* h, const int16_t* d_pcm, const int64_t*
     rc = check_corpus(h, d_pcm, h_offsets, n_rec, divisor, PB_CORPUS_LISTENER, 1, d_inputs, true, nullptr, nullptr);
     if (rc != PB_OK) return rc;
     if (max_samples < 1) return fail(PB_ERR_INVALID, "max_samples = %lld must be >= 1", (long long)max_samples);
-    for (int64_t r = 0; r < n_rec; ++r)
-        if (h_offsets[r + 1] == h_offsets[r]) return fail(PB_ERR_INVALID, "recording %lld is empty: cannot vectorize empty audio", (long long)r);
+    rc = check_nonempty(h_offsets, n_rec);
+    if (rc != PB_OK) return rc;
     if (n_rec == 0) return PB_OK;
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    const CorpusPlan plan = corpus_plan(h, d_pcm, h_offsets, n_rec, PB_CORPUS_LISTENER, 1, max_samples);
-    rc = corpus_reserve(h, plan, n_rec, CorpusPoolSizes{}, s);
+    const CorpusPlan plan = corpus_plan(h, (uintptr_t)d_pcm % 16 == 0, h_offsets, n_rec, PB_CORPUS_LISTENER, 1, max_samples);
+    CorpusWs w;
+    rc = reserve_workspace(h, s, [&](Carve& c) { w = corpus_ws(c, h, plan); });
     if (rc != PB_OK) return rc;
-    auto launch = [&]() -> int {
-        rc = corpus_k1(h, plan, d_pcm, n_rec, divisor, PB_CORPUS_LISTENER, 1, s);
-        if (rc != PB_OK) return rc;
-        const int T = h->cfg.n_features, F = h->feat;
-        const long long total = (long long)n_rec * T * F;
-        vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->row_stride,
-                                                                               T, F, n_rec, d_inputs);
-        CK(cudaGetLastError());
-        return PB_OK;
-    };
-    return corpus_done(h, s, launch());
+    return corpus_done(h, s, vectorize(h, plan, w, d_pcm, n_rec, divisor, d_inputs, s));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2625,49 +2632,32 @@ PB_API int pb_add_noise(pb_handle* h, const int16_t* d_pcm, const int64_t* h_off
 
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
-    DevArray<NoiseItem> f_items; DevArray<long long> f_seg0; DevArray<unsigned long long> f_sums; DevArray<int16_t> f_pcm;
-    cudaError_t e = corpus_grow(h->d_nz_items, (size_t)n_items, f_items);
-    if (e == cudaSuccess) e = corpus_grow(h->d_nz_seg0, (size_t)n_items + 1, f_seg0);
-    if (e == cudaSuccess) e = corpus_grow(h->d_nz_sums, 2 * (size_t)n_items, f_sums);
-    if (e == cudaSuccess) e = corpus_grow(h->d_nz_pcm, (size_t)ws, f_pcm);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return fail(PB_ERR_CUDA, "noise workspace allocation failed (%lld items): %s", (long long)n_items, cudaGetErrorString(e));
-    }
-    if (f_items.get() || f_seg0.get() || f_sums.get() || f_pcm.get()) CK(cudaEventSynchronize(h->corpus_ev));
-    if (f_items.get()) h->d_nz_items = std::move(f_items);
-    if (f_seg0.get()) h->d_nz_seg0 = std::move(f_seg0);
-    if (f_sums.get()) h->d_nz_sums = std::move(f_sums);
-    if (f_pcm.get()) h->d_nz_pcm = std::move(f_pcm);
+    // the workspace's audio starts at a multiple of 256 bytes, so every item may take the fast K1
     CorpusPlan plan;
-    if (d_inputs) {
-        plan = corpus_plan(h, h->d_nz_pcm.get(), ws_off.data(), n_items, PB_CORPUS_LISTENER, 1, max_samples, ws_len.data());
-        rc = corpus_reserve(h, plan, n_items, CorpusPoolSizes{}, s);
-        if (rc != PB_OK) return rc;
-    } else {
-        CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
-    }
+    if (d_inputs) plan = corpus_plan(h, true, ws_off.data(), n_items, PB_CORPUS_LISTENER, 1, max_samples, ws_len.data());
+    // the items, each item's first segment, their (sum x^2, sum n^2), and with d_inputs the mixed clips' cropped tails
+    CorpusWs w{};
+    NoiseItem* d_items;
+    long long* d_seg0;
+    unsigned long long* d_sums;
+    int16_t* d_ws_pcm = nullptr;
+    rc = reserve_workspace(h, s, [&](Carve& c) {
+        if (d_inputs) w = corpus_ws(c, h, plan);
+        d_items = c.take<NoiseItem>((size_t)n_items); d_seg0 = c.take<long long>(seg0.size());
+        d_sums = c.take<unsigned long long>(2 * (size_t)n_items);
+        if (d_inputs) d_ws_pcm = c.take<int16_t>((size_t)ws);
+    });
+    if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        CK(cudaMemcpyAsync(h->d_nz_items.get(), items.data(), items.size() * sizeof(NoiseItem), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_nz_seg0.get(), seg0.data(), seg0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-        CK(cudaMemsetAsync(h->d_nz_sums.get(), 0, 2 * (size_t)n_items * sizeof(unsigned long long), s));
-        noise_sums_kernel<<<(unsigned)n_seg, NZ_THREADS, 0, s>>>(d_pcm, d_noise, n_noise, h->d_nz_items.get(), h->d_nz_seg0.get(),
-                                                                 (int)n_items, h->d_nz_sums.get());
+        CK(cudaMemcpyAsync(d_items, items.data(), items.size() * sizeof(NoiseItem), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_seg0, seg0.data(), seg0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(d_sums, 0, 2 * (size_t)n_items * sizeof(unsigned long long), s));
+        noise_sums_kernel<<<(unsigned)n_seg, NZ_THREADS, 0, s>>>(d_pcm, d_noise, n_noise, d_items, d_seg0, (int)n_items, d_sums);
         CK(cudaGetLastError());
-        noise_mix_kernel<<<(unsigned)n_seg, NZ_THREADS, 0, s>>>(d_pcm, d_noise, n_noise, h->d_nz_items.get(), h->d_nz_seg0.get(),
-                                                                (int)n_items, h->d_nz_sums.get(), d_out,
-                                                                d_inputs ? h->d_nz_pcm.get() : nullptr);
+        noise_mix_kernel<<<(unsigned)n_seg, NZ_THREADS, 0, s>>>(d_pcm, d_noise, n_noise, d_items, d_seg0, (int)n_items, d_sums, d_out,
+                                                                d_ws_pcm);
         CK(cudaGetLastError());
-        if (!d_inputs) return PB_OK;
-        rc = corpus_k1(h, plan, h->d_nz_pcm.get(), n_items, divisor, PB_CORPUS_LISTENER, 1, s);
-        if (rc != PB_OK) return rc;
-        const int T = h->cfg.n_features, F = h->feat;
-        const long long total = (long long)n_items * T * F;
-        vectorize_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->row_stride,
-                                                                               T, F, n_items, d_inputs);
-        CK(cudaGetLastError());
-        return PB_OK;
+        return d_inputs ? vectorize(h, plan, w, d_ws_pcm, n_items, divisor, d_inputs, s) : PB_OK;
     };
     return corpus_done(h, s, launch());
 }
@@ -2789,67 +2779,56 @@ PB_API int pb_generate(pb_handle* h, const int16_t* d_bg, const int64_t* h_bg_of
 
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
-    DevArray<GenRec> f_recs; DevArray<long long> f_rseg0, f_tile0, f_wins; DevArray<unsigned long long> f_sums;
-    DevArray<GenItem> f_items; DevArray<GenSeg> f_segs; DevArray<int16_t> f_pcm;
-    cudaError_t e = corpus_grow(h->d_gen_recs, (size_t)n_recs, f_recs);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_rseg0, rseg0.size(), f_rseg0);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_sums, (size_t)n_recs, f_sums);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_items, (size_t)n_items, f_items);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_tile0, tile0.size(), f_tile0);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_segs, (size_t)n_dsegs, f_segs);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_wins, (size_t)n_windows, f_wins);
-    if (e == cudaSuccess) e = corpus_grow(h->d_gen_pcm, (size_t)ws, f_pcm);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return fail(PB_ERR_CUDA, "generate workspace allocation failed (%lld items, %lld samples): %s", (long long)n_items, out,
-                    cudaGetErrorString(e));
-    }
-    if (f_recs.get() || f_rseg0.get() || f_sums.get() || f_items.get() || f_tile0.get() || f_segs.get() || f_wins.get() || f_pcm.get())
-        CK(cudaEventSynchronize(h->corpus_ev));        // the previous call may still read what is replaced
-    if (f_recs.get()) h->d_gen_recs = std::move(f_recs);
-    if (f_rseg0.get()) h->d_gen_rseg0 = std::move(f_rseg0);
-    if (f_sums.get()) h->d_gen_sums = std::move(f_sums);
-    if (f_items.get()) h->d_gen_items = std::move(f_items);
-    if (f_tile0.get()) h->d_gen_tile0 = std::move(f_tile0);
-    if (f_segs.get()) h->d_gen_segs = std::move(f_segs);
-    if (f_wins.get()) h->d_gen_wins = std::move(f_wins);
-    if (f_pcm.get()) h->d_gen_pcm = std::move(f_pcm);
+    // the workspace's audio starts at a multiple of 256 bytes, so every stream may take the fast K1
     CorpusPlan plan;
     std::vector<long long> wins;
     if (vec) {
-        plan = corpus_plan(h, h->d_gen_pcm.get(), ws_off.data(), n_items, PB_CORPUS_LISTENER, chunk, 0, ws_len.data());
+        plan = corpus_plan(h, true, ws_off.data(), n_items, PB_CORPUS_LISTENER, chunk, 0, ws_len.data());
         wins.resize((size_t)n_windows);
         for (int64_t w = 0; w < n_windows; ++w) wins[w] = plan.win0[h_windows[2 * w]] + h_windows[2 * w + 1];
-        rc = corpus_reserve(h, plan, n_items, CorpusPoolSizes{}, s);
-        if (rc != PB_OK) return rc;
-    } else {
-        CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
     }
+    // the recordings whose sums of squares the mix needs, each one's first CTA of the sums, their sums, the items, each item's
+    // first CTA of the mix, each item's own copy of the segments covering it; with d_inputs the chosen windows' places in the
+    // window table and the generated streams
+    CorpusWs w{};
+    GenRec* d_recs;
+    long long* d_rseg0;
+    unsigned long long* d_sums;
+    GenItem* d_items;
+    long long* d_tile0;
+    GenSeg* d_segs;
+    long long* d_wins = nullptr;
+    int16_t* d_ws_pcm = nullptr;
+    rc = reserve_workspace(h, s, [&](Carve& c) {
+        if (vec) w = corpus_ws(c, h, plan);
+        d_recs = c.take<GenRec>((size_t)n_recs); d_rseg0 = c.take<long long>(rseg0.size());
+        d_sums = c.take<unsigned long long>((size_t)n_recs); d_items = c.take<GenItem>((size_t)n_items);
+        d_tile0 = c.take<long long>(tile0.size()); d_segs = c.take<GenSeg>((size_t)n_dsegs);
+        if (vec) { d_wins = c.take<long long>((size_t)n_windows); d_ws_pcm = c.take<int16_t>((size_t)ws); }
+    });
+    if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        CK(cudaMemcpyAsync(h->d_gen_recs.get(), recs.data(), recs.size() * sizeof(GenRec), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_gen_rseg0.get(), rseg0.data(), rseg0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_gen_items.get(), items.data(), items.size() * sizeof(GenItem), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(h->d_gen_tile0.get(), tile0.data(), tile0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
-        if (n_dsegs > 0) CK(cudaMemcpyAsync(h->d_gen_segs.get(), segs.data(), segs.size() * sizeof(GenSeg), cudaMemcpyHostToDevice, s));
-        CK(cudaMemsetAsync(h->d_gen_sums.get(), 0, (size_t)n_recs * sizeof(unsigned long long), s));
+        CK(cudaMemcpyAsync(d_recs, recs.data(), recs.size() * sizeof(GenRec), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_rseg0, rseg0.data(), rseg0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_items, items.data(), items.size() * sizeof(GenItem), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_tile0, tile0.data(), tile0.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        if (n_dsegs > 0) CK(cudaMemcpyAsync(d_segs, segs.data(), segs.size() * sizeof(GenSeg), cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(d_sums, 0, (size_t)n_recs * sizeof(unsigned long long), s));
         if (n_rseg > 0) {
-            gen_sums_kernel<<<(unsigned)n_rseg, GEN_THREADS, 0, s>>>(d_bg, d_clips, h->d_gen_recs.get(), h->d_gen_rseg0.get(), (int)n_recs,
-                                                                    h->d_gen_sums.get());
+            gen_sums_kernel<<<(unsigned)n_rseg, GEN_THREADS, 0, s>>>(d_bg, d_clips, d_recs, d_rseg0, (int)n_recs, d_sums);
             CK(cudaGetLastError());
         }
-        gen_mix_kernel<<<(unsigned)n_tiles, GEN_THREADS, 0, s>>>(d_bg, d_clips, h->d_gen_recs.get(), h->d_gen_sums.get(), h->d_gen_items.get(),
-                                                                h->d_gen_tile0.get(), (int)n_items, h->d_gen_segs.get(), d_out,
-                                                                vec ? h->d_gen_pcm.get() : nullptr);
+        gen_mix_kernel<<<(unsigned)n_tiles, GEN_THREADS, 0, s>>>(d_bg, d_clips, d_recs, d_sums, d_items, d_tile0, (int)n_items, d_segs,
+                                                                d_out, d_ws_pcm);
         CK(cudaGetLastError());
         if (!vec) return PB_OK;
-        rc = corpus_k1(h, plan, h->d_gen_pcm.get(), n_items, divisor, PB_CORPUS_LISTENER, chunk, s);
+        rc = corpus_k1(h, plan, w, d_ws_pcm, n_items, divisor, PB_CORPUS_LISTENER, chunk, s);
         if (rc != PB_OK) return rc;
-        CK(cudaMemcpyAsync(h->d_gen_wins.get(), wins.data(), wins.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_wins, wins.data(), wins.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
         const int T = h->cfg.n_features, F = h->feat;
         const long long total = (long long)n_windows * T * F;
-        gen_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->d_cw_rows.get(), h->d_cw_starts.get(), h->d_gen_wins.get(),
-                                                                         h->row_stride, T, F, n_windows, d_inputs);
+        gen_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w.rows, w.starts, d_wins, h->row_stride, T, F, n_windows,
+                                                                         d_inputs);
         CK(cudaGetLastError());
         return PB_OK;
     };
@@ -2993,18 +2972,6 @@ static std::vector<TrainGroup> train_groups(const TrainEntries& te, int64_t k, i
     return out;
 }
 
-// Carves typed arrays out of the training arena (a null base only measures).
-struct TrainCarve {
-    uint8_t* base;
-    size_t at = 0;
-    template <typename T> T* take(size_t n) {
-        at = (at + TRAIN_ALIGN - 1) / TRAIN_ALIGN * TRAIN_ALIGN;
-        T* p = base ? reinterpret_cast<T*>(base + at) : nullptr;
-        at += std::max<size_t>(n, 1) * sizeof(T);
-        return p;
-    }
-};
-
 struct TrainWs {
     TrainRowDev* rows; uint8_t* targets; double* loss_acc;
     int* ent; int* order; int* vals; uint64_t* keys; uint64_t* keys2; int* seg; int* seg_row;
@@ -3012,9 +2979,8 @@ struct TrainWs {
     long long* soff; float* state;   // wide calls only (state_floats > 0)
 };
 
-static TrainWs train_layout(uint8_t* base, int64_t k, int64_t n_rec, int64_t n, int64_t rows, int64_t tiles, int64_t steps,
-                            int64_t max_tiles, size_t sort_bytes, size_t stride, size_t state_floats, size_t* bytes) {
-    TrainCarve c{base};
+static TrainWs train_layout(Carve& c, int64_t k, int64_t n_rec, int64_t n, int64_t rows, int64_t tiles, int64_t steps,
+                            int64_t max_tiles, size_t sort_bytes, size_t stride, size_t state_floats) {
     TrainWs w{};
     w.rows = c.take<TrainRowDev>((size_t)k); w.targets = c.take<uint8_t>((size_t)n_rec); w.loss_acc = c.take<double>((size_t)k);
     w.ent = c.take<int>((size_t)n); w.order = c.take<int>((size_t)n); w.vals = c.take<int>((size_t)n);
@@ -3024,7 +2990,6 @@ static TrainWs train_layout(uint8_t* base, int64_t k, int64_t n_rec, int64_t n, 
     w.part = c.take<float>((size_t)max_tiles * stride); w.part_loss = c.take<double>((size_t)max_tiles);
     w.sort_tmp = c.take<uint8_t>(sort_bytes);
     if (state_floats) { w.soff = c.take<long long>((size_t)tiles); w.state = c.take<float>(state_floats); }
-    if (bytes) *bytes = c.at;
     return w;
 }
 
@@ -3076,23 +3041,12 @@ static int train_run(pb_handle* h, const float* d_inputs, int64_t n_rec, const u
         sort_max = std::max(sort_max, g.sort_bytes);
         state_max = std::max(state_max, g.state_floats);
     }
-    size_t bytes = 0;
-    train_layout(nullptr, k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, stride, state_max, &bytes);
-    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
-    if (h->d_tr_ws.size() < bytes) {
-        DevArray<uint8_t> fresh;
-        const cudaError_t e = fresh.alloc(bytes);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(PB_ERR_CUDA, "training workspace allocation failed (%zu bytes): %s", bytes, cudaGetErrorString(e));
-        }
-        CK(cudaEventSynchronize(h->corpus_ev));                     // the previous call may still use the arena
-        h->d_tr_ws = std::move(fresh);
-    }
     if (!wide) CK(ensure_dyn_smem(train_grad_kernel, train_smem(h->cfg.n_features)));
-    CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
-    const TrainWs w = train_layout(h->d_tr_ws.get(), k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, stride,
-                                   state_max, nullptr);
+    TrainWs w;
+    const int rc = reserve_workspace(h, s, [&](Carve& c) {
+        w = train_layout(c, k, n_rec, n_max, rows_max, tiles_max, steps_max, ptiles_max, sort_max, stride, state_max);
+    });
+    if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
         const int n_loss = train ? epochs : 1;
         if (d_loss) {
@@ -3245,14 +3199,14 @@ PB_API int pb_train_wide_loss(pb_handle* h, const float* d_inputs, int64_t n_rec
 // networks from weight rows over labelled clips (rows.cuh)
 
 constexpr size_t ROWS_FRAG_CAP = size_t(256) << 20;   // fragments of one group of networks
-constexpr int64_t ROWS_RAW_CAP = 256ll << 20;         // raw of one cross-product batch kept in the arena (no d_raw)
+constexpr int64_t ROWS_RAW_CAP = 256ll << 20;         // raw of one cross-product batch kept in the workspace (no d_raw)
 constexpr int64_t ROWS_PAIRS_BATCH = 1ll << 25;       // pairs per batch: 8 B of window start and 4 B of raw each
 constexpr int ROWS_MAX_NETS = 65535;                  // networks per group (gridDim.y of the split and the scan)
 
-// Arena bytes of one network's fragments, bias and table entry at feature size F (upload_wide's sizes, each part aligned).
+// Workspace bytes of one network's fragments, bias and table entry at feature size F (upload_wide's sizes, each part aligned).
 static size_t rows_net_bytes(int H, int F) {
     const size_t FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
-    auto al = [](size_t b) { return (b + TRAIN_ALIGN - 1) / TRAIN_ALIGN * TRAIN_ALIGN; };
+    auto al = [](size_t b) { return (b + WS_ALIGN - 1) / WS_ALIGN * WS_ALIGN; };
     return al(KS * (HP / 4) * 32 * sizeof(uint4)) + al(KS * (HP / 8) * 32 * sizeof(uint4)) + al(3 * HP * sizeof(float)) +
            sizeof(GruWideW) + sizeof(int);
 }
@@ -3300,15 +3254,7 @@ PB_API int pb_score_rows(pb_handle* h, const float* d_inputs, int64_t n_rec, con
     const bool by_pairs = n_pairs > 0;
     CK(cudaSetDevice(h->cfg.device));
     cudaStream_t s = (cudaStream_t)stream;
-    const int bins = 2 * n_thr + 1;
-    auto zero = [&]() -> int {
-        if (d_count) CK(cudaMemsetAsync(d_count, 0, (size_t)k * 2 * sizeof(int64_t), s));
-        if (d_hist) CK(cudaMemsetAsync(d_hist, 0, (size_t)k * 2 * bins * sizeof(int64_t), s));
-        if (d_fit) CK(cudaMemsetAsync(d_fit, 0, (size_t)k * 6 * sizeof(int64_t), s));
-        if (misses) CK(cudaMemsetAsync(d_n_miss, 0, sizeof(unsigned long long), s));
-        return PB_OK;
-    };
-    if (n_rec == 0 || k == 0) return zero();
+    if (n_rec == 0 || k == 0) return zero_stats(k, n_thr, d_count, d_hist, d_fit, d_n_miss, s);
 
     const int T = h->cfg.n_features, F = h->feat;
     const int net_cap = h->rows_group_nets > 0 ? std::min(h->rows_group_nets, ROWS_MAX_NETS) : ROWS_MAX_NETS;
@@ -3387,34 +3333,17 @@ PB_API int pb_score_rows(pb_handle* h, const float* d_inputs, int64_t n_rec, con
         long long* starts; float* raw_slot; float* raw;
     };
     const size_t raw_n = d_raw ? 0 : by_pairs ? (size_t)batch_cap : (size_t)(batch_rows * n_rec);
-    auto layout = [&](uint8_t* base, size_t* bytes) {
-        TrainCarve c{base};
-        RowsWs w{};
+    CK(ensure_dyn_smem(gru_wide_rows_kernel, smem_max));
+    RowsWs w;
+    rc = reserve_workspace(h, s, [&](Carve& c) {
         w.nets = c.take<GruWideW>(net_max); w.rows = c.take<int>(net_max); w.frag = c.take<uint8_t>(bytes_max);
         w.targets = c.take<uint8_t>(stats ? (size_t)n_rec : 0); w.thr = c.take<float>((size_t)n_thr);
         w.pairs = c.take<int2>((size_t)n_pairs); w.slot_pair = c.take<int>(slots_max); w.tile_net = c.take<int>(slots_max / WG_STREAMS);
         w.starts = c.take<long long>(slots_max); w.raw_slot = c.take<float>(slots_max); w.raw = c.take<float>(raw_n);
-        if (bytes) *bytes = c.at;
-        return w;
-    };
-    size_t bytes = 0;
-    layout(nullptr, &bytes);
-    if (!h->corpus_ev) CK(cudaEventCreateWithFlags(&h->corpus_ev, cudaEventDisableTiming));
-    if (h->d_tr_ws.size() < bytes) {
-        DevArray<uint8_t> fresh;
-        const cudaError_t e = fresh.alloc(bytes);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(PB_ERR_CUDA, "workspace allocation failed (%zu bytes): %s", bytes, cudaGetErrorString(e));
-        }
-        CK(cudaEventSynchronize(h->corpus_ev));                     // the previous call may still use the arena
-        h->d_tr_ws = std::move(fresh);
-    }
-    CK(ensure_dyn_smem(gru_wide_rows_kernel, smem_max));
-    CK(cudaStreamWaitEvent(s, h->corpus_ev, 0));
-    const RowsWs w = layout(h->d_tr_ws.get(), nullptr);
+    });
+    if (rc != PB_OK) return rc;
     auto launch = [&]() -> int {
-        rc = zero();
+        rc = zero_stats(k, n_thr, d_count, d_hist, d_fit, d_n_miss, s);
         if (rc != PB_OK) return rc;
         if (d_hist) CK(cudaMemcpyAsync(w.thr, thr.data(), thr.size() * sizeof(float), cudaMemcpyHostToDevice, s));
         if (stats) CK(cudaMemcpyAsync(w.targets, h_targets, (size_t)n_rec, cudaMemcpyHostToDevice, s));
@@ -3432,10 +3361,10 @@ PB_API int pb_score_rows(pb_handle* h, const float* d_inputs, int64_t n_rec, con
         D.miss_thr = (float)miss_threshold; D.miss = d_miss; D.capacity = miss_capacity; D.n_miss = d_n_miss;
         std::vector<GruWideW> table;
         for (const RowsGroup& g : groups) {
-            // the group's table: fragment pointers into the arena (rows_split_kernel fills them and bd), dense_w in the row; the
+            // the group's table: fragment pointers into the workspace (rows_split_kernel fills them and bd), dense_w in the row; the
             // host buffers are staged by the copies, so the next group may refill them
             table.assign(g.nets.size(), GruWideW{});
-            TrainCarve c{w.frag};
+            Carve c{w.frag};
             for (size_t j = 0; j < g.nets.size(); ++j) {
                 const int H = h_rows[g.nets[j]].hidden, FP = (F + 7) & ~7, HP = (H + 15) & ~15, KS = (FP + HP) / 8;
                 GruWideW& n = table[j];
